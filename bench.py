@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the SchNetPack message-passing hot path on B200 (driver contract: one JSON line on rank 0).
+"""Benchmark of the SchNetPack message-passing hot path on H100 (one JSON line on rank 0).
 
     python bench.py --gpus 1 --steps 20 --warmup 5                  # CUDA path (this repo)
     python bench.py --impl reference --gpus 1 --steps 5 --warmup 1  # reference arm: CPU path on the host cores
@@ -39,7 +39,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth)"
 
 
 def workload(name: str, rank: int, batch: int | None):
@@ -308,7 +308,7 @@ def cpu_baseline_leg(args):
 
 def eager_gpu_leg(spec, params, data, dev, B, n_it=10):
     """The reference's own single-GPU eager PyTorch path (modules .to(cuda), cuBLAS SGEMM, index_select / index_add_ atomics,
-    autograd backward) on the same B200, inputs resident: the denominator of the north-star's >= 5x target."""
+    autograd backward) on the same GPU, inputs resident: the denominator of the north-star's >= 5x target."""
     try:
         run, kind = reference_engine(spec, params, data, device=dev)
         for _ in range(3):
@@ -320,12 +320,33 @@ def eager_gpu_leg(spec, params, data, dev, B, n_it=10):
         torch.cuda.synchronize()
         dt = (time.perf_counter() - t0) / n_it
         return {"value": B / dt, "unit": UNIT, "ms_per_step": 1e3 * dt, "kind": kind,
-                "what": "the reference's modules in eager PyTorch on the same B200 (wall clock, synchronised), inputs resident"}
+                "what": "the reference's modules in eager PyTorch on the same GPU (wall clock, synchronised), inputs resident"}
     except Exception as exc:  # pragma: no cover
         return {"error": repr(exc)[:200]}
 
 
 # ------------------------------------------------------------------------------------------------- CUDA arm
+DUMP_BUDGET = 64 << 20
+
+
+def dump_outputs(path, outputs):
+    """--dump-outputs: write the floating-point arrays the timed path returned in its last step as ``path/<name>.npy``
+    (float64 kept, everything else float32), so that two builds can be compared output for output on identical inputs.
+    When they exceed 64 MB in all, every array keeps the same fixed, seeded sample of its rows."""
+    os.makedirs(path, exist_ok=True)
+    arrays = {}
+    for name, t in outputs.items():
+        if torch.is_tensor(t) and t.is_floating_point():
+            a = t.detach().cpu().numpy()
+            arrays[name] = a if a.dtype == np.float64 else a.astype(np.float32)
+    total = sum(a.nbytes for a in arrays.values())
+    for name, a in arrays.items():
+        if total > DUMP_BUDGET and a.ndim > 0 and a.shape[0] > 1:
+            keep = max(1, int(a.shape[0] * (DUMP_BUDGET / total)))
+            a = a[np.sort(np.random.default_rng(0).choice(a.shape[0], keep, replace=False))]
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def run_cuda(args, rank, world, local_rank):
     import schnetpack_b200 as sb
     from schnetpack_b200 import _lib, ops
@@ -474,6 +495,8 @@ def run_cuda(args, rank, world, local_rank):
             for kind in ("fwd", "bwd"):
                 kernel_ms[kind] += [(a.elapsed_time(b), hm) for a, b, hm in pairs[kind]]
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(args.dump_outputs, out)
     t_wall = time.perf_counter() - t_wall0
     launches = launches_per_step * args.steps if use_graph else _lib.launch_count - launches0
     timing["on"] = False
@@ -559,7 +582,7 @@ def run_cuda(args, rank, world, local_rank):
                               "avg_us": 1e3 * tot_ms / n, "algorithmic_bytes_per_launch": tot_bytes / n,
                               "share_of_step": tot_ms / dev_ms, "peak_source": peak_src,
                               "model": "algorithmic bytes = no-reuse gather model of SURVEY 8(d): every gathered row counted as "
-                                       "HBM traffic; rows served by the 126 MB L2 let frac approach or exceed 1 -- `traffic` is "
+                                       "HBM traffic; rows served by the 50 MB L2 let frac approach or exceed 1 -- `traffic` is "
                                        "the DRAM bytes ncu measured",
                               "timing": "CUDA events around the kernel, inside the timed region"
                                         + (" (external event nodes of the replayed graph)" if use_graph else "")}
@@ -574,7 +597,7 @@ def run_cuda(args, rank, world, local_rank):
 
     if cf_ev:      # fused SchNet block kernel: tensor-pipe bound (SURVEY 8d: 2(R F + F^2) = 37.9 kFLOP per edge and layer)
         d = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-        tpeak = float(d.get("bf16_tflops", 1750.0))
+        tpeak = float(d.get("bf16_tflops", 989.0))     # H100 SXM data sheet, dense BF16
         n_act = int(cf_ev[0][2][0])
         ms_l = [a.elapsed_time(b) for a, b, _ in cf_ev]
         flops = n_act * 2.0 * (spec.get("n_rbf", 20) * F + F * F)
@@ -582,7 +605,7 @@ def run_cuda(args, rank, world, local_rank):
         roof = {"bound": "tensor", "achieved": ach, "peak": tpeak, "unit": "TFLOP/s", "frac": ach / tpeak, "traffic": None,
                 "kernel": "k_schnet_cfconv_fwd_tc", "launches_timed": len(ms_l), "avg_us": 1e3 * sum(ms_l) / len(ms_l),
                 "active_edges": n_act, "edge_slots": E, "share_of_step": sum(ms_l) / dev_ms,
-                "peak_source": "MEASURED_PEAKS.json bf16 dense burst" if d else "fallback (B200_PROFILING.md)",
+                "peak_source": "MEASURED_PEAKS.json bf16 dense burst" if d else "fallback (H100 SXM data sheet, dense BF16)",
                 "model": "algorithmic fp32 FLOPs of the filter network over the ACTIVE edges (padding slots dropped); the kernel "
                          "computes in 3xTF32 (3 MMAs per product, TF32 = 1/2 of the bf16 rate): its own ceiling is peak / 6",
                 "timing": "CUDA events around the kernel, inside the timed region"}
@@ -593,7 +616,7 @@ def run_cuda(args, rank, world, local_rank):
     if world == 1 and not args.no_cpu_baseline:
         cpu = cpu_baseline_leg(args)
 
-    # ---- the reference's eager single-GPU path (its own modules .to(cuda)) on this B200, for the >=5x target ---------------
+    # ---- the reference's eager single-GPU path (its own modules .to(cuda)) on this GPU, for the >=5x target ---------------
     eager = None
     if world == 1 and not args.no_cpu_baseline:
         eager = eager_gpu_leg(spec, params, data, dev, B)
@@ -653,12 +676,12 @@ def run_cuda(args, rank, world, local_rank):
 
 
 # ------------------------------------------------------------------------------------------------- spatial (cfg5) arm
-def run_spatial(args, rank, world, local_rank, steps=None, warmup=None, cpu_leg=True):
+def run_spatial(args, rank, world, local_rank, steps=None, warmup=None, cpu_leg=True, dump=True):
     """cfg5: ONE periodic box (default 262144 atoms, PaiNN 128x3, E+F) cut into `world` slabs; every rank owns a slab, holds
     read-only ghost rows of the senders it does not own, and exchanges (x, mu) ghost rows per interaction block over NCCL
     point-to-point (gradients back in the reverse sweep).  STRONG scaling: the box is fixed, `value` = whole-box evaluations
     per second.  At N=1 the same pipeline runs without a halo -- the single-GPU workload whose gathered tables (400 MB per
-    [N,3F] table) exceed the 126 MB L2, where the roofline fraction of the edge kernels is an HBM statement."""
+    [N,3F] table) exceed the 50 MB L2, where the roofline fraction of the edge kernels is an HBM statement."""
     from schnetpack_b200 import _lib, ops, parallel as P
     from schnetpack_b200.model import from_spec
     from schnetpack_b200.neighbors import neighbor_list
@@ -786,6 +809,8 @@ def run_spatial(args, rank, world, local_rank, steps=None, warmup=None, cpu_leg=
         step_ev.append((s_, e_))
     torch.cuda.synchronize()
     timing["on"] = False
+    if dump and args.dump_outputs and rank == 0 and steps > 0:
+        dump_outputs(args.dump_outputs, {"energy": energy, "forces": forces})
     launches = _lib.launch_count - c0
     clocks = sampler.stop() if sampler is not None else None
     dev_ms = sum(a.elapsed_time(b) for a, b in step_ev)
@@ -853,7 +878,7 @@ def run_spatial(args, rank, world, local_rank, steps=None, warmup=None, cpu_leg=
                           "algorithmic_bytes_per_launch": tot_bytes / len(ms_l), "share_of_step": tot_ms / dev_ms,
                           "peak_source": peak_src,
                           "model": "SURVEY 8(d) no-reuse gather model over this rank's edges / local rows; the gathered "
-                                   "tables (N_local x 1.5 KB x 2) exceed the 126 MB L2 here",
+                                   "tables (N_local x 1.5 KB x 2) exceed the 50 MB L2 here",
                           "timing": "CUDA events around the kernel, inside the timed region (rank 0)"}
     roof = None
     if roof_all:
@@ -909,6 +934,8 @@ def main():
     ap.add_argument("--spatial-steps", type=int, default=8)
     ap.add_argument("--md", action="store_true", help="also time the device-resident MD step (rows f1+f2); not part of the metric")
     ap.add_argument("--no-graph", action="store_true", help="time eager model(inputs) calls (value and e2e) instead of CUDA-graph replays")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (energy, forces, ...) as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -917,7 +944,7 @@ def main():
         run_reference(args, rank, world)
         return
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device -- the B200 path has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device -- the CUDA path has no CPU fallback")
     # the contract is ONE JSON line on stdout: libraries (NCCL's version banner, symmetric-memory set-up) write to fd 1, so
     # everything but the final line is diverted to stderr for the duration of the run
     sys.stdout.flush()
@@ -931,7 +958,7 @@ def main():
             # second leg, same run: STRONG scaling of the one-box workload (cfg5) on the same N GPUs, so that a 1/2/4/8-GPU
             # sweep of the default command also yields a curve with a real collective (the halo) in the data path
             try:
-                sp = run_spatial(args, rank, world, local_rank, steps=args.spatial_steps, warmup=3, cpu_leg=False)
+                sp = run_spatial(args, rank, world, local_rank, steps=args.spatial_steps, warmup=3, cpu_leg=False, dump=False)
             except Exception as exc:  # pragma: no cover
                 sp = {"error": repr(exc)[:300]}
             if line is not None:

@@ -1,5 +1,5 @@
 /*
- * spk_b200.h -- C ABI of the B200-native (sm_100a) message-passing hot path for SchNetPack models.
+ * spk_b200.h -- C ABI of the H100-native (sm_90a) message-passing hot path for SchNetPack models.
  *
  * The reference (atomistic-machine-learning/schnetpack @ 4c967da) has NO native interface for this path: every op is
  * an ATen kernel dispatched from Python (SURVEY.md section 2, "CUDA kernel inventory: empty").  The entry points below
@@ -123,10 +123,10 @@ int spk_dense(const float* A, int64_t M, int K, int64_t lda, const float* a_pre,
  * a static operand.  The tensor-core kernels fetch it by TMA BEFORE their programmatic-launch dependency wait, so it must be
  * written only by these pack entry points (whose kernels never release their dependents early) or be complete before the
  * preceding kernels of the stream were launched; do not overwrite it with other kernels while evaluations are in flight. */
-/* Same layer on the tcgen05 tensor cores with 3xTF32 error compensation (fp32-grade results: split accumulators, K-tile
+/* Same layer on the Hopper tensor cores (wgmma) with 3xTF32 error compensation (fp32-grade results: split accumulators, K-tile
  * draining; see csrc/gemm_tc.cu).  The weight the A rows are contracted with -- the torch weight [N,K] itself for a
  * forward layer, its transpose for the input-gradient -- is packed once by spk_tc_pack_weight into per-(64-row, 16-column)
- * operand tiles [tf32_round(W) | W - tf32_round(W)] laid out exactly as the kernel's shared-memory UMMA operand, so one TMA
+ * operand tiles [tf32_round(W) | W - tf32_round(W)] laid out exactly as the kernel's shared-memory wgmma operand, so one TMA
  * bulk copy stages a tile.  Requirements: K, N, lda, ldy, ld_add multiples of 4, 16 B-aligned pointers, and at most one of
  * (a_act, act) active; otherwise SPK_ERR_UNSUPPORTED is returned and the caller uses spk_dense. */
 size_t spk_tc_packed_floats(int N, int K);
@@ -249,7 +249,7 @@ size_t spk_atom_chain_workspace_ints(int n_steps, int64_t n_atoms);
 int spk_atom_chain(const spk_chain_step_t* steps /* host array */, int n_steps, int64_t n_atoms, int32_t* workspace,
                    size_t workspace_ints, int flags, spk_stream_t stream);
 /* development aid: the same launch writing 8 int64 stamps per work item (claimed, dependencies satisfied, K-loop done,
- * published in ns of %globaltimer; CTA; step; atom tile; unused) to trace[8 * items] (tools/chain_trace.py) */
+ * published in ns of %globaltimer; CTA; step; atom tile; unused) to trace[8 * items] */
 int spk_atom_chain_debug(const spk_chain_step_t* steps, int n_steps, int64_t n_atoms, int32_t* workspace,
                          size_t workspace_ints, int flags, long long* trace, spk_stream_t stream);
 
@@ -260,7 +260,7 @@ int spk_atom_chain_debug(const spk_chain_step_t* steps, int n_steps, int64_t n_a
  * the filter-network output per CSR slot. */
 int spk_cfconv_fwd(const float* h, const float* w_raw, const float* geo, const int32_t* rowptr, const int32_t* slot_j,
                    int64_t n_atoms, int64_t n_edges, int F, float* m, spk_stream_t stream);
-/* The whole interaction-block forward edge pipeline fused, filter network on tcgen05 (csrc/schnet_tc.cu):
+/* The whole interaction-block forward edge pipeline fused, filter network on wgmma (csrc/schnet_tc.cu):
  *   m[i] = sum_{s in row i} h[j_s] * ( W1 act(W0 phi_s + b0) + b1 ) * fc_s          schnet.py:61-67
  * filter_packed = spk_schnet_pack_filter(filter_network.0.{weight,bias}, filter_network.1.weight) (hi|lo operand tiles,
  * spk_schnet_filter_packed_floats() floats); b1 = filter_network.1.bias; act = SPK_ACT_SSP | SPK_ACT_SILU | SPK_ACT_NONE.

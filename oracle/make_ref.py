@@ -8,7 +8,7 @@ transform/{base,atomistic,casting,neighborlist}, model/base}) -- plus the two sm
 
 ``/root/reference`` does not exist on the GPU box, ``oracle/_ref`` travels there with the snapshot (it is git-ignored but not
 gpurun-ignored), so the ``-m gpu`` tests can hold the CUDA path against the UNMODIFIED reference modules running on the same
-B200 (``tests/test_reference_live.py``), and ``bench.py --impl reference`` / ``cpu_baseline`` time the reference itself
+GPU (``tests/test_reference_live.py``), and ``bench.py --impl reference`` / ``cpu_baseline`` time the reference itself
 (``kind: "reference"``) instead of the oracle port.  Nothing is ever written to the reference tree, and no reference source
 enters the git history.
 """

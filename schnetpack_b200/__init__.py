@@ -1,4 +1,4 @@
-"""schnetpack_b200 -- B200-native (sm_100a) implementation of SchNetPack's message-passing hot path.
+"""schnetpack_b200 -- H100-native (sm_90a) implementation of SchNetPack's message-passing hot path.
 
 Drop-in module mirrors (same constructor signatures, tensor-dict protocol and ``state_dict`` keys as the reference):
 ``representation.{PaiNN,SchNet}``, ``nn.{GaussianRBF,BesselRBF,CosineCutoff,Dense,shifted_softplus,scatter_add,...}``,

@@ -121,7 +121,7 @@ def check(rc: int, name: str):
     if rc == -1:
         raise ValueError(f"{name}: invalid argument (SPK_ERR_ARG)")
     if rc == -2:
-        raise NotImplementedError(f"{name}: shape outside the compiled sm_100a templates (SPK_ERR_UNSUPPORTED)")
+        raise NotImplementedError(f"{name}: shape outside the compiled sm_90a templates (SPK_ERR_UNSUPPORTED)")
     raise RuntimeError(f"{name}: CUDA error {-rc - 1000}")
 
 

@@ -1,4 +1,4 @@
-"""Mirror of the hot-path output/input modules of ``schnetpack.atomistic`` on the B200 kernels:
+"""Mirror of the hot-path output/input modules of ``schnetpack.atomistic`` on the CUDA kernels:
 ``PairwiseDistances`` (atomistic/distances.py:9-26), ``Atomwise`` (atomistic/atomwise.py:14-88) and ``Forces``
 (atomistic/response.py:18-92)."""
 from __future__ import annotations

@@ -1,7 +1,7 @@
-"""In-tree build of the sm_100a CUDA library (``schnetpack_b200/csrc/libspk_b200.so``) with plain nvcc.
+"""In-tree build of the sm_90a (H100) CUDA library (``schnetpack_b200/csrc/libspk_b200.so``) with plain nvcc.
 
 The library has a C ABI only (``include/spk_b200.h``); it does not link against torch.  ``nvcc`` cross-compiles for
-sm_100a without a GPU, so this runs in the CPU build container; the resulting .so travels to the GPU box.
+sm_90a without a GPU, so the library can be built on a machine without one.
 """
 from __future__ import annotations
 
@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libspk_b200.so")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",

@@ -1,8 +1,7 @@
 // Persistent per-atom stage ("atom chain"): ALL the per-atom work that sits between two fused edge kernels of a PaiNN
 // evaluation -- mu_channel_mix, norm/context glue, intraatomic_context_net (2 Dense), gated update, and the NEXT block's
-// interatomic_context_net (2 Dense); or their reverses -- as ONE launch (reference: representation/painn.py:54,103-116 and
-// nn/base.py:52-55; previously 7 launches per stage, 44 % + 11 % of the cfg2 step in ~13 us pieces whose tensor pipe was
-// 6-20 % active because every launch paid TMEM allocation, barrier set-up, pipeline fill and a full grid drain).
+// interatomic_context_net (2 Dense); or their reverses -- as ONE launch (reference: representation/painn.py and
+// nn/base.py; otherwise 7 launches per stage, each paying barrier set-up, pipeline fill and a full grid drain).
 //
 // Every operation of the stage is ROW-LOCAL: the rows of a 128-atom tile produced by step k are all that step k+1 needs
 // for the same tile.  So the stage is a static list of STEPS (GEMM or elementwise glue, given by the host as plain structs)
@@ -13,41 +12,27 @@
 // schedule cannot deadlock however many CTAs are co-resident.  Data between steps goes through global memory (L2-resident,
 // read with ld.global.cg): what is saved is the launch boundary, not the bytes.
 //
-// A GEMM item is one 128 x 128 output tile computed by the warp-specialised tcgen05 pipeline of gemm_tc.cu (3xTF32 with
-// split accumulators and per-K-tile draining, see there), kept WARM across items: TMEM is allocated once, the mbarrier
-// phases run on (stage = global K-tile count % NST), weight tiles still arrive pre-packed by one TMA bulk copy each.
-// Three main accumulators (3 x 128 TMEM columns + 128 for the correction terms = all 512 columns) instead of two deepen
-// the MMA -> drain pipeline.  Activation codes and the "x act'(pre)" prologue are run-time here (one kernel, any program).
+// A GEMM item is one 128 x 128 output tile computed by the warp-specialised wgmma pipeline of gemm_tc.cu (3xTF32 with a
+// fresh accumulator per K-tile added to fp32 registers, see there), kept WARM across items: the mbarrier phases run on
+// (stage = global K-tile count % NST), weight tiles still arrive pre-packed by one TMA bulk copy each.  Activation codes and
+// the "x act'(pre)" prologue are run-time here (one kernel, any program).
 //
 // The last CTA to finish resets the dependency counters, so the caller-owned workspace only has to be zero once.
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int TM = 128, TN = 128, TK = 16;
-constexpr int N_DRAIN = 8, W_MMA = 8, W_PROD0 = 9;
+constexpr int N_CONS = 8, W_PROD0 = 8;
 constexpr int NST = 6, NPROD = 6;
 constexpr int OPER_A = TM * TK * 4, OPER_B = TN * TK * 4;
 constexpr int STAGE_BYTES = 2 * OPER_A + 2 * OPER_B;        // A_hi, A_lo, W_hi, W_lo
 constexpr int EP_LD = TN + 4;
 constexpr int SMEM_BYTES = NST * STAGE_BYTES + 1024;
-constexpr int NTHREADS = (W_PROD0 + NPROD) * 32;            // 480
-constexpr int TMEM_COLS = 512;                              // main[0..2] | corr
-constexpr int CW = TN / 2;
+constexpr int NTHREADS = (W_PROD0 + NPROD) * 32;            // 448
+constexpr int NB = TN / 64;                                 // m64n64 column blocks per consumer warpgroup
 static_assert(NST * STAGE_BYTES >= TM * EP_LD * 4, "epilogue staging tile reuses the pipeline stages");
 static_assert(NST % NPROD == 0, "a stage must be owned by exactly one producer warp");
-// Two accumulation schemes for the 3xTF32 products of a K-tile (A = Ah + Al, W = Wh + Wl):
-//   NFOLD = false   3 MMAs per k-step: Ah*Wh -> main[buf] (fresh per K-tile, 3 buffers), Al*Wh and Ah*Wl -> corr (over all K);
-//   NFOLD = true    2 MMAs per k-step: the packed tile [W_hi ; W_lo] is ONE operand of 256 rows, so Ah*[Wh;Wl]^T gives the main
-//                   product and the Ah*Wl terms in one N = 256 instruction (an MMA costs about the same for any N <= 256) and
-//                   Al*Wh accumulates onto the correction columns; [main | corr] = 256 columns per buffer, 2 buffers, both
-//                   halves fresh per K-tile and drained into fp32 registers (round-1 experiment gemm_tc_nfold, now selectable).
-template <bool NFOLD>
-struct Acc {
-    static constexpr int NBUF = NFOLD ? 2 : 3;
-    static constexpr int BUF_COLS = NFOLD ? 2 * TN : TN;
-};
-static_assert(3 * TN + TN <= TMEM_COLS && 2 * 2 * TN <= TMEM_COLS, "accumulators exceed TMEM");
 
 struct ChainArgs {
     spk_chain_step_t step[SPK_CHAIN_MAX_STEPS];
@@ -55,7 +40,7 @@ struct ChainArgs {
     int n_tiles;            // ceil(n_atoms / 128)
     int64_t n_atoms;
     int* ws;                // [n_steps * n_tiles] done counters, then [1] finished-CTA counter, [1] next-item counter
-    long long* trace;       // optional (spk_atom_chain_debug): 8 stamps per item, see tools/chain_trace.py
+    long long* trace;       // optional (spk_atom_chain_debug): 8 stamps per item
 };
 
 __device__ __forceinline__ long long gtime() {
@@ -67,19 +52,6 @@ __device__ __forceinline__ long long gtime() {
     do {                                                                         \
         if (g.trace && tid == 0) g.trace[(int64_t)item * 8 + (slot)] = (val);    \
     } while (0)
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 
 __device__ __forceinline__ int ld_acquire(const int* p) {
     int v;
@@ -93,7 +65,7 @@ __device__ __forceinline__ int items_per_tile(const spk_chain_step_t& s) {
 }
 
 // activation value and derivative for the epilogue of a 128 x 128 tile: 16 k elements on ONE SM, so the instruction count per
-// element is what the tile's latency pays (expf + two IEEE divisions cost 3.3 us per tile; measured).  silu keeps expf
+// element is what the tile's latency pays (expf + two IEEE divisions per element).  silu keeps expf
 // (accuracy of the reference's sigmoid) but takes ONE reciprocal; shifted softplus as in common.cuh.
 __device__ __forceinline__ void chain_act_both(float x, int act, float& y, float& dy) {
     if (act == SPK_ACT_SILU) {
@@ -198,16 +170,11 @@ __device__ void glue_item(const spk_chain_step_t& s, int64_t a0, int64_t a1, int
     }
 }
 
-template <bool NFOLD>
 __global__ void __launch_bounds__(NTHREADS, 1) k_atom_chain(const __grid_constant__ ChainArgs g) {
-    constexpr int NBUF = Acc<NFOLD>::NBUF, BUF_COLS = Acc<NFOLD>::BUF_COLS;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     __shared__ __align__(8) uint64_t full_bar[NST];
     __shared__ __align__(8) uint64_t empty_bar[NST];
-    __shared__ __align__(8) uint64_t acc_full[3];
-    __shared__ __align__(8) uint64_t acc_empty[3];
-    __shared__ uint32_t s_tmem;
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // broadcast: the compiler may treat the role index as warp-uniform
@@ -216,24 +183,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_atom_chain(const __grid_constan
 #pragma unroll
         for (int s = 0; s < NST; ++s) {
             mbar_init(&full_bar[s], 2);      // expect_tx arrive (weight TMA) + arrive after the A tile is stored
-            mbar_init(&empty_bar[s], 1);
-        }
-#pragma unroll
-        for (int b = 0; b < NBUF; ++b) {
-            mbar_init(&acc_full[b], 1);
-            mbar_init(&acc_empty[b], N_DRAIN);
+            mbar_init(&empty_bar[s], N_CONS);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)),
-                     "n"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = s_tmem;
     SPK_PDL_WAIT();
 
     // step-major item numbering
@@ -308,7 +262,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_atom_chain(const __grid_constan
                         const int k = kt * TK + chunk * 4;
                         // every load unconditional (clamped row, zeroed afterwards) and the a_pre variant chosen by a
                         // warp-uniform branch OUTSIDE the batch: loads under a data-dependent branch are serialised by
-                        // the compiler (profiles/FINDINGS.md) -- the first version of this loop cost 2.4 k cycles per K-tile
+                        // the compiler
                         float4 av[16];
                         const int64_t m_last = M - 1;
 #pragma unroll
@@ -354,95 +308,38 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_atom_chain(const __grid_constan
                         __syncwarp();
                         if (lane == 0) mbar_arrive(&full_bar[s]);
                     }
-                } else if (warp == W_MMA) {
-                    // =========================================== MMA issuer ===========================================
-                    if (lane == 0) {
-                        const uint32_t idesc =
-                            (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-                        for (int kt = 0; kt < nk; ++kt) {
-                            const uint32_t gk = ktg + kt;
-                            const int s = gk % NST, buf = gk % NBUF;
-                            mbar_wait(&full_bar[s], (gk / NST) & 1);
-                            if (gk >= NBUF) mbar_wait(&acc_empty[buf], ((gk / NBUF) - 1) & 1);
-                            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                            const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
-                            const uint32_t d_main = tmem_base + (uint32_t)(buf * BUF_COLS);
-                            const uint32_t d_corr = tmem_base + (uint32_t)(NBUF * TN);           // !NFOLD only
-                            const uint32_t idesc_w = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)((2 * TN) >> 3) << 17) |
-                                                     ((uint32_t)(TM >> 4) << 24);
-#pragma unroll
-                            for (int ks = 0; ks < TK / 8; ++ks) {
-                                const uint64_t ah = make_desc(sa + 32 * ks);
-                                const uint64_t al = make_desc(sa + OPER_A + 32 * ks);
-                                const uint64_t bh = make_desc(sa + 2 * OPER_A + 32 * ks);        // W_hi tile; W_lo follows it
-                                if (NFOLD) {
-                                    umma_tf32(d_main, ah, bh, idesc_w, ks ? 1u : 0u);            // [Ah Wh | Ah Wl], fresh per K-tile
-                                    umma_tf32(d_main + (uint32_t)TN, al, bh, idesc, 1u);         // Al Wh onto the correction half
-                                } else {
-                                    const uint64_t bl = make_desc(sa + 2 * OPER_A + OPER_B + 32 * ks);
-                                    umma_tf32(d_corr, al, bh, idesc, (kt | ks) ? 1u : 0u);       // small terms: over all of K
-                                    umma_tf32(d_corr, ah, bl, idesc, 1u);
-                                    umma_tf32(d_main, ah, bh, idesc, ks ? 1u : 0u);              // fresh accumulator per K-tile
-                                }
-                            }
-                            umma_commit(&empty_bar[s]);
-                            umma_commit(&acc_full[buf]);
-                        }
-                    }
                 } else {
-                    // =========================================== drain ===========================================
-                    const int q = warp & 3, ch = warp >> 2;
-                    const int row = q * 32 + lane;
-                    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(ch * CW);
-                    float accr[CW];
+                    // =========================================== consumers: wgmma ===========================================
+                    const int wg = warp >> 2;
+                    float acc[NB][32];
 #pragma unroll
-                    for (int i = 0; i < CW; ++i) accr[i] = 0.f;
+                    for (int cb = 0; cb < NB; ++cb)
+#pragma unroll
+                        for (int i = 0; i < 32; ++i) acc[cb][i] = 0.f;
                     for (int kt = 0; kt < nk; ++kt) {
                         const uint32_t gk = ktg + kt;
-                        const int buf = gk % NBUF;
-                        mbar_wait(&acc_full[buf], (gk / NBUF) & 1);
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-                        for (int c0 = 0; c0 < CW; c0 += 32) {
-                            uint32_t r[32];
-                            if (NFOLD) {                                      // corrections of this K-tile first (small)
-                                tmem_ld32(lane_addr + (uint32_t)(buf * BUF_COLS + TN + c0), r);
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) accr[c0 + j] += __uint_as_float(r[j]);
-                            }
-                            tmem_ld32(lane_addr + (uint32_t)(buf * BUF_COLS + c0), r);
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) accr[c0 + j] += __uint_as_float(r[j]);
-                        }
-                        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+                        const int s = gk % NST;
+                        mbar_wait(&full_bar[s], (gk / NST) & 1);
+                        const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
+                        wg_ktile_3xtf32<NB>(acc, sa + wg * SPK_WG_ROWS_BYTES, sa + OPER_A + wg * SPK_WG_ROWS_BYTES,
+                                            sa + 2 * OPER_A, sa + 2 * OPER_A + OPER_B);
                         __syncwarp();
-                        if (lane == 0) mbar_arrive(&acc_empty[buf]);
+                        if (lane == 0) mbar_arrive(&empty_bar[s]);
                     }
-                    // the last acc_full commit also covers every correction MMA, and all MMAs have finished reading the
-                    // stages: their memory now stages the raw fp32 tile for the CTA-wide epilogue
-                    float* ep = reinterpret_cast<float*>(smem) + row * EP_LD + ch * CW;
-                    if (NFOLD) {
+                    // every wgmma of both warpgroups has completed and the producers are done with this item: the stages
+                    // now stage the raw fp32 tile for the CTA-wide epilogue
+                    wg_bar(1, N_CONS * 32);
+                    const int t = tid & 127;
 #pragma unroll
-                        for (int c0 = 0; c0 < CW; c0 += 4)
-                            *reinterpret_cast<float4*>(ep + c0) = make_float4(accr[c0], accr[c0 + 1], accr[c0 + 2], accr[c0 + 3]);
-                    } else {
+                    for (int cb = 0; cb < NB; ++cb)
 #pragma unroll
-                        for (int c0 = 0; c0 < CW; c0 += 32) {
-                            uint32_t r[32];
-                            tmem_ld32(lane_addr + (uint32_t)(NBUF * TN + c0), r);
-#pragma unroll
-                            for (int j = 0; j < 32; j += 4)
-                                *reinterpret_cast<float4*>(ep + c0 + j) = make_float4(
-                                    accr[c0 + j + 0] + __uint_as_float(r[j + 0]), accr[c0 + j + 1] + __uint_as_float(r[j + 1]),
-                                    accr[c0 + j + 2] + __uint_as_float(r[j + 2]), accr[c0 + j + 3] + __uint_as_float(r[j + 3]));
-                        }
-                    }
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+                        for (int i = 0; i < 32; i += 2)
+                            *reinterpret_cast<float2*>(reinterpret_cast<float*>(smem) + (wg * 64 + wg_frag_row(t, i)) * EP_LD +
+                                                       cb * 64 + wg_frag_col(t, i)) = make_float2(acc[cb][i], acc[cb][i + 1]);
                 }
                 ktg += nk;
             }
             __syncthreads();
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
             CTRACE(2, gtime());                                                      // K-loop done, tile staged
             if (live) {
                 // =========================================== epilogue: all warps, coalesced ===========================================
@@ -498,10 +395,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_atom_chain(const __grid_constan
             __threadfence();
         }
     }
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
-    }
 }
 
 }  // namespace
@@ -556,15 +449,14 @@ extern "C" int spk_atom_chain_debug(const spk_chain_step_t* steps, int n_steps, 
         }
     }
     if (items >= (1ll << 31)) return SPK_ERR_UNSUPPORTED;
-    static SpkSmemOnce once_a, once_b;
-    if (cudaError_t e = once_a.set(k_atom_chain<false>, SMEM_BYTES); e != cudaSuccess) return SPK_CUDA_ERR(e);
-    if (cudaError_t e = once_b.set(k_atom_chain<true>, SMEM_BYTES); e != cudaSuccess) return SPK_CUDA_ERR(e);
+    // SPK_CHAIN_FLAG_NFOLD selects nothing here: with register accumulators both accumulation schemes of the 3xTF32
+    // products are the same fresh-accumulator-per-K-tile scheme (wg_ktile_3xtf32)
+    (void)flags;
+    static SpkSmemOnce once;
+    if (cudaError_t e = once.set(k_atom_chain, SMEM_BYTES); e != cudaSuccess) return SPK_CUDA_ERR(e);
     int64_t nb = spk_num_sms();                       // one persistent CTA per SM
     if (nb > items) nb = items;
-    if (flags & SPK_CHAIN_FLAG_NFOLD)
-        spk_launch(k_atom_chain<true>, (unsigned)nb, NTHREADS, SMEM_BYTES, spk_st(stream), g);
-    else
-        spk_launch(k_atom_chain<false>, (unsigned)nb, NTHREADS, SMEM_BYTES, spk_st(stream), g);
+    spk_launch(k_atom_chain, (unsigned)nb, NTHREADS, SMEM_BYTES, spk_st(stream), g);
     SPK_LAUNCH_CHECK();
     return SPK_OK;
 }

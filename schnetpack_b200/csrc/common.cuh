@@ -1,4 +1,4 @@
-// Shared device/host helpers for the sm_100a kernels of the SchNetPack hot path.
+// Shared device/host helpers for the sm_90a (H100) kernels of the SchNetPack hot path.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -16,8 +16,8 @@
 static inline cudaStream_t spk_st(spk_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
 
 // ---- programmatic dependent launch ----------------------------------------------------------------------------------
-// One E+F evaluation is a chain of ~65 short kernels (median 10 us); a normal launch lets kernel n+1 start only after
-// kernel n has drained and its completion has been processed (~3 us per boundary).  Every kernel of the library is
+// One E+F evaluation is a chain of ~65 short kernels; a normal launch lets kernel n+1 start only after kernel n has drained
+// and its completion has been processed.  Every kernel of the library is
 // therefore launched with the programmatic-stream-serialization attribute and begins with
 //     griddepcontrol.launch_dependents   -- the next kernel's CTAs may be scheduled as soon as all of ours are resident
 //     griddepcontrol.wait                -- block until the previous kernel has completed and its writes are visible
@@ -28,7 +28,7 @@ static inline cudaStream_t spk_st(spk_stream_t s) { return reinterpret_cast<cuda
 #define SPK_PDL_LAUNCH_DEPENDENTS() asm volatile("griddepcontrol.launch_dependents;" ::: "memory")
 #define SPK_PDL_WAIT() asm volatile("griddepcontrol.wait;" ::: "memory")
 #else
-// Debug build (tools/build_variant.sh timeline -DSPK_TIMELINE, tools/timeline.py): thread 0 of block 0 of EVERY kernel stamps
+// Debug build (-DSPK_TIMELINE): thread 0 of block 0 of EVERY kernel stamps
 // %globaltimer at entry and when its griddepcontrol.wait returns (= the previous kernel has completed), tagged with the
 // source line of the macro.  The differences between consecutive wait-return stamps are the kernels' durations INSIDE the
 // programmatic-launch chain of a graph replay -- which neither CUDA events (they break the programmatic edges) nor ncu
@@ -120,7 +120,7 @@ static inline void spk_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 
 static inline int64_t spk_cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-constexpr int SPK_NUM_SMS = 148;  // B200: 2 dies x 74 SMs
+constexpr int SPK_NUM_SMS = 132;  // H100 SXM
 
 // Per-device caches (a process may drive several GPUs): indexed by the CURRENT device of the calling thread, which the
 // host side sets to the device of the tensors before every call.  Entries are write-once values, so concurrent callers
@@ -132,7 +132,7 @@ static inline int spk_device() {
     return dev;
 }
 
-// SM count of the current device (148 on B200).
+// SM count of the current device (132 on H100 SXM).
 static inline int spk_num_sms() {
     static int n[SPK_MAX_DEVICES] = {0};
     const int dev = spk_device();
@@ -210,6 +210,12 @@ __device__ __forceinline__ void spk_act_both(float x, int act, float& y, float& 
     }
 }
 
+// (a * b + c) per component with IEEE round-to-nearest: on sm_90 scalar FFMA runs at the full fp32 rate, so the float2
+// accumulators of the CUDA-core kernels are two independent FFMAs
+__device__ __forceinline__ float2 spk_fma2(float2 a, float2 b, float2 c) {
+    return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
+
 __device__ __forceinline__ float spk_warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -227,8 +233,8 @@ __device__ __forceinline__ int spk_lower_bound(const int32_t* __restrict__ ptr, 
 }
 
 // The same lower bound found by a whole warp: 32 probes per round instead of one, so the chain of DEPENDENT global loads is
-// log32(n) + 1 long instead of log2(n) (5376 rows: 3 instead of 13 -- at ~0.35 us of L2 latency each, the two serial
-// searches per group were ~9 us at the head of every edge kernel, tools/timeline.py).  All lanes must call; all get the result.
+// log32(n) + 1 long instead of log2(n) (5376 rows: 3 instead of 13 dependent L2 round trips at
+// the head of every edge kernel).  All lanes must call; all get the result.
 __device__ __forceinline__ int spk_lower_bound_warp(const int32_t* __restrict__ ptr, int n, int target) {
     const int lane = threadIdx.x & 31;
     int lo = 0, hi = n;                                        // the answer stays in [lo, hi]; ptr[n] is never read

@@ -3,7 +3,7 @@
 // reference's default torch matmul precision ("highest", cli.py:95-97), so 1e-5 parity holds by construction.
 //
 // Tiling: BM x 64 output tile per CTA (BM = 128 / 256 threads, or 64 / 128 threads for grids that would not fill the
-// chip), BK=16, 8x4 register micro-tile per thread computed with packed FFMA2, A tile stored k-major in shared memory
+// chip), BK=16, 8x4 register micro-tile per thread computed as float2 pairs (spk_fma2), A tile stored k-major in shared memory
 // so both operand fetches are conflict-free 128-bit LDS; double-buffered shared memory (one barrier per k-tile) with
 // the next k-tile prefetched into registers while the current one is multiplied.
 #include "common.cuh"
@@ -26,7 +26,7 @@ struct GemmArgs {
 
 // activation helpers kept out of line and selected at compile time: inlining the runtime-switched expf/log1pf code into
 // the unrolled load / epilogue loops made the kernel 6.3k SASS instructions long and 22 % of its stalls were
-// instruction-cache misses (profiles/r1_ncu_dense.txt)
+// instruction-cache misses
 template <int ACT>
 __device__ __noinline__ float act_grad1(float q) { return ACT == SPK_ACT_GIVEN ? q : spk_act_grad(q, ACT); }
 template <int ACT>
@@ -38,7 +38,7 @@ __device__ __noinline__ float2 act_both1(float v) {
     return make_float2(y, dy);
 }
 
-// BM = 128 (256 threads) for tall problems, BM = 64 / 32 when the 128-row grid would not fill the 148 SMs.
+// BM = 128 (256 threads) for tall problems, BM = 64 / 32 when the 128-row grid would not fill the 132 SMs.
 template <int BM, int A_ACT, int ACT>
 __global__ void __launch_bounds__(BM * 2) k_dense(GemmArgs g) {
     SPK_PDL_ENTER();
@@ -124,8 +124,7 @@ __global__ void __launch_bounds__(BM * 2) k_dense(GemmArgs g) {
             *reinterpret_cast<float4*>(&Bs[buf][b_k + it * (NT / 16)][b_n]) = rb[it];
     };
 
-    // 8x4 micro-tile held as 4x4 float2 accumulators paired along M: Blackwell issues scalar FFMA at half rate, the
-    // packed FFMA2 (fma.rn.f32x2, __ffma2_rn) restores the full fp32 rate with IEEE round-to-nearest per component.
+    // 8x4 micro-tile held as 4x4 float2 accumulators paired along M (spk_fma2: IEEE round-to-nearest per component).
     float2 acc2[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
@@ -151,7 +150,7 @@ __global__ void __launch_bounds__(BM * 2) k_dense(GemmArgs g) {
 #pragma unroll
             for (int i = 0; i < 4; ++i)
 #pragma unroll
-                for (int j = 0; j < 4; ++j) acc2[i][j] = __ffma2_rn(ap[i], bd[j], acc2[i][j]);
+                for (int j = 0; j < 4; ++j) acc2[i][j] = spk_fma2(ap[i], bd[j], acc2[i][j]);
         }
         if (kt + 1 < nk) store_tiles(buf ^ 1);           // the other buffer was last read before the previous barrier
         __syncthreads();

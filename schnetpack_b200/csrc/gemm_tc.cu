@@ -1,68 +1,44 @@
-// Dense layer on the 5th-generation tensor cores (tcgen05, TMEM accumulators) with 3xTF32 error compensation:
+// Dense layer on the Hopper tensor cores (wgmma, register accumulators) with 3xTF32 error compensation:
 //
 //     Y = act( (A .* act'(a_pre)) * W^T + bias ) + addend            A [M,K] fp32, W [N,K] fp32 (K contiguous)
 //
-// The reference computes these layers with true-fp32 cuBLAS SGEMM (torch matmul precision "highest",
-// /root/reference/src/schnetpack/cli.py:95-97, nn/base.py:52-55); single-pass TF32 would miss the 1e-5 parity bar by two
-// orders of magnitude.  Scheme (validated on B200, DESIGN.md section 3):
+// The reference computes these layers with true-fp32 cuBLAS SGEMM (torch matmul precision "highest"); single-pass TF32
+// would miss the 1e-5 parity bar by two orders of magnitude.  Scheme (DESIGN.md section 3):
 //   * every operand is split  x = hi + lo  (hi = round-to-nearest TF32, lo = x - hi exact in fp32); three tensor-core
 //     products Ah*Bh + Al*Bh + Ah*Bl are formed (Al*Bl is O(2^-24));
-//   * the tensor core adds into its TMEM accumulator with TRUNCATION, which biases long K-sums toward zero (measured: 8x
-//     worse end-to-end parity).  Therefore the main Ah*Bh product of each K-tile (16 floats = 2 MMA k-steps) goes into a
-//     FRESH accumulator that is drained into fp32 registers and summed there with IEEE round-to-nearest, while the small
-//     lo products accumulate over all of K in a separate TMEM accumulator (their truncation error is 2^-12 smaller).
+//   * the tensor core adds into its accumulator with TRUNCATION, which biases long K-sums toward zero.  Therefore the products
+//     of each K-tile (16 floats = 2 k-steps) go into a FRESH accumulator that is added to the fp32 running sum with IEEE
+//     round-to-nearest (wg_ktile_3xtf32, wgmma.cuh).
 //
-// Measured on B200 (tools/tc_trace.cu, clock64 phase stamps): one tcgen05.mma.kind::tf32 with M = 128 takes ~130 cycles for
-// every N <= 256, from shared memory or from TMEM alike, so a CTA's K-loop is a serial chain of 3 * K/8 MMAs and the
-// tensor-pipe work of a GEMM is proportional to the NUMBER of MMAs.  Hence the widest tile that still fills the GPU:
-// TN = 128 columns when N >= 256, 64 otherwise.
-//
-// Warp-specialised pipeline, one CTA per 128 x TN output tile, cta_group::1, UMMA 128 x TN x 8:
-//   warps 9..  producers: K-tile kt belongs to warp kt % NPROD and stage kt % NST (NPROD divides NST).  Lane 0 arms
-//              full[stage] with the byte count of the weight tile and issues ONE TMA bulk copy (cp.async.bulk) of the
-//              pre-packed W_hi|W_lo operand tile (the weights are static, so the host packs them once in the exact
-//              shared-memory operand layout, spk_tc_pack_weight); all lanes load the A tile with coalesced 128-bit loads
-//              (optional backward prologue x act'(a_pre)), split hi/lo in registers and st.shared it K-major with the
-//              64-byte swizzle (row = 64 B, 8-row atoms of 512 B, 16 B chunk index XOR row bits [1,3));
-//              fence.proxy.async; arrive on full[stage];
-//   warp 8     MMA issuer (one lane): waits full[stage] and acc_empty[buf], issues 6 tcgen05.mma.kind::tf32, then
-//              tcgen05.commit -> empty[stage] and -> acc_full[buf];
-//   warps 0-7  drain: warp w reads TMEM lane quarter w % 4 (thread = output row), column half w / 4, with
-//              tcgen05.ld.32x32b.x32, adds into fp32 registers, arrives acc_empty[buf]; after the last K-tile adds the
-//              correction accumulator and stages the raw tile in shared memory (the pipeline stages are free by then);
-//   all warps  epilogue: bias / activation (+ saved derivative) / addend / stores, 16 B per thread, whole 128 B lines
-//              per row segment (a thread-per-row epilogue kept only 4 warps busy and cost up to 60 % of the kernel).
-#include "tcgen05.cuh"
+// Warp-specialised pipeline, one CTA per 128 x TN output tile:
+//   warps 8..   producers: K-tile kt belongs to warp kt % NPROD and stage kt % NST (NPROD divides NST).  Lane 0 arms
+//               full[stage] with the byte count of the weight tile and issues ONE TMA bulk copy (cp.async.bulk) of the
+//               pre-packed W_hi|W_lo operand tile (the weights are static, so the host packs them once in the exact
+//               shared-memory operand layout, spk_tc_pack_weight); all lanes load the A tile with coalesced 128-bit loads
+//               (optional backward prologue x act'(a_pre)), split hi/lo in registers and st.shared it K-major with the
+//               64-byte swizzle (row = 64 B, 8-row atoms of 512 B, 16 B chunk index XOR row bits [1,3));
+//               fence.proxy.async; arrive on full[stage];
+//   warps 0-7   two consumer warpgroups, rows 0-63 and 64-127 of the tile: wait full[stage], issue the stage's wgmma
+//               (m64n64k8, TN / 64 column blocks), accumulate in registers, arrive on empty[stage]; after the last K-tile
+//               the raw tile is staged in shared memory (the pipeline stages are free by then);
+//   all warps   epilogue: bias / activation (+ saved derivative) / addend / stores, 16 B per thread, whole 128 B lines
+//               per row segment.
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int TM = 128;                        // rows per CTA tile (UMMA M)
-constexpr int TK = 16;                         // floats per K-tile = 2 UMMA k-steps
-constexpr int N_DRAIN = 8;                     // drain warps 0-7
-constexpr int W_MMA = 8;
-constexpr int W_PROD0 = 9;
+constexpr int TM = 128;                        // rows per CTA tile (two m64 warpgroups)
+constexpr int TK = 16;                         // floats per K-tile = 2 k-steps
+constexpr int N_CONS = 8;                      // consumer warps 0-7 (two warpgroups)
+constexpr int W_PROD0 = 8;
 constexpr int OPER_A = TM * TK * 4;            // 8192 B: A tile, K-major, SWIZZLE_64B
-// K-tiles accumulated in one TMEM main accumulator before it is drained into fp32 registers.  1 (default) is the validated
-// precision scheme; 2 halves the TMEM -> register traffic of the drain warps (the K-loop is drain-bound: ~1000 cycles per
-// K-tile in the round-2 item trace) at the price of 4 instead of 2 truncating accumulations per main accumulator.
-#ifndef SPK_TC_ACC_KT
-#define SPK_TC_ACC_KT 1
-#endif
-constexpr int ACC_KT = SPK_TC_ACC_KT;
-// The two small products A_lo*W_hi and A_hi*W_lo share one correction accumulator (0) or get one each (1).  Measured inside
-// the programmatic-launch chain (tools/timeline.py): no difference -- the K-loop's ~400 ns per K-tile of 6 MMAs is the
-// tensor pipe's issue rate for M = 128 tf32 instructions, not a read-modify-write dependence on one TMEM tile.
-#ifndef SPK_TC_DUAL_CORR
-#define SPK_TC_DUAL_CORR 0
-#endif
 #ifndef SPK_TC_STAGGER
 #define SPK_TC_STAGGER 300
 #endif
-constexpr int N_CORR = SPK_TC_DUAL_CORR ? 2 : 1;
 
 template <int TN>
 struct Cfg {
-    static constexpr int NST = TN == 64 ? 7 : 6;           // shared-memory stages (16 / 15 warps: 128 registers each)
+    static constexpr int NST = TN == 64 ? 7 : 6;           // shared-memory stages
     static constexpr int NPROD = NST;                       // producer warps; NPROD divides NST, so all uses of a stage belong
                                                             // to ONE warp and are strictly ordered (a parity wait cannot
                                                             // tell phase u from phase u+2)
@@ -71,39 +47,20 @@ struct Cfg {
     static constexpr int EP_LD = TN + 4;                    // padded row of the epilogue staging tile (floats)
     static constexpr int SMEM_BYTES = NST * STAGE_BYTES + 1024;   // + slack to align the stages to 1024 B
     static constexpr int NTHREADS = (W_PROD0 + NPROD) * 32;
-    static constexpr int TMEM_COLS = TN == 64 ? 256 : 512;  // main[0] | main[1] | corr[0] | corr[1]
-    static constexpr int CW = TN / 2;                       // columns drained by one warp
+    static constexpr int NB = TN / 64;                      // m64n64 column blocks per consumer warpgroup
     static_assert(NST * STAGE_BYTES >= TM * EP_LD * 4, "epilogue staging tile reuses the pipeline stages");
     static_assert(NST % NPROD == 0, "a stage must be owned by exactly one producer warp");
 };
 
-#ifdef SPK_TC_TRACE
-#define TRACE(slot)                                                                                     \
-    do {                                                                                                \
-        if (g.dbg && (threadIdx.x & 31) == 0)                                                           \
-            g.dbg[((int64_t)blockIdx.y * gridDim.x + blockIdx.x) * 128 + (slot)] = clock64();           \
-    } while (0)
-#else
-#define TRACE(slot) do { } while (0)
-#endif
-
-
-
-
-
-
-// 32 consecutive accumulator columns of this thread's TMEM lane -> registers
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// raw accumulator fragments of a consumer warpgroup (rows wg*64..) -> row-major fp32 staging tile with rows of ld floats
+template <int NB>
+__device__ __forceinline__ void wg_stage_tile(const float (&acc)[NB][32], float* ep, int ld, int wg, int t) {
+#pragma unroll
+    for (int cb = 0; cb < NB; ++cb)
+#pragma unroll
+        for (int i = 0; i < 32; i += 2)
+            *reinterpret_cast<float2*>(ep + (wg * 64 + wg_frag_row(t, i)) * ld + cb * 64 + wg_frag_col(t, i)) =
+                make_float2(acc[cb][i], acc[cb][i + 1]);
 }
 
 // activation-gradient helper kept out of line: the producer loop is fully unrolled over a register array, inlining
@@ -123,9 +80,6 @@ struct TcArgs {
     float* y_pre;
     int64_t M, lda, ld_add, ldy;
     int K, N, a_act, act, save_deriv;
-#ifdef SPK_TC_TRACE
-    long long* dbg;
-#endif
 };
 
 
@@ -172,19 +126,15 @@ template <int TN, int A_ACT, int ACT>
 __global__ void __launch_bounds__(Cfg<TN>::NTHREADS, 1) k_dense_tc(TcArgs g) {
     using C = Cfg<TN>;
     constexpr int NST = C::NST, NPROD = C::NPROD, OPER_B = C::OPER_B, STAGE_BYTES = C::STAGE_BYTES, EP_LD = C::EP_LD,
-                  NTHREADS = C::NTHREADS, TMEM_COLS = C::TMEM_COLS, CW = C::CW;
+                  NTHREADS = C::NTHREADS, NB = C::NB;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     __shared__ __align__(8) uint64_t full_bar[NST];
     __shared__ __align__(8) uint64_t empty_bar[NST];
-    __shared__ __align__(8) uint64_t acc_full[2];
-    __shared__ __align__(8) uint64_t acc_empty[2];
-    __shared__ uint32_t s_tmem;
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // broadcast: the compiler may treat the role index as warp-uniform
     SPK_PDL_LAUNCH_DEPENDENTS();
-    if (tid == 0) TRACE(0);
     const int64_t m0 = (int64_t)blockIdx.x * TM;
     const int n0 = blockIdx.y * TN;
     const int nk = (g.K + TK - 1) / TK;
@@ -193,12 +143,8 @@ __global__ void __launch_bounds__(Cfg<TN>::NTHREADS, 1) k_dense_tc(TcArgs g) {
 #pragma unroll
         for (int s = 0; s < NST; ++s) {
             mbar_init(&full_bar[s], 2);      // expect_tx arrive (weight TMA) + arrive after the A tile is stored
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], N_CONS);
         }
-        mbar_init(&acc_full[0], 1);
-        mbar_init(&acc_full[1], 1);
-        mbar_init(&acc_empty[0], N_DRAIN);
-        mbar_init(&acc_empty[1], N_DRAIN);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         // the weight tiles of the first NST K-tiles are static operands: their TMA copies are issued here, BEFORE
         // griddepcontrol.wait, and land while the previous kernel is still running (pack kernels never trigger their
@@ -209,17 +155,8 @@ __global__ void __launch_bounds__(Cfg<TN>::NTHREADS, 1) k_dense_tc(TcArgs g) {
             tma_load(smem + s * STAGE_BYTES + 2 * OPER_A, wp0 + (int64_t)s * (2 * OPER_B / 4), 2 * OPER_B, &full_bar[s]);
         }
     }
-    if (warp == W_MMA) {   // the MMA warp owns the TMEM allocation
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)),
-                     "n"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = s_tmem;
-    SPK_PDL_WAIT();      // barrier init and TMEM allocation above overlap the previous kernel's tail; no global access yet
-    if (tid == 0) TRACE(1);
+    SPK_PDL_WAIT();      // barrier init above overlaps the previous kernel's tail; no global access yet
 
     if (warp >= W_PROD0) {
         // =========================================== producers ===========================================
@@ -231,9 +168,8 @@ __global__ void __launch_bounds__(Cfg<TN>::NTHREADS, 1) k_dense_tc(TcArgs g) {
             const int k = kt * TK + chunk * 4;
             const bool k_ok = k < g.K;                         // K % 4 == 0: a 16 B chunk is entirely in or out
 #if SPK_TC_STAGGER > 0
-            // The first NPROD K-tiles are requested in K order, SPK_TC_STAGGER cycles apart: issued all at once, 6 x (8 KB of
-            // A + 16 KB of W) share the SM's ~50 B/clk L2 port and K-tile 0 -- which the first MMA waits for -- lands last
-            // as likely as first (measured: first stage published 1.9 us after the wait returned).
+            // The first NPROD K-tiles are requested in K order, SPK_TC_STAGGER cycles apart: issued all at once they share
+            // the SM's L2 port and K-tile 0 -- which the first MMA waits for -- lands last as likely as first.
             if (kt < NPROD && kt > 0) {
                 const long long t0 = clock64();
                 while (clock64() - t0 < (long long)kt * SPK_TC_STAGGER) { }
@@ -257,8 +193,7 @@ __global__ void __launch_bounds__(Cfg<TN>::NTHREADS, 1) k_dense_tc(TcArgs g) {
                 }
                 av[p] = v;
             }
-            if (kt < 16) TRACE(16 + kt);                       // loads issued
-            if (use >= 1) mbar_wait(&empty_bar[s], (use - 1) & 1);      // MMAs that read this stage have retired
+            if (use >= 1) mbar_wait(&empty_bar[s], (use - 1) & 1);      // wgmma that read this stage have completed
             if (lane == 0 && use >= 1) {   // weight tile (hi|lo, operand layout): one TMA bulk copy (first uses: prefetched above)
                 mbar_expect_tx(&full_bar[s], 2 * OPER_B);
                 tma_load(st + 2 * OPER_A, wp_tile0 + (int64_t)kt * (2 * OPER_B / 4), 2 * OPER_B, &full_bar[s]);
@@ -273,102 +208,41 @@ __global__ void __launch_bounds__(Cfg<TN>::NTHREADS, 1) k_dense_tc(TcArgs g) {
                 *reinterpret_cast<float4*>(st + off) = hi;
                 *reinterpret_cast<float4*>(st + OPER_A + off) = lo;
             }
-            // generic-proxy stores -> visible to the tensor core (async proxy), then signal the MMA warp
+            // generic-proxy stores -> visible to the tensor core (async proxy), then signal the consumers
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             __syncwarp();
             if (lane == 0) mbar_arrive(&full_bar[s]);
-            if (kt < 16) TRACE(32 + kt);                       // stage published
             if (lane == 0 && (kt == 0 || kt == nk - 1)) SPK_TL_PHASE(kt == 0 ? 2 : 3);   // first / last stage published
         }
-    } else if (warp == W_MMA) {
-        // =========================================== MMA issuer ===========================================
-        if (lane == 0) {
-            // instruction descriptor: D=F32 (1<<4), A=B=TF32 (2<<7, 2<<10), K-major, N>>3 at [17,23), M>>4 at [24,29)
-            const uint32_t idesc =
-                (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-            for (int kt = 0; kt < nk; ++kt) {
-                const int s = kt % NST;
-                const int grp = kt / ACC_KT, buf = grp & 1;                     // accumulator group of ACC_KT K-tiles
-                const bool first = (kt % ACC_KT) == 0, last = (kt % ACC_KT) == ACC_KT - 1 || kt == nk - 1;
-                mbar_wait(&full_bar[s], (kt / NST) & 1);
-                if (first && grp >= 2) mbar_wait(&acc_empty[buf], ((grp >> 1) - 1) & 1);   // drain warps are done with it
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
-                const uint32_t d_main = tmem_base + (uint32_t)(buf * TN);
-                const uint32_t d_corr = tmem_base + (uint32_t)(2 * TN);
-                const uint32_t d_corr2 = tmem_base + (uint32_t)((1 + N_CORR) * TN);
-#pragma unroll
-                for (int ks = 0; ks < TK / 8; ++ks) {
-                    const uint64_t ah = make_desc(sa + 32 * ks);                     // k-step = 8 floats = 32 B
-                    const uint64_t al = make_desc(sa + OPER_A + 32 * ks);
-                    const uint64_t bh = make_desc(sa + 2 * OPER_A + 32 * ks);
-                    const uint64_t bl = make_desc(sa + 2 * OPER_A + OPER_B + 32 * ks);
-                    umma_tf32(d_corr, al, bh, idesc, (kt | ks) ? 1u : 0u);   // small terms: accumulate over all of K
-                    umma_tf32(d_corr2, ah, bl, idesc, (N_CORR == 1 || (kt | ks)) ? 1u : 0u);
-                    umma_tf32(d_main, ah, bh, idesc, (ks || !first) ? 1u : 0u);   // main term: fresh accumulator per group
-                }
-                umma_commit(&empty_bar[s]);      // stage reusable once these MMAs have read it
-                if (last) umma_commit(&acc_full[buf]);   // main buffer (and, after the last tile, the corrections) ready
-                if (kt < 16) TRACE(48 + kt);     // MMAs of this K-tile issued
-                if (kt == 0 || kt == nk - 1) SPK_TL_PHASE(kt == 0 ? 4 : 5);   // first / last K-tile's MMAs issued
-            }
-        }
     } else {
-        // =========================================== drain ===========================================
-        const int q = warp & 3;                          // TMEM lane quarter this warp may access
-        const int ch = warp >> 2;                        // column half
-        const int row = q * 32 + lane;                   // output row inside the tile == TMEM lane
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(ch * CW);
-        float accr[CW];
+        // =========================================== consumers: wgmma, fp32 accumulation in registers ===========================
+        const int wg = warp >> 2;                        // rows wg * 64 .. wg * 64 + 63 of the tile
+        float acc[NB][32];
 #pragma unroll
-        for (int i = 0; i < CW; ++i) accr[i] = 0.f;
-        const int ngrp = (nk + ACC_KT - 1) / ACC_KT;
-        for (int kt = 0; kt < ngrp; ++kt) {                    // kt counts accumulator groups here
-            const int buf = kt & 1;
-            mbar_wait(&acc_full[buf], (kt >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (warp == 0 && kt < 16) TRACE(80 + kt);          // accumulator ready
+        for (int cb = 0; cb < NB; ++cb)
 #pragma unroll
-            for (int c0 = 0; c0 < CW; c0 += 32) {
-                uint32_t r[32];
-                tmem_ld32(lane_addr + (uint32_t)(buf * TN + c0), r);
-#pragma unroll
-                for (int j = 0; j < 32; ++j) accr[c0 + j] += __uint_as_float(r[j]);
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+            for (int i = 0; i < 32; ++i) acc[cb][i] = 0.f;
+        for (int kt = 0; kt < nk; ++kt) {
+            const int s = kt % NST;
+            mbar_wait(&full_bar[s], (kt / NST) & 1);
+            const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
+            wg_ktile_3xtf32<NB>(acc, sa + wg * SPK_WG_ROWS_BYTES, sa + OPER_A + wg * SPK_WG_ROWS_BYTES, sa + 2 * OPER_A,
+                                sa + 2 * OPER_A + OPER_B);
             __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[buf]);
-            if (warp == 0 && kt < 16) TRACE(64 + kt);          // drained
+            if (lane == 0) mbar_arrive(&empty_bar[s]);
+            if (warp == 0 && lane == 0 && (kt == 0 || kt == nk - 1)) SPK_TL_PHASE(kt == 0 ? 4 : 5);
         }
-        // the last acc_full commit also covers every correction MMA, and every MMA has finished reading the stages:
-        // their memory now stages the raw fp32 tile (row-major, padded rows) for the CTA-wide epilogue
-        float* ep = reinterpret_cast<float*>(smem) + row * EP_LD + ch * CW;
-#pragma unroll
-        for (int c0 = 0; c0 < CW; c0 += 32) {
-            uint32_t r[32];
-            if (N_CORR == 2) {
-                tmem_ld32(lane_addr + (uint32_t)(3 * TN + c0), r);
-#pragma unroll
-                for (int j = 0; j < 32; ++j) accr[c0 + j] += __uint_as_float(r[j]);
-            }
-            tmem_ld32(lane_addr + (uint32_t)(2 * TN + c0), r);
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-                *reinterpret_cast<float4*>(ep + c0 + j) =
-                    make_float4(accr[c0 + j + 0] + __uint_as_float(r[j + 0]), accr[c0 + j + 1] + __uint_as_float(r[j + 1]),
-                                accr[c0 + j + 2] + __uint_as_float(r[j + 2]), accr[c0 + j + 3] + __uint_as_float(r[j + 3]));
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        if (warp == 0) TRACE(2);                               // tile staged
+        // both warpgroups have completed every wgmma (and the producers every store): the stages now hold the raw tile
+        wg_bar(1, N_CONS * 32);
+        wg_stage_tile<NB>(acc, reinterpret_cast<float*>(smem), EP_LD, wg, tid & 127);
         if (warp == 0 && lane == 0) SPK_TL_PHASE(6);
     }
     __syncthreads();
     // =========================================== epilogue: all warps, coalesced ===========================================
     {
         // Every thread owns ONE float4 column group (NTHREADS is a multiple of TN / 4) and walks down the rows: the bias is
-        // loaded once, pointers advance by constant strides (the index arithmetic of a flat loop was most of the epilogue's
-        // instructions), and the loads of RB rows are issued before their stores (the outputs may alias the inputs as
-        // far as the compiler knows, so it cannot hoist them itself).
+        // loaded once, pointers advance by constant strides, and the loads of RB rows are issued before their stores (the
+        // outputs may alias the inputs as far as the compiler knows, so it cannot hoist them itself).
         static_assert(NTHREADS % (TN / 4) == 0, "one column group per thread");
         constexpr int RSTEP = NTHREADS / (TN / 4), RB = 3;
         const float* ept = reinterpret_cast<const float*>(smem);
@@ -416,13 +290,7 @@ __global__ void __launch_bounds__(Cfg<TN>::NTHREADS, 1) k_dense_tc(TcArgs g) {
             }
         }
     }
-    if (tid == 0) TRACE(3);
     if (tid == 0) SPK_TL_PHASE(7);                                // this CTA's epilogue stores issued
-    __syncthreads();
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
-    }
 }
 
 }  // namespace
@@ -487,9 +355,6 @@ extern "C" int spk_dense_tc(const float* A, int64_t M, int K, int64_t lda, const
     TcArgs g;
     g.A = A; g.a_pre = a_pre; g.Wp = W_packed; g.bias = bias; g.addend = addend; g.Y = Y; g.y_pre = y_pre;
     g.M = M; g.lda = lda; g.ld_add = ld_add; g.ldy = ldy; g.K = K; g.N = N; g.a_act = a_act; g.act = act; g.save_deriv = save_deriv;
-#ifdef SPK_TC_TRACE
-    g.dbg = nullptr;
-#endif
     cudaStream_t st = spk_st(stream);
     int rc;
     if (tile_n(M, N) == 128) {

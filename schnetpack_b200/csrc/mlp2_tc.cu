@@ -1,27 +1,25 @@
-// Two Dense layers as ONE launch on the tcgen05 tensor cores, hidden tile resident in shared memory (round 2):
+// Two Dense layers as ONE launch on the Hopper tensor cores (wgmma), hidden tile resident in shared memory:
 //
 //     H = act(A W0^T + b0)            A [M,K1], W0 [128,K1]                (also stored: act'(pre) [M,128] for the reverse pass)
 //     Y = H W1^T + b1 [+ addend]      W1 [N2,128]
 //
 // Reference: every Dense -> Dense pair of the per-atom path -- interatomic_context_net and intraatomic_context_net of PaiNN
-// (/root/reference/src/schnetpack/representation/painn.py:39-44, 84-91: Dense(F, F, silu) -> Dense(F, 3F)).
+// (representation/painn.py of the reference: Dense(F, F, silu) -> Dense(F, 3F)).
 //
-// Why (tools/timeline.py, profiles/r2_timeline_cfg2.txt): inside the programmatic-launch chain a K = 128 k_dense_tc launch is
-// 8.7-10 us of which 3.3 us is MMA issue; the rest is paid per LAUNCH -- 1.4 us until the first operand stage is published,
-// ~2 us of epilogue (64 KB of stores from one SM), 1.4 us until the next kernel's dependency wait returns.  For a pair, the
+// Why: a K = 128 k_dense_tc launch pays a launch boundary, a pipeline fill and an epilogue of its own, and for a pair the
 // hidden activations make a round trip through L2 in between.  Here a CTA owns a 128-row tile and ONE 128-column tile of the
-// final output; it computes the whole hidden tile itself (every column-tile CTA repeats that GEMM: 48 more MMAs, but no second
+// final output; it computes the whole hidden tile itself (every column-tile CTA repeats that GEMM, but there is no second
 // launch boundary, no hidden-layer store/load, one load phase), writes act(.) hi/lo-split straight into shared memory in the
-// UMMA operand layout (K-major, 64-byte swizzle: exactly what the producers of gemm_tc.cu build from global memory), and runs
+// wgmma operand layout (K-major, 64-byte swizzle: exactly what the producers of gemm_tc.cu build from global memory), and runs
 // the second GEMM from there while the W1 tiles stream through the same TMA ring.  Precision scheme, pipeline roles, operand
-// layout and epilogue are those of gemm_tc.cu (3xTF32, fresh main accumulator per K-tile drained into fp32 registers, small
-// products in a correction accumulator).
-#include "tcgen05.cuh"
+// layout and epilogue are those of gemm_tc.cu (3xTF32, fresh accumulator per K-tile added to fp32 registers).  Each consumer
+// warpgroup owns 64 rows of both GEMMs, so the hidden rows it writes are exactly the A rows it reads back.
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int TM = 128, TK = 16, TN = 128, HID = 128;
-constexpr int N_DRAIN = 8, W_MMA = 8, W_PROD0 = 9, NST = 3, NPROD = 3;
+constexpr int N_CONS = 8, W_PROD0 = 8, NST = 3, NPROD = 3;
 constexpr int OPER_A = TM * TK * 4;            // 8192 B
 constexpr int OPER_B = TN * TK * 4;            // 8192 B
 constexpr int STAGE_BYTES = 2 * OPER_A + 2 * OPER_B;       // A_hi, A_lo, W_hi, W_lo
@@ -30,23 +28,10 @@ constexpr int A2_BYTES = 2 * NK2 * OPER_A;     // hidden operand [hi, lo][k-tile
 constexpr int EP_LD = TN + 4;
 constexpr int SMEM_BYTES = NST * STAGE_BYTES + A2_BYTES + 1024;
 constexpr int NTHREADS = (W_PROD0 + NPROD) * 32;
-constexpr int TMEM_COLS = 512;                 // main[0] | main[1] | corr | (unused)
+constexpr int NB = TN / 64;                    // m64n64 column blocks per consumer warpgroup
 static_assert(A2_BYTES >= TM * EP_LD * 4, "the epilogue staging tile reuses the hidden operand");
 static_assert(NST == NPROD, "a stage is owned by exactly one producer warp in both phases");
 static_assert(NTHREADS % (TN / 4) == 0, "one column group per thread in the epilogue");
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 
 struct Mlp2Args {
     const float* A;
@@ -67,11 +52,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp2_tc(Mlp2Args g) {
     uint8_t* sA2 = smem + NST * STAGE_BYTES;
     __shared__ __align__(8) uint64_t full_bar[NST];
     __shared__ __align__(8) uint64_t empty_bar[NST];
-    __shared__ __align__(8) uint64_t acc_full[2];
-    __shared__ __align__(8) uint64_t acc_empty[2];
-    __shared__ __align__(8) uint64_t h_ready;
-    __shared__ uint32_t s_tmem;
-
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // broadcast: the compiler may treat the role index as warp-uniform
     SPK_PDL_LAUNCH_DEPENDENTS();
@@ -85,13 +65,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp2_tc(Mlp2Args g) {
 #pragma unroll
         for (int s = 0; s < NST; ++s) {
             mbar_init(&full_bar[s], 2);      // expect_tx arrive (weight TMA) + arrive after the A tile is stored (phase 2: plain)
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], N_CONS);
         }
-        mbar_init(&acc_full[0], 1);
-        mbar_init(&acc_full[1], 1);
-        mbar_init(&acc_empty[0], N_DRAIN);
-        mbar_init(&acc_empty[1], N_DRAIN);
-        mbar_init(&h_ready, N_DRAIN);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         // static operands: the first W0 tiles are fetched BEFORE griddepcontrol.wait (pack kernels never trigger early)
         for (int s = 0; s < NST && s < nk1; ++s) {
@@ -99,15 +74,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp2_tc(Mlp2Args g) {
             tma_load(smem + s * STAGE_BYTES + 2 * OPER_A, g.W0p + (int64_t)s * (2 * OPER_B / 4), 2 * OPER_B, &full_bar[s]);
         }
     }
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)),
-                     "n"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = s_tmem;
     SPK_PDL_WAIT();
 
     if (warp >= W_PROD0) {
@@ -161,114 +128,62 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp2_tc(Mlp2Args g) {
             }
             __syncwarp();
         }
-    } else if (warp == W_MMA) {
-        // =========================================== MMA issuer ===========================================
-        if (lane == 0) {
-            const uint32_t idesc =
-                (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-            const uint32_t d_corr = tmem_base + (uint32_t)(2 * TN);
-            for (int kt = 0; kt < nkt; ++kt) {
-                const int s = kt % NST, buf = kt & 1;
-                const bool second = kt >= nk1;
-                if (kt == nk1) {
-                    SPK_TL_PHASE(3);                              // GEMM 1 issued
-                    mbar_wait(&h_ready, 0);                       // hidden operand stored; GEMM 1's accumulators fully read
-                    SPK_TL_PHASE(4);                              // hidden tile ready
-                }
+    } else {
+        // =========================================== consumers: wgmma, fp32 accumulation in registers ===========================
+        const int wg = warp >> 2, t = tid & 127;         // rows wg * 64 .. wg * 64 + 63 of both GEMMs
+        float acc[NB][32];
+        auto gemm = [&](int kt_begin, int kt_end) {
+#pragma unroll
+            for (int cb = 0; cb < NB; ++cb)
+#pragma unroll
+                for (int i = 0; i < 32; ++i) acc[cb][i] = 0.f;
+            for (int kt = kt_begin; kt < kt_end; ++kt) {
+                const int s = kt % NST;
                 mbar_wait(&full_bar[s], (kt / NST) & 1);
-                if (kt >= 2) mbar_wait(&acc_empty[buf], ((kt >> 1) - 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
                 const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
+                const bool second = kt >= nk1;
                 const uint32_t a_hi = second ? smem_u32(sA2 + (kt - nk1) * OPER_A) : sa;
                 const uint32_t a_lo = second ? smem_u32(sA2 + (NK2 + kt - nk1) * OPER_A) : sa + OPER_A;
-                const uint32_t d_main = tmem_base + (uint32_t)(buf * TN);
-                const bool first_of_gemm = kt == 0 || kt == nk1;
-#pragma unroll
-                for (int ks = 0; ks < TK / 8; ++ks) {
-                    const uint64_t ah = make_desc(a_hi + 32 * ks);
-                    const uint64_t al = make_desc(a_lo + 32 * ks);
-                    const uint64_t bh = make_desc(sa + 2 * OPER_A + 32 * ks);
-                    const uint64_t bl = make_desc(sa + 2 * OPER_A + OPER_B + 32 * ks);
-                    umma_tf32(d_corr, al, bh, idesc, (first_of_gemm && ks == 0) ? 0u : 1u);   // small terms over all of K
-                    umma_tf32(d_corr, ah, bl, idesc, 1u);
-                    umma_tf32(d_main, ah, bh, idesc, ks ? 1u : 0u);                            // fresh main per K-tile
-                }
-                umma_commit(&empty_bar[s]);
-                umma_commit(&acc_full[buf]);
-                if (kt == nkt - 1) SPK_TL_PHASE(5);               // GEMM 2 issued
-            }
-        }
-    } else {
-        // =========================================== drain ===========================================
-        const int q = warp & 3, ch = warp >> 2;
-        const int row = q * 32 + lane;
-        constexpr int CW = TN / 2;
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(ch * CW);
-        float accr[CW];
-        auto drain = [&](int kt_begin, int kt_end) {
-#pragma unroll
-            for (int i = 0; i < CW; ++i) accr[i] = 0.f;
-            for (int kt = kt_begin; kt < kt_end; ++kt) {
-                const int buf = kt & 1;
-                mbar_wait(&acc_full[buf], (kt >> 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-                for (int c0 = 0; c0 < CW; c0 += 32) {
-                    uint32_t r[32];
-                    tmem_ld32(lane_addr + (uint32_t)(buf * TN + c0), r);
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) accr[c0 + j] += __uint_as_float(r[j]);
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+                wg_ktile_3xtf32<NB>(acc, a_hi + wg * SPK_WG_ROWS_BYTES, a_lo + wg * SPK_WG_ROWS_BYTES, sa + 2 * OPER_A,
+                                    sa + 2 * OPER_A + OPER_B);
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&acc_empty[buf]);
+                if (lane == 0) mbar_arrive(&empty_bar[s]);
             }
         };
-        // ---- GEMM 1 -> hidden tile: + corrections + b0, activation (value and derivative), hi/lo split into the operand
-        drain(0, nk1);
-        const bool store_deriv = g.h_deriv != nullptr && blockIdx.y == 0 && m0 + row < g.M;
+        // ---- GEMM 1 -> hidden tile: + b0, activation (value and derivative), hi/lo split into the operand
+        gemm(0, nk1);
+        SPK_TL_PHASE(3);
 #pragma unroll
-        for (int c0 = 0; c0 < CW; c0 += 32) {
-            uint32_t r[32];
-            tmem_ld32(lane_addr + (uint32_t)(2 * TN + c0), r);
+        for (int cb = 0; cb < NB; ++cb) {
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-                const int c = ch * CW + c0 + j;                 // hidden unit == K index of GEMM 2
-                float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (g.b0) bv = *reinterpret_cast<const float4*>(g.b0 + c);
-                float x[4] = {accr[c0 + j + 0] + __uint_as_float(r[j + 0]) + bv.x, accr[c0 + j + 1] + __uint_as_float(r[j + 1]) + bv.y,
-                              accr[c0 + j + 2] + __uint_as_float(r[j + 2]) + bv.z, accr[c0 + j + 3] + __uint_as_float(r[j + 3]) + bv.w};
-                float y[4], d[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) spk_act_both(x[u], g.act, y[u], d[u]);
-                if (store_deriv)
-                    *reinterpret_cast<float4*>(g.h_deriv + (m0 + row) * HID + c) = make_float4(d[0], d[1], d[2], d[3]);
-                float4 hi, lo;
-                hi.x = tf32_rn(y[0]); hi.y = tf32_rn(y[1]); hi.z = tf32_rn(y[2]); hi.w = tf32_rn(y[3]);
-                lo.x = y[0] - hi.x; lo.y = y[1] - hi.y; lo.z = y[2] - hi.z; lo.w = y[3] - hi.w;
-                const int kt2 = c >> 4, off = tile_off(row, (c & 15) >> 2);
-                *reinterpret_cast<float4*>(sA2 + kt2 * OPER_A + off) = hi;
-                *reinterpret_cast<float4*>(sA2 + (NK2 + kt2) * OPER_A + off) = lo;
+            for (int i = 0; i < 32; i += 2) {
+                const int row = wg * 64 + wg_frag_row(t, i);
+                const int c = cb * 64 + wg_frag_col(t, i);                // hidden unit == K index of GEMM 2 (even)
+                float2 bv = make_float2(0.f, 0.f);
+                if (g.b0) bv = *reinterpret_cast<const float2*>(g.b0 + c);
+                float y0, y1, d0, d1;
+                spk_act_both(acc[cb][i] + bv.x, g.act, y0, d0);
+                spk_act_both(acc[cb][i + 1] + bv.y, g.act, y1, d1);
+                if (g.h_deriv != nullptr && blockIdx.y == 0 && m0 + row < g.M)
+                    *reinterpret_cast<float2*>(g.h_deriv + (m0 + row) * HID + c) = make_float2(d0, d1);
+                const float h0 = tf32_rn(y0), h1 = tf32_rn(y1);
+                const int kt2 = c >> 4, off = tile_off(row, (c & 15) >> 2) + (c & 3) * 4;
+                *reinterpret_cast<float2*>(sA2 + kt2 * OPER_A + off) = make_float2(h0, h1);
+                *reinterpret_cast<float2*>(sA2 + (NK2 + kt2) * OPER_A + off) = make_float2(y0 - h0, y1 - h1);
             }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy stores -> visible to the tensor core
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&h_ready);
-        // ---- GEMM 2 -> raw output tile staged in shared memory (the hidden operand is dead once its MMAs have completed)
-        drain(nk1, nkt);
-        float* ep = reinterpret_cast<float*>(sA2) + row * EP_LD + ch * CW;
+        wg_bar(1 + wg);                                                   // this warpgroup's hidden rows are complete
+        SPK_TL_PHASE(4);
+        // ---- GEMM 2 -> raw output tile staged in shared memory once both warpgroups are done reading the hidden operand
+        gemm(nk1, nkt);
+        wg_bar(3, N_CONS * 32);
 #pragma unroll
-        for (int c0 = 0; c0 < CW; c0 += 32) {
-            uint32_t r[32];
-            tmem_ld32(lane_addr + (uint32_t)(2 * TN + c0), r);
+        for (int cb = 0; cb < NB; ++cb)
 #pragma unroll
-            for (int j = 0; j < 32; j += 4)
-                *reinterpret_cast<float4*>(ep + c0 + j) =
-                    make_float4(accr[c0 + j + 0] + __uint_as_float(r[j + 0]), accr[c0 + j + 1] + __uint_as_float(r[j + 1]),
-                                accr[c0 + j + 2] + __uint_as_float(r[j + 2]), accr[c0 + j + 3] + __uint_as_float(r[j + 3]));
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+            for (int i = 0; i < 32; i += 2)
+                *reinterpret_cast<float2*>(reinterpret_cast<float*>(sA2) + (wg * 64 + wg_frag_row(t, i)) * EP_LD + cb * 64 +
+                                           wg_frag_col(t, i)) = make_float2(acc[cb][i], acc[cb][i + 1]);
         if (warp == 0 && lane == 0) SPK_TL_PHASE(6);              // output tile staged
     }
     __syncthreads();
@@ -306,11 +221,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp2_tc(Mlp2Args g) {
         }
     }
     if (tid == 0) SPK_TL_PHASE(7);                                // epilogue stores issued
-    __syncthreads();
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
-    }
 }
 
 }  // namespace

@@ -112,13 +112,13 @@ __global__ void __launch_bounds__(NW * 32, SPK_EDGE_MINB(NW)) k_painn_edge_fwd(
             for (int k4 = 0; k4 < NRB / 4; ++k4) {
                 const float4 p = ph[k4];
                 const float2 p01 = make_float2(p.x, p.y), p23 = make_float2(p.z, p.w);
-                pa2 = __ffma2_rn(p01, w.a[2 * k4], pa2);
-                pb2 = __ffma2_rn(p01, w.b[2 * k4], pb2);
-                pa2 = __ffma2_rn(p23, w.a[2 * k4 + 1], pa2);
-                pb2 = __ffma2_rn(p23, w.b[2 * k4 + 1], pb2);
+                pa2 = spk_fma2(p01, w.a[2 * k4], pa2);
+                pb2 = spk_fma2(p01, w.b[2 * k4], pb2);
+                pa2 = spk_fma2(p23, w.a[2 * k4 + 1], pa2);
+                pb2 = spk_fma2(p23, w.b[2 * k4 + 1], pb2);
                 if (HAS_MU) {
-                    pc2 = __ffma2_rn(p01, w.c[2 * k4], pc2);
-                    pc2 = __ffma2_rn(p23, w.c[2 * k4 + 1], pc2);
+                    pc2 = spk_fma2(p01, w.c[2 * k4], pc2);
+                    pc2 = spk_fma2(p23, w.c[2 * k4 + 1], pc2);
                 }
             }
             const float pa = pa2.x + pa2.y, pb = pb2.x + pb2.y, pc = pc2.x + pc2.y;
@@ -269,19 +269,19 @@ __global__ void __launch_bounds__(NW * 32, SPK_EDGE_MINB(NW)) k_painn_edge_bwd(
                         const float4 d4 = dh[k4];
                         const float2 p01 = make_float2(p4.x, p4.y), p23 = make_float2(p4.z, p4.w);
                         const float2 d01 = make_float2(d4.x, d4.y), d23 = make_float2(d4.z, d4.w);
-                        pa2 = __ffma2_rn(p01, w.a[2 * k4], pa2);
-                        da2 = __ffma2_rn(d01, w.a[2 * k4], da2);
-                        pb2 = __ffma2_rn(p01, w.b[2 * k4], pb2);
-                        db2 = __ffma2_rn(d01, w.b[2 * k4], db2);
-                        pa2 = __ffma2_rn(p23, w.a[2 * k4 + 1], pa2);
-                        da2 = __ffma2_rn(d23, w.a[2 * k4 + 1], da2);
-                        pb2 = __ffma2_rn(p23, w.b[2 * k4 + 1], pb2);
-                        db2 = __ffma2_rn(d23, w.b[2 * k4 + 1], db2);
+                        pa2 = spk_fma2(p01, w.a[2 * k4], pa2);
+                        da2 = spk_fma2(d01, w.a[2 * k4], da2);
+                        pb2 = spk_fma2(p01, w.b[2 * k4], pb2);
+                        db2 = spk_fma2(d01, w.b[2 * k4], db2);
+                        pa2 = spk_fma2(p23, w.a[2 * k4 + 1], pa2);
+                        da2 = spk_fma2(d23, w.a[2 * k4 + 1], da2);
+                        pb2 = spk_fma2(p23, w.b[2 * k4 + 1], pb2);
+                        db2 = spk_fma2(d23, w.b[2 * k4 + 1], db2);
                         if (HAS_MU) {
-                            pc2 = __ffma2_rn(p01, w.c[2 * k4], pc2);
-                            dc2 = __ffma2_rn(d01, w.c[2 * k4], dc2);
-                            pc2 = __ffma2_rn(p23, w.c[2 * k4 + 1], pc2);
-                            dc2 = __ffma2_rn(d23, w.c[2 * k4 + 1], dc2);
+                            pc2 = spk_fma2(p01, w.c[2 * k4], pc2);
+                            dc2 = spk_fma2(d01, w.c[2 * k4], dc2);
+                            pc2 = spk_fma2(p23, w.c[2 * k4 + 1], pc2);
+                            dc2 = spk_fma2(d23, w.c[2 * k4 + 1], dc2);
                         }
                     }
                     const float pa = pa2.x + pa2.y, pb = pb2.x + pb2.y, pc = pc2.x + pc2.y;
@@ -438,7 +438,7 @@ int launch_edge_fwd(const float* x, const float* mu, const float* q, const float
                     const int* rowptr, const int* slot_j, const float* wf, const float* bf, int n_atoms, int n_edges,
                     int n_rbf, float* q_out, float* mu_out, cudaStream_t st) {
     // exactly one resident wave of CTAs (no tail), >= 32 edges per CTA, at most one CTA per atom
-    static int occ_mu = 0, occ_nomu = 0;      // occupancy of a template instantiation: the same on every B200 of a box
+    static int occ_mu = 0, occ_nomu = 0;      // occupancy of a template instantiation: the same on every GPU of a box
     if (!occ_mu) {
         int a = 0, b = 0;
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, k_painn_edge_fwd<NW, NRB, true>, NW * 32, 0);

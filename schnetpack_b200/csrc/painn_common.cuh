@@ -3,8 +3,8 @@
 #include "common.cuh"
 
 // Filter weights of one channel as k-PAIRS (w[2m], w[2m+1]): with the radial basis read from shared memory as natural
-// (phi[2m], phi[2m+1]) pairs, one packed FFMA2 (fma.rn.f32x2 -- Blackwell's full-rate fp32 path; scalar FFMA issues at
-// half rate) advances an even-k and an odd-k partial sum at once; the two partials are added at the end.
+// (phi[2m], phi[2m+1]) pairs, one spk_fma2 advances an even-k and an odd-k partial sum (two independent dependency chains);
+// the two partials are added at the end.
 template <int NRB>
 struct FilterRegs {
     float2 a[NRB / 2], b[NRB / 2], c[NRB / 2];

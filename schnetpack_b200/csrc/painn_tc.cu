@@ -1,36 +1,33 @@
-// PaiNN fused edge kernel with the continuous filter evaluated on the tensor cores (tcgen05, TMEM).
-// Reference: representation/painn.py:55-65 (message), :232 (filter = filter_net(phi) * fcut), nn/scatter.py:26-34.
+// PaiNN fused edge kernel with the continuous filter evaluated on the tensor cores (wgmma).
+// Reference: representation/painn.py (message, filter = filter_net(phi) * fcut), nn/scatter.py.
 //
-// Why: the streaming kernel of painn.cu is bound by the load/store unit, not by HBM, L2, FMA or latency (measured on
-// B200: more resident warps, deeper gather pipelines and TMA staging all left it at ~210 cycles per edge and SM, which is
-// 4 warps x 13 LSU operations x 4 cycles): every warp re-reads the edge's 20 radial-basis values as warp-broadcast LDS.128
-// (4 LSU cycles each -- a broadcast 16 B load costs as much as four 4 B loads) to feed 60 FFMA2.  The filter
+// Why: evaluated per channel on the CUDA cores (painn.cu), every warp re-reads the edge's radial-basis values as warp-broadcast
+// shared-memory loads to feed its FMAs, and the load/store unit, not HBM, bounds the kernel.  The filter
 //       W[e, c] = fc_e * (b_c + sum_k phi_k(d_e) w_ck)            c in [0, 3F)
-// is a GEMM with K = n_rbf + 1, so here it runs on the tensor pipe instead and the LSU only carries the gathers:
+// is a GEMM with K = n_rbf + 1, so here it runs on the tensor cores instead and the LSU only carries the gathers:
 //
 //   * orientation: channels on the M side.  For each filter third t the A operand is W_t = [w | b] (128 channels x 32,
 //     static, packed once by spk_painn_pack_filter in the shared-memory operand layout and fetched by ONE TMA bulk copy),
 //     the B operand is a chunk of 64 edge rows  Phi' = fc * [phi | 1]  (K-major, 64 B swizzle, produced per chunk by
-//     two producer warps with the hi/lo split of 3xTF32), and D_t = W_t Phi'^T lands in TMEM as
-//     lane = channel, column = edge -- exactly the thread = channel mapping of the gather/accumulate code, so a consumer
-//     reads the filter values of its channel for 16 edges with one tcgen05.ld.32x32b.x16 per third;
-//   * 3xTF32 (Wh*Ph + Wl*Ph + Wh*Pl, small terms first) keeps the filter at fp32 accuracy; K = 24 is three k-steps, so a
-//     chunk costs 27 MMAs (~130 cycles each for any N <= 256);
-//   * one persistent CTA per SM: 16 consumer warps = 4 groups x 4 warps (a group owns 128 channels of its own
-//     edge-balanced receiver range, as a CTA of painn.cu did), 1 MMA-issuer warp, 2 producer warps; two Phi' stages and
-//     two TMEM accumulator sets (3 x 64 columns each) let chunk k+1's staging and MMAs overlap chunk k's gathers.
+//     the producer warps with the hi/lo split of 3xTF32);
+//   * one persistent CTA per SM: 4 consumer warpgroups (a group owns 128 channels of its own edge-balanced receiver range,
+//     as a CTA of painn.cu did) and the producer warps.  Group g multiplies W_t by ITS 16 rows of the chunk (wgmma m64n16,
+//     two m64 halves), so no group waits for another; the fragments go through a small shared-memory transpose to
+//     thread = channel, the mapping of the gather/accumulate code;
+//   * 3xTF32 (Wl*Ph + Wh*Pl + Wh*Ph, small terms first) keeps the filter at fp32 accuracy; K = 24 is three k-steps;
+//   * NST Phi' stages let the producers stage chunk k+1.. while the groups gather chunk k.
 // The reduction over a receiver's edges stays a private register accumulation in CSR order: deterministic, no atomics.
 #include "painn_common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 
 #ifdef SPK_EDGE_TRACE                          // -DSPK_EDGE_TRACE=1: forward kernel stamps, =2: reverse kernel stamps
-__device__ long long g_edge_trace[148 * 256];
+__device__ long long g_edge_trace[SPK_NUM_SMS * 256];
 #define EDGE_STAMP(slot)                                                                 \
     do {                                                                                 \
         if ((threadIdx.x & 31) == 0 && (slot) < 256) g_edge_trace[blockIdx.x * 256 + (slot)] = clock64(); \
     } while (0)
 extern "C" int spk_debug_edge_trace(long long* host) {
-    return (int)cudaMemcpyFromSymbol(host, g_edge_trace, sizeof(long long) * 148 * 256);
+    return (int)cudaMemcpyFromSymbol(host, g_edge_trace, sizeof(long long) * SPK_NUM_SMS * 256);
 }
 #endif
 #if defined(SPK_EDGE_TRACE) && SPK_EDGE_TRACE == 2
@@ -46,13 +43,12 @@ extern "C" int spk_debug_edge_trace(long long* host) {
 
 namespace {
 
-constexpr int F_TC = 128;                      // channels per filter third == UMMA M
-constexpr int EG = 16;                         // edges per group and chunk
-constexpr int NG = 4;                          // consumer groups
-constexpr int NE = EG * NG;                    // Phi' rows per chunk == UMMA N
+constexpr int F_TC = 128;                      // channels per filter third (two m64 halves)
+constexpr int EG = 16;                         // edges per group and chunk (wgmma N)
+constexpr int NG = 4;                          // consumer groups = warpgroups
+constexpr int NE = EG * NG;                    // Phi' rows per chunk
 constexpr int NCW = NG * 4;                    // consumer warps
-constexpr int W_MMA = NCW;
-constexpr int W_PROD0 = NCW + 1;
+constexpr int W_PROD0 = NCW;
 constexpr int NPROD = 3;                       // producer warps: chunk k -> warp k % NPROD
 constexpr int NST = 3;                         // Phi' stages: chunk k -> stage k % NST (NPROD divides NST: one owner per stage)
 constexpr int NTHREADS = (W_PROD0 + NPROD) * 32;
@@ -62,20 +58,49 @@ constexpr int A_BYTES = 3 * 2 * 2 * A_TILE;    // [third][hi,lo][k-tile]
 constexpr int B_TILE = NE * KT * 4;            // 4096 B
 constexpr int B_STAGE = 2 * 2 * B_TILE;        // [hi,lo][k-tile]
 constexpr int META_STAGE = NE * 4 + NE * 16;   // sender index + (ux, uy, uz, -) per row
-constexpr int SMEM_BYTES = A_BYTES + NST * B_STAGE + NST * META_STAGE + 1024;
-constexpr int TMEM_COLS = 512;                 // [buf][third][64 edge columns] = 384 used
-constexpr int BUF_COLS = 3 * NE;
+constexpr int T_LD = F_TC + 4;                 // row of the per-group transpose tile [column][channel] (floats)
+constexpr int T_BYTES = NG * 16 * T_LD * 4;    // 16 columns per group (forward: 16 edges; reverse: 8 edges x {W, dW/dd})
+constexpr int SMEM_BYTES = A_BYTES + NST * B_STAGE + NST * META_STAGE + T_BYTES + 1024;
 
-// 8 consecutive accumulator columns of this thread's TMEM lane -> registers (no wait: several loads are batched)
-__device__ __forceinline__ void tmem_ld8_nowait(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr));
+// The group's 3xTF32 filter products of one chunk for NT thirds: d[t][m-half] (+)= W_t * B^T over the three k-steps
+// (K = n_rbf + 1 <= 24), B = 16 (forward) or 8 (reverse) operand rows starting at byte offset b_row of the stage.
+template <int NT, int N>
+__device__ __forceinline__ void filter_mma(float (&d)[NT][2][N / 2], uint32_t aB, uint32_t bB) {
+    wgmma_fence();
 #pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
+    for (int t = 0; t < NT; ++t)
+#pragma unroll
+        for (int s3 = 0; s3 < 3; ++s3) {                     // k-steps 0..2 = (tile 0, 0), (tile 0, 32 B), (tile 1, 0)
+            const int kt = s3 >> 1, ko = (s3 & 1) * 32;
+            const uint64_t bh = make_desc(bB + (0 * 2 + kt) * B_TILE + ko);
+            const uint64_t bl = make_desc(bB + (1 * 2 + kt) * B_TILE + ko);
+#pragma unroll
+            for (int mh = 0; mh < 2; ++mh) {
+                const uint64_t ah = make_desc(aB + ((t * 2 + 0) * 2 + kt) * A_TILE + mh * SPK_WG_ROWS_BYTES + ko);
+                const uint64_t al = make_desc(aB + ((t * 2 + 1) * 2 + kt) * A_TILE + mh * SPK_WG_ROWS_BYTES + ko);
+                if constexpr (N == 16) {
+                    wgmma_n16(d[t][mh], al, bh, s3 ? 1 : 0);       // small terms first
+                    wgmma_n16(d[t][mh], ah, bl, 1);
+                    wgmma_n16(d[t][mh], ah, bh, 1);
+                } else {
+                    wgmma_n8(d[t][mh], al, bh, s3 ? 1 : 0);
+                    wgmma_n8(d[t][mh], ah, bl, 1);
+                    wgmma_n8(d[t][mh], ah, bh, 1);
+                }
+            }
+        }
+    wgmma_commit();
+    wgmma_wait_all();
 }
 
+// fragment (m64nN, two m-halves) of the warpgroup -> columns col0.. of the [column][channel] tile tg
+template <int N>
+__device__ __forceinline__ void frag_to_tile(const float (&d)[2][N / 2], float* tg, int col0, int t) {
+#pragma unroll
+    for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) tg[(col0 + wg_frag_col(t, i)) * T_LD + mh * 64 + wg_frag_row(t, i)] = d[mh][i];
+}
 
 // [third][hi,lo][k-tile][128 x 16] operand tiles of  [w | b | 0]  (k = n_rbf is the bias column)
 __global__ void k_pack_filter(const float* __restrict__ wf, const float* __restrict__ bf, int n_rbf,
@@ -106,8 +131,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
     uint8_t* sA = smem;
     uint8_t* sB = smem + A_BYTES;
     uint8_t* sMeta = sB + NST * B_STAGE;
-    __shared__ __align__(8) uint64_t a_full, full_bar[NST], empty_bar[NST], acc_full[2], acc_empty[2], meta_empty[NST];
-    __shared__ uint32_t s_tmem;
+    float* sT = reinterpret_cast<float*>(sMeta + NST * META_STAGE);
+    __shared__ __align__(8) uint64_t a_full, full_bar[NST], empty_bar[NST], meta_empty[NST];
     __shared__ int s_rlo[NG], s_rhi[NG], s_sb[NG], s_se[NG];
 
     const int tid = threadIdx.x, lane = tid & 31;
@@ -119,21 +144,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
 #pragma unroll
         for (int s = 0; s < NST; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], NCW);
             mbar_init(&meta_empty[s], NCW);
         }
-        mbar_init(&acc_full[0], 1);
-        mbar_init(&acc_full[1], 1);
-        mbar_init(&acc_empty[0], NCW);
-        mbar_init(&acc_empty[1], NCW);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         mbar_expect_tx(&a_full, A_BYTES);          // static operand: fetched BEFORE griddepcontrol.wait (pack kernels never trigger their dependents early, common.cuh)
         tma_load(sA, wpk, A_BYTES, &a_full);
-    }
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)),
-                     "n"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
     }
     SPK_PDL_WAIT();                                // everything below reads memory written by earlier kernels
     if (warp <= NG) {                              // warp w finds boundary w of this CTA's NG group ranges (warp-wide search)
@@ -150,10 +166,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = s_tmem;
     int n_chunks = 0;
 #pragma unroll
     for (int g = 0; g < NG; ++g) n_chunks = max(n_chunks, (s_se[g] - s_sb[g] + EG - 1) / EG);
@@ -173,7 +186,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
             float4* st_u = reinterpret_cast<float4*>(sMeta + st * META_STAGE + NE * 4);
             // all loads are unconditional (rows past a group's end read slot 0 and are zeroed afterwards) and issued in
             // two batches of 8 rows: branchy loads, or more loads than the register budget holds, are serialised by the
-            // compiler and cost one full memory latency EACH (measured: 17k cycles per chunk)
+            // compiler and cost one full memory latency EACH
             int mj[2];
             float4 mu4[2];
 #pragma unroll
@@ -232,51 +245,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
             if (lane == 0) mbar_arrive(&full_bar[st]);
             if (p == 0 && k < 48) ETRACE(32 + k / 3);          // producer 0: published
         }
-    } else if (warp == W_MMA) {
-        // =========================================== MMA issuer ===========================================
-        if (lane == 0) {
-            const uint32_t idesc =
-                (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(NE >> 3) << 17) | ((uint32_t)(F_TC >> 4) << 24);
-            mbar_wait(&a_full, 0);
-            for (int k = 0; k < n_chunks; ++k) {
-                const int st = k % NST, buf = k & 1;
-                mbar_wait(&full_bar[st], (k / NST) & 1);
-                if (k >= 2) mbar_wait(&acc_empty[buf], ((k >> 1) - 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t bB = smem_u32(sB + st * B_STAGE);
-                const uint32_t aB = smem_u32(sA);
-#pragma unroll
-                for (int t = 0; t < NT; ++t) {
-                    const uint32_t d = tmem_base + (uint32_t)(buf * BUF_COLS + t * NE);
-#pragma unroll
-                    for (int s3 = 0; s3 < 3; ++s3) {                     // k-steps 0..2 = (tile 0, 0), (tile 0, 32 B), (tile 1, 0)
-                        const int kt = s3 >> 1, ko = (s3 & 1) * 32;
-                        const uint64_t ah = make_desc(aB + ((t * 2 + 0) * 2 + kt) * A_TILE + ko);
-                        const uint64_t al = make_desc(aB + ((t * 2 + 1) * 2 + kt) * A_TILE + ko);
-                        const uint64_t bh = make_desc(bB + (0 * 2 + kt) * B_TILE + ko);
-                        const uint64_t bl = make_desc(bB + (1 * 2 + kt) * B_TILE + ko);
-                        umma_tf32(d, al, bh, idesc, s3 ? 1u : 0u);       // small terms first
-                        umma_tf32(d, ah, bl, idesc, 1u);
-                        umma_tf32(d, ah, bh, idesc, 1u);
-                    }
-                }
-                umma_commit(&empty_bar[st]);
-                umma_commit(&acc_full[buf]);
-                if (k < 16) ETRACE(48 + k);                    // MMAs issued
-            }
-        }
     } else {
         // =========================================== consumers ===========================================
         const int g = warp >> 2, qd = warp & 3;
-        const int c = qd * 32 + lane;                          // channel == TMEM lane
+        const int c = qd * 32 + lane;                          // channel (thread of the warpgroup)
         const int row_hi = s_rhi[g], s_begin = s_sb[g], s_end = s_se[g];
         int i = s_rlo[g];
         int next_boundary = i < row_hi ? rowptr[i + 1] : 0x7fffffff;
         float dq = 0.f, dm0 = 0.f, dm1 = 0.f, dm2 = 0.f;
         // The residual inputs of the CURRENT receiver row and the row pointer after next are fetched when the row starts,
         // not when it ends: a row switch then costs four stores instead of two dependent memory latencies (row pointer ->
-        // q / mu rows -> stores) in front of the next edge (measured: the switch, not the gathers, was the consumers'
-        // stall -- the kernel ran as fast with every gather hitting L1).
+        // q / mu rows -> stores) in front of the next edge.
         float bq = 0.f, bm0 = 0.f, bm1 = 0.f, bm2 = 0.f;
         int boundary2 = 0x7fffffff;
         auto prefetch_row = [&](int row) {                     // row <= row_hi <= n_atoms; clamped reads are never used
@@ -299,37 +278,39 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
             mu_out[om + 2 * F] = bm2 + dm2;
             dq = dm0 = dm1 = dm2 = 0.f;
         };
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(g * EG);
+        float* tg = sT + g * 16 * T_LD;                        // this group's [edge][channel] transpose tile
+        const uint32_t aB = smem_u32(sA);
+        mbar_wait(&a_full, 0);
         for (int k = 0; k < n_chunks; ++k) {
-            const int st = k % NST, buf = k & 1;
+            const int st = k % NST;
             if (warp == 0 && k < 16) ETRACE(64 + k);           // consumer 0: starts waiting
-            mbar_wait(&acc_full[buf], (k >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (warp == 0 && k < 16) ETRACE(80 + k);           // accumulators ready
+            mbar_wait(&full_bar[st], (k / NST) & 1);           // Phi' rows and metadata of the chunk
+            float d[NT][2][8];
+            filter_mma<NT, 16>(d, aB, smem_u32(sB + st * B_STAGE) + (uint32_t)(g * EG * SPK_SW64_ROW));
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[st]);        // the group's wgmma have read the stage
+            float wv[3][EG];
+#pragma unroll
+            for (int t = 0; t < NT; ++t) {                     // fragments -> thread = channel, one third at a time
+                frag_to_tile<16>(d[t], tg, 0, c);
+                wg_bar(1 + g);
+#pragma unroll
+                for (int u = 0; u < EG; ++u) wv[t][u] = tg[u * T_LD + c];
+                wg_bar(1 + g);
+            }
+            if (warp == 0 && k < 16) ETRACE(80 + k);           // filter values ready
             if (warp == 0 && lane == 0 && k == 0) SPK_TL_PHASE(2);
             const int* st_j = reinterpret_cast<const int*>(sMeta + st * META_STAGE) + g * EG;
             const float4* st_u = reinterpret_cast<const float4*>(sMeta + st * META_STAGE + NE * 4) + g * EG;
             const int base = s_begin + k * EG;
-            // eight edges at a time: their filter values come out of TMEM with one tcgen05.ld.x8 per third, and all their
-            // gathers are issued before the first use (rows past the range read sender 0, their filter values are exactly
-            // 0), so eight memory latencies overlap instead of following each other
+            // eight edges at a time: all their gathers are issued before the first use (rows past the range read sender 0,
+            // their filter values are exactly 0), so eight memory latencies overlap instead of following each other
 #pragma unroll
             for (int half = 0; half < 2; ++half) {
                 constexpr int HB = EG / 2;
-                float wa[HB], wb[HB], wc[HB];
-                const uint32_t ta = lane_addr + (uint32_t)(buf * BUF_COLS + half * HB);
-                tmem_ld8_nowait(ta, wa);
-                tmem_ld8_nowait(ta + NE, wb);
-                if (HAS_MU) tmem_ld8_nowait(ta + 2 * NE, wc);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (warp == 0 && k < 16) ETRACE((half ? 144 : 112) + k);   // filter values of this half in registers
-                if (half == 1) {
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&acc_empty[buf]);   // all accumulators are in registers: free the TMEM set
-                } else {
-                    mbar_wait(&full_bar[st], (k / NST) & 1);       // acquire the producer's metadata writes directly
-                }
+                const float* wa = wv[0] + half * HB;
+                const float* wb = wv[1] + half * HB;
+                const float* wc = wv[2] + half * HB;
                 if (base + half * HB < s_end) {
                     float xa[HB], xb[HB], xc[HB], m0[HB], m1[HB], m2[HB];
 #pragma unroll
@@ -391,12 +372,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
         }
         if (warp == 0) ETRACE(3);
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
-    }
 }
 
 
@@ -404,20 +379,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
 // reverse pass, grouped by sender (same structure; reference: autograd of painn.py:55-65)
 // ------------------------------------------------------------------------------------------------------------------
 // A chunk is 4 groups x 8 edges.  Its operand has 64 rows: rows 0..31 = fc [phi | 1] (-> W) and rows 32..63 =
-// dfc [phi | 1] + fc [dphi | 0] (-> dW/dd), so ONE set of 27 MMAs yields both the filter and its radial derivative.
+// dfc [phi | 1] + fc [dphi | 0] (-> dW/dd); group g multiplies its 8 rows of each half, so one pass yields both the filter
+// and its radial derivative.
 constexpr int EGB = 8;                         // edges per group and chunk
 constexpr int NEB = EGB * NG;                  // 32 edges per chunk (x 2 operand rows each)
 constexpr int META_B = NEB * 4 + NEB * 4 + NEB * 16;   // receiver index, edge id, (ux, uy, uz, 1/d) per edge
-constexpr int SMEM_BYTES_B = A_BYTES + NST * B_STAGE + NST * META_B + 1024;
-
-__device__ __forceinline__ void tmem_ld4_nowait(uint32_t taddr, float (&v)[4]) {
-    uint32_t r[4];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-                 : "r"(taddr));
-#pragma unroll
-    for (int i = 0; i < 4; ++i) v[i] = __uint_as_float(r[i]);
-}
+constexpr int SMEM_BYTES_B = A_BYTES + NST * B_STAGE + NST * META_B + T_BYTES + 1024;
 
 
 template <bool HAS_MU>
@@ -435,8 +402,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
     uint8_t* sA = smem;
     uint8_t* sB = smem + A_BYTES;
     uint8_t* sMeta = sB + NST * B_STAGE;
-    __shared__ __align__(8) uint64_t a_full, full_bar[NST], empty_bar[NST], acc_full[2], acc_empty[2], meta_empty[NST];
-    __shared__ uint32_t s_tmem;
+    float* sT = reinterpret_cast<float*>(sMeta + NST * META_B);
+    __shared__ __align__(8) uint64_t a_full, full_bar[NST], empty_bar[NST], meta_empty[NST];
     __shared__ int s_rlo[NG], s_rhi[NG], s_sb[NG], s_se[NG];
     __shared__ float s_red[2][NG][EGB][4][4];      // [chunk parity][group][edge][warp][scalar]
 
@@ -448,21 +415,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
 #pragma unroll
         for (int s = 0; s < NST; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], NCW);
             mbar_init(&meta_empty[s], NCW);
         }
-        mbar_init(&acc_full[0], 1);
-        mbar_init(&acc_full[1], 1);
-        mbar_init(&acc_empty[0], NCW);
-        mbar_init(&acc_empty[1], NCW);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         mbar_expect_tx(&a_full, A_BYTES);          // static operand: fetched BEFORE griddepcontrol.wait (pack kernels never trigger their dependents early, common.cuh)
         tma_load(sA, wpk, A_BYTES, &a_full);
-    }
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)),
-                     "n"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
     }
     if (tid == 0) BTRACE(0);
     SPK_PDL_WAIT();
@@ -481,10 +439,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = s_tmem;
     int n_chunks = 0;
 #pragma unroll
     for (int g = 0; g < NG; ++g) n_chunks = max(n_chunks, (s_se[g] - s_sb[g] + EGB - 1) / EGB);
@@ -574,39 +529,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
             __syncwarp();
             if (lane == 0) mbar_arrive(&full_bar[st]);
         }
-    } else if (warp == W_MMA) {
-        // =========================================== MMA issuer ===========================================
-        if (lane == 0) {
-            const uint32_t idesc =
-                (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(NE >> 3) << 17) | ((uint32_t)(F_TC >> 4) << 24);
-            mbar_wait(&a_full, 0);
-            for (int k = 0; k < n_chunks; ++k) {
-                const int st = k % NST, buf = k & 1;
-                mbar_wait(&full_bar[st], (k / NST) & 1);
-                if (k >= 2) mbar_wait(&acc_empty[buf], ((k >> 1) - 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t bB = smem_u32(sB + st * B_STAGE);
-                const uint32_t aB = smem_u32(sA);
-#pragma unroll
-                for (int t = 0; t < NT; ++t) {
-                    const uint32_t d = tmem_base + (uint32_t)(buf * BUF_COLS + t * NE);
-#pragma unroll
-                    for (int s3 = 0; s3 < 3; ++s3) {
-                        const int kt = s3 >> 1, ko = (s3 & 1) * 32;
-                        const uint64_t ah = make_desc(aB + ((t * 2 + 0) * 2 + kt) * A_TILE + ko);
-                        const uint64_t al = make_desc(aB + ((t * 2 + 1) * 2 + kt) * A_TILE + ko);
-                        const uint64_t bh = make_desc(bB + (0 * 2 + kt) * B_TILE + ko);
-                        const uint64_t bl = make_desc(bB + (1 * 2 + kt) * B_TILE + ko);
-                        umma_tf32(d, al, bh, idesc, s3 ? 1u : 0u);
-                        umma_tf32(d, ah, bl, idesc, 1u);
-                        umma_tf32(d, ah, bh, idesc, 1u);
-                    }
-                }
-                umma_commit(&empty_bar[st]);
-                umma_commit(&acc_full[buf]);
-                if (k < 16) BTRACE(48 + k);                    // MMAs issued
-            }
-        }
     } else {
         // =========================================== consumers ===========================================
         const int g = warp >> 2, qd = warp & 3;
@@ -642,14 +564,33 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
         };
         if (j < j_hi) load_own(j);
         const int my_idx = ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(g * EGB);
+        float* tg = sT + g * 16 * T_LD;                        // this group's [W edge | dW edge][channel] transpose tile
+        const uint32_t aB = smem_u32(sA);
+        mbar_wait(&a_full, 0);
         for (int k = 0; k < n_chunks; ++k) {
-            const int st = k % NST, buf = k & 1;
+            const int st = k % NST;
             if (warp == 0 && k < 16) BTRACE(64 + k);           // consumer 0: starts waiting
-            mbar_wait(&acc_full[buf], (k >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            mbar_wait(&full_bar[st], (k / NST) & 1);           // acquire the producer's metadata writes
-            if (warp == 0 && k < 16) BTRACE(80 + k);           // accumulators + metadata ready
+            mbar_wait(&full_bar[st], (k / NST) & 1);           // operand rows and metadata of the chunk
+            const uint32_t bB = smem_u32(sB + st * B_STAGE);
+            float dw[NT][2][4], dd[NT][2][4];
+            filter_mma<NT, 8>(dw, aB, bB + (uint32_t)(g * EGB * SPK_SW64_ROW));           // W rows of the group
+            filter_mma<NT, 8>(dd, aB, bB + (uint32_t)((NEB + g * EGB) * SPK_SW64_ROW));   // dW/dd rows of the group
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[st]);
+            float wv[3][EGB], dv[3][EGB];
+#pragma unroll
+            for (int t = 0; t < NT; ++t) {                     // fragments -> thread = channel, one third at a time
+                frag_to_tile<8>(dw[t], tg, 0, c);
+                frag_to_tile<8>(dd[t], tg, EGB, c);
+                wg_bar(1 + g);
+#pragma unroll
+                for (int u = 0; u < EGB; ++u) {
+                    wv[t][u] = tg[u * T_LD + c];
+                    dv[t][u] = tg[(EGB + u) * T_LD + c];
+                }
+                wg_bar(1 + g);
+            }
+            if (warp == 0 && k < 16) BTRACE(80 + k);           // filter values + metadata ready
             if (warp == 0 && lane == 0 && k == 0) SPK_TL_PHASE(2);
             const int* st_i = reinterpret_cast<const int*>(sMeta + st * META_B) + g * EGB;
             const int* st_e = reinterpret_cast<const int*>(sMeta + st * META_B) + NEB + g * EGB;
@@ -657,22 +598,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
             const int base = p_begin + k * EGB;
 #pragma unroll
             for (int half = 0; half < 2; ++half) {
-                float Wa[4], Wb[4], Wc[4], Da[4], Db[4], Dc[4];
-                const uint32_t ta = lane_addr + (uint32_t)(buf * BUF_COLS + half * 4);
-                tmem_ld4_nowait(ta, Wa);
-                tmem_ld4_nowait(ta + NEB, Da);
-                tmem_ld4_nowait(ta + NE, Wb);
-                tmem_ld4_nowait(ta + NE + NEB, Db);
-                if (HAS_MU) {
-                    tmem_ld4_nowait(ta + 2 * NE, Wc);
-                    tmem_ld4_nowait(ta + 2 * NE + NEB, Dc);
-                }
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (half == 1) {
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&acc_empty[buf]);
-                }
+                const float *Wa = wv[0] + half * 4, *Wb = wv[1] + half * 4, *Wc = wv[2] + half * 4;
+                const float *Da = dv[0] + half * 4, *Db = dv[1] + half * 4, *Dc = dv[2] + half * 4;
                 float gq[4], g0[4], g1[4], g2[4];
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {                  // rows past the range gather receiver 0; their W, dW are 0
@@ -763,12 +690,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
         if (warp == 0) BTRACE(2);
         for (; j < j_hi; ++j) flush(j);
         if (warp == 0) BTRACE(3);
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
     }
 }
 

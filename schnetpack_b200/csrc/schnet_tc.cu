@@ -1,59 +1,40 @@
-// SchNet interaction block, forward, as ONE fused edge kernel with the filter network on the tensor cores (tcgen05, TMEM).
-// Reference: representation/schnet.py:56-70
-//     Wij = filter_network(f_ij) * rcut_ij        filter_network = Dense(n_rbf -> F, ssp) -> Dense(F -> F)      :61-62
-//     x   = scatter_add( x[idx_j] * Wij, idx_i )                                                                :65-67
-// The reference (and round 1 of this repo) materialises the [E,F] hidden layer and the [E,F] filter in HBM per block (2 x
-// 512 B per edge and layer, round trips included ~2 KB) -- 38 kFLOP per edge and layer of dense work that is tensor-pipe
-// bound (SURVEY.md section 8d).  Here a chunk of 32 edges goes through both layers without leaving the SM:
+// SchNet interaction block, forward, as ONE fused edge kernel with the filter network on the tensor cores (wgmma).
+// Reference: representation/schnet.py
+//     Wij = filter_network(f_ij) * rcut_ij        filter_network = Dense(n_rbf -> F, ssp) -> Dense(F -> F)
+//     x   = scatter_add( x[idx_j] * Wij, idx_i )
+// The reference materialises the [E,F] hidden layer and the [E,F] filter in HBM per block (2 x 512 B per edge and layer,
+// round trips included ~2 KB) -- 38 kFLOP per edge and layer of dense work.  Here a chunk of 32 edges goes through both
+// layers without leaving the SM:
 //
 //   producers   Phi' = [phi | 1 | 0] rows of the chunk (hi/lo TF32 split) -> shared memory (K-major, 64 B swizzle);
-//   MMA 1       H = [W0 | b0] Phi'^T        128 hidden channels (TMEM lanes) x 32 edges (columns), 3xTF32, K = n_rbf + 1;
-//               "N-folded": the hi and lo tiles of an edge operand are adjacent, so [X_hi ; X_lo] is ONE operand of 64 rows
-//               and W_hi [X_hi ; X_lo]^T yields the main product (columns 0..31) and the W_hi X_lo terms (32..63) in one
-//               instruction, W_lo X_hi accumulates onto the latter: 2 MMAs per k-step instead of 3 (an MMA costs ~130 cycles
-//               for any N <= 256, and the chunk's serial MMA chain is what bounds this kernel);
-//   activation  the 16 consumer warps (all 512 threads: lane = hidden channel, a group takes its own 8 edges of the NEXT chunk)
-//               read H with tcgen05.ld, apply shifted softplus (nn/activations.py:9-22), split hi/lo and write it to shared
-//               memory as the K-major B operand of the second layer -- 4 dedicated activation warps needed 7.2 k cycles per
-//               chunk for the 32 log1p(exp()) per thread and were the chunk period (phase trace, profiles/);
-//   MMA 2       D = W1 ssp(H)            128 output channels (lanes) x 32 edges, 3xTF32, K = 128: the main products in one
-//               accumulator, the small hi*lo terms in a second one (the tensor core truncates when it accumulates);
-//   consumers   16 warps = 4 groups x 128 channels, thread = channel as in the PaiNN kernels: filter value
-//               W = (D_main + D_corr + b1) * fc for the group's 8 edges of the chunk with two tcgen05.ld.x8, gather
-//               h[j, c], accumulate the receiver's row in registers (CSR order, deterministic, no atomics), m[i] on flush.
+//   groups      4 consumer warpgroups; group g owns 8 edges of every chunk (and its own edge-balanced receiver range).  It
+//               computes with wgmma, 3xTF32 (small products first; wgmma.cuh):
+//       MMA 1   H = [W0 | b0] Phi'_g^T       128 hidden channels (two m64 halves) x 8 edges, K = n_rbf + 1;
+//       act     shifted softplus on the fragment registers, hi/lo split, written as the group's 8 rows of the K-major
+//               B operand of the second layer (only this warpgroup reads them);
+//       MMA 2   D = W1 ssp(H)                 128 output channels x 8 edges, K = 128: the main products in one accumulator,
+//               the small hi*lo terms in a second one (the tensor core truncates when it accumulates);
+//       gather  D goes through a small shared-memory transpose to thread = channel; filter value
+//               W = (D + b1) * fc, gather h[j, c], accumulate the receiver's row in registers (CSR order, deterministic, no
+//               atomics), m[i] on flush.
 //
 // Both weight operands ([W0|b0]: 32 KB, W1: 128 KB as hi|lo tiles) stay resident in shared memory for the life of the
 // persistent CTA (one per SM) and arrive by two TMA bulk copies.  The receiver ranges come from a CSR that may have been
 // built from the ACTIVE edges only (spk_graph_build_active: d < cutoff), so the padding slots of a padded neighbour list
-// (cfg3: 62 % of 831 488 slots) cost nothing -- their filter is exactly 0 in the reference (nn/cutoff.py:30-32).
-// The reverse pass (forces) keeps the round-1 pipeline (filter tensors materialised): the named SchNet workload with forces is
-// the 9-atom cfg1; cfg3 is energy-only inference.
-#include "tcgen05.cuh"
-
-// development aid (build with -DSPK_SCHNET_TRACE, tools/build_variant.sh): clock64 stamps of CTA 0, one row of 16 per chunk
-#ifdef SPK_SCHNET_TRACE
-__device__ long long g_schnet_trace[256 * 16];
-#define STRACE(k, slot)                                                                              \
-    do {                                                                                             \
-        if (blockIdx.x == 0 && (threadIdx.x & 31) == 0 && (k) < 256) g_schnet_trace[(k) * 16 + (slot)] = clock64(); \
-    } while (0)
-extern "C" int spk_debug_schnet_trace(long long* host) {
-    return (int)cudaMemcpyFromSymbol(host, g_schnet_trace, sizeof(long long) * 256 * 16);
-}
-#else
-#define STRACE(k, slot) do { } while (0)
-#endif
+// cost nothing -- their filter is exactly 0 in the reference (nn/cutoff.py).
+// The reverse pass (forces) keeps the materialised-filter pipeline: the named SchNet workload with forces is the 9-atom cfg1;
+// cfg3 is energy-only inference.
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int F_TC = 128;
-constexpr int EG = 8, NG = 4, NE = EG * NG;              // 32 edge rows per chunk == UMMA N
-constexpr int NCW = NG * 4;                              // 16 consumer warps
-constexpr int W_MMA = NCW;
-constexpr int W_PROD0 = NCW + 1;
+constexpr int EG = 8, NG = 4, NE = EG * NG;              // 32 edge rows per chunk, 8 per group (wgmma N)
+constexpr int NCW = NG * 4;                              // 16 consumer warps = 4 warpgroups
+constexpr int W_PROD0 = NCW;
 constexpr int NPROD = 2, NST = 2;                        // Phi' stages (chunk k -> stage k % 2 -> producer k % 2)
 constexpr int NMETA = 4;                                 // (sender, fc) ring
-constexpr int NTHREADS = (W_PROD0 + NPROD) * 32;         // 608
+constexpr int NTHREADS = (W_PROD0 + NPROD) * 32;         // 576
 constexpr int KT = 16;
 constexpr int A_TILE = F_TC * KT * 4;                    // 8192 B
 constexpr int W0_BYTES = 2 * 2 * A_TILE;                 // [hi,lo][2 k-tiles]
@@ -62,30 +43,13 @@ constexpr int B_TILE = NE * KT * 4;                      // 2048 B
 constexpr int PHI_STAGE = 2 * 2 * B_TILE;                // [hi,lo][2 k-tiles]
 constexpr int B2_BYTES = 2 * 8 * B_TILE;                 // [hi,lo][8 k-tiles]
 constexpr int META_STAGE = NE * 8;                       // int sender + float fc per row
-constexpr int SMEM_BYTES = W0_BYTES + W1_BYTES + NST * PHI_STAGE + B2_BYTES + NMETA * META_STAGE + 1024;
-constexpr int TMEM_COLS = 256;                           // H[2] x (main 32 | corr 32) | D[2] x (main 32 | corr 32)
-constexpr int COL_H = 0, COL_D = 128;
-static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
-
-__device__ __forceinline__ void tmem_ld8_nowait(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr));
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
+constexpr int T_LD = F_TC + 4;                           // row of the per-group transpose tile [edge][channel] (floats)
+constexpr int T_BYTES = NG * EG * T_LD * 4;
+// the 64-byte swizzle repeats every 512 B, so 512 B alignment suffices; the static shared variables round up to the same
+// 512 B and count against the 227 KB a block may use
+constexpr int SMEM_ALIGN = 512;
+constexpr int SMEM_BYTES = W0_BYTES + W1_BYTES + NST * PHI_STAGE + B2_BYTES + NMETA * META_STAGE + T_BYTES + SMEM_ALIGN;
+static_assert(SMEM_BYTES + SMEM_ALIGN <= 227 * 1024, "shared memory budget (dynamic + static)");
 
 // packed operands: [W0|b0|0] as [hi,lo][2 k-tiles][128 x 16], then W1 as [hi,lo][8 k-tiles][128 x 16]
 __global__ void k_pack_schnet_filter(const float* __restrict__ w0, const float* __restrict__ b0,
@@ -123,16 +87,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_schnet_cfconv_fwd_tc(
     const int* __restrict__ rowptr, const int* __restrict__ slot_j, const float* __restrict__ wpk,
     const float* __restrict__ b1, int act, int n_atoms, int n_rbf, float* __restrict__ m) {
     constexpr int F = F_TC;
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    extern __shared__ __align__(SMEM_ALIGN) uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((SMEM_ALIGN - (smem_u32(smem_raw) & (SMEM_ALIGN - 1))) & (SMEM_ALIGN - 1));
     uint8_t* sW0 = smem;
     uint8_t* sW1 = sW0 + W0_BYTES;
     uint8_t* sPhi = sW1 + W1_BYTES;
     uint8_t* sB2 = sPhi + NST * PHI_STAGE;
     uint8_t* sMeta = sB2 + B2_BYTES;
-    __shared__ __align__(8) uint64_t w_full, phi_full[NST], phi_empty[NST], h_full[2], h_empty[2], b2_full, b2_empty,
-        d_full[2], d_empty[2], meta_full[NMETA], meta_empty[NMETA];
-    __shared__ uint32_t s_tmem;
+    float* sT = reinterpret_cast<float*>(sMeta + NMETA * META_STAGE);
+    __shared__ __align__(8) uint64_t w_full, phi_full[NST], phi_empty[NST], meta_full[NMETA], meta_empty[NMETA];
     __shared__ int s_rlo[NG], s_rhi[NG], s_sb[NG], s_se[NG];
 
     const int tid = threadIdx.x, lane = tid & 31;
@@ -143,17 +106,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_schnet_cfconv_fwd_tc(
 #pragma unroll
         for (int s = 0; s < NST; ++s) {
             mbar_init(&phi_full[s], 1);
-            mbar_init(&phi_empty[s], 1);
+            mbar_init(&phi_empty[s], NCW);
         }
-#pragma unroll
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&h_full[b], 1);
-            mbar_init(&h_empty[b], NCW);
-            mbar_init(&d_full[b], 1);
-            mbar_init(&d_empty[b], NCW);
-        }
-        mbar_init(&b2_full, NCW);
-        mbar_init(&b2_empty, 1);
 #pragma unroll
         for (int s = 0; s < NMETA; ++s) {
             mbar_init(&meta_full[s], 1);
@@ -163,11 +117,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_schnet_cfconv_fwd_tc(
         mbar_expect_tx(&w_full, W0_BYTES + W1_BYTES);      // static operand: fetched BEFORE griddepcontrol.wait (pack kernels never trigger their dependents early, common.cuh)
         tma_load(sW0, wpk, W0_BYTES, &w_full);
         tma_load(sW1, wpk + W0_BYTES / 4, W1_BYTES, &w_full);
-    }
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)),
-                     "n"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
     }
     SPK_PDL_WAIT();
     if (warp <= NG) {                              // warp w finds boundary w of this CTA's NG group ranges (warp-wide search)
@@ -185,10 +134,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_schnet_cfconv_fwd_tc(
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = s_tmem;
     int n_chunks = 0;
 #pragma unroll
     for (int g = 0; g < NG; ++g) n_chunks = max(n_chunks, (s_se[g] - s_sb[g] + EG - 1) / EG);
@@ -249,124 +195,86 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_schnet_cfconv_fwd_tc(
                 mbar_arrive(&phi_full[st]);
                 mbar_arrive(&meta_full[ms]);
             }
-            STRACE(k, 0);                                   // producer: chunk published
-        }
-    } else if (warp == W_MMA) {
-        // =========================================== MMA issuer ===========================================
-        if (lane == 0) {
-            const uint32_t idesc =
-                (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(NE >> 3) << 17) | ((uint32_t)(F_TC >> 4) << 24);
-            const uint32_t idesc_w =                                       // N = 2 NE: [X_hi ; X_lo] as one operand
-                (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)((2 * NE) >> 3) << 17) | ((uint32_t)(F_TC >> 4) << 24);
-            mbar_wait(&w_full, 0);
-            const uint32_t a0 = smem_u32(sW0), a1 = smem_u32(sW1), bb2 = smem_u32(sB2);
-            auto mma1 = [&](int k) {                                      // H(k) = [W0|b0] Phi'(k)^T
-                const int st = k % NST, hb = k & 1;
-                mbar_wait(&phi_full[st], (k / NST) & 1);
-                if (k >= 2) mbar_wait(&h_empty[hb], ((k >> 1) - 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t bp = smem_u32(sPhi + st * PHI_STAGE);
-                const uint32_t d = tmem_base + (uint32_t)(COL_H + hb * 2 * NE);
-                for (int s3 = 0; s3 < nks1; ++s3) {
-                    const int kt = s3 >> 1, ko = (s3 & 1) * 32;
-                    const uint64_t ah = make_desc(a0 + (0 * 2 + kt) * A_TILE + ko);
-                    const uint64_t al = make_desc(a0 + (1 * 2 + kt) * A_TILE + ko);
-                    const uint64_t bw = make_desc(bp + (kt * 2) * B_TILE + ko);       // hi tile, lo tile follows
-                    umma_tf32(d, ah, bw, idesc_w, s3 ? 1u : 0u);                      // [Wh Xh | Wh Xl]
-                    umma_tf32(d + (uint32_t)NE, al, bw, idesc, 1u);                   // Wl Xh onto the small-term columns
-                }
-                umma_commit(&phi_empty[st]);
-                umma_commit(&h_full[hb]);
-                STRACE(k, 1);                               // MMA 1 issued
-            };
-            if (n_chunks > 0) mma1(0);
-            for (int k = 0; k < n_chunks; ++k) {
-                if (k + 1 < n_chunks) mma1(k + 1);                        // keeps the activation warps one chunk ahead
-                const int db = k & 1;
-                mbar_wait(&b2_full, k & 1);
-                STRACE(k, 2);                               // B2 of this chunk available
-                if (k >= 2) mbar_wait(&d_empty[db], ((k >> 1) - 1) & 1);
-                STRACE(k, 3);                               // D buffer free
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t d_main = tmem_base + (uint32_t)(COL_D + db * 2 * NE);
-#pragma unroll
-                for (int s16 = 0; s16 < 16; ++s16) {                      // D(k) = W1 ssp(H(k)), K = 128
-                    const int kt = s16 >> 1, ko = (s16 & 1) * 32;
-                    const uint64_t ah = make_desc(a1 + (0 * 8 + kt) * A_TILE + ko);
-                    const uint64_t al = make_desc(a1 + (1 * 8 + kt) * A_TILE + ko);
-                    const uint64_t bw = make_desc(bb2 + (kt * 2) * B_TILE + ko);      // [act_hi ; act_lo]
-                    umma_tf32(d_main, ah, bw, idesc_w, s16 ? 1u : 0u);
-                    umma_tf32(d_main + (uint32_t)NE, al, bw, idesc, 1u);
-                }
-                umma_commit(&b2_empty);
-                umma_commit(&d_full[db]);
-                STRACE(k, 4);                               // MMA 2 issued
-            }
         }
     } else {
-        // =========================================== consumers ===========================================
-        const int g = warp >> 2, qd = warp & 3;
-        const int c = qd * 32 + lane;
+        // =========================================== consumer warpgroups ===========================================
+        const int g = warp >> 2;
+        const int c = tid & 127;                                       // channel of the gather / accumulate phase
         const float b1c = b1 ? b1[c] : 0.f;
         const int row_hi = s_rhi[g], s_begin = s_sb[g], s_end = s_se[g];
         int i = s_rlo[g];
         int next_boundary = i < row_hi ? rowptr[i + 1] : 0x7fffffff;
         float acc = 0.f;
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(COL_D + g * EG);
-        // activation of chunk ka for this group's 8 edges: H[lane = hidden channel c, columns g*8..] -> ssp -> B2 rows g*8..
-        const uint32_t lane_h = tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(COL_H + g * EG);
-        const int akt = c >> 4, akk = c & 15;
-        auto activate = [&](int ka) {
-            const int hb = ka & 1;
-            mbar_wait(&h_full[hb], (ka >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (warp == 0) STRACE(ka, 5);                  // H ready
-            float hm[EG], hc[EG];
-            tmem_ld8_nowait(lane_h + (uint32_t)(hb * 2 * NE), hm);
-            tmem_ld8_nowait(lane_h + (uint32_t)(hb * 2 * NE + NE), hc);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&h_empty[hb]);
-            float a[EG];
-            if (act == SPK_ACT_SSP) {                      // the block's own activation (schnet.py:45), SFU version
+        float* tg = sT + g * EG * T_LD;                                // this group's [edge][channel] transpose tile
+        const uint32_t a0 = smem_u32(sW0), a1 = smem_u32(sW1), bb2 = smem_u32(sB2) + (uint32_t)(g * EG * SPK_SW64_ROW);
+        mbar_wait(&w_full, 0);
+        for (int k = 0; k < n_chunks; ++k) {
+            const int st = k % NST, ms = k % NMETA;
+            // ---- MMA 1: H = [W0|b0] Phi'^T for the group's 8 edges
+            mbar_wait(&phi_full[st], (k / NST) & 1);
+            const uint32_t bp = smem_u32(sPhi + st * PHI_STAGE) + (uint32_t)(g * EG * SPK_SW64_ROW);
+            float hf[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+            wgmma_fence();
+            for (int s3 = 0; s3 < nks1; ++s3) {
+                const int kt = s3 >> 1, ko = (s3 & 1) * 32;
 #pragma unroll
-                for (int e = 0; e < EG; ++e) a[e] = spk_ssp_fast(hm[e] + hc[e]);
-            } else {
-#pragma unroll
-                for (int e = 0; e < EG; ++e) a[e] = spk_act(hm[e] + hc[e], act);
+                for (int mh = 0; mh < 2; ++mh) {
+                    const uint32_t ah = a0 + (0 * 2 + kt) * A_TILE + mh * SPK_WG_ROWS_BYTES + ko;
+                    const uint32_t al = a0 + (1 * 2 + kt) * A_TILE + mh * SPK_WG_ROWS_BYTES + ko;
+                    const uint32_t bh = bp + (kt * 2 + 0) * B_TILE + ko, bl = bp + (kt * 2 + 1) * B_TILE + ko;
+                    wgmma_n8(hf[mh], make_desc(al), make_desc(bh), s3);   // small terms first
+                    wgmma_n8(hf[mh], make_desc(ah), make_desc(bl), 1);
+                    wgmma_n8(hf[mh], make_desc(ah), make_desc(bh), 1);
+                }
             }
-            if (warp == 0) STRACE(ka, 6);                  // values computed
-            if (ka >= 1) mbar_wait(&b2_empty, (ka - 1) & 1);              // MMA 2 of the previous chunk has read B2
-            if (warp == 0) STRACE(ka, 7);                  // B2 free
-            uint8_t* hi_t = sB2 + (akt * 2 + 0) * B_TILE;                 // [k-tile][hi | lo]
-            uint8_t* lo_t = sB2 + (akt * 2 + 1) * B_TILE;
+            wgmma_commit();
+            wgmma_wait_all();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&phi_empty[st]);
+            // ---- activation (the block's own, schnet.py; SFU version of shifted softplus) -> the group's rows of B2
 #pragma unroll
-            for (int e = 0; e < EG; ++e) {
-                const float hi = tf32_rn(a[e]);
-                const int off = tile_off(g * EG + e, akk >> 2) + (akk & 3) * 4;
-                *reinterpret_cast<float*>(hi_t + off) = hi;
-                *reinterpret_cast<float*>(lo_t + off) = a[e] - hi;
+            for (int mh = 0; mh < 2; ++mh) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const int ch = mh * 64 + wg_frag_row(c, q), e = wg_frag_col(c, q);
+                    const float a = act == SPK_ACT_SSP ? spk_ssp_fast(hf[mh][q]) : spk_act(hf[mh][q], act);
+                    const float hi = tf32_rn(a);
+                    const int off = tile_off(g * EG + e, (ch & 15) >> 2) + (ch & 3) * 4;
+                    *reinterpret_cast<float*>(sB2 + ((ch >> 4) * 2 + 0) * B_TILE + off) = hi;
+                    *reinterpret_cast<float*>(sB2 + ((ch >> 4) * 2 + 1) * B_TILE + off) = a - hi;
+                }
             }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&b2_full);
-            if (warp == 0) STRACE(ka, 8);                  // B2 stored
-        };
-        if (n_chunks > 0) activate(0);
-        for (int k = 0; k < n_chunks; ++k) {
-            const int db = k & 1, ms = k % NMETA;
-            if (k + 1 < n_chunks) activate(k + 1);          // the next chunk's hidden layer, while MMA 2 of this one runs
-            mbar_wait(&d_full[db], (k >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (warp == 0) STRACE(k, 9);                    // consumer: D ready
-            float wm[EG], wc[EG];
-            tmem_ld8_nowait(lane_addr + (uint32_t)(db * 2 * NE), wm);
-            tmem_ld8_nowait(lane_addr + (uint32_t)(db * 2 * NE + NE), wc);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&d_empty[db]);
+            wg_bar(1 + g);
+            // ---- MMA 2: D = W1 ssp(H), K = 128
+            float dm[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+            float dc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+            wgmma_fence();
+#pragma unroll
+            for (int s16 = 0; s16 < 16; ++s16) {
+                const int kt = s16 >> 1, ko = (s16 & 1) * 32;
+                const uint32_t bh = bb2 + (kt * 2 + 0) * B_TILE + ko, bl = bb2 + (kt * 2 + 1) * B_TILE + ko;
+#pragma unroll
+                for (int mh = 0; mh < 2; ++mh) {
+                    const uint32_t ah = a1 + (0 * 8 + kt) * A_TILE + mh * SPK_WG_ROWS_BYTES + ko;
+                    const uint32_t al = a1 + (1 * 8 + kt) * A_TILE + mh * SPK_WG_ROWS_BYTES + ko;
+                    wgmma_n8(dm[mh], make_desc(ah), make_desc(bh), s16 ? 1 : 0);
+                    wgmma_n8(dc[mh], make_desc(al), make_desc(bh), s16 ? 1 : 0);
+                    wgmma_n8(dc[mh], make_desc(ah), make_desc(bl), 1);
+                }
+            }
+            wgmma_commit();
+            wgmma_wait_all();
+            // ---- fragments -> [edge][channel] -> thread = channel
+#pragma unroll
+            for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+                for (int q = 0; q < 4; ++q)
+                    tg[wg_frag_col(c, q) * T_LD + mh * 64 + wg_frag_row(c, q)] = dm[mh][q] + dc[mh][q];
+            wg_bar(1 + g);
+            float w[EG];
+#pragma unroll
+            for (int u = 0; u < EG; ++u) w[u] = tg[u * T_LD + c];
             mbar_wait(&meta_full[ms], (k / NMETA) & 1);
             const int* st_j = reinterpret_cast<const int*>(sMeta + ms * META_STAGE) + g * EG;
             const float* st_fc = reinterpret_cast<const float*>(sMeta + ms * META_STAGE + NE * 4) + g * EG;
@@ -388,24 +296,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_schnet_cfconv_fwd_tc(
                             ++i;
                             next_boundary = rowptr[i + 1];
                         }
-                        acc = fmaf((wm[u] + wc[u] + b1c) * fc[u], hv[u], acc);
+                        acc = fmaf((w[u] + b1c) * fc[u], hv[u], acc);
                     }
                 }
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&meta_empty[ms]);
-            if (warp == 0) STRACE(k, 10);                   // consumer: chunk done
         }
         for (; i < row_hi; ++i) {
             m[(size_t)i * F + c] = acc;
             acc = 0.f;
         }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
     }
 }
 

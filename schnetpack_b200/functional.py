@@ -453,7 +453,7 @@ def _schnet_filter_packed(b, n_rbf: int):
 
 def schnet_forward_fused(pk: SchNetPack, x0: Tensor, r_ij: Tensor, idx_i: Tensor, idx_j: Tensor, rbf_kind: int, n_rbf: int,
                          rbf_p0, rbf_p1, cutoff: float, act: int) -> Tensor:
-    """Inference forward (no tape) with ONE fused edge kernel per interaction block (filter network on tcgen05 inside it,
+    """Inference forward (no tape) with ONE fused edge kernel per interaction block (filter network on the tensor cores inside it,
     csrc/schnet_tc.cu) over the ACTIVE edges only (d < cutoff: padding slots of a padded neighbour list are dropped when the
     receiver CSR is built), and the per-atom layers f2out + residual + the next block's in2f as one persistent launch
     (csrc/atom_chain.cu).  schnet.py:56-70,160-171."""

@@ -1,8 +1,8 @@
 """Minimal mirror of the boundary caller ``schnetpack.model.NeuralNetworkPotential``
-(/root/reference/src/schnetpack/model/base.py:16-190) so that the B200 modules can be assembled and driven exactly
+(/root/reference/src/schnetpack/model/base.py:16-190) so that the CUDA modules can be assembled and driven exactly
 like the reference's (input modules -> representation -> output modules -> postprocessors) on a box where the
 reference package is absent, plus ``convert_model`` which swaps the hot-path modules of an already-loaded reference
-model for their B200 counterparts (identical ``state_dict`` keys)."""
+model for their CUDA counterparts (identical ``state_dict`` keys)."""
 from __future__ import annotations
 
 from typing import Dict, List, Optional
@@ -110,7 +110,7 @@ def _convert_rbf(rb):
     elif name == "BesselRBF":
         out = snn.BesselRBF(rb.n_rbf, 1.0)
     else:
-        raise NotImplementedError(f"radial basis {name} has no B200 kernel")
+        raise NotImplementedError(f"radial basis {name} has no CUDA kernel")
     out.load_state_dict(rb.state_dict())
     return out
 
@@ -120,7 +120,7 @@ def _convert_representation(rep):
     rbf = _convert_rbf(rep.radial_basis)
     cut = snn.CosineCutoff(float(rep.cutoff_fn.cutoff))
     if type(rep.cutoff_fn).__name__ != "CosineCutoff":
-        raise NotImplementedError(f"cutoff {type(rep.cutoff_fn).__name__} has no B200 kernel")
+        raise NotImplementedError(f"cutoff {type(rep.cutoff_fn).__name__} has no CUDA kernel")
     emb = rep.embedding if not isinstance(rep.embedding, nn.Embedding) else None
     eemb = list(rep.electronic_embeddings) if len(getattr(rep, "electronic_embeddings", [])) else None
     if name == "PaiNN":
@@ -136,7 +136,7 @@ def _convert_representation(rep):
                                     shared_interactions=shared, activation=_map_act(act), nuclear_embedding=emb,
                                     electronic_embeddings=eemb)
     else:
-        raise NotImplementedError(f"representation {name} is outside the B200 hot path")
+        raise NotImplementedError(f"representation {name} is outside the CUDA hot path")
     new.load_state_dict(rep.state_dict())
     return new
 
@@ -148,7 +148,7 @@ def _map_act(act):
 
 
 def convert_model(model: nn.Module) -> NeuralNetworkPotential:
-    """Build a B200 ``NeuralNetworkPotential`` from a loaded reference model (duck-typed on class names; weights are
+    """Build a CUDA ``NeuralNetworkPotential`` from a loaded reference model (duck-typed on class names; weights are
     copied through ``state_dict`` whose keys are identical).  Modules outside the hot path (postprocessors, custom
     embeddings, other output heads) are reused as they are."""
     in_mods = []

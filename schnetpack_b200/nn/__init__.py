@@ -1,4 +1,4 @@
-"""Mirror of the reference's ``schnetpack.nn`` primitives that sit on the hot path, backed by the sm_100a kernels.
+"""Mirror of the reference's ``schnetpack.nn`` primitives that sit on the hot path, backed by the sm_90a CUDA kernels.
 
 Same constructor signatures, buffers/parameters and ``state_dict`` keys as
 /root/reference/src/schnetpack/nn/{radial,cutoff,base,activations,scatter,blocks,utils}.py.  Forward passes on CUDA

@@ -1,6 +1,6 @@
 """Python-side plumbing over the C ABI: tensor checks, buffer allocation (torch owns device memory), stream handoff.
 
-Every function here launches hand-written sm_100a kernels from ``csrc/`` through ``include/spk_b200.h``; there is no
+Every function here launches hand-written sm_90a kernels from ``csrc/`` through ``include/spk_b200.h``; there is no
 torch arithmetic on the hot path and no CPU fallback (non-CUDA tensors raise).
 """
 from __future__ import annotations
@@ -309,7 +309,7 @@ def tc_pack_weight(w: Tensor) -> Tensor:
 def dense_tc(A: Tensor, w_packed: Tensor, n_out: int, bias: Optional[Tensor] = None, act: int = ACT_NONE,
              a_pre: Optional[Tensor] = None, a_act: int = ACT_NONE, addend: Optional[Tensor] = None,
              save_pre: bool = False, k: Optional[int] = None, out: Optional[Tensor] = None):
-    """tcgen05 / 3xTF32 variant of ``dense``: Y = act((A .* act'(a_pre)) @ W^T + bias) + addend with W [n_out, K] given
+    """wgmma / 3xTF32 variant of ``dense``: Y = act((A .* act'(a_pre)) @ W^T + bias) + addend with W [n_out, K] given
     in packed form (``tc_pack_weight``)."""
     f32(A, "A")
     M, lda = A.shape
@@ -338,7 +338,7 @@ def split_tf32(w: Tensor):
 
 
 # dense-layer kernel (both meet the 1e-5 parity bar; r1: equal speed on cfg2 within run-to-run noise):
-#   "tc"   (default) tcgen05 3xTF32 tensor-core kernel csrc/gemm_tc.cu -- split accumulators + K-tile draining give
+#   "tc"   (default) wgmma 3xTF32 tensor-core kernel csrc/gemm_tc.cu -- fresh accumulator per K-tile added in fp32 gives
 #          fp32-grade error; shapes outside its vector fast path fall back to "ffma" per call
 #   "ffma" fp32 CUDA-core kernel csrc/gemm.cu (packed FFMA2, IEEE fp32 accumulation like the reference SGEMM)
 DENSE_IMPL = os.environ.get("SPK_B200_DENSE", "tc")
@@ -421,10 +421,9 @@ def mlp2(A: Tensor, l0: "Lin", l1: "Lin", act: int, addend: Optional[Tensor] = N
 
 # ------------------------------------------------------------------------------------------------------------ atom chain
 # persistent per-atom stage (csrc/atom_chain.cu): one launch for mixing(t) + context(t+1) (or their reverses) instead of
-# seven.  SPK_B200_CHAIN=0 restores the launch-per-layer pipeline (same kernels as round 1) for A/B measurements.
-CHAIN_IMPL = os.environ.get("SPK_B200_CHAIN", "0") != "0"      # opt-in: measured slower than the launch-per-layer pipeline at the
-#                                                                named sizes (DESIGN.md section 3: per-SM bandwidth of tile-local items)
-CHAIN_NFOLD = os.environ.get("SPK_B200_CHAIN_NFOLD", "0") != "0"    # 2 MMAs per k-step ([W_hi;W_lo] as one operand)
+# seven.  Opt-in (SPK_B200_CHAIN=1); the default is the launch-per-layer pipeline.
+CHAIN_IMPL = os.environ.get("SPK_B200_CHAIN", "0") != "0"
+CHAIN_NFOLD = os.environ.get("SPK_B200_CHAIN_NFOLD", "0") != "0"    # SPK_CHAIN_FLAG_NFOLD; the sm_90a kernel has one scheme
 CHAIN_TRACE = None          # set to a list to collect (stamps, program) of every stage launch
 _CHAIN_WS: "dict[tuple, Tensor]" = {}
 
@@ -494,7 +493,7 @@ def atom_chain(steps, n_atoms: int, device):
         if ws is None or ws.numel() < need:
             ws = torch.zeros(max(need, 4096), dtype=torch.int32, device=device)   # zero once; the kernel leaves it zero
             _CHAIN_WS[key] = ws
-    if CHAIN_TRACE is not None:      # development: per-item time stamps of every stage launch (tools/chain_trace.py)
+    if CHAIN_TRACE is not None:      # development: per-item time stamps of every stage launch (spk_atom_chain_debug)
         items = sum((s.rows_per_atom * (s.N // 128) if s.kind == _lib.CHAIN_GEMM else 1) for s in steps) * ((n_atoms + 127) // 128)
         tr = torch.zeros((items, 8), dtype=torch.int64, device=device)
         CHAIN_TRACE.append((tr, [(s.kind, s.K, s.N, s.rows_per_atom) for s in steps]))
@@ -506,10 +505,8 @@ def atom_chain(steps, n_atoms: int, device):
 
 # ------------------------------------------------------------------------------------------------------------ PaiNN
 # edge kernels: "tc" (default) = persistent kernels with the continuous filter on the tensor cores (csrc/painn_tc.cu:
-# tcgen05 3xTF32, channels on TMEM lanes) for F == 128, n_rbf <= 31 and >= EDGE_TC_MIN_EDGES edges; everything else, and
-# SPK_B200_EDGE=ldg, runs the streaming kernels with the filter in packed FFMA2 (csrc/painn.cu).  The round-1 TMA-ring,
-# cp.async-ring and system-resident variants measured slower (DESIGN.md section 3) and live on as
-# tools/experiments/edge_variants_r1.patch.
+# wgmma 3xTF32, channels on the M side) for F == 128, n_rbf <= 31 and >= EDGE_TC_MIN_EDGES edges; everything else, and
+# SPK_B200_EDGE=ldg, runs the streaming kernels with the filter on the CUDA cores (csrc/painn.cu).
 EDGE_IMPL = os.environ.get("SPK_B200_EDGE", "tc")
 EDGE_TC_MIN_EDGES = 4096
 
@@ -620,7 +617,7 @@ def cfconv_fwd(h, w_raw, geo, graph: EdgeGraph, F: int):
     return m
 
 
-# fused forward block (csrc/schnet_tc.cu): filter network on tcgen05 inside the edge kernel; F == n_filters == 128, n_rbf <= 31.
+# fused forward block (csrc/schnet_tc.cu): filter network on wgmma inside the edge kernel; F == n_filters == 128, n_rbf <= 31.
 # SPK_B200_CFCONV=mat restores the materialised-filter pipeline (two dense kernels over [E, .] + spk_cfconv_fwd).
 CFCONV_IMPL = os.environ.get("SPK_B200_CFCONV", "tc")
 CFCONV_TC_MIN_EDGES = 2048

@@ -391,7 +391,7 @@ def _halo(rows: torch.Tensor, plan: RankPlan, group, peer: Optional["PeerHalo"] 
 
 class PartitionedPotential:
     """Energy + forces of ONE large system evaluated by the ranks of a process group (SURVEY.md section 8e, cfg5), every
-    rank running the sm_100a kernels on its part of the graph:
+    rank running the sm_90a kernels on its part of the graph:
 
         owned atoms  -> context net (dense kernels)            x [n_owned, 3F]
         halo         -> ghost rows of (x, mu) from their owners  (HaloExchange: NCCL point-to-point, autograd-aware)

@@ -1,4 +1,4 @@
-"""PaiNN representation on the B200 kernels -- drop-in for ``schnetpack.representation.PaiNN``.
+"""PaiNN representation on the CUDA kernels -- drop-in for ``schnetpack.representation.PaiNN``.
 
 Constructor signature, attributes, tensor-dict protocol and ``state_dict`` keys follow
 /root/reference/src/schnetpack/representation/painn.py:120-256; the arithmetic is the fused kernel pipeline of
@@ -87,7 +87,7 @@ class PaiNNMixing(nn.Module):
 
 
 class PaiNN(nn.Module):
-    """PaiNN - polarizable interaction neural network (painn.py:120-256), B200 kernel path."""
+    """PaiNN - polarizable interaction neural network (painn.py:120-256), CUDA kernel path."""
 
     def __init__(self, n_atom_basis: int, n_interactions: int, radial_basis: nn.Module,
                  cutoff_fn: Optional[Callable] = None, activation: Optional[Callable] = F.silu,

@@ -1,4 +1,4 @@
-"""SchNet representation on the B200 kernels -- drop-in for ``schnetpack.representation.SchNet``
+"""SchNet representation on the CUDA kernels -- drop-in for ``schnetpack.representation.SchNet``
 (/root/reference/src/schnetpack/representation/schnet.py:73-173)."""
 from __future__ import annotations
 
@@ -43,7 +43,7 @@ class SchNetInteraction(nn.Module):
 
 
 class SchNet(nn.Module):
-    """SchNet (schnet.py:73-173), B200 kernel path."""
+    """SchNet (schnet.py:73-173), CUDA kernel path."""
 
     def __init__(self, n_atom_basis: int, n_interactions: int, radial_basis: nn.Module, cutoff_fn: Callable,
                  n_filters: int = None, shared_interactions: bool = False,

@@ -1,4 +1,4 @@
-"""TorchScript deployment of the B200 path (SURVEY.md section 8 f4).
+"""TorchScript deployment of the CUDA path (SURVEY.md section 8 f4).
 
 The reference deploys models with ``torch.jit.script`` (``src/scripts/spkdeploy:16-38``; MD with ``script_model=True``,
 ``md/calculators/schnetpack_calculator.py:105-107``).  The kernel pipelines of this package are driven from Python
@@ -364,7 +364,7 @@ class ScriptedPotential(nn.Module):
 
 
 def to_scriptable(model: NeuralNetworkPotential) -> ScriptedPotential:
-    """TorchScript-compatible twin of a B200 ``NeuralNetworkPotential`` (``convert_model`` output or ``from_spec``): same
+    """TorchScript-compatible twin of a CUDA ``NeuralNetworkPotential`` (``convert_model`` output or ``from_spec``): same
     weights (shared storage), ``torch.jit.script`` -able, ``save`` / ``load`` -able."""
     ins = []
     for m in model.input_modules:

@@ -24,7 +24,7 @@ MODEL_CASES = [
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on a GPU machine with -m gpu)")
 
 
 def load_case(name):

@@ -167,7 +167,7 @@ def test_dense(M, K, N):
                                         (4100, 128, 20, None), (16128, 128, 256, None), (130, 128, 64, None),
                                         (77, 384, 128, None), (2000, 20, 128, 24), (5, 64, 128, None)])
 def test_dense_tcgen05_3xtf32(M, K, N, lda):
-    """tcgen05 tensor-core layer with 3xTF32 compensation must be fp32-grade (the reference GEMMs are true fp32)."""
+    """wgmma tensor-core layer with 3xTF32 compensation must be fp32-grade (the reference GEMMs are true fp32)."""
     from schnetpack_b200 import ops
 
     torch.manual_seed(3)
@@ -200,7 +200,7 @@ def test_dense_tcgen05_3xtf32(M, K, N, lda):
 @pytest.mark.gpu
 @pytest.mark.parametrize("M,K1,N2", [(300, 128, 384), (5376, 128, 384), (1000, 256, 384), (77, 64, 128), (129, 20, 256)])
 def test_mlp2_one_launch_matches_fp64_and_two_launches(M, K1, N2):
-    """Dense(K1,128,act) -> Dense(128,N2) as one tcgen05 launch with the hidden tile resident in shared memory
+    """Dense(K1,128,act) -> Dense(128,N2) as one wgmma launch with the hidden tile resident in shared memory
     (csrc/mlp2_tc.cu) against the fp64 restatement and against two spk_dense_tc launches: values, saved act'(pre), addend,
     ragged last row tile, K1 not a multiple of the 16-float K-tile."""
     from schnetpack_b200 import ops
@@ -423,7 +423,7 @@ def test_lin_saved_derivative_backward(impl):
 
 @pytest.mark.parametrize("gen,n_rbf", [("aspirin", 20), ("qm9like", 20), ("aspirin", 13), ("periodic", 20)])
 def test_painn_edge_tensor_core_filter_matches_streaming(gen, n_rbf):
-    """csrc/painn_tc.cu (filter on tcgen05, channels on TMEM lanes) == csrc/painn.cu (filter in FFMA2) to fp32 rounding,
+    """csrc/painn_tc.cu (filter on wgmma) == csrc/painn.cu (filter on the CUDA cores) to fp32 rounding,
     forward and reverse, with and without mu, on ragged row lengths, tail chunks and an n_rbf that is not a multiple of 4."""
     from schnetpack_b200 import ops
     from schnetpack_b200 import synthetic as S
@@ -621,7 +621,7 @@ def test_atom_chain_matches_per_layer_pipeline(batch, nfold):
 
 @pytest.mark.parametrize("case", ["qm9", "qm9_padded", "box", "bessel18"])
 def test_schnet_fused_forward_block_vs_fp64(case):
-    """csrc/schnet_tc.cu (filter network on tcgen05 inside the edge kernel, CSR over the active edges only) against a torch
+    """csrc/schnet_tc.cu (filter network on wgmma inside the edge kernel, CSR over the active edges only) against a torch
     fp64 restatement of schnet.py:56-67 for one block, incl. a padded neighbour list (padding slots at d == cutoff are
     dropped by spk_graph_build_active), a periodic box, and n_rbf % 4 != 0 with the Bessel basis."""
     from schnetpack_b200 import ops

@@ -1,4 +1,4 @@
-"""GPU: the CUDA path (through the module API -> C ABI -> sm_100a kernels) against
+"""GPU: the CUDA path (through the module API -> C ABI -> sm_90a kernels) against
   (1) the committed golden fixtures produced by the UNMODIFIED reference (tests/golden/*.npz), and
   (2) the oracle (oracle/spk_oracle.py, fp64) on seeded inputs of the named configurations.
 

@@ -106,7 +106,7 @@ def test_ranks_over_nccl(tmp_path, transport, monkeypatch):
     monkeypatch.setenv("SPK_B200_HALO", transport)
     world = min(torch.cuda.device_count(), 4)
     if world < 2:
-        pytest.skip("needs >= 2 GPUs (NCCL cannot put two ranks on one device); covered by the 2-GPU gpurun of tools/gpu_r2_halo.sh")
+        pytest.skip("needs >= 2 GPUs (NCCL cannot put two ranks on one device))")
     out = str(tmp_path / "res.npz")
     n_atoms = 3000
     mp.spawn(_worker, args=(world, _free_port(), "nccl", n_atoms, out), nprocs=world, join=True)

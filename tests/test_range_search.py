@@ -51,7 +51,7 @@ def test_warp_lower_bound_matches_searchsorted(n):
         ptr = np.concatenate([[0], np.cumsum(deg)]).astype(np.int64)
         E = int(ptr[-1])
         targets = list(rng.integers(-3, E + 4, size=40)) + [0, E, E + 1, -1]
-        nb = 592                                                                # 148 CTAs x 4 groups
+        nb = 528                                                                # 132 CTAs x 4 groups
         targets += [(E * b) // nb for b in range(0, nb + 1, 37)]
         for t in targets:
             want = min(int(np.searchsorted(ptr[:n], t, side="left")), n)
@@ -60,10 +60,10 @@ def test_warp_lower_bound_matches_searchsorted(n):
 
 
 def test_group_ranges_cover_every_row_once():
-    """the four group ranges of all 148 CTAs tile [0, n) without gaps or overlap (what the kernels rely on)"""
+    """the four group ranges of all 132 CTAs tile [0, n) without gaps or overlap (what the kernels rely on)"""
     rng = np.random.default_rng(5)
     n = 5376
     ptr = np.concatenate([[0], np.cumsum(rng.integers(0, 30, size=n))]).astype(np.int64)
-    E, nb = int(ptr[-1]), 148 * 4
+    E, nb = int(ptr[-1]), 132 * 4
     b = [0 if k <= 0 else (n if k >= nb else lower_bound_warp(ptr, n, (E * k) // nb)) for k in range(nb + 1)]
     assert b[0] == 0 and b[-1] == n and all(x <= y for x, y in zip(b, b[1:]))

@@ -1,9 +1,11 @@
-"""The UNMODIFIED reference modules as the live checker (oracle/ref_loader.py: from /root/reference in the build container,
-from the git-ignored byte-identical copy oracle/_ref on the GPU box -- recipe oracle/make_ref.py).
+"""The UNMODIFIED reference modules as the checker (oracle/ref_loader.py: from a reference checkout or from the git-ignored
+copy oracle/_ref -- recipe oracle/make_ref.py); at the full sizes of the named configurations the reference's fp64 outputs
+are stored under tests/golden/full_size_<cfg>.npz (tests/golden/make_golden_full_size.py), so that comparison needs no
+reference tree.
 
 CPU part (``-m "not gpu"``): the restatement oracle/spk_oracle.py against the live reference, and ``convert_model`` on the
 reference's shipped trained model (class swap, identical state_dict, fp64 -> fp32 cast).
-GPU part: the CUDA path against the reference running in fp64 ON THE SAME GPU at the FULL sizes of the named configurations
+GPU part: the CUDA path against the reference's fp64 results at the FULL sizes of the named configurations
 (cfg2 B=256, cfg3 B=1024 padded, cfg4 8192 atoms), ``convert_model`` end to end (incl. custom nuclear / electronic
 embeddings), and the reference's block-level API (PaiNNInteraction / PaiNNMixing / SchNetInteraction forward + gradients).
 Tolerance: 1e-5 relative (max-norm) against fp64, BASELINE.json north_star.
@@ -39,7 +41,7 @@ def test_oracle_matches_live_reference_cpu():
 
 @needs_ref
 def test_convert_model_swaps_classes_and_keeps_state_dict():
-    """INTEGRATION.md section 1: convert_model(reference model) -> B200 modules with the SAME state_dict (keys and values),
+    """INTEGRATION.md section 1: convert_model(reference model) -> CUDA modules with the SAME state_dict (keys and values),
     postprocessors reused, fp64 models cast to fp32 with input casting switched on."""
     import schnetpack_b200 as sb
     from schnetpack_b200 import atomistic, representation
@@ -104,21 +106,22 @@ def _cuda_eval(model, data, dev):
 
 
 @pytest.mark.gpu
-@needs_ref
 @pytest.mark.parametrize("cfg", ["cfg2", "cfg3", "cfg4"])
 def test_full_size_parity_against_reference_on_gpu(cfg):
     """The benchmarked sizes themselves: cfg2 = aspirin x 256 (5376 atoms / 78 k edges, PaiNN E+F), cfg3 = QM9-like x 1024
     with the padded neighbour list (831 488 edge slots, SchNet 128x6, energy), cfg4 = 8192-atom periodic box (PaiNN E+F).
-    Checker: the reference's own modules in fp64 on the same GPU."""
+    Checker: the reference's own modules in fp64 on the same inputs and weights (stored, tests/golden/full_size_<cfg>.npz)."""
+    from conftest import GOLDEN
     from schnetpack_b200 import synthetic as S
     from schnetpack_b200.model import from_spec
 
     dev = torch.device("cuda:0")
     spec, data = S.make_config(cfg)
-    params = S.init_params(spec, seed=7)
+    z = np.load(os.path.join(GOLDEN, f"full_size_{cfg}.npz"))
+    assert int(z["n_atoms"]) == data[S.Z].shape[0] and int(z["n_edges"]) == data[S.idx_i].shape[0]
+    params = S.init_params(spec, seed=int(z["seed"]))
     out = _cuda_eval(from_spec(spec, params, dev), data, dev)
-    ref_model = rl.build_from_spec(spec, params, torch.float64, dev)
-    ref = rl.evaluate(ref_model, data, torch.float64, dev, forces=bool(spec.get("forces", True)))
+    ref = {k[6:]: torch.as_tensor(z[k]) for k in z.files if k.startswith("ref64:")}
     e = rel_err(out["energy"], ref["energy"].cpu().numpy())
     print(cfg, "N", data["_atomic_numbers"].shape[0], "E", data["_idx_i"].shape[0], "energy rel err", e)
     assert e < TOL
