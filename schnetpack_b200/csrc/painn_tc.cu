@@ -8,14 +8,17 @@
 //
 //   * orientation: channels on the M side.  For each filter third t the A operand is W_t = [w | b] (128 channels x 32,
 //     static, packed once by spk_painn_pack_filter in the shared-memory operand layout and fetched by ONE TMA bulk copy),
-//     the B operand is a chunk of 64 edge rows  Phi' = fc * [phi | 1]  (K-major, 64 B swizzle, produced per chunk by
-//     the producer warps with the hi/lo split of 3xTF32);
+//     the B operand is a chunk of NR = 32 operand rows  Phi' = fc * [phi | 1]  (K-major, 64 B swizzle, hi/lo split of 3xTF32);
 //   * one persistent CTA per SM: 4 consumer warpgroups (a group owns 128 channels of its own edge-balanced receiver range,
-//     as a CTA of painn.cu did) and the producer warps.  Group g multiplies W_t by ITS 16 rows of the chunk (wgmma m64n16,
-//     two m64 halves), so no group waits for another; the fragments go through a small shared-memory transpose to
-//     thread = channel, the mapping of the gather/accumulate code;
+//     as a CTA of painn.cu did) and one producer warpgroup.  The producer stages the Phi' rows of a whole chunk (every
+//     group's rows), multiplies them with wide wgmma (m64n32k8: 3 thirds x 2 m-halves x 3 k-steps x 3 products = 54
+//     instructions per chunk) and stores the fragments straight into a [operand row][third * 128 + channel] fp32 tile;
+//     the consumers read their rows of it with thread = channel, the mapping of the gather/accumulate code.  They never
+//     issue or wait on a wgmma, so the tensor core and the gathers run side by side;
 //   * 3xTF32 (Wl*Ph + Wh*Pl + Wh*Ph, small terms first) keeps the filter at fp32 accuracy; K = 24 is three k-steps;
-//   * NST Phi' stages let the producers stage chunk k+1.. while the groups gather chunk k.
+//   * NBUF = 2 filter tiles (with their metadata) behind full/empty mbarriers: the producer stages, multiplies and stores
+//     chunk k+1 while the groups gather chunk k.  The global loads of chunk k+1 are issued before the MMAs of chunk k and
+//     land while they run.
 // The reduction over a receiver's edges stays a private register accumulation in CSR order: deterministic, no atomics.
 #include "painn_common.cuh"
 #include "wgmma.cuh"
@@ -40,66 +43,74 @@ extern "C" int spk_debug_edge_trace(long long* host) {
 #define ETRACE(slot) do { } while (0)
 #define BTRACE(slot) do { } while (0)
 #endif
+// Stamp slots (consumer warp 0, chunks k < 16): 64+k the wait for the chunk starts, 176+k it returns, 80+k the filter
+// values are in registers, 96+k the chunk is done; 16+k (producer warp 0): the chunk's filter tile is published.
 
 namespace {
 
 constexpr int F_TC = 128;                      // channels per filter third (two m64 halves)
-constexpr int EG = 16;                         // edges per group and chunk (wgmma N)
 constexpr int NG = 4;                          // consumer groups = warpgroups
-constexpr int NE = EG * NG;                    // Phi' rows per chunk
 constexpr int NCW = NG * 4;                    // consumer warps
-constexpr int W_PROD0 = NCW;
-constexpr int NPROD = 3;                       // producer warps: chunk k -> warp k % NPROD
-constexpr int NST = 3;                         // Phi' stages: chunk k -> stage k % NST (NPROD divides NST: one owner per stage)
-constexpr int NTHREADS = (W_PROD0 + NPROD) * 32;
+constexpr int W_PROD0 = NCW;                   // the producer warpgroup: warps NCW .. NCW + 3
+constexpr int NTHREADS = (NCW + 4) * 32;
+constexpr int PROD_BAR = 1 + NG;               // named barrier of the producer warpgroup (1..NG: consumer groups)
+constexpr int NR = 32;                         // operand rows per chunk = wgmma N
+constexpr int NBUF = 2;                        // filter tiles (and their metadata) in flight
 constexpr int KT = 16;                         // floats per operand K-tile (64 B rows, SWIZZLE_64B)
 constexpr int A_TILE = F_TC * KT * 4;          // 8192 B
 constexpr int A_BYTES = 3 * 2 * 2 * A_TILE;    // [third][hi,lo][k-tile]
-constexpr int B_TILE = NE * KT * 4;            // 4096 B
-constexpr int B_STAGE = 2 * 2 * B_TILE;        // [hi,lo][k-tile]
-constexpr int META_STAGE = NE * 4 + NE * 16;   // sender index + (ux, uy, uz, -) per row
-constexpr int T_LD = F_TC + 4;                 // row of the per-group transpose tile [column][channel] (floats)
-constexpr int T_BYTES = NG * 16 * T_LD * 4;    // 16 columns per group (forward: 16 edges; reverse: 8 edges x {W, dW/dd})
-constexpr int SMEM_BYTES = A_BYTES + NST * B_STAGE + NST * META_STAGE + T_BYTES + 1024;
+constexpr int B_TILE = NR * KT * 4;            // 2048 B
+constexpr int B_BYTES = 2 * 2 * B_TILE;        // [hi,lo][k-tile]
+constexpr int T_LD = 3 * F_TC + 4;             // row of the filter tile (floats); = 4 mod 32: conflict-free fragment stores
+constexpr int T_FLOATS = NR * T_LD;
+constexpr int T_BYTES = T_FLOATS * 4;
 
-// The group's 3xTF32 filter products of one chunk for NT thirds: d[t][m-half] (+)= W_t * B^T over the three k-steps
-// (K = n_rbf + 1 <= 24), B = 16 (forward) or 8 (reverse) operand rows starting at byte offset b_row of the stage.
-template <int NT, int N>
-__device__ __forceinline__ void filter_mma(float (&d)[NT][2][N / 2], uint32_t aB, uint32_t bB) {
+// Forward: a chunk is NG groups x EG edges, one operand row each.
+constexpr int EG = NR / NG;                    // 8 edges per group and chunk
+constexpr int META_F = NR * 4 + NR * 16;       // sender index + (ux, uy, uz, -) per row
+constexpr int SMEM_BYTES = A_BYTES + B_BYTES + NBUF * (T_BYTES + META_F) + 1024;
+
+// One filter third on the producer warpgroup: d[m-half] = W_t * B^T over the three k-steps (K = n_rbf + 1 <= 24) for the
+// NR operand rows of the stage at bB, as one commit group.
+__device__ __forceinline__ void filter_third(float (&d)[2][16], uint32_t aB, uint32_t bB, int t) {
     wgmma_fence();
 #pragma unroll
-    for (int t = 0; t < NT; ++t)
+    for (int s3 = 0; s3 < 3; ++s3) {                         // k-steps 0..2 = (tile 0, 0), (tile 0, 32 B), (tile 1, 0)
+        const int kt = s3 >> 1, ko = (s3 & 1) * 32;
+        const uint64_t bh = make_desc(bB + (0 * 2 + kt) * B_TILE + ko);
+        const uint64_t bl = make_desc(bB + (1 * 2 + kt) * B_TILE + ko);
 #pragma unroll
-        for (int s3 = 0; s3 < 3; ++s3) {                     // k-steps 0..2 = (tile 0, 0), (tile 0, 32 B), (tile 1, 0)
-            const int kt = s3 >> 1, ko = (s3 & 1) * 32;
-            const uint64_t bh = make_desc(bB + (0 * 2 + kt) * B_TILE + ko);
-            const uint64_t bl = make_desc(bB + (1 * 2 + kt) * B_TILE + ko);
-#pragma unroll
-            for (int mh = 0; mh < 2; ++mh) {
-                const uint64_t ah = make_desc(aB + ((t * 2 + 0) * 2 + kt) * A_TILE + mh * SPK_WG_ROWS_BYTES + ko);
-                const uint64_t al = make_desc(aB + ((t * 2 + 1) * 2 + kt) * A_TILE + mh * SPK_WG_ROWS_BYTES + ko);
-                if constexpr (N == 16) {
-                    wgmma_n16(d[t][mh], al, bh, s3 ? 1 : 0);       // small terms first
-                    wgmma_n16(d[t][mh], ah, bl, 1);
-                    wgmma_n16(d[t][mh], ah, bh, 1);
-                } else {
-                    wgmma_n8(d[t][mh], al, bh, s3 ? 1 : 0);
-                    wgmma_n8(d[t][mh], ah, bl, 1);
-                    wgmma_n8(d[t][mh], ah, bh, 1);
-                }
-            }
+        for (int mh = 0; mh < 2; ++mh) {
+            const uint64_t ah = make_desc(aB + ((t * 2 + 0) * 2 + kt) * A_TILE + mh * SPK_WG_ROWS_BYTES + ko);
+            const uint64_t al = make_desc(aB + ((t * 2 + 1) * 2 + kt) * A_TILE + mh * SPK_WG_ROWS_BYTES + ko);
+            wgmma_n32(d[mh], al, bh, s3 ? 1 : 0);              // small terms first
+            wgmma_n32(d[mh], ah, bl, 1);
+            wgmma_n32(d[mh], ah, bh, 1);
         }
+    }
     wgmma_commit();
-    wgmma_wait_all();
 }
 
-// fragment (m64nN, two m-halves) of the warpgroup -> columns col0.. of the [column][channel] tile tg
-template <int N>
-__device__ __forceinline__ void frag_to_tile(const float (&d)[2][N / 2], float* tg, int col0, int t) {
+// The chunk's 3xTF32 filter for NT thirds -> tile[row][t * 128 + channel].  Third t+1 is on the tensor core while the
+// fragments of third t are stored (pt: thread of the producer warpgroup).
+template <int NT>
+__device__ __forceinline__ void filter_to_tile(uint32_t aB, uint32_t bB, float* tile, int pt) {
+    float d[2][2][16];                                       // [third parity][m-half]
+    filter_third(d[0], aB, bB, 0);
 #pragma unroll
-    for (int mh = 0; mh < 2; ++mh)
+    for (int t = 0; t < NT; ++t) {
+        if (t + 1 < NT) {
+            filter_third(d[(t + 1) & 1], aB, bB, t + 1);
+            wgmma_wait<1>();
+        } else {
+            wgmma_wait<0>();
+        }
 #pragma unroll
-        for (int i = 0; i < N / 2; ++i) tg[(col0 + wg_frag_col(t, i)) * T_LD + mh * 64 + wg_frag_row(t, i)] = d[mh][i];
+        for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+            for (int i = 0; i < 16; ++i)
+                tile[wg_frag_col(pt, i) * T_LD + t * F_TC + mh * 64 + wg_frag_row(pt, i)] = d[t & 1][mh][i];
+    }
 }
 
 // [third][hi,lo][k-tile][128 x 16] operand tiles of  [w | b | 0]  (k = n_rbf is the bias column)
@@ -118,6 +129,26 @@ __global__ void k_pack_filter(const float* __restrict__ wf, const float* __restr
     out[((third * 2 + 1) * 2 + kt) * (A_TILE / 4) + off] = lo;
 }
 
+// 16-byte chunk of one Phi' row -> the hi/lo operand tiles of the stage
+__device__ __forceinline__ void put_row(uint8_t* stB, int r, int qc, float4 v) {
+    float4 hi, lo;
+    hi.x = tf32_rn(v.x); hi.y = tf32_rn(v.y); hi.z = tf32_rn(v.z); hi.w = tf32_rn(v.w);
+    lo.x = v.x - hi.x; lo.y = v.y - hi.y; lo.z = v.z - hi.z; lo.w = v.w - hi.w;
+    const int off = tile_off(r, qc & 3);
+    *reinterpret_cast<float4*>(stB + (0 * 2 + (qc >> 2)) * B_TILE + off) = hi;
+    *reinterpret_cast<float4*>(stB + (1 * 2 + (qc >> 2)) * B_TILE + off) = lo;
+}
+
+// [phi | 1] restricted to the 16-byte K-chunk qc (the bias column k = n_rbf is 1, chunks past KP are 0)
+__device__ __forceinline__ float4 with_bias(float4 v, bool q_in, int qc, int n_rbf) {
+    if (!q_in) v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (qc == (n_rbf >> 2)) {
+        const int kb = n_rbf & 3;
+        if (kb == 0) v.x = 1.f; else if (kb == 1) v.y = 1.f; else if (kb == 2) v.z = 1.f; else v.w = 1.f;
+    }
+    return v;
+}
+
 template <bool HAS_MU>
 __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
     const float* __restrict__ x, const float* __restrict__ mu, const float* __restrict__ q,
@@ -130,9 +161,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* sA = smem;
     uint8_t* sB = smem + A_BYTES;
-    uint8_t* sMeta = sB + NST * B_STAGE;
-    float* sT = reinterpret_cast<float*>(sMeta + NST * META_STAGE);
-    __shared__ __align__(8) uint64_t a_full, full_bar[NST], empty_bar[NST], meta_empty[NST];
+    float* sT = reinterpret_cast<float*>(sB + B_BYTES);
+    uint8_t* sMeta = sB + B_BYTES + NBUF * T_BYTES;
+    __shared__ __align__(8) uint64_t a_full, full_bar[NBUF], empty_bar[NBUF];
     __shared__ int s_rlo[NG], s_rhi[NG], s_sb[NG], s_se[NG];
 
     const int tid = threadIdx.x, lane = tid & 31;
@@ -142,10 +173,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
     if (tid == 0) {
         mbar_init(&a_full, 1);
 #pragma unroll
-        for (int s = 0; s < NST; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], NCW);
-            mbar_init(&meta_empty[s], NCW);
+        for (int b = 0; b < NBUF; ++b) {
+            mbar_init(&full_bar[b], 4);
+            mbar_init(&empty_bar[b], NCW);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         mbar_expect_tx(&a_full, A_BYTES);          // static operand: fetched BEFORE griddepcontrol.wait (pack kernels never trigger their dependents early, common.cuh)
@@ -175,75 +205,69 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
 
     if (warp >= W_PROD0) {
         // =========================================== producers ===========================================
-        const int p = warp - W_PROD0;
-        const int qc = lane & 7, rsub = lane >> 3;             // 8 x 16 B K-chunks per row, 4 rows per pass, 16 passes
+        const int pt = tid - W_PROD0 * 32;                     // thread of the producer warpgroup
+        const int qc = pt & 7, rsub = pt >> 3;                 // 8 x 16 B K-chunks per row, 16 rows per pass, 2 passes
         const bool q_in = qc * 4 < KP;
-        const int kb_chunk = n_rbf >> 2, kb = n_rbf & 3;       // the bias column k = n_rbf
-        for (int k = p; k < n_chunks; k += NPROD) {
-            const int st = k % NST, use = k / NST;
-            uint8_t* stB = sB + st * B_STAGE;
-            int* st_j = reinterpret_cast<int*>(sMeta + st * META_STAGE);
-            float4* st_u = reinterpret_cast<float4*>(sMeta + st * META_STAGE + NE * 4);
-            // all loads are unconditional (rows past a group's end read slot 0 and are zeroed afterwards) and issued in
-            // two batches of 8 rows: branchy loads, or more loads than the register budget holds, are serialised by the
-            // compiler and cost one full memory latency EACH
-            int mj[2];
-            float4 mu4[2];
+        // one chunk in registers: all loads are unconditional (rows past a group's end read slot 0, fc = 0 zeroes them)
+        float4 pv[2];
+        float fcv[2];
+        int mj = 0;                                            // metadata: threads pt < NR, row = pt
+        float4 mu4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        auto load = [&](int k) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int r = lane + 32 * h, g = r / EG;
+                const int r = rsub + 16 * h, g = r / EG;
                 const int s = s_sb[g] + k * EG + (r % EG);
+                const bool ok = s < s_se[g];
+                const int sl = ok ? s : 0;
+                const float fc = geo[(int64_t)sl * SPK_GEO_STRIDE + 4];
+                fcv[h] = ok ? fc : 0.f;
+                pv[h] = *reinterpret_cast<const float4*>(phi + (int64_t)sl * KP + (q_in ? qc * 4 : 0));
+            }
+            if (pt < NR) {
+                const int g = pt / EG;
+                const int s = s_sb[g] + k * EG + (pt % EG);
                 const int sl = s < s_se[g] ? s : 0;
-                mj[h] = slot_j[sl];
-                mu4[h] = *reinterpret_cast<const float4*>(geo + (int64_t)sl * SPK_GEO_STRIDE);   // ux uy uz d
+                mj = slot_j[sl];
+                mu4 = *reinterpret_cast<const float4*>(geo + (int64_t)sl * SPK_GEO_STRIDE);   // ux uy uz d
             }
-#pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                float4 pv[8];
-                float fcv[8];
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const int r = (half * 8 + i) * 4 + rsub, g = r / EG;
-                    const int s = s_sb[g] + k * EG + (r % EG);
-                    const bool ok = s < s_se[g];
-                    const int sl = ok ? s : 0;
-                    const float fc = geo[(int64_t)sl * SPK_GEO_STRIDE + 4];
-                    fcv[i] = ok ? fc : 0.f;
-                    pv[i] = *reinterpret_cast<const float4*>(phi + (int64_t)sl * KP + (q_in ? qc * 4 : 0));
-                }
-                if (half == 0) {
-                    if (p == 0 && k < 48) ETRACE(16 + k / 3);  // producer 0: loads issued
-                    if (use >= 1) {
-                        mbar_wait(&empty_bar[st], (use - 1) & 1);      // MMAs of chunk k-NST have read this Phi' stage
-                        mbar_wait(&meta_empty[st], (use - 1) & 1);     // consumers are done with its metadata
-                    }
-                }
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const int r = (half * 8 + i) * 4 + rsub;
-                    const float fc = fcv[i];                   // 0 for rows past the group's end
-                    float4 v = q_in ? pv[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (qc == kb_chunk) {
-                        if (kb == 0) v.x = 1.f; else if (kb == 1) v.y = 1.f; else if (kb == 2) v.z = 1.f; else v.w = 1.f;
-                    }
-                    v.x *= fc; v.y *= fc; v.z *= fc; v.w *= fc;  // Phi' = fc * [phi | 1]: the MMA yields W itself
-                    float4 hi, lo;
-                    hi.x = tf32_rn(v.x); hi.y = tf32_rn(v.y); hi.z = tf32_rn(v.z); hi.w = tf32_rn(v.w);
-                    lo.x = v.x - hi.x; lo.y = v.y - hi.y; lo.z = v.z - hi.z; lo.w = v.w - hi.w;
-                    const int off = tile_off(r, qc & 3);
-                    *reinterpret_cast<float4*>(stB + (0 * 2 + (qc >> 2)) * B_TILE + off) = hi;
-                    *reinterpret_cast<float4*>(stB + (1 * 2 + (qc >> 2)) * B_TILE + off) = lo;
-                }
-            }
+        };
+        auto stage = [&](int k) {                              // Phi' = fc * [phi | 1]: the MMA yields W itself
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                st_j[lane + 32 * h] = mj[h];
-                st_u[lane + 32 * h] = mu4[h];
+                float4 v = with_bias(pv[h], q_in, qc, n_rbf);
+                const float fc = fcv[h];
+                v.x *= fc; v.y *= fc; v.z *= fc; v.w *= fc;
+                put_row(sB, rsub + 16 * h, qc, v);
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            if (pt < NR) {
+                uint8_t* m = sMeta + (k % NBUF) * META_F;
+                reinterpret_cast<int*>(m)[pt] = mj;
+                reinterpret_cast<float4*>(m + NR * 4)[pt] = mu4;
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the stage is read by the async proxy
+            wg_bar(PROD_BAR);
+        };
+        const uint32_t aB = smem_u32(sA), bB = smem_u32(sB);
+        if (n_chunks > 0) {
+            load(0);
+            stage(0);
+        }
+        mbar_wait(&a_full, 0);
+        for (int k = 0; k < n_chunks; ++k) {
+            const int b = k % NBUF;
+            const bool more = k + 1 < n_chunks;
+            if (more) load(k + 1);                             // in flight during the MMAs of chunk k
+            filter_to_tile<NT>(aB, bB, sT + b * T_FLOATS, pt);
             __syncwarp();
-            if (lane == 0) mbar_arrive(&full_bar[st]);
-            if (p == 0 && k < 48) ETRACE(32 + k / 3);          // producer 0: published
+            if (lane == 0) mbar_arrive(&full_bar[b]);
+            if (warp == W_PROD0 && k < 16) ETRACE(16 + k);
+            if (more) {
+                const int nb = (k + 1) % NBUF, use = (k + 1) / NBUF;
+                if (use >= 1) mbar_wait(&empty_bar[nb], (use - 1) & 1);   // tile and metadata of chunk k+1-NBUF consumed
+                wg_bar(PROD_BAR);                              // every warp's MMAs of chunk k have read the stage
+                stage(k + 1);
+            }
         }
     } else {
         // =========================================== consumers ===========================================
@@ -278,89 +302,67 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
             mu_out[om + 2 * F] = bm2 + dm2;
             dq = dm0 = dm1 = dm2 = 0.f;
         };
-        float* tg = sT + g * 16 * T_LD;                        // this group's [edge][channel] transpose tile
-        const uint32_t aB = smem_u32(sA);
-        mbar_wait(&a_full, 0);
         for (int k = 0; k < n_chunks; ++k) {
-            const int st = k % NST;
+            const int b = k % NBUF;
             if (warp == 0 && k < 16) ETRACE(64 + k);           // consumer 0: starts waiting
-            mbar_wait(&full_bar[st], (k / NST) & 1);           // Phi' rows and metadata of the chunk
-            float d[NT][2][8];
-            filter_mma<NT, 16>(d, aB, smem_u32(sB + st * B_STAGE) + (uint32_t)(g * EG * SPK_SW64_ROW));
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty_bar[st]);        // the group's wgmma have read the stage
-            float wv[3][EG];
-#pragma unroll
-            for (int t = 0; t < NT; ++t) {                     // fragments -> thread = channel, one third at a time
-                frag_to_tile<16>(d[t], tg, 0, c);
-                wg_bar(1 + g);
-#pragma unroll
-                for (int u = 0; u < EG; ++u) wv[t][u] = tg[u * T_LD + c];
-                wg_bar(1 + g);
-            }
+            mbar_wait(&full_bar[b], (k / NBUF) & 1);           // filter tile and metadata of the chunk
+            if (warp == 0 && k < 16) ETRACE(176 + k);
+            // this group's rows of the filter tile, thread = channel: read where they are used, which keeps 24 registers free
+            const float* tg = sT + b * T_FLOATS + g * EG * T_LD + c;
             if (warp == 0 && k < 16) ETRACE(80 + k);           // filter values ready
             if (warp == 0 && lane == 0 && k == 0) SPK_TL_PHASE(2);
-            const int* st_j = reinterpret_cast<const int*>(sMeta + st * META_STAGE) + g * EG;
-            const float4* st_u = reinterpret_cast<const float4*>(sMeta + st * META_STAGE + NE * 4) + g * EG;
+            const int* st_j = reinterpret_cast<const int*>(sMeta + b * META_F) + g * EG;
+            const float4* st_u = reinterpret_cast<const float4*>(sMeta + b * META_F + NR * 4) + g * EG;
             const int base = s_begin + k * EG;
-            // eight edges at a time: all their gathers are issued before the first use (rows past the range read sender 0,
-            // their filter values are exactly 0), so eight memory latencies overlap instead of following each other
+            // all eight gathers are issued before the first use (rows past the range read sender 0, their filter values
+            // are exactly 0), so eight memory latencies overlap instead of following each other
+            if (base < s_end) {
+                float xa[EG], xb[EG], xc[EG], m0[EG], m1[EG], m2[EG];
 #pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                constexpr int HB = EG / 2;
-                const float* wa = wv[0] + half * HB;
-                const float* wb = wv[1] + half * HB;
-                const float* wc = wv[2] + half * HB;
-                if (base + half * HB < s_end) {
-                    float xa[HB], xb[HB], xc[HB], m0[HB], m1[HB], m2[HB];
-#pragma unroll
-                    for (int u = 0; u < HB; ++u) {
+                for (int u = 0; u < EG; ++u) {
 #ifdef SPK_EDGE_EXP_JMASK
-                        const int j = st_j[half * HB + u] & 7;     // experiment: all gathers hit L1 (timing only)
+                    const int j = st_j[u] & 7;                 // experiment: all gathers hit L1 (timing only)
 #else
-                        const int j = st_j[half * HB + u];
+                    const int j = st_j[u];
 #endif
-                        const float* __restrict__ xj = x + (size_t)j * (3 * F) + c;
-                        xa[u] = xj[0];
-                        xb[u] = xj[F];
-                        if (HAS_MU) {
-                            xc[u] = xj[2 * F];
-                            const float* __restrict__ mj = mu + (size_t)j * (3 * F) + c;
-                            m0[u] = mj[0];
-                            m1[u] = mj[F];
-                            m2[u] = mj[2 * F];
-                        }
+                    const float* __restrict__ xj = x + (size_t)j * (3 * F) + c;
+                    xa[u] = xj[0];
+                    xb[u] = xj[F];
+                    if (HAS_MU) {
+                        xc[u] = xj[2 * F];
+                        const float* __restrict__ mj = mu + (size_t)j * (3 * F) + c;
+                        m0[u] = mj[0];
+                        m1[u] = mj[F];
+                        m2[u] = mj[2 * F];
                     }
+                }
 #pragma unroll
-                    for (int u = 0; u < HB; ++u) {
-                        const int t = half * HB + u;
-                        const int s = base + t;
-                        if (s < s_end) {
-                            while (s >= next_boundary) {
-                                flush(i);
-                                ++i;
-                                next_boundary = boundary2;
-                                prefetch_row(i);
-                            }
-                            const float4 uv = st_u[t];
-                            dq = fmaf(wa[u], xa[u], dq);
-                            const float tb = wb[u] * xb[u];
-                            dm0 = fmaf(tb, uv.x, dm0);
-                            dm1 = fmaf(tb, uv.y, dm1);
-                            dm2 = fmaf(tb, uv.z, dm2);
-                            if (HAS_MU) {
-                                const float tc = wc[u] * xc[u];
-                                dm0 = fmaf(tc, m0[u], dm0);
-                                dm1 = fmaf(tc, m1[u], dm1);
-                                dm2 = fmaf(tc, m2[u], dm2);
-                            }
+                for (int u = 0; u < EG; ++u) {
+                    const int s = base + u;
+                    if (s < s_end) {
+                        while (s >= next_boundary) {
+                            flush(i);
+                            ++i;
+                            next_boundary = boundary2;
+                            prefetch_row(i);
+                        }
+                        const float4 uv = st_u[u];
+                        dq = fmaf(tg[u * T_LD], xa[u], dq);
+                        const float tb = tg[u * T_LD + F] * xb[u];
+                        dm0 = fmaf(tb, uv.x, dm0);
+                        dm1 = fmaf(tb, uv.y, dm1);
+                        dm2 = fmaf(tb, uv.z, dm2);
+                        if (HAS_MU) {
+                            const float tc = tg[u * T_LD + 2 * F] * xc[u];
+                            dm0 = fmaf(tc, m0[u], dm0);
+                            dm1 = fmaf(tc, m1[u], dm1);
+                            dm2 = fmaf(tc, m2[u], dm2);
                         }
                     }
                 }
-                if (half == 0 && warp == 0 && k < 16) ETRACE(128 + k);     // first half's edges done
             }
             __syncwarp();
-            if (lane == 0) mbar_arrive(&meta_empty[st]);
+            if (lane == 0) mbar_arrive(&empty_bar[b]);
             if (warp == 0 && k < 16) ETRACE(96 + k);           // chunk's edges done
         }
         if (warp == 0) ETRACE(2);
@@ -378,13 +380,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
 // ------------------------------------------------------------------------------------------------------------------
 // reverse pass, grouped by sender (same structure; reference: autograd of painn.py:55-65)
 // ------------------------------------------------------------------------------------------------------------------
-// A chunk is 4 groups x 8 edges.  Its operand has 64 rows: rows 0..31 = fc [phi | 1] (-> W) and rows 32..63 =
-// dfc [phi | 1] + fc [dphi | 0] (-> dW/dd); group g multiplies its 8 rows of each half, so one pass yields both the filter
-// and its radial derivative.
-constexpr int EGB = 8;                         // edges per group and chunk
-constexpr int NEB = EGB * NG;                  // 32 edges per chunk (x 2 operand rows each)
+// A chunk is 4 groups x 4 edges.  Its operand has NR = 32 rows: rows 0..15 = fc [phi | 1] (-> W) and rows 16..31 =
+// dfc [phi | 1] + fc [dphi | 0] (-> dW/dd), so one m64n32 product yields both the filter and its radial derivative.
+constexpr int EGB = NR / 2 / NG;               // 4 edges per group and chunk
+constexpr int NEB = EGB * NG;                  // 16 edges per chunk (x 2 operand rows each)
 constexpr int META_B = NEB * 4 + NEB * 4 + NEB * 16;   // receiver index, edge id, (ux, uy, uz, 1/d) per edge
-constexpr int SMEM_BYTES_B = A_BYTES + NST * B_STAGE + NST * META_B + T_BYTES + 1024;
+constexpr int SMEM_BYTES_B = A_BYTES + B_BYTES + NBUF * (T_BYTES + META_B) + 1024;
 
 
 template <bool HAS_MU>
@@ -401,9 +402,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* sA = smem;
     uint8_t* sB = smem + A_BYTES;
-    uint8_t* sMeta = sB + NST * B_STAGE;
-    float* sT = reinterpret_cast<float*>(sMeta + NST * META_B);
-    __shared__ __align__(8) uint64_t a_full, full_bar[NST], empty_bar[NST], meta_empty[NST];
+    float* sT = reinterpret_cast<float*>(sB + B_BYTES);
+    uint8_t* sMeta = sB + B_BYTES + NBUF * T_BYTES;
+    __shared__ __align__(8) uint64_t a_full, full_bar[NBUF], empty_bar[NBUF];
     __shared__ int s_rlo[NG], s_rhi[NG], s_sb[NG], s_se[NG];
     __shared__ float s_red[2][NG][EGB][4][4];      // [chunk parity][group][edge][warp][scalar]
 
@@ -413,10 +414,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
     if (tid == 0) {
         mbar_init(&a_full, 1);
 #pragma unroll
-        for (int s = 0; s < NST; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], NCW);
-            mbar_init(&meta_empty[s], NCW);
+        for (int b = 0; b < NBUF; ++b) {
+            mbar_init(&full_bar[b], 4);
+            mbar_init(&empty_bar[b], NCW);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         mbar_expect_tx(&a_full, A_BYTES);          // static operand: fetched BEFORE griddepcontrol.wait (pack kernels never trigger their dependents early, common.cuh)
@@ -447,22 +447,28 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
 
     if (warp >= W_PROD0) {
         // =========================================== producers ===========================================
-        const int p = warp - W_PROD0;
-        const int qc = lane & 7, rsub = lane >> 3;             // 8 x 16 B K-chunks per row, 4 edges per pass, 8 passes
+        const int pt = tid - W_PROD0 * 32;
+        const int qc = pt & 7, e = pt >> 3;                    // 8 x 16 B K-chunks per row, one edge per 8 threads
         const bool q_in = qc * 4 < KP;
-        const int kb_chunk = n_rbf >> 2, kb = n_rbf & 3;
-        for (int k = p; k < n_chunks; k += NPROD) {
-            const int st = k % NST, use = k / NST;
-            uint8_t* stB = sB + st * B_STAGE;
-            int* st_i = reinterpret_cast<int*>(sMeta + st * META_B);
-            int* st_e = st_i + NEB;
-            float4* st_u = reinterpret_cast<float4*>(sMeta + st * META_B + 2 * NEB * 4);
-            // consumer metadata: lane = edge of the chunk
-            int m_i, m_e;
-            float4 m_u;
+        float4 pv, dv;
+        float fc = 0.f, dfc = 0.f;
+        int m_i = 0, m_e = 0;                                  // metadata: threads pt < NEB, edge = pt
+        float4 m_u = make_float4(0.f, 0.f, 0.f, 0.f);
+        auto load = [&](int k) {
             {
-                const int g = lane / EGB;
-                const int pp = s_sb[g] + k * EGB + (lane % EGB);
+                const int g = e / EGB;
+                const int pp = s_sb[g] + k * EGB + (e % EGB);
+                const bool ok = pp < s_se[g];
+                const int sl = pos_slot[ok ? pp : 0];
+                const float2 f2 = *reinterpret_cast<const float2*>(geo + (int64_t)sl * SPK_GEO_STRIDE + 4);   // fc, dfc
+                fc = ok ? f2.x : 0.f;
+                dfc = ok ? f2.y : 0.f;
+                pv = *reinterpret_cast<const float4*>(phi + (int64_t)sl * KP + (q_in ? qc * 4 : 0));
+                dv = *reinterpret_cast<const float4*>(dphi + (int64_t)sl * KP + (q_in ? qc * 4 : 0));
+            }
+            if (pt < NEB) {
+                const int g = pt / EGB;
+                const int pp = s_sb[g] + k * EGB + (pt % EGB);
                 const bool ok = pp < s_se[g];
                 const int sl = pos_slot[ok ? pp : 0];
                 m_i = pos_i[ok ? pp : 0];
@@ -470,64 +476,49 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
                 const float4 g0 = *reinterpret_cast<const float4*>(geo + (int64_t)sl * SPK_GEO_STRIDE);
                 m_u = make_float4(g0.x, g0.y, g0.z, geo[(int64_t)sl * SPK_GEO_STRIDE + 6]);
             }
-#pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                float4 pv[4], dv[4];
-                float fcv[4], dfcv[4];
-                int sl[4];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int r = (half * 4 + i) * 4 + rsub, g = r / EGB;
-                    const int pp = s_sb[g] + k * EGB + (r % EGB);
-                    const bool ok = pp < s_se[g];
-                    sl[i] = pos_slot[ok ? pp : 0];
-                    fcv[i] = ok ? 1.f : 0.f;
-                }
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const float2 f2 = *reinterpret_cast<const float2*>(geo + (int64_t)sl[i] * SPK_GEO_STRIDE + 4);   // fc, dfc
-                    dfcv[i] = f2.y * fcv[i];
-                    fcv[i] *= f2.x;
-                    pv[i] = *reinterpret_cast<const float4*>(phi + (int64_t)sl[i] * KP + (q_in ? qc * 4 : 0));
-                    dv[i] = *reinterpret_cast<const float4*>(dphi + (int64_t)sl[i] * KP + (q_in ? qc * 4 : 0));
-                }
-                if (half == 0 && use >= 1) {
-                    mbar_wait(&empty_bar[st], (use - 1) & 1);
-                    mbar_wait(&meta_empty[st], (use - 1) & 1);
-                }
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int r = (half * 4 + i) * 4 + rsub;
-                    const float fc = fcv[i], dfc = dfcv[i];
-                    float4 v = q_in ? pv[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-                    float4 d = q_in ? dv[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (qc == kb_chunk) {                      // bias column: [phi | 1], [dphi | 0]
-                        if (kb == 0) { v.x = 1.f; d.x = 0.f; } else if (kb == 1) { v.y = 1.f; d.y = 0.f; }
-                        else if (kb == 2) { v.z = 1.f; d.z = 0.f; } else { v.w = 1.f; d.w = 0.f; }
-                    }
-                    float4 w, dw;                              // rows of the W and dW/dd operands
-                    w.x = fc * v.x; w.y = fc * v.y; w.z = fc * v.z; w.w = fc * v.w;
-                    dw.x = fmaf(dfc, v.x, fc * d.x); dw.y = fmaf(dfc, v.y, fc * d.y);
-                    dw.z = fmaf(dfc, v.z, fc * d.z); dw.w = fmaf(dfc, v.w, fc * d.w);
-                    float4 hi, lo;
-                    hi.x = tf32_rn(w.x); hi.y = tf32_rn(w.y); hi.z = tf32_rn(w.z); hi.w = tf32_rn(w.w);
-                    lo.x = w.x - hi.x; lo.y = w.y - hi.y; lo.z = w.z - hi.z; lo.w = w.w - hi.w;
-                    int off = tile_off(r, qc & 3);
-                    *reinterpret_cast<float4*>(stB + (0 * 2 + (qc >> 2)) * B_TILE + off) = hi;
-                    *reinterpret_cast<float4*>(stB + (1 * 2 + (qc >> 2)) * B_TILE + off) = lo;
-                    hi.x = tf32_rn(dw.x); hi.y = tf32_rn(dw.y); hi.z = tf32_rn(dw.z); hi.w = tf32_rn(dw.w);
-                    lo.x = dw.x - hi.x; lo.y = dw.y - hi.y; lo.z = dw.z - hi.z; lo.w = dw.w - hi.w;
-                    off = tile_off(NEB + r, qc & 3);
-                    *reinterpret_cast<float4*>(stB + (0 * 2 + (qc >> 2)) * B_TILE + off) = hi;
-                    *reinterpret_cast<float4*>(stB + (1 * 2 + (qc >> 2)) * B_TILE + off) = lo;
-                }
+        };
+        auto stage = [&](int k) {                              // rows of the W and dW/dd operands
+            const float4 v = with_bias(pv, q_in, qc, n_rbf);   // [phi | 1]
+            float4 d = q_in ? dv : make_float4(0.f, 0.f, 0.f, 0.f);
+            if (qc == (n_rbf >> 2)) {                          // bias column of [dphi | 0]
+                const int kb = n_rbf & 3;
+                if (kb == 0) d.x = 0.f; else if (kb == 1) d.y = 0.f; else if (kb == 2) d.z = 0.f; else d.w = 0.f;
             }
-            st_i[lane] = m_i;
-            st_e[lane] = m_e;
-            st_u[lane] = m_u;
+            float4 w, dw;
+            w.x = fc * v.x; w.y = fc * v.y; w.z = fc * v.z; w.w = fc * v.w;
+            dw.x = fmaf(dfc, v.x, fc * d.x); dw.y = fmaf(dfc, v.y, fc * d.y);
+            dw.z = fmaf(dfc, v.z, fc * d.z); dw.w = fmaf(dfc, v.w, fc * d.w);
+            put_row(sB, e, qc, w);
+            put_row(sB, NEB + e, qc, dw);
+            if (pt < NEB) {
+                uint8_t* m = sMeta + (k % NBUF) * META_B;
+                reinterpret_cast<int*>(m)[pt] = m_i;
+                reinterpret_cast<int*>(m)[NEB + pt] = m_e;
+                reinterpret_cast<float4*>(m + 2 * NEB * 4)[pt] = m_u;
+            }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            wg_bar(PROD_BAR);
+        };
+        const uint32_t aB = smem_u32(sA), bB = smem_u32(sB);
+        if (n_chunks > 0) {
+            load(0);
+            stage(0);
+        }
+        mbar_wait(&a_full, 0);
+        for (int k = 0; k < n_chunks; ++k) {
+            const int b = k % NBUF;
+            const bool more = k + 1 < n_chunks;
+            if (more) load(k + 1);
+            filter_to_tile<NT>(aB, bB, sT + b * T_FLOATS, pt);
             __syncwarp();
-            if (lane == 0) mbar_arrive(&full_bar[st]);
+            if (lane == 0) mbar_arrive(&full_bar[b]);
+            if (warp == W_PROD0 && k < 16) BTRACE(16 + k);
+            if (more) {
+                const int nb = (k + 1) % NBUF, use = (k + 1) / NBUF;
+                if (use >= 1) mbar_wait(&empty_bar[nb], (use - 1) & 1);
+                wg_bar(PROD_BAR);
+                stage(k + 1);
+            }
         }
     } else {
         // =========================================== consumers ===========================================
@@ -564,46 +555,31 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
         };
         if (j < j_hi) load_own(j);
         const int my_idx = ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
-        float* tg = sT + g * 16 * T_LD;                        // this group's [W edge | dW edge][channel] transpose tile
-        const uint32_t aB = smem_u32(sA);
-        mbar_wait(&a_full, 0);
         for (int k = 0; k < n_chunks; ++k) {
-            const int st = k % NST;
+            const int b = k % NBUF;
             if (warp == 0 && k < 16) BTRACE(64 + k);           // consumer 0: starts waiting
-            mbar_wait(&full_bar[st], (k / NST) & 1);           // operand rows and metadata of the chunk
-            const uint32_t bB = smem_u32(sB + st * B_STAGE);
-            float dw[NT][2][4], dd[NT][2][4];
-            filter_mma<NT, 8>(dw, aB, bB + (uint32_t)(g * EGB * SPK_SW64_ROW));           // W rows of the group
-            filter_mma<NT, 8>(dd, aB, bB + (uint32_t)((NEB + g * EGB) * SPK_SW64_ROW));   // dW/dd rows of the group
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty_bar[st]);
-            float wv[3][EGB], dv[3][EGB];
+            mbar_wait(&full_bar[b], (k / NBUF) & 1);           // filter tile and metadata of the chunk
+            if (warp == 0 && k < 16) BTRACE(176 + k);
+            const float* tg = sT + b * T_FLOATS + g * EGB * T_LD + c;   // W rows of the group; dW/dd rows NEB further
+            float Wv[3][EGB], Dv[3][EGB];
 #pragma unroll
-            for (int t = 0; t < NT; ++t) {                     // fragments -> thread = channel, one third at a time
-                frag_to_tile<8>(dw[t], tg, 0, c);
-                frag_to_tile<8>(dd[t], tg, EGB, c);
-                wg_bar(1 + g);
+            for (int t = 0; t < NT; ++t)
 #pragma unroll
                 for (int u = 0; u < EGB; ++u) {
-                    wv[t][u] = tg[u * T_LD + c];
-                    dv[t][u] = tg[(EGB + u) * T_LD + c];
+                    Wv[t][u] = tg[u * T_LD + t * F];
+                    Dv[t][u] = tg[(NEB + u) * T_LD + t * F];
                 }
-                wg_bar(1 + g);
-            }
-            if (warp == 0 && k < 16) BTRACE(80 + k);           // filter values + metadata ready
+            if (warp == 0 && k < 16) BTRACE(80 + k);           // filter values ready
             if (warp == 0 && lane == 0 && k == 0) SPK_TL_PHASE(2);
-            const int* st_i = reinterpret_cast<const int*>(sMeta + st * META_B) + g * EGB;
-            const int* st_e = reinterpret_cast<const int*>(sMeta + st * META_B) + NEB + g * EGB;
-            const float4* st_u = reinterpret_cast<const float4*>(sMeta + st * META_B + 2 * NEB * 4) + g * EGB;
+            const int* st_i = reinterpret_cast<const int*>(sMeta + b * META_B) + g * EGB;
+            const int* st_e = reinterpret_cast<const int*>(sMeta + b * META_B) + NEB + g * EGB;
+            const float4* st_u = reinterpret_cast<const float4*>(sMeta + b * META_B + 2 * NEB * 4) + g * EGB;
             const int base = p_begin + k * EGB;
+            {
+                float gq[EGB], g0[EGB], g1[EGB], g2[EGB];
 #pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                const float *Wa = wv[0] + half * 4, *Wb = wv[1] + half * 4, *Wc = wv[2] + half * 4;
-                const float *Da = dv[0] + half * 4, *Db = dv[1] + half * 4, *Dc = dv[2] + half * 4;
-                float gq[4], g0[4], g1[4], g2[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {                  // rows past the range gather receiver 0; their W, dW are 0
-                    const int i = st_i[half * 4 + u];
+                for (int u = 0; u < EGB; ++u) {                // rows past the range gather receiver 0; their W, dW are 0
+                    const int i = st_i[u];
                     gq[u] = g_q[(size_t)i * F + c];
                     const float* __restrict__ gmi = g_mu + (size_t)i * (3 * F) + c;
                     g0[u] = gmi[0];
@@ -612,9 +588,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
                 }
                 float red[16];
 #pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int t = half * 4 + u;
-                    const int p = base + t;
+                for (int u = 0; u < EGB; ++u) {
+                    const int p = base + u;
                     float part_d = 0.f, pu0 = 0.f, pu1 = 0.f, pu2 = 0.f;
                     if (p < p_end) {
                         if (p >= next_boundary) {
@@ -625,23 +600,23 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
                             } while (p >= next_boundary);
                             load_own(j);
                         }
-                        const float4 ge = st_u[t];                 // ux uy uz 1/d
+                        const float4 ge = st_u[u];                 // ux uy uz 1/d
                         const float gu = g0[u] * ge.x + g1[u] * ge.y + g2[u] * ge.z;
-                        gxa = fmaf(Wa[u], gq[u], gxa);
-                        gxb = fmaf(Wb[u], gu, gxb);
-                        part_d = gq[u] * xa * Da[u] + gu * xb * Db[u];
-                        const float wbx = Wb[u] * xb;
+                        gxa = fmaf(Wv[0][u], gq[u], gxa);
+                        gxb = fmaf(Wv[1][u], gu, gxb);
+                        part_d = gq[u] * xa * Dv[0][u] + gu * xb * Dv[1][u];
+                        const float wbx = Wv[1][u] * xb;
                         pu0 = g0[u] * wbx;
                         pu1 = g1[u] * wbx;
                         pu2 = g2[u] * wbx;
                         if (HAS_MU) {
                             const float gm = g0[u] * m0 + g1[u] * m1 + g2[u] * m2;
-                            gxc = fmaf(Wc[u], gm, gxc);
-                            const float wcx = Wc[u] * xc;
+                            gxc = fmaf(Wv[2][u], gm, gxc);
+                            const float wcx = Wv[2][u] * xc;
                             gm0 = fmaf(wcx, g0[u], gm0);
                             gm1 = fmaf(wcx, g1[u], gm1);
                             gm2 = fmaf(wcx, g2[u], gm2);
-                            part_d = fmaf(gm * xc, Dc[u], part_d);
+                            part_d = fmaf(gm * xc, Dv[2][u], part_d);
                         }
                     }
                     red[4 * u + 0] = part_d;
@@ -650,13 +625,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
                     red[4 * u + 3] = pu2;
                 }
                 const float tot = butterfly16(red, lane);
-                const int te = half * 4 + (my_idx >> 2);
-                if (!(lane & 1)) s_red[k & 1][g][te][qd][my_idx & 3] = tot;
-                if (warp == 0 && k < 16) BTRACE((half ? 128 : 112) + k);   // half done (4 edges + butterfly)
+                if (!(lane & 1)) s_red[k & 1][g][my_idx >> 2][qd][my_idx & 3] = tot;
             }
-            // the four warps of the group have published their partial sums of this chunk's 8 edges
+            // the four warps of the group have published their partial sums of this chunk's edges
             asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");
-            if (warp == 0 && k < 16) BTRACE(144 + k);          // group barrier passed
             if (qd == 0 && lane < EGB && base + lane < p_end) {
                 const int t = lane;
                 float gd = 0.f, u0 = 0.f, u1 = 0.f, u2 = 0.f;
@@ -683,7 +655,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
                 out[2] = r2;
             }
             __syncwarp();
-            if (lane == 0) mbar_arrive(&meta_empty[st]);
+            if (lane == 0) mbar_arrive(&empty_bar[b]);
             if (warp == 0 && k < 16) BTRACE(96 + k);           // chunk done (incl. the g_rij tail of warp qd == 0)
         }
         if (warp == 0 && lane == 0) SPK_TL_PHASE(3);           // main loop done
@@ -721,7 +693,7 @@ extern "C" int spk_painn_edge_fwd_tc(const float* x, const float* mu, const floa
     if (cudaError_t e = once_mu.set(k_painn_edge_fwd_tc<true>, SMEM_BYTES); e != cudaSuccess) return SPK_CUDA_ERR(e);
     if (cudaError_t e = once_nomu.set(k_painn_edge_fwd_tc<false>, SMEM_BYTES); e != cudaSuccess) return SPK_CUDA_ERR(e);
     int64_t nb = spk_num_sms();
-    if (nb > spk_cdiv(n_edges, NE)) nb = spk_cdiv(n_edges, NE);
+    if (nb > spk_cdiv(n_edges, NR)) nb = spk_cdiv(n_edges, NR);
     if (nb > n_atoms) nb = n_atoms;
     if (nb < 1) nb = 1;
     cudaStream_t st = spk_st(stream);
