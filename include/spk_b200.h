@@ -334,6 +334,47 @@ int spk_md_velocity_verlet(float* momenta, float* positions, float* model_positi
                            const float* masses, int64_t n_atoms, float dt, float force_conversion,
                            float position_conversion, int drift, spk_stream_t stream);
 
+/* ---- thermostats of the device MD step (md/simulation_hooks/thermostats.py:149-513, md/system.py:374-421).  Applied to the
+ * momenta before the first and after the second half kick (md/simulator.py:127-150).  Systems are those of a collated batch:
+ * idx_m [n_atoms] int64 sorted, sys_ptr [n_sys+1] int32 (spk_segment_ptr); masses [n_atoms] fp32; momenta [n_atoms,3] fp32
+ * in place.  Every per-system sum is accumulated in fp64 in a fixed order (no atomics): bitwise reproducible.
+ * workspace: spk_md_thermostat_workspace_bytes(n_atoms, n_sys) bytes, 8-byte aligned, no initialisation needed.
+ *   spk_md_kinetic_energy  ke[s] = 1/2 sum_{a in s} |p_a|^2 / m_a, temperature[s] = 2 ke[s] / (3 n_s kB)  (fp64, nullable)
+ *   spk_md_berendsen       p *= sqrt(1 + dt_over_tau (temperature_bath / T_s - 1)) per system (unchanged where T_s = 0)
+ *   spk_md_nhc             Nose-Hoover chains (:398-468) propagated with params, p *= the chain's scaling.  Chain state
+ *                          chain_v, chain_f, chain_m [n_chain, chain_length] fp64, n_chain = n_sys, or 3 n_atoms when
+ *                          massive (one chain per degree of freedom, row 3a+d; idx_m / sys_ptr / workspace unused then).
+ *                          chain_m holds the thermostat masses (:375-396); velocities and forces start at zero and are
+ *                          advanced in place.
+ *   spk_md_langevin        p = c1 p + c2 sqrt(m kb_temperature) xi, xi ~ N(0,1) from Philox4x32-10 with key = seed and
+ *                          counter = (atom index, counter[0]) through Box-Muller (normals 0..2 of the draw for x, y, z).
+ *                          counter [2] uint64 on the DEVICE: [0] = application index, advanced by one in stream order by
+ *                          every call (so a replayed graph draws fresh noise each time), [1] = 0 (internal ticket).
+ *   spk_philox4x32_10      out[4 i + k] = word k of the Philox4x32-10 draw for element i, application counter[0], key
+ *                          seed (counter not advanced): the raw bits behind spk_md_langevin. */
+typedef struct {
+    int32_t chain_length;  /* >= 1 */
+    int32_t multi_step;    /* >= 1 */
+    int32_t order;         /* Yoshida-Suzuki order 3, 5 or 7 = entries of time_step used */
+    int32_t massive;       /* 0: one chain per system, 1: one chain per degree of freedom */
+    double kb_temperature; /* kB * T_bath in MD energy units */
+    double time_step[7];   /* dt * w_k / multi_step, w = Yoshida-Suzuki weights (md/utils/thermostat_utils.py:18-44) */
+} spk_nhc_params_t;
+
+size_t spk_md_thermostat_workspace_bytes(int64_t n_atoms, int64_t n_sys);
+int spk_md_kinetic_energy(const float* momenta, const float* masses, const int64_t* idx_m, const int32_t* sys_ptr,
+                          int64_t n_atoms, int64_t n_sys, double kB, double* ke, double* temperature, void* workspace,
+                          size_t workspace_bytes, spk_stream_t stream);
+int spk_md_berendsen(float* momenta, const float* masses, const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms,
+                     int64_t n_sys, double kB, double dt_over_tau, double temperature_bath, void* workspace,
+                     size_t workspace_bytes, spk_stream_t stream);
+int spk_md_nhc(float* momenta, const float* masses, const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms,
+               int64_t n_sys, const spk_nhc_params_t* params, double* chain_v, double* chain_f, const double* chain_m,
+               void* workspace, size_t workspace_bytes, spk_stream_t stream);
+int spk_md_langevin(float* momenta, const float* masses, int64_t n_atoms, double c1, double c2, double kb_temperature,
+                    uint64_t seed, uint64_t* counter, spk_stream_t stream);
+int spk_philox4x32_10(uint64_t seed, const uint64_t* counter, int64_t n, uint32_t* out, spk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, Structure, c_float, c_int, c_int32, c_int64, c_size_t, c_void_p
+from ctypes import POINTER, Structure, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint64, c_void_p
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SPK_B200_LIB") or os.path.join(HERE, "csrc", "libspk_b200.so")   # override: A/B builds
@@ -31,6 +31,12 @@ class ChainStep(Structure):
                 ("ld_add", c_int64), ("A", c_void_p), ("a_pre", c_void_p), ("Wp", c_void_p), ("bias", c_void_p),
                 ("addend", c_void_p), ("Y", c_void_p), ("y_pre", c_void_p), ("g0", c_void_p), ("g1", c_void_p),
                 ("g2", c_void_p), ("g3", c_void_p), ("o0", c_void_p), ("o1", c_void_p)]
+
+
+class NHCParams(Structure):
+    """spk_nhc_params_t of include/spk_b200.h."""
+    _fields_ = [("chain_length", c_int32), ("multi_step", c_int32), ("order", c_int32), ("massive", c_int32),
+                ("kb_temperature", c_double), ("time_step", c_double * 7)]
 
 
 # name -> argument ctypes (return type is int unless listed in _RESTYPE)
@@ -83,11 +89,18 @@ SIGNATURES = {
     "spk_md_velocity_verlet": [P, P, P, P, P, c_int64, c_float, c_float, c_float, c_int, P],
     "spk_neighbor_list_workspace_bytes": [c_int64, c_int64],
     "spk_neighbor_list": [P, P, P, P, c_int64, c_int64, c_float, c_int64, c_int, P, P, P, P, P, P, c_size_t, P],
+    "spk_md_thermostat_workspace_bytes": [c_int64, c_int64],
+    "spk_md_kinetic_energy": [P, P, P, P, c_int64, c_int64, c_double, P, P, P, c_size_t, P],
+    "spk_md_berendsen": [P, P, P, P, c_int64, c_int64, c_double, c_double, c_double, P, c_size_t, P],
+    "spk_md_nhc": [P, P, P, P, c_int64, c_int64, POINTER(NHCParams), P, P, P, P, c_size_t, P],
+    "spk_md_langevin": [P, P, c_int64, c_double, c_double, c_double, c_uint64, P, P],
+    "spk_philox4x32_10": [c_uint64, P, c_int64, P, P],
 }
 _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_size_t,
             "spk_tc_packed_floats_tn": c_size_t, "spk_atom_chain_workspace_ints": c_size_t,
             "spk_schnet_filter_packed_floats": c_size_t,
-            "spk_painn_filter_packed_floats": c_size_t, "spk_neighbor_list_workspace_bytes": c_size_t}
+            "spk_painn_filter_packed_floats": c_size_t, "spk_neighbor_list_workspace_bytes": c_size_t,
+            "spk_md_thermostat_workspace_bytes": c_size_t}
 
 _lib = None
 
@@ -126,7 +139,8 @@ def check(rc: int, name: str):
 
 
 # kernels launched per C-ABI call (default 1); bench.py reports the running total as ``gpu_launches``
-LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out": 2, "spk_neighbor_list": 6}
+LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out": 2, "spk_neighbor_list": 6,
+            "spk_md_kinetic_energy": 2, "spk_md_berendsen": 3}
 launch_count = 0
 
 
