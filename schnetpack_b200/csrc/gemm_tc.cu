@@ -11,7 +11,7 @@
 //     round-to-nearest (wg_ktile_3xtf32, wgmma.cuh).
 //
 // Warp-specialised pipeline, one CTA per 128 x TN output tile:
-//   warps 8..   producers: K-tile kt belongs to warp kt % NPROD and stage kt % NST (NPROD divides NST).  Lane 0 arms
+//   warps 8-11  producers: K-tile kt belongs to warp kt % NPROD and stage kt % NST (NPROD divides NST).  Lane 0 arms
 //               full[stage] with the byte count of the weight tile and issues ONE TMA bulk copy (cp.async.bulk) of the
 //               pre-packed W_hi|W_lo operand tile (the weights are static, so the host packs them once in the exact
 //               shared-memory operand layout, spk_tc_pack_weight); all lanes load the A tile with coalesced 128-bit loads
@@ -19,8 +19,9 @@
 //               64-byte swizzle (row = 64 B, 8-row atoms of 512 B, 16 B chunk index XOR row bits [1,3));
 //               fence.proxy.async; arrive on full[stage];
 //   warps 0-7   two consumer warpgroups, rows 0-63 and 64-127 of the tile: wait full[stage], issue the stage's wgmma
-//               (m64n64k8, TN / 64 column blocks), accumulate in registers, arrive on empty[stage]; after the last K-tile
-//               the raw tile is staged in shared memory (the pipeline stages are free by then);
+//               (m64n64k8, one commit group per 64-column block), add each completed group to the register sum while
+//               the next one runs, arrive on empty[stage]; after the last K-tile the raw tile is staged in shared
+//               memory (the pipeline stages are free by then);
 //   all warps   epilogue: bias / activation (+ saved derivative) / addend / stores, 16 B per thread, whole 128 B lines
 //               per row segment.
 #include "wgmma.cuh"
@@ -38,10 +39,12 @@ constexpr int OPER_A = TM * TK * 4;            // 8192 B: A tile, K-major, SWIZZ
 
 template <int TN>
 struct Cfg {
-    static constexpr int NST = TN == 64 ? 7 : 6;           // shared-memory stages
-    static constexpr int NPROD = NST;                       // producer warps; NPROD divides NST, so all uses of a stage belong
+    static constexpr int NST = TN == 64 ? 8 : 4;           // shared-memory stages (8 x 32 KB would not fit at TN = 128)
+    static constexpr int NPROD = 4;                         // producer warps; NPROD divides NST, so all uses of a stage belong
                                                             // to ONE warp and are strictly ordered (a parity wait cannot
-                                                            // tell phase u from phase u+2)
+                                                            // tell phase u from phase u+2).  384 threads leave the
+                                                            // consumers' sum and two fresh accumulators (128 floats at
+                                                            // TN = 128) room in registers without spills
     static constexpr int OPER_B = TN * TK * 4;              // weight tile, same layout as the A tile
     static constexpr int STAGE_BYTES = 2 * OPER_A + 2 * OPER_B;   // A_hi, A_lo, W_hi, W_lo
     static constexpr int EP_LD = TN + 4;                    // padded row of the epilogue staging tile (floats)
@@ -216,21 +219,57 @@ __global__ void __launch_bounds__(Cfg<TN>::NTHREADS, 1) k_dense_tc(TcArgs g) {
         }
     } else {
         // =========================================== consumers: wgmma, fp32 accumulation in registers ===========================
+        // The work is a sequence of units u = (K-tile u / NB, column block u % NB), each one wgmma group into a fresh
+        // accumulator.  Two fresh accumulators alternate: unit u + 1 is on the tensor core while unit u is added to its
+        // column block's sum, so the tensor core is not drained between units.  Each column block still receives its
+        // K-tiles in ascending order, one fresh accumulator per K-tile (the numerics of wg_ktile_3xtf32).
         const int wg = warp >> 2;                        // rows wg * 64 .. wg * 64 + 63 of the tile
-        float acc[NB][32];
+        float acc[NB][32], t0[32], t1[32];
 #pragma unroll
-        for (int cb = 0; cb < NB; ++cb)
+        for (int i = 0; i < 32; ++i) {
 #pragma unroll
-            for (int i = 0; i < 32; ++i) acc[cb][i] = 0.f;
-        for (int kt = 0; kt < nk; ++kt) {
-            const int s = kt % NST;
-            mbar_wait(&full_bar[s], (kt / NST) & 1);
-            const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
-            wg_ktile_3xtf32<NB>(acc, sa + wg * SPK_WG_ROWS_BYTES, sa + OPER_A + wg * SPK_WG_ROWS_BYTES, sa + 2 * OPER_A,
-                                sa + 2 * OPER_A + OPER_B);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty_bar[s]);
-            if (warp == 0 && lane == 0 && (kt == 0 || kt == nk - 1)) SPK_TL_PHASE(kt == 0 ? 4 : 5);
+            for (int cb = 0; cb < NB; ++cb) acc[cb][i] = 0.f;
+            t0[i] = t1[i] = 0.f;                         // defined operands; each unit's first product overwrites them
+        }
+        const int nu = nk * NB;
+        auto issue = [&](float (&t)[32], int u) {
+            const int kt = u / NB, cb = u % NB, s = kt % NST;
+            if (cb == 0) mbar_wait(&full_bar[s], (kt / NST) & 1);
+            const uint32_t sa = smem_u32(smem + s * STAGE_BYTES), bo = (uint32_t)(cb * SPK_WG_ROWS_BYTES);
+            wg_ktile_3xtf32_issue(t, sa + wg * SPK_WG_ROWS_BYTES, sa + OPER_A + wg * SPK_WG_ROWS_BYTES,
+                                  sa + 2 * OPER_A + bo, sa + 2 * OPER_A + OPER_B + bo);
+        };
+        auto retire = [&](const float (&t)[32], float (&a)[32], int u) {   // unit u has completed
+#pragma unroll
+            for (int i = 0; i < 32; ++i) a[i] += t[i];
+            const int kt = u / NB;
+            if (u % NB == NB - 1) {                      // every wgmma that read this K-tile's stage has completed
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[kt % NST]);
+                if (warp == 0 && lane == 0 && (kt == 0 || kt == nk - 1)) SPK_TL_PHASE(kt == 0 ? 4 : 5);
+            }
+        };
+        // u is even: t0 holds column block 0 and t1 column block NB - 1 (both block 0 when NB == 1).  The loop body issues
+        // unconditionally (a conditional issue makes ptxas serialise every wgmma of the kernel); the tail is peeled.
+        issue(t0, 0);
+        int u = 0;
+        for (; u + 2 < nu; u += 2) {
+            issue(t1, u + 1);
+            wgmma_wait<1>();
+            retire(t0, acc[0], u);
+            issue(t0, u + 2);
+            wgmma_wait<1>();
+            retire(t1, acc[NB - 1], u + 1);
+        }
+        if (u + 1 < nu) {
+            issue(t1, u + 1);
+            wgmma_wait<1>();
+            retire(t0, acc[0], u);
+            wgmma_wait<0>();
+            retire(t1, acc[NB - 1], u + 1);
+        } else {
+            wgmma_wait<0>();
+            retire(t0, acc[0], u);
         }
         // both warpgroups have completed every wgmma (and the producers every store): the stages now hold the raw tile
         wg_bar(1, N_CONS * 32);

@@ -103,11 +103,27 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b
 }
 #undef SPK_WGMMA_PRE
 
-// One K-tile (16 floats = 2 k-steps) of a dense layer in 3xTF32 on the calling warpgroup: its 64 rows of A (a_hi / a_lo:
-// shared addresses of the warpgroup's first operand row) times NB column blocks of 64 rows of W (b_hi / b_lo: tile start).
-// The tensor core truncates when it accumulates, which biases long K-sums toward zero; so the three products of the tile
-// (small terms first: Al*Wh, Ah*Wl, then Ah*Wh) go into a FRESH accumulator that is added to `acc` in fp32 with
-// round-to-nearest, and the truncation never runs over more than one K-tile.
+// Issue the 3xTF32 products of one K-tile (16 floats = 2 k-steps) for one 64-column block on the calling warpgroup and
+// commit them as ONE wgmma group, without waiting: its 64 rows of A (a_hi / a_lo: shared addresses of the warpgroup's
+// first operand row) times 64 rows of W (b_hi / b_lo).  The tensor core truncates when it accumulates, which biases long
+// K-sums toward zero; so the three products of the tile (small terms first: Al*Wh, Ah*Wl, then Ah*Wh) go into the FRESH
+// accumulator t (the first product overwrites it), which the caller adds to its fp32 sum with round-to-nearest once the
+// group has completed: the truncation never runs over more than one K-tile.
+__device__ __forceinline__ void wg_ktile_3xtf32_issue(float (&t)[32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
+                                                      uint32_t b_lo) {
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+        wgmma_n64(t, make_desc(a_lo + 32 * ks), make_desc(b_hi + 32 * ks), ks);
+        wgmma_n64(t, make_desc(a_hi + 32 * ks), make_desc(b_lo + 32 * ks), 1);
+    }
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) wgmma_n64(t, make_desc(a_hi + 32 * ks), make_desc(b_hi + 32 * ks), 1);
+    wgmma_commit();
+}
+
+// One K-tile for NB column blocks of 64 rows of W (b_hi / b_lo: tile start), each block issued, drained and added to
+// acc[cb] in turn (wg_ktile_3xtf32_issue).
 template <int NB>
 __device__ __forceinline__ void wg_ktile_3xtf32(float (&acc)[NB][32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
                                                 uint32_t b_lo) {
@@ -117,15 +133,7 @@ __device__ __forceinline__ void wg_ktile_3xtf32(float (&acc)[NB][32], uint32_t a
 #pragma unroll
         for (int i = 0; i < 32; ++i) t[i] = 0.f;
         const uint32_t bo = (uint32_t)(cb * SPK_WG_ROWS_BYTES);
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) {
-            wgmma_n64(t, make_desc(a_lo + 32 * ks), make_desc(b_hi + bo + 32 * ks), ks);
-            wgmma_n64(t, make_desc(a_hi + 32 * ks), make_desc(b_lo + bo + 32 * ks), 1);
-        }
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) wgmma_n64(t, make_desc(a_hi + 32 * ks), make_desc(b_hi + bo + 32 * ks), 1);
-        wgmma_commit();
+        wg_ktile_3xtf32_issue(t, a_hi, a_lo, b_hi + bo, b_lo + bo);
         wgmma_wait_all();
 #pragma unroll
         for (int i = 0; i < 32; ++i) acc[cb][i] += t[i];
