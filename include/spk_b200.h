@@ -375,6 +375,77 @@ int spk_md_langevin(float* momenta, const float* masses, int64_t n_atoms, double
                     uint64_t seed, uint64_t* counter, spk_stream_t stream);
 int spk_philox4x32_10(uint64_t seed, const uint64_t* counter, int64_t n, uint32_t* out, spk_stream_t stream);
 
+/* ---- per-system virial (csrc/geometry.cu): W[m][b][a] = sum_{e in m} g_rij[e][b] * r_ij[e][a] in fp64, the strain
+ * derivative dE/d(strain) of atomistic/response.py:78-90 (Strain maps r_e -> r_e (1 + strain^T)); the stress is W / V.
+ * The edges of system m are the receiver slots [rowptr[sys_ptr[m]], rowptr[sys_ptr[m+1]]) of the graph view of
+ * spk_graph_build, mapped to edge ids by slot_eid; sys_ptr [n_sys+1] int32 = first atom of every system
+ * (spk_segment_ptr).  g_rij, r_ij [n_edges,3] fp32 in edge order; virial [n_sys,3,3] fp64, overwritten.  Reduced with
+ * fixed-shape CTA partials and an ordered per-system pass (no atomics): bitwise reproducible for any mix of system sizes.
+ * workspace: spk_pairwise_virial_workspace_bytes(n_edges, n_sys) bytes, 8-byte aligned, no initialisation needed. */
+size_t spk_pairwise_virial_workspace_bytes(int64_t n_edges, int64_t n_sys);
+int spk_pairwise_virial(const float* g_rij, const float* r_ij, const int32_t* rowptr, const int32_t* slot_eid,
+                        const int32_t* sys_ptr, int64_t n_edges, int64_t n_sys, double* virial, void* workspace,
+                        size_t workspace_bytes, spk_stream_t stream);
+
+/* ---- Nose-Hoover-chain barostats of the device MD step (csrc/barostat.cu; md/simulation_hooks/barostats.py:162-927 with
+ * md/integrators.py:232-263 NPTVelocityVerlet).  Systems, masses and momenta as for the thermostats above; positions
+ * [n_atoms,3] fp32 in MD units; cell [n_sys,3,3] fp64 in MD units (rows = lattice vectors).  One step (simulator.py:124-150):
+ * thermostat, kick, half_step, main_step, forces + virial, half_step, kick, thermostat.
+ * workspace: spk_md_barostat_workspace_bytes(n_atoms, n_sys) bytes, 8-byte aligned, no initialisation needed; the operators
+ * of half_step / main_step live there between their two launches only.
+ *   spk_md_kinetic_energy_tensor  ke_tensor[s] = 1/2 sum_{a in s} p_a p_a^T / m_a  [n_sys,3,3] fp64 (system.py:389-404)
+ *   spk_md_barostat_thermostat    _update_thermostat (:408-481): the particle chains (per system, or per degree of freedom
+ *                                 when massive) scale the momenta, the cell chain (per system) scales b_v
+ *   spk_md_barostat_kick          _update_barostat (:604-631 isotropic, :822-842 anisotropic): b_f from the pressure with
+ *                                 stress = virial_scale * virial / V (virial [n_sys,3,3] fp64, V = det(cell)), then
+ *                                 b_v += 1/2 dt b_f
+ *   spk_md_barostat_half_step     propagate_half_step (:661-686, :885-926): p = p A + 1/2 dt (forces * force_conversion) B
+ *   spk_md_barostat_main_step     propagate_main_step (:633-659, :844-883): x = x A + dt (p / m) B, cell scaled (isotropic:
+ *                                 cell * exp(dt b_v); anisotropic: cell @ A), model_cell [n_sys,3,3] fp32 = cell *
+ *                                 position_conversion and model_positions = x * position_conversion (both nullable).
+ * The anisotropic operators come from a per-system fp64 Jacobi eigendecomposition of b_v that reads its upper triangle (as
+ * torch.symeig(upper=True) did).  sinh(x)/x is md/utils/thermostat_utils.py:181-201 StableSinhDiv exactly as written. */
+typedef struct {
+    int32_t anisotropic;     /* 0: one cell velocity per system (b_v, b_f [n_sys]); 1: 3x3 (b_v, b_f [n_sys,3,3]) */
+    int32_t massive;         /* 0: one particle chain per system; 1: one per degree of freedom (row 3a+d) */
+    int32_t chain_length;    /* >= 1, both chains */
+    int32_t multi_step;      /* >= 1 */
+    int32_t order;           /* Yoshida-Suzuki order 3, 5 or 7 = entries of ys_time_step used */
+    int32_t reserved;
+    double kb_temperature;   /* kB * T_bath in MD energy units */
+    double time_step;        /* dt in MD time units */
+    double target_pressure;  /* P0 in MD pressure units (energy / length^3) */
+    double ys_time_step[7];  /* dt * w_k / multi_step */
+    double* t_v;             /* particle chains [n_chain, chain_length] fp64: velocities, forces, masses */
+    double* t_f;
+    const double* t_m;
+    double* c_v;             /* cell chain [n_sys, chain_length] fp64 */
+    double* c_f;
+    const double* c_m;
+    double* b_v;             /* cell velocities, forces [n_sys] or [n_sys,3,3], masses [n_sys] fp64 */
+    double* b_f;
+    const double* b_m;
+} spk_nhc_barostat_t;
+
+size_t spk_md_barostat_workspace_bytes(int64_t n_atoms, int64_t n_sys);
+int spk_md_kinetic_energy_tensor(const float* momenta, const float* masses, const int64_t* idx_m, const int32_t* sys_ptr,
+                                 int64_t n_atoms, int64_t n_sys, double* ke_tensor, void* workspace,
+                                 size_t workspace_bytes, spk_stream_t stream);
+int spk_md_barostat_thermostat(const spk_nhc_barostat_t* barostat, float* momenta, const float* masses,
+                               const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms, int64_t n_sys,
+                               void* workspace, size_t workspace_bytes, spk_stream_t stream);
+int spk_md_barostat_kick(const spk_nhc_barostat_t* barostat, const float* momenta, const float* masses,
+                         const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms, int64_t n_sys, const double* cell,
+                         const double* virial, double virial_scale, void* workspace, size_t workspace_bytes,
+                         spk_stream_t stream);
+int spk_md_barostat_half_step(const spk_nhc_barostat_t* barostat, float* momenta, const float* forces,
+                              double force_conversion, const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms,
+                              int64_t n_sys, void* workspace, size_t workspace_bytes, spk_stream_t stream);
+int spk_md_barostat_main_step(const spk_nhc_barostat_t* barostat, float* positions, float* model_positions,
+                              const float* momenta, const float* masses, const int64_t* idx_m, const int32_t* sys_ptr,
+                              int64_t n_atoms, int64_t n_sys, double* cell, float* model_cell, double position_conversion,
+                              void* workspace, size_t workspace_bytes, spk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

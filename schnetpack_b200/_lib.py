@@ -8,6 +8,7 @@ from __future__ import annotations
 import ctypes
 import os
 from ctypes import POINTER, Structure, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint64, c_void_p
+from typing import Optional
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SPK_B200_LIB") or os.path.join(HERE, "csrc", "libspk_b200.so")   # override: A/B builds
@@ -37,6 +38,15 @@ class NHCParams(Structure):
     """spk_nhc_params_t of include/spk_b200.h."""
     _fields_ = [("chain_length", c_int32), ("multi_step", c_int32), ("order", c_int32), ("massive", c_int32),
                 ("kb_temperature", c_double), ("time_step", c_double * 7)]
+
+
+class NHCBarostat(Structure):
+    """spk_nhc_barostat_t of include/spk_b200.h (parameters and device pointers of the chain / cell state)."""
+    _fields_ = [("anisotropic", c_int32), ("massive", c_int32), ("chain_length", c_int32), ("multi_step", c_int32),
+                ("order", c_int32), ("reserved", c_int32), ("kb_temperature", c_double), ("time_step", c_double),
+                ("target_pressure", c_double), ("ys_time_step", c_double * 7),
+                ("t_v", c_void_p), ("t_f", c_void_p), ("t_m", c_void_p), ("c_v", c_void_p), ("c_f", c_void_p),
+                ("c_m", c_void_p), ("b_v", c_void_p), ("b_f", c_void_p), ("b_m", c_void_p)]
 
 
 # name -> argument ctypes (return type is int unless listed in _RESTYPE)
@@ -95,8 +105,18 @@ SIGNATURES = {
     "spk_md_nhc": [P, P, P, P, c_int64, c_int64, POINTER(NHCParams), P, P, P, P, c_size_t, P],
     "spk_md_langevin": [P, P, c_int64, c_double, c_double, c_double, c_uint64, P, P],
     "spk_philox4x32_10": [c_uint64, P, c_int64, P, P],
+    "spk_pairwise_virial_workspace_bytes": [c_int64, c_int64],
+    "spk_pairwise_virial": [P, P, P, P, P, c_int64, c_int64, P, P, c_size_t, P],
+    "spk_md_barostat_workspace_bytes": [c_int64, c_int64],
+    "spk_md_kinetic_energy_tensor": [P, P, P, P, c_int64, c_int64, P, P, c_size_t, P],
+    "spk_md_barostat_thermostat": [POINTER(NHCBarostat), P, P, P, P, c_int64, c_int64, P, c_size_t, P],
+    "spk_md_barostat_kick": [POINTER(NHCBarostat), P, P, P, P, c_int64, c_int64, P, P, c_double, P, c_size_t, P],
+    "spk_md_barostat_half_step": [POINTER(NHCBarostat), P, P, c_double, P, P, c_int64, c_int64, P, c_size_t, P],
+    "spk_md_barostat_main_step": [POINTER(NHCBarostat), P, P, P, P, P, P, c_int64, c_int64, P, P, c_double, P, c_size_t,
+                                  P],
 }
 _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_size_t,
+            "spk_pairwise_virial_workspace_bytes": c_size_t, "spk_md_barostat_workspace_bytes": c_size_t,
             "spk_tc_packed_floats_tn": c_size_t, "spk_atom_chain_workspace_ints": c_size_t,
             "spk_schnet_filter_packed_floats": c_size_t,
             "spk_painn_filter_packed_floats": c_size_t, "spk_neighbor_list_workspace_bytes": c_size_t,
@@ -140,12 +160,15 @@ def check(rc: int, name: str):
 
 # kernels launched per C-ABI call (default 1); bench.py reports the running total as ``gpu_launches``
 LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out": 2, "spk_neighbor_list": 6,
-            "spk_md_kinetic_energy": 2, "spk_md_berendsen": 3}
+            "spk_md_kinetic_energy": 2, "spk_md_berendsen": 3, "spk_pairwise_virial": 2,
+            "spk_md_kinetic_energy_tensor": 3, "spk_md_barostat_thermostat": 4, "spk_md_barostat_kick": 3,
+            "spk_md_barostat_half_step": 2, "spk_md_barostat_main_step": 2}
 launch_count = 0
 
 
-def call(name: str, *args):
+def call(name: str, *args, launches: Optional[int] = None):
+    """``launches``: kernels this call enqueues when it differs from the entry point's usual count in LAUNCHES"""
     global launch_count
     rc = getattr(lib(), name)(*args)
     check(rc, name)
-    launch_count += LAUNCHES.get(name, 1)
+    launch_count += LAUNCHES.get(name, 1) if launches is None else launches

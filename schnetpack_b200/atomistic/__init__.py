@@ -20,11 +20,21 @@ __all__ = ["PairwiseDistances", "Atomwise", "Forces", "Strain"]
 
 class PairwiseDistances(nn.Module):
     """Rij = R[idx_j] - R[idx_i] + offsets (distances.py:14-26).  The backward assembles dE/dR per atom from the
-    receiver- and sender-grouped edge views (deterministic; the reference uses index_put atomics)."""
+    receiver- and sender-grouped edge views (deterministic; the reference uses index_put atomics).
+
+    Virial on request: with a caller-owned fp64 ``[n_sys, 3, 3]`` CUDA tensor under ``properties.virial`` the backward also
+    writes W[m] = sum_{e in m} dE/dr_e (x) r_e into it (fp64 sums in a fixed order), so that stress = W / V without a strain
+    leaf.  This costs one ``spk_segment_ptr`` launch in the forward and the two launches of ``spk_pairwise_virial`` (plus
+    its small workspace) in the backward; the buffer is only written when a backward runs, so the evaluation needs grad
+    mode and positions that require grad.  Without the key nothing changes."""
 
     @ops.on_tensor_device
     def forward(self, inputs: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        virial = inputs.get(properties.virial)
         if self.training and torch.is_grad_enabled():     # training graph: differentiable twice (functional_torch)
+            if virial is not None:
+                raise ValueError(f"PairwiseDistances: the '{properties.virial}' output is computed by the CUDA kernels "
+                                 "only; evaluate the model in eval() mode (or under no trainable parameters) to get it")
             from .. import functional_torch as T
 
             return T.pairwise(inputs)
@@ -35,8 +45,20 @@ class PairwiseDistances(nn.Module):
         graph = ops.get_graph(inputs[properties.idx_i] if inputs[properties.idx_i].dtype == torch.int64 else idx_i,
                               inputs[properties.idx_j] if inputs[properties.idx_j].dtype == torch.int64 else idx_j,
                               R.shape[0])
-        inputs[properties.Rij] = K.PairwiseDistancesFunction.apply(
-            R, offsets, dict(idx_i=idx_i.contiguous(), idx_j=idx_j.contiguous(), graph=graph))
+        holder = dict(idx_i=idx_i.contiguous(), idx_j=idx_j.contiguous(), graph=graph)
+        if virial is not None:
+            idx_m = inputs[properties.idx_m]
+            off_grad = offsets is not None and offsets.requires_grad
+            if not (torch.is_grad_enabled() and (R.requires_grad or off_grad)):
+                raise ValueError(f"PairwiseDistances: '{properties.virial}' is filled by the backward pass; evaluate with "
+                                 "grad enabled and positions that require grad (a Forces output does both)")
+            if (not virial.is_cuda or virial.dtype != torch.float64 or not virial.is_contiguous() or virial.dim() != 3
+                    or virial.shape[1:] != (3, 3) or virial.device != R.device):
+                raise ValueError(f"PairwiseDistances: '{properties.virial}' must be a contiguous float64 [n_sys, 3, 3] "
+                                 f"tensor on {R.device}")
+            idx_m = idx_m if idx_m.dtype == torch.int64 else idx_m.long()
+            holder.update(virial=virial, sys_ptr=ops.segment_ptr(idx_m.contiguous(), virial.shape[0]))
+        inputs[properties.Rij] = K.PairwiseDistancesFunction.apply(R, offsets, holder)
         return inputs
 
 

@@ -1,7 +1,7 @@
 // Edge geometry, radial basis, cutoff, embedding and force assembly kernels (HBM-bound elementwise / segmented work).
 // Reference: atomistic/distances.py:14-26, representation/painn.py:227-230, schnet.py:156-158, nn/radial.py,
 // nn/cutoff.py:14-33, nn/activations.py:9-22, nn/scatter.py:26-34.
-#include "common.cuh"
+#include "segscan.cuh"
 
 namespace {
 
@@ -200,6 +200,58 @@ __global__ void k_velocity_verlet(float* __restrict__ momenta, float* __restrict
     }
 }
 
+// Per-system virial W_m[b][a] = sum_{e in m} g_e[b] r_e[a] (the strain derivative of atomistic/response.py:78-90 without the
+// 1/V).  The edges of system m are the receiver slots [rowptr[sys_ptr[m]], rowptr[sys_ptr[m+1]]); CTAs take VIR_T
+// consecutive slots, reduce them with a fixed-shape segmented scan in fp64 and leave one partial per (system, CTA) pair, which
+// k_seg_finish adds in a fixed order -- the scheme of the kinetic-energy sums in thermostat.cu, so the result is bitwise the
+// same on every call for any mix of system sizes.  Padding pairs (distance 2 cutoff) have g_e = 0 and add nothing.
+constexpr int VIR_T = 256;
+
+__device__ __forceinline__ int64_t slot_of_sys(const int* __restrict__ rowptr, const int* __restrict__ sys_ptr, int64_t m) {
+    return rowptr[sys_ptr[m]];
+}
+
+__global__ void __launch_bounds__(VIR_T) k_virial_partials(const float* __restrict__ g, const float* __restrict__ r,
+                                                           const int* __restrict__ rowptr, const int* __restrict__ slot_eid,
+                                                           const int* __restrict__ sys_ptr, int64_t n_sys,
+                                                           double* __restrict__ sys_part, double* __restrict__ head) {
+    __shared__ double sv[9][VIR_T];
+    __shared__ int sf[VIR_T];
+    SPK_PDL_ENTER();
+    const int t = threadIdx.x;
+    const int64_t b0 = (int64_t)blockIdx.x * VIR_T;
+    const int64_t s = b0 + t;
+    const int64_t n_slots = slot_of_sys(rowptr, sys_ptr, n_sys);
+    double v[9];
+    int f = 1;
+    int64_t m = -1;
+#pragma unroll
+    for (int c = 0; c < 9; ++c) v[c] = 0.0;
+    if (s < n_slots) {
+        int64_t lo = 0, hi = n_sys;   // last system whose first slot is <= s (skips empty systems)
+        while (lo < hi) {
+            const int64_t mid = (lo + hi + 1) >> 1;
+            if (slot_of_sys(rowptr, sys_ptr, mid) <= s) lo = mid;
+            else hi = mid - 1;
+        }
+        m = lo;
+        const int64_t e = slot_eid[s];
+        const double gx = g[3 * e], gy = g[3 * e + 1], gz = g[3 * e + 2];
+        const double rx = r[3 * e], ry = r[3 * e + 1], rz = r[3 * e + 2];
+        v[0] = gx * rx; v[1] = gx * ry; v[2] = gx * rz;
+        v[3] = gy * rx; v[4] = gy * ry; v[5] = gy * rz;
+        v[6] = gz * rx; v[7] = gz * ry; v[8] = gz * rz;
+        f = (t == 0) || (s == slot_of_sys(rowptr, sys_ptr, m));
+    }
+    seg_scan<VIR_T, 9>(v, f, sv, sf);
+    if (s >= n_slots) return;
+    const bool seg_end = (t == VIR_T - 1) || (s == n_slots - 1) || (s + 1 == slot_of_sys(rowptr, sys_ptr, m + 1));
+    if (!seg_end) return;
+    double* dst = slot_of_sys(rowptr, sys_ptr, m) >= b0 ? sys_part + m * 9 : head + (int64_t)blockIdx.x * 9;
+#pragma unroll
+    for (int c = 0; c < 9; ++c) dst[c] = v[c];
+}
+
 }  // namespace
 
 #define GRID1D(n, T) (unsigned)spk_cdiv((n), (T)), (T), 0, spk_st(stream)
@@ -307,6 +359,29 @@ extern "C" int spk_md_velocity_verlet(float* momenta, float* positions, float* m
     if (!momenta || !forces || (drift && (!positions || !masses))) return SPK_ERR_ARG;
     spk_launch(k_velocity_verlet, GRID1D(n_atoms * 3, 256), momenta, positions, model_positions, forces, masses, n_atoms, dt,
                force_conversion, position_conversion, drift);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" size_t spk_pairwise_virial_workspace_bytes(int64_t n_edges, int64_t n_sys) {
+    const int64_t nb = n_edges > 0 ? spk_cdiv(n_edges, VIR_T) : 0;
+    return sizeof(double) * 9 * (size_t)((n_sys > 0 ? n_sys : 0) + nb + 1);
+}
+
+extern "C" int spk_pairwise_virial(const float* g_rij, const float* r_ij, const int32_t* rowptr, const int32_t* slot_eid,
+                                   const int32_t* sys_ptr, int64_t n_edges, int64_t n_sys, double* virial, void* workspace,
+                                   size_t workspace_bytes, spk_stream_t stream) {
+    if (n_edges < 0 || n_sys <= 0 || n_edges >= (1ll << 31) - 1) return SPK_ERR_ARG;
+    if (!rowptr || !sys_ptr || !virial || !workspace) return SPK_ERR_ARG;
+    if (workspace_bytes < spk_pairwise_virial_workspace_bytes(n_edges, n_sys)) return SPK_ERR_ARG;
+    if (n_edges > 0 && (!g_rij || !r_ij || !slot_eid)) return SPK_ERR_ARG;
+    double* sys_part = reinterpret_cast<double*>(workspace);
+    double* head = sys_part + 9 * n_sys;
+    if (n_edges > 0)
+        spk_launch(k_virial_partials, (unsigned)spk_cdiv(n_edges, VIR_T), VIR_T, 0, spk_st(stream), g_rij, r_ij, rowptr,
+                   slot_eid, sys_ptr, n_sys, sys_part, head);
+    spk_launch(k_seg_finish<VIR_T, 9>, (unsigned)n_sys, SEG_FIN_T, 0, spk_st(stream), rowptr, sys_ptr, sys_part, head,
+               virial);
     SPK_LAUNCH_CHECK();
     return SPK_OK;
 }

@@ -8,7 +8,7 @@
 // continuation).  The per-system pass then adds a system's partials in CTA order.  No atomics touch a sum, so the result is
 // bitwise the same on every call, whatever the size mix of the batch (one 262 144-atom box spans 1024 CTAs, a 1-atom system
 // one).
-#include "common.cuh"
+#include "md_common.cuh"
 
 namespace {
 
@@ -85,34 +85,6 @@ __device__ __forceinline__ double system_sum(const int32_t* __restrict__ sys_ptr
     return acc;
 }
 
-// thermostats.py:398-468 for one chain; v, f, M point at its chain_length entries.  Operation order as in the reference.
-__device__ double nhc_propagate(double ke, double dof, const spk_nhc_params_t& q, double* __restrict__ v,
-                                double* __restrict__ f, const double* __restrict__ M) {
-    const int L = q.chain_length;
-    const double kbt = q.kb_temperature;
-    f[0] = (ke - dof * kbt) / M[0];
-    double scaling = 1.0;
-    for (int ms = 0; ms < q.multi_step; ++ms) {
-        for (int k = 0; k < q.order; ++k) {
-            const double h = q.time_step[k];
-            v[L - 1] += 0.25 * f[L - 1] * h;
-            for (int c = L - 2; c >= 0; --c) {
-                const double coeff = exp(-0.125 * h * v[c + 1]);
-                v[c] = v[c] * (coeff * coeff) + 0.25 * f[c] * coeff * h;
-            }
-            scaling *= exp(-0.5 * h * v[0]);
-            f[0] = (scaling * scaling * ke - dof * kbt) / M[0];
-            for (int c = 0; c < L - 1; ++c) {
-                const double coeff = exp(-0.125 * h * v[c + 1]);
-                v[c] = v[c] * (coeff * coeff) + 0.25 * f[c] * coeff * h;
-                f[c + 1] = (M[c] * (v[c] * v[c]) - kbt) / M[c + 1];
-            }
-            v[L - 1] += 0.25 * f[L - 1] * h;
-        }
-    }
-    return scaling;
-}
-
 // one thread per system: finish the sum, then the temperature (system.py:407-421) and the mode's scaling factor
 __global__ void k_thermo_system(const int32_t* __restrict__ sys_ptr, int64_t n_sys, const double* __restrict__ sys_part,
                                 const double* __restrict__ head, int mode, double kB, double dt_over_tau, double t_bath,
@@ -140,29 +112,6 @@ __global__ void k_thermo_system(const int32_t* __restrict__ sys_ptr, int64_t n_s
         sc = nhc_propagate(2.0 * ke, 3.0 * n, q, chain_v + s * L, chain_f + s * L, chain_m + s * L);   // :489
     }
     scale[s] = sc;
-}
-
-__global__ void k_scale_momenta(float* __restrict__ p, const int64_t* __restrict__ idx_m,
-                                const double* __restrict__ scale, int64_t n) {
-    SPK_PDL_ENTER();
-    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    p[i] = (float)(scale[idx_m[i / 3]] * (double)p[i]);
-}
-
-// massive NHC: one chain per degree of freedom (thermostats.py:348-354,483-487), one thread per chain
-__global__ void k_nhc_massive(float* __restrict__ p, const float* __restrict__ m, int64_t n_dof,
-                              const __grid_constant__ spk_nhc_params_t q,
-                              double* __restrict__ chain_v, double* __restrict__ chain_f,
-                              const double* __restrict__ chain_m) {
-    SPK_PDL_ENTER();
-    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (i >= n_dof) return;
-    const double pi = (double)p[i];
-    const double ke = pi * pi / (double)m[i / 3];
-    const int L = q.chain_length;
-    const double sc = nhc_propagate(ke, 1.0, q, chain_v + i * L, chain_f + i * L, chain_m + i * L);
-    p[i] = (float)(pi * sc);
 }
 
 // ---- Philox4x32-10 (Salmon, Moraes, Dror, Shaw, SC'11) + Box-Muller ---------------------------------------------------

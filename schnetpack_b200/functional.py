@@ -634,14 +634,22 @@ class PairwiseDistancesFunction(torch.autograd.Function):
         ctx.holder = holder
         ctx.off_grad = offsets is not None and offsets.requires_grad
         with ops.device_of(R, idx_i, idx_j):
-            return ops.pairwise_fwd(R.detach().contiguous(), idx_i, idx_j,
+            r_ij = ops.pairwise_fwd(R.detach().contiguous(), idx_i, idx_j,
                                     offsets.detach().contiguous() if offsets is not None else None)
+        if holder.get("virial") is not None:
+            # the virial contracts the edge gradient with r_ij itself: keep the output (no copy, no recompute launch)
+            ctx.save_for_backward(r_ij)
+        return r_ij
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, g_rij):
         g_rij = g_rij.contiguous()
-        graph = ctx.holder["graph"]
+        h = ctx.holder
+        graph = h["graph"]
         with ops.device_of(g_rij):
             g_R = ops.pairwise_bwd(g_rij, graph, 1.0)
+            if h.get("virial") is not None:
+                (r_ij,) = ctx.saved_tensors
+                ops.pairwise_virial(g_rij, r_ij, graph, h["sys_ptr"], h["virial"])
         return g_R, (g_rij if ctx.off_grad else None), None

@@ -24,6 +24,14 @@ second half kick, as the reference's ThermostatHook does at on_step_begin / on_s
 same captured graph.  Systems are those of the batch (``_idx_m`` / ``_n_atoms``); per-system kinetic energies are fp64 sums
 in a fixed order, the chain state of the Nose-Hoover thermostat and the application counter of the Langevin noise live in
 device memory, so a replayed step neither syncs with the host nor repeats its noise.
+
+Constant-pressure runs (DESIGN.md section 9): ``DeviceMD(..., barostat=...)`` with an ``NHCBarostatIsotropic`` or
+``NHCBarostatAnisotropic`` (md/simulation_hooks/barostats.py:162-927) runs the step of NPTVelocityVerlet
+(md/integrators.py:232-263, md/simulator.py:124-150): barostat on_step_begin, half step, main step (positions and cell),
+neighbour list on the new cell, energy + forces + virial, half step, on_step_end -- all in the same captured graph.  The
+virial W = sum_e dE/dr_e (x) r_e comes out of the backward of ``PairwiseDistances`` (one fp64 kernel with a fixed summation
+order); the stress in MD units is W / V * energy_conversion / position_conversion^3 (base_calculator.py:97,218-222) with V
+the volume of the model cell.  ``compute_stress=True`` keeps the same virial up to date in NVE / NVT runs.
 """
 from __future__ import annotations
 
@@ -37,7 +45,8 @@ from . import _lib, ops
 from . import properties as P
 from .neighbors import CellListNeighborList
 
-__all__ = ["DeviceMD", "BerendsenThermostat", "LangevinThermostat", "NHCThermostat", "KB_MD", "FS_MD"]
+__all__ = ["DeviceMD", "BerendsenThermostat", "LangevinThermostat", "NHCThermostat", "NHCBarostatIsotropic",
+           "NHCBarostatAnisotropic", "KB_MD", "FS_MD", "BAR_MD"]
 
 Tensor = torch.Tensor
 
@@ -50,6 +59,8 @@ _MD_ENERGY = 1e3 / _CODATA_E / _CODATA_NA                      # kJ/mol in eV
 _MD_TIME = 10.0 * math.sqrt(1.0 / _MD_ENERGY)                 # units.py:37, in ASE time units
 KB_MD = (_CODATA_K / _CODATA_E) / _MD_ENERGY                   # units.py:79: ~0.0083144598 kJ/mol/K
 FS_MD = 1e-15 * 1e10 * math.sqrt(_CODATA_E / _CODATA_AMU) / _MD_TIME   # units.py:59: ~1.0e-3
+# units.py:37-40,64-65: 1 bar = 1e5 Pa = 1e5 J/m^3 = 1e5 N_A / 1e30 kJ/mol/nm^3 (~0.0602214)
+BAR_MD = 1e5 * _CODATA_NA / 1e30
 
 
 class _Systems:
@@ -76,6 +87,22 @@ class _Systems:
         temp = torch.empty(self.n_sys, dtype=torch.float64, device=dev)
         self.call("spk_md_kinetic_energy", momenta, float(kB), ops._p(ke), ops._p(temp))
         return ke, temp
+
+    @property
+    def baro_ws(self) -> Tensor:
+        """fp64 workspace of the barostat kernels (allocated on first use, outside any capture)"""
+        if getattr(self, "_baro_ws", None) is None:
+            nbytes = int(_lib.lib().spk_md_barostat_workspace_bytes(self.n_atoms, self.n_sys))
+            self._baro_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.masses.device)
+        return self._baro_ws
+
+    def kinetic_energy_tensor(self, momenta: Tensor) -> Tensor:
+        """1/2 sum_a p_a p_a^T / m_a per system, [n_sys, 3, 3] fp64 (system.py:389-404)"""
+        out = torch.empty(self.n_sys, 3, 3, dtype=torch.float64, device=momenta.device)
+        ws = self.baro_ws
+        _lib.call("spk_md_kinetic_energy_tensor", ops._p(momenta), ops._p(self.masses), ops._p(self.idx_m),
+                  ops._p(self.sys_ptr), self.n_atoms, self.n_sys, ops._p(out), ops._p(ws), ws.numel(), ops._stream())
+        return out
 
 
 class _Thermostat:
@@ -201,17 +228,147 @@ class NHCThermostat(_Thermostat):
         return {"velocities": self.velocities, "forces": self.forces}
 
 
+class _NHCBarostat:
+    """Nose-Hoover-chain barostat (barostats.py:162-705) with the reference's keywords and defaults: target pressure in bar,
+    bath temperature in K, time constants in fs; ``kB``, ``fs`` and ``bar`` define the caller's MD units (defaults: the
+    reference's kJ/mol, nm, Da).  Two chains as in the reference: one on the particles (per system, or per degree of freedom
+    with ``massive``) and one on the cell (per system).  It thermostats the particles itself, so ``DeviceMD`` takes no
+    separate thermostat with it.  State (chains, cell velocities and forces) is fp64 on the device."""
+
+    anisotropic = False
+    YS_WEIGHTS = NHCThermostat.YS_WEIGHTS
+
+    def __init__(self, target_pressure: float, temperature_bath: float, time_constant: float,
+                 time_constant_cell: Optional[float] = None, time_constant_barostat: Optional[float] = None,
+                 chain_length: int = 4, multi_step: int = 4, integration_order: int = 7, massive: bool = False,
+                 kB: float = KB_MD, fs: float = FS_MD, bar: float = BAR_MD):
+        if integration_order not in self.YS_WEIGHTS:
+            raise ValueError(f"Order {integration_order:d} not supported for YS integration weights")
+        if int(chain_length) < 1 or int(multi_step) < 1:
+            raise ValueError("chain_length and multi_step must be >= 1")
+        self.target_pressure = float(target_pressure) * float(bar)               # :51-53
+        self.temperature_bath = float(temperature_bath)
+        self.time_constant = float(time_constant) * float(fs)
+        self.frequency = 1.0 / self.time_constant                               # :209
+        self.cell_frequency = self.frequency if time_constant_cell is None else 1.0 / (float(time_constant_cell) * fs)
+        self.barostat_frequency = (self.frequency if time_constant_barostat is None
+                                   else 1.0 / (float(time_constant_barostat) * fs))
+        self.kB = float(kB)
+        self.kb_temperature = self.temperature_bath * self.kB                   # :227
+        self.chain_length = int(chain_length)
+        self.multi_step = int(multi_step)
+        self.integration_order = int(integration_order)
+        self.massive = bool(massive)
+        self.systems: Optional[_Systems] = None
+
+    def bind(self, systems: _Systems, time_step: float):
+        """on_simulation_start (:263-383, :760-796): masses and zero state for the systems of a batch."""
+        self.systems = s = systems
+        self.time_step = float(time_step)
+        dev = s.masses.device
+        f64 = dict(dtype=torch.float64, device=dev)
+        kbt, L = self.kb_temperature, self.chain_length
+        dof = 3.0 * s.n_atoms_sys                                                # :285-287
+        self.b_masses = (dof + 3.0) * kbt / self.barostat_frequency ** 2         # :318-322
+        if self.anisotropic:
+            self.b_masses = self.b_masses / 3.0                                  # :771-776
+            self.b_velocities = torch.zeros(s.n_sys, 3, 3, **f64)
+        else:
+            self.b_velocities = torch.zeros(s.n_sys, **f64)
+        self.b_forces = torch.zeros_like(self.b_velocities)
+        dof_p = torch.ones(3 * s.n_atoms, **f64) if self.massive else dof       # :293-302
+        self.t_masses = torch.full((dof_p.shape[0], L), kbt / self.frequency ** 2, **f64)       # :343-371
+        self.t_masses[:, 0] = dof_p * kbt / self.frequency ** 2
+        dof_cell = 6.0 if self.anisotropic else 1.0                              # :328-330, :794-796
+        self.t_masses_cell = torch.full((s.n_sys, L), kbt / self.cell_frequency ** 2, **f64)
+        self.t_masses_cell[:, 0] = dof_cell * kbt / self.cell_frequency ** 2
+        self.t_velocities = torch.zeros_like(self.t_masses)
+        self.t_forces = torch.zeros_like(self.t_masses)
+        self.t_velocities_cell = torch.zeros_like(self.t_masses_cell)
+        self.t_forces_cell = torch.zeros_like(self.t_masses_cell)
+        w = self.YS_WEIGHTS[self.integration_order]
+        steps = [self.time_step * wk / self.multi_step for wk in w] + [0.0] * (7 - len(w))   # :273-281
+        p = ops._p
+        self.params = _lib.NHCBarostat(
+            int(self.anisotropic), int(self.massive), L, self.multi_step, self.integration_order, 0, kbt, self.time_step,
+            self.target_pressure, (ctypes.c_double * 7)(*steps), p(self.t_velocities), p(self.t_forces), p(self.t_masses),
+            p(self.t_velocities_cell), p(self.t_forces_cell), p(self.t_masses_cell), p(self.b_velocities),
+            p(self.b_forces), p(self.b_masses))
+
+    def _call(self, name: str, *args, launches: Optional[int] = None):
+        s = self.systems
+        ws = s.baro_ws
+        _lib.call(name, ctypes.byref(self.params), *args, ops._p(ws), ws.numel(), ops._stream(), launches=launches)
+
+    def apply_thermostat(self, momenta: Tensor):
+        """_update_thermostat (:408-481): particle and cell chains; scales the momenta and the cell velocities."""
+        s = self.systems
+        self._call("spk_md_barostat_thermostat", ops._p(momenta), ops._p(s.masses), ops._p(s.idx_m), ops._p(s.sys_ptr),
+                   s.n_atoms, s.n_sys, launches=2 if self.massive else 4)   # massive: no kinetic-energy passes
+
+    def kick(self, momenta: Tensor, cell: Tensor, virial: Tensor, virial_scale: float):
+        """_update_barostat (:604-631, :822-842) with stress = virial_scale * virial / det(cell)."""
+        s = self.systems
+        self._call("spk_md_barostat_kick", ops._p(momenta), ops._p(s.masses), ops._p(s.idx_m), ops._p(s.sys_ptr),
+                   s.n_atoms, s.n_sys, ops._p(cell), ops._p(virial), float(virial_scale))
+
+    def half_step(self, momenta: Tensor, forces: Tensor, force_conversion: float = 1.0):
+        """propagate_half_step (:661-686, :885-926) with forces * force_conversion in MD units."""
+        s = self.systems
+        self._call("spk_md_barostat_half_step", ops._p(momenta), ops._p(forces), float(force_conversion),
+                   ops._p(s.idx_m), ops._p(s.sys_ptr), s.n_atoms, s.n_sys)
+
+    def main_step(self, positions: Tensor, momenta: Tensor, cell: Tensor, model_positions: Optional[Tensor] = None,
+                  model_cell: Optional[Tensor] = None, position_conversion: float = 1.0):
+        """propagate_main_step (:633-659, :844-883): positions and the MD cell in place, plus their model-unit copies."""
+        s = self.systems
+        self._call("spk_md_barostat_main_step", ops._p(positions), ops._p(model_positions), ops._p(momenta),
+                   ops._p(s.masses), ops._p(s.idx_m), ops._p(s.sys_ptr), s.n_atoms, s.n_sys, ops._p(cell),
+                   ops._p(model_cell), float(position_conversion))
+
+    def _state(self) -> Dict[str, Tensor]:
+        return {"t_velocities": self.t_velocities, "t_forces": self.t_forces,
+                "t_velocities_cell": self.t_velocities_cell, "t_forces_cell": self.t_forces_cell,
+                "b_velocities": self.b_velocities, "b_forces": self.b_forces}
+
+    def state_dict(self) -> Dict[str, Tensor]:
+        return {k: v.clone() for k, v in self._state().items()}
+
+    def load_state_dict(self, state: Dict[str, Tensor]):
+        for k, v in self._state().items():
+            v.copy_(state[k])
+
+
+class NHCBarostatIsotropic(_NHCBarostat):
+    """Isotropic cell fluctuations (barostats.py:162-705): one cell velocity per system; the barostat force uses the
+    pressure without its kinetic part, -tr(stress) / 3."""
+
+
+class NHCBarostatAnisotropic(_NHCBarostat):
+    """Full 3x3 cell fluctuations (barostats.py:707-927): the barostat force uses the pressure tensor -stress + 2 K / V with
+    the kinetic-energy tensor K; the propagators come from a per-system fp64 Jacobi eigendecomposition of the cell velocity
+    (the reference's torch.symeig no longer exists in current torch)."""
+
+    anisotropic = True
+
+
 class DeviceMD:
     def __init__(self, model: torch.nn.Module, batch: Dict[str, Tensor], masses: Tensor, time_step: float, cutoff: float,
                  capacity: int, momenta: Optional[Tensor] = None, use_graph: bool = True,
                  position_conversion: float = 1.0, energy_conversion: float = 1.0,
-                 thermostat: Optional[_Thermostat] = None):
+                 thermostat: Optional[_Thermostat] = None, barostat: Optional[_NHCBarostat] = None,
+                 compute_stress: bool = False):
         """``batch[_positions]`` (and ``_cell``) are in MODEL units as everywhere in this package; ``self.positions`` is the
         MD-unit state (= model positions / position_conversion).  ``thermostat`` (None = NVE) is bound to the systems of
-        the batch and applied around every step."""
+        the batch and applied around every step.  ``barostat`` (an NHC barostat, which thermostats the particles itself)
+        makes the run NPT: every system must be periodic on all three axes.  ``compute_stress`` keeps the virial (and so
+        ``stress`` / ``pressure``) up to date in an NVE / NVT run."""
         dev = batch[P.R].device
         if dev.type != "cuda":
             raise ValueError("DeviceMD needs a CUDA batch (no CPU fallback)")
+        if barostat is not None and thermostat is not None:
+            raise ValueError("DeviceMD: the NHC barostats contain their own thermostat (temperature_control = True); "
+                             "pass either a thermostat or a barostat")
         self.model = model
         self.dt = float(time_step)
         self.p_conv = float(position_conversion)
@@ -237,6 +394,26 @@ class DeviceMD:
         self.thermostat = thermostat
         if thermostat is not None:
             thermostat.bind(self.systems, self.dt)                                # on_simulation_start
+        self.barostat = barostat
+        self.cell: Optional[Tensor] = None          # MD-unit cell [n_sys, 3, 3] fp64 (the model reads static[_cell])
+        self.virial: Optional[Tensor] = None        # model-unit virial [n_sys, 3, 3] fp64, written by every evaluation
+        if barostat is not None or compute_stress:
+            n_sys = self.systems.n_sys
+            if P.cell not in self.static:
+                raise ValueError("DeviceMD: stress and NPT need a periodic batch with a '_cell'")
+            self.model_cell = self.static[P.cell]
+            if (self.model_cell.dtype != torch.float32 or not self.model_cell.is_contiguous()
+                    or self.model_cell.numel() != 9 * n_sys):
+                raise ValueError("DeviceMD: '_cell' must be a contiguous float32 [n_sys, 3, 3] tensor")
+            self.cell = self.model_cell.reshape(n_sys, 3, 3).double() / self.p_conv
+            self.virial = torch.zeros(n_sys, 3, 3, dtype=torch.float64, device=dev)
+        if barostat is not None:
+            pbc = self.static.get(P.pbc)
+            if pbc is None or not bool(pbc.reshape(-1, 3).all()) or pbc.reshape(-1, 3).shape[0] not in (1, n_sys):
+                raise ValueError("DeviceMD: NPT needs every system periodic on all three axes (system.py:599-602)")
+            if bool((self.volume() == 0.0).any()):
+                raise ValueError("DeviceMD: NPT needs a non-zero cell volume for every system (system.py:599-602)")
+            barostat.bind(self.systems, self.dt)                                  # on_simulation_start
         self._calculate()                       # forces at t = 0 (simulator.py:118)
 
     @property
@@ -254,6 +431,8 @@ class DeviceMD:
     def _calculate(self):
         ops._GRAPH_CACHE.clear()
         x = {k: (v.detach() if v.is_floating_point() else v) for k, v in self.static.items()}
+        if self.virial is not None:
+            x[P.virial] = self.virial
         x = self.nl(x)
         out = self.model(x)
         e, f = out["energy"].detach(), out["forces"].detach()
@@ -271,7 +450,25 @@ class DeviceMD:
         _lib.call("spk_md_velocity_verlet", ops._p(self.momenta), ops._p(self.positions), ops._p(mp), ops._p(self.forces),
                   ops._p(self.masses), n, self.dt, self.f_conv, self.p_conv, 1 if drift else 0, ops._stream())
 
+    def _virial_scale(self) -> float:
+        # stress_MD = W / V_model * e_conv / p_conv^3 with V_model = V_MD p_conv^3 (base_calculator.py:97,218-222)
+        return self.e_conv / self.p_conv ** 6
+
+    def _npt_step(self):
+        b = self.barostat
+        mp = self.model_positions if self.model_positions is not self.positions else None
+        b.apply_thermostat(self.momenta)                                           # simulator.py:127-128 on_step_begin
+        b.kick(self.momenta, self.cell, self.virial, self._virial_scale())
+        b.half_step(self.momenta, self.forces, self.f_conv)                        # integrators.py:249-257
+        b.main_step(self.positions, self.momenta, self.cell, mp, self.model_cell, self.p_conv)   # :259-263
+        self._calculate()                                                          # neighbour list on the new cell
+        b.half_step(self.momenta, self.forces, self.f_conv)
+        b.kick(self.momenta, self.cell, self.virial, self._virial_scale())        # simulator.py:149-150 on_step_end
+        b.apply_thermostat(self.momenta)
+
     def _step(self):
+        if self.barostat is not None:
+            return self._npt_step()
         if self.thermostat is not None:
             self.thermostat.apply(self.momenta)   # simulator.py:127-128 on_step_begin
         self._verlet(True)        # integrators.py:70 half_step + :108 main_step (momenta, then positions with the new momenta)
@@ -288,6 +485,10 @@ class DeviceMD:
             state.append(self.model_positions)
         if self.thermostat is not None:
             state.extend(self.thermostat._state().values())
+        if self.virial is not None:
+            state.extend([self.virial, self.cell, self.model_cell])
+        if self.barostat is not None:
+            state.extend(self.barostat._state().values())
         saved = [t.clone() for t in state]
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
@@ -336,7 +537,8 @@ class DeviceMD:
         """Instantaneous temperature of every system in K (system.py:407-421), fp64 on the device; ``kB`` in MD energy per
         kelvin defaults to the thermostat's, else to the reference's MD units."""
         if kB is None:
-            kB = self.thermostat.kB if self.thermostat is not None else KB_MD
+            hook = self.thermostat if self.thermostat is not None else self.barostat
+            kB = hook.kB if hook is not None else KB_MD
         return self.systems.kinetic_energy_and_temperature(self.momenta, kB)[1]
 
     def state_dict(self) -> Dict[str, object]:
@@ -349,6 +551,10 @@ class DeviceMD:
             sd["model_positions"] = self.model_positions.clone()
         if self.thermostat is not None:
             sd["thermostat"] = self.thermostat.state_dict()
+        if self.virial is not None:
+            sd.update(cell=self.cell.clone(), model_cell=self.model_cell.clone(), virial=self.virial.clone())
+        if self.barostat is not None:
+            sd["barostat"] = self.barostat.state_dict()
         return sd
 
     def load_state_dict(self, state: Dict[str, object]):
@@ -359,4 +565,41 @@ class DeviceMD:
             self.model_positions.copy_(state["model_positions"])
         if self.thermostat is not None:
             self.thermostat.load_state_dict(state["thermostat"])
+        if self.virial is not None:
+            for k in ("cell", "model_cell", "virial"):
+                getattr(self, k).copy_(state[k])
+        if self.barostat is not None:
+            self.barostat.load_state_dict(state["barostat"])
         self.steps_done = int(state["steps_done"])
+
+    # ---- cell, stress and pressure (system.py:567-614), MD units, per system, fp64 on the device ----------------------------
+    def volume(self) -> Tensor:
+        """cell volumes [n_sys] (system.py:567-581)"""
+        c = self._need_cell()
+        return torch.sum(c[:, 0] * torch.cross(c[:, 1], c[:, 2], dim=1), dim=1)
+
+    def _need_cell(self) -> Tensor:
+        if self.cell is None:
+            raise RuntimeError("DeviceMD: create it with compute_stress=True or a barostat to track the cell and stress")
+        return self.cell
+
+    @property
+    def stress(self) -> Tensor:
+        """stress of the last evaluation [n_sys, 3, 3] in MD units: W / V_model * energy_conversion /
+        position_conversion^3 (base_calculator.py:97,218-222)"""
+        v_model = self.volume() * self.p_conv ** 3
+        return self.virial / v_model[:, None, None] * (self.e_conv / self.p_conv ** 3)
+
+    def pressure(self, tensor: bool = False, kinetic_component: bool = False) -> Tensor:
+        """system.py:583-614: -stress ([n_sys, 3, 3]) or its trace / 3 ([n_sys]), optionally with the kinetic part."""
+        vol = self.volume()
+        p = -self.stress
+        if tensor:
+            if kinetic_component:
+                p = p + 2.0 * self.systems.kinetic_energy_tensor(self.momenta) / vol[:, None, None]
+            return p
+        p = torch.diagonal(p, dim1=1, dim2=2).sum(-1) / 3.0
+        if kinetic_component:
+            ke = self.systems.kinetic_energy_and_temperature(self.momenta, KB_MD)[0]
+            p = p + 2.0 * ke / vol / 3.0
+        return p

@@ -13,6 +13,7 @@ import torch.nn as nn
 from . import atomistic, representation
 from . import nn as snn
 from . import ops
+from . import properties
 
 __all__ = ["AtomisticModel", "NeuralNetworkPotential", "convert_model"]
 
@@ -86,7 +87,7 @@ class NeuralNetworkPotential(AtomisticModel):
         out_dtype = None
         if self.cast_inputs:
             for k, v in list(inputs.items()):
-                if v.is_floating_point() and v.dtype != torch.float32:
+                if v.is_floating_point() and v.dtype != torch.float32 and k != properties.virial:
                     out_dtype = v.dtype
                     inputs[k] = v.to(torch.float32)
         inputs = self.initialize_derivatives(inputs)
@@ -292,6 +293,8 @@ class GraphedPotential:
         for k, v in inputs.items():
             static_in[k].copy_(v, non_blocking=True)
         graph.replay()
+        if properties.virial in inputs:             # the caller's virial buffer is an output: hand the replay's back
+            inputs[properties.virial].copy_(static_in[properties.virial], non_blocking=True)
         self._last = entry
         return static_out
 

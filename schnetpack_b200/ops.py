@@ -200,6 +200,17 @@ def pairwise_bwd(g_rij: Tensor, graph: EdgeGraph, sign: float = 1.0) -> Tensor:
     return out
 
 
+def pairwise_virial(g_rij: Tensor, r_ij: Tensor, graph: EdgeGraph, sys_ptr: Tensor, virial: Tensor):
+    """virial[m] = sum over the edges received by the atoms of system m of g_rij (x) r_ij, fp64, in place."""
+    f32(g_rij, "g_rij")
+    f32(r_ij, "_Rij")
+    n_sys = virial.shape[0]
+    nbytes = int(_lib.lib().spk_pairwise_virial_workspace_bytes(graph.n_edges, n_sys))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=g_rij.device)
+    _lib.call("spk_pairwise_virial", _p(g_rij), _p(r_ij), _p(graph.rowptr), _p(graph.slot_eid), _p(sys_ptr), graph.n_edges,
+              n_sys, _p(virial), _p(ws), nbytes, _stream())
+
+
 def edge_geometry(r_ij: Tensor, graph: Optional[EdgeGraph], rbf_kind: int, n_rbf: int, p0: Tensor, p1: Optional[Tensor],
                   cutoff: float, need_grad: bool = True, active_only: bool = False):
     """``active_only``: ``graph`` was built from the active edges (EdgeGraph(..., r_ij, cutoff)); only its
