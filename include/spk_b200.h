@@ -446,6 +446,44 @@ int spk_md_barostat_main_step(const spk_nhc_barostat_t* barostat, float* positio
                               int64_t n_atoms, int64_t n_sys, double* cell, float* model_cell, double position_conversion,
                               void* workspace, size_t workspace_bytes, spk_stream_t stream);
 
+/* ---- ring-polymer MD of the device MD step (csrc/rpmd.cu; md/integrators.py:113-229 RingPolymer,
+ * md/utils/normal_model_transformation.py, md/simulation_hooks/thermostats_rpmd.py:33-234,373-501).  Bead arrays
+ * [n_beads, n_atoms, 3] fp32 in MD units, replica-major (bead r of atom a at row r n_atoms + a); masses [n_atoms] fp32 of
+ * the base batch (one copy of every atom); 1 <= n_beads <= 64.  c_transform [n_beads, n_beads] fp64 on the device is the
+ * normal-mode matrix C (modes = C beads, beads = C^T modes).  Arithmetic is fp64 with fp32 loads and stores.  Systems
+ * (idx_m, sys_ptr, n_sys) are those of the base batch, as for the thermostats above; they are read by the global variants
+ * only.  workspace: spk_rpmd_workspace_bytes(n_atoms, n_sys) bytes, 8-byte aligned, no initialisation needed.  One step
+ * (md/simulator.py:124-150): thermostat, half kick on every bead (spk_md_velocity_verlet, drift = 0), main step, forces on
+ * all beads, half kick, thermostat.
+ *   spk_rpmd_normal_modes  out = C in (inverse = 0) or C^T in (inverse = 1) over the bead axis; may run in place
+ *   spk_rpmd_main_step     integrators.py:221-230 per degree of freedom: (p~, x~) of mode k -> propagator [n_beads,2,2]
+ *                          fp64 (p~' = U00 p~ + U01 m x~, x~' = U10 p~ / m + U11 x~); positions and momenta in place,
+ *                          model_positions = positions * position_conversion (nullable)
+ *   spk_rpmd_pile          p~_k = c1[k] p~_k + c2[k] sqrt(m kb_temperature) xi (kb_temperature = n_beads kB T; c1, c2
+ *                          [n_beads] fp64 on the device) with xi from Philox4x32-10, key = seed, counter = (k n_atoms + a,
+ *                          counter[0]), normals 0..2 of the draw for x, y, z; counter as for spk_md_langevin.  global != 0:
+ *                          mode 0 is instead rescaled per system by the stochastic velocity rescaling factor of
+ *                          thermostats_rpmd.py:160-189 from K0 = sum |p~_0|^2 / m, S = sum |xi_0|^2 and R = the x-noise of
+ *                          the system's first atom (a system with K0 = 0 is left as it is)
+ *   spk_rpmd_nhc           one Nose-Hoover chain per (mode, degree of freedom) on p~ (params->massive is ignored):
+ *                          kinetic energy p~^2 / m, chain state chain_v, chain_f, chain_m [n_beads 3 n_atoms, chain_length]
+ *                          fp64, row k 3 n_atoms + 3 a + d.  global != 0: mode 0 sees its system's sum |p~_0|^2 / m with
+ *                          3 n_s degrees of freedom. */
+size_t spk_rpmd_workspace_bytes(int64_t n_atoms, int64_t n_sys);
+int spk_rpmd_normal_modes(const float* in, float* out, int64_t n_atoms, int32_t n_beads, const double* c_transform,
+                          int32_t inverse, spk_stream_t stream);
+int spk_rpmd_main_step(float* positions, float* momenta, float* model_positions, const float* masses, int64_t n_atoms,
+                       int32_t n_beads, const double* c_transform, const double* propagator, double position_conversion,
+                       spk_stream_t stream);
+int spk_rpmd_pile(float* momenta, const float* masses, const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms,
+                  int64_t n_sys, int32_t n_beads, const double* c_transform, const double* c1, const double* c2,
+                  double kb_temperature, int32_t global, uint64_t seed, uint64_t* counter, void* workspace,
+                  size_t workspace_bytes, spk_stream_t stream);
+int spk_rpmd_nhc(float* momenta, const float* masses, const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms,
+                 int64_t n_sys, int32_t n_beads, const double* c_transform, const spk_nhc_params_t* params, int32_t global,
+                 double* chain_v, double* chain_f, const double* chain_m, void* workspace, size_t workspace_bytes,
+                 spk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

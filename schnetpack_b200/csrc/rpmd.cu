@@ -1,0 +1,376 @@
+// Ring-polymer MD of the device MD step: the normal-mode transform (md/utils/normal_model_transformation.py:37-101), the
+// free ring-polymer propagation of the RingPolymer integrator (md/integrators.py:154-229) and the ring-polymer thermostats
+// PILE-L / PILE-G / TRPMD and NHC (md/simulation_hooks/thermostats_rpmd.py:33-234,373-501).  Every entry point only
+// enqueues work, so the whole RPMD step stays one CUDA graph.
+//
+// Bead arrays are [P, n_atoms, 3] fp32, replica-major, so for a fixed bead a run of consecutive degrees of freedom (atom,
+// component) is contiguous.  The mode kernels give a CTA RP_T = 32 consecutive degrees of freedom across all P beads: the
+// bead values are staged in shared memory with coalesced loads, every (mode, dof) pair is formed as an fp64 dot product with
+// a row of C, the per-mode operator is applied in registers, and the back-transform C^T writes the beads.  Threads of a warp
+// share one mode (or bead) index, so their reads of C are warp-uniform broadcasts from L1.  Shared memory: 24 P RP_T bytes,
+// 48 KB at P = 64.
+//
+// The per-system centroid sums of the global thermostats use the fixed-shape segmented scan of segscan.cuh and one ordered
+// finishing pass per system: no atomics touch a sum, so every call is bitwise reproducible.
+#include "md_common.cuh"
+
+namespace {
+
+constexpr int RP_T = 32;          // degrees of freedom per CTA of the mode kernels
+constexpr int RP_THREADS = 256;
+constexpr int RP_KT = 256;        // atoms per CTA of the centroid partial pass
+constexpr int RP_NV = 2;          // centroid sums: sum |p~_0|^2 / m, sum |xi_0|^2
+constexpr int RP_MAX_BEADS = 64;
+
+enum RpmdOp { OP_MAIN = 0, OP_PILE = 1, OP_NHC = 2 };
+
+struct RpmdArgs {
+    float* x;                     // bead positions (OP_MAIN)
+    float* p;                     // bead momenta
+    float* model_x;               // nullable: x * pos_conv (OP_MAIN)
+    const float* m;               // [n_atoms]
+    const int64_t* idx_m;
+    const int32_t* sys_ptr;
+    const double* C;              // [P, P]
+    const double* prop;           // [P, 2, 2] (OP_MAIN)
+    const double* c1;             // [P] (OP_PILE)
+    const double* c2;
+    const double* tot;            // [n_sys, RP_NV] centroid sums (global variants)
+    double* chain_v;              // [P * 3 n_atoms, L] (OP_NHC)
+    double* chain_f;
+    const double* chain_m;
+    unsigned long long* counter;  // [2]: application index, ticket (OP_PILE)
+    int64_t n_atoms;
+    double pos_conv;
+    double kbt_p;                 // P kB T (OP_PILE)
+    uint64_t seed;
+    int32_t P;
+    int32_t global;
+    spk_nhc_params_t q;           // (OP_NHC)
+};
+
+struct Workspace {
+    double* sys_part;  // [n_sys, RP_NV]
+    double* tot;       // [n_sys, RP_NV]
+    double* head;      // [n_blocks, RP_NV]
+};
+
+static inline int64_t rp_blocks(int64_t n_atoms) { return spk_cdiv(n_atoms, RP_KT); }
+
+static inline Workspace carve(void* ws, int64_t n_sys) {
+    double* d = reinterpret_cast<double*>(ws);
+    return Workspace{d, d + RP_NV * n_sys, d + 2 * RP_NV * n_sys};
+}
+
+static inline size_t mode_smem(int P) { return (size_t)P * RP_T * (2 * sizeof(double) + 2 * sizeof(float)); }
+
+// normal d (0, 1, 2 = x, y, z) of the draw for element elem: the first three Box-Muller normals, as k_langevin
+__device__ __forceinline__ double mode_noise(uint64_t seed, uint64_t app, int64_t elem, int d) {
+    const uint4 r = philox_draw(seed, app, elem);
+    if (d == 2) return box_muller(r.z, r.w).x;
+    const double2 z = box_muller(r.x, r.y);
+    return d == 0 ? z.x : z.y;
+}
+
+// PILE-G centroid factor of system s (thermostats_rpmd.py:160-195) with R = the x-noise of the system's own first atom;
+// a system whose centroid kinetic energy is zero keeps its centroid (alpha = 1)
+__device__ __forceinline__ double pile_alpha(const RpmdArgs& A, uint64_t app, int64_t s) {
+    const double k0 = A.tot[RP_NV * s], S = A.tot[RP_NV * s + 1];
+    if (!(k0 > 0.0)) return 1.0;
+    const double c = A.c1[0];
+    const double factor = k0 / A.kbt_p;                                         // :167-169
+    const double cf = (1.0 - c) / factor;                                       // :171
+    const double R = mode_noise(A.seed, app, A.sys_ptr[s], 0);
+    const double a2 = c + S * cf + 2.0 * R * sqrt(c * cf);                      // :173-181
+    const double sg = R + sqrt(c / cf);                                         // :183-186 torch.sign
+    return sqrt(a2) * (double)((sg > 0.0) - (sg < 0.0));
+}
+
+// beads -> normal modes, the per-mode operator OP, normal modes -> beads, for RP_T degrees of freedom per CTA
+template <int OP>
+__global__ void __launch_bounds__(RP_THREADS) k_rpmd_modes(const __grid_constant__ RpmdArgs A) {
+    extern __shared__ double smem[];
+    const int P = A.P;
+    const int PT = P * RP_T;
+    double* mx = smem;                                   // [P][RP_T] normal modes of x
+    double* mp = smem + PT;                              // [P][RP_T] normal modes of p
+    float* bx = reinterpret_cast<float*>(smem + 2 * PT); // [P][RP_T] bead values
+    float* bp = bx + PT;
+    SPK_PDL_ENTER();
+    unsigned long long app = 0;
+    if (OP == OP_PILE) app = *(volatile unsigned long long*)A.counter;
+    const int64_t n_dof = 3 * A.n_atoms;
+    const int64_t i0 = (int64_t)blockIdx.x * RP_T;
+    for (int j = threadIdx.x; j < PT; j += RP_THREADS) {
+        const int b = j / RP_T;
+        const int64_t i = i0 + (j % RP_T);
+        if (i < n_dof) {
+            if (OP == OP_MAIN) bx[j] = A.x[b * n_dof + i];
+            bp[j] = A.p[b * n_dof + i];
+        }
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < PT; j += RP_THREADS) {
+        const int k = j / RP_T, t = j % RP_T;
+        const int64_t i = i0 + t;
+        if (i >= n_dof) continue;
+        const double* Ck = A.C + (int64_t)k * P;
+        double xn = 0.0, pn = 0.0;
+        for (int b = 0; b < P; ++b) {                    // normal_model_transformation.py:78-80 beads2normal
+            const double c = Ck[b];
+            if (OP == OP_MAIN) xn += c * (double)bx[b * RP_T + t];
+            pn += c * (double)bp[b * RP_T + t];
+        }
+        const int64_t a = i / 3;
+        const double ma = (double)A.m[a];
+        if (OP == OP_MAIN) {                             // integrators.py:221-230
+            const double* u = A.prop + 4 * k;
+            const double np = u[0] * pn + u[1] * xn * ma;
+            xn = u[2] * pn / ma + u[3] * xn;
+            pn = np;
+        } else if (OP == OP_PILE) {
+            if (k == 0 && A.global) {                    // thermostats_rpmd.py:188-189
+                pn *= pile_alpha(A, app, A.idx_m[a]);
+            } else {                                     // :115-119, :191-195
+                const double xi = mode_noise(A.seed, app, (int64_t)k * A.n_atoms + a, (int)(i - 3 * a));
+                pn = A.c1[k] * pn + sqrt(ma * A.kbt_p) * A.c2[k] * xi;
+            }
+        } else {                                         // thermostats_rpmd.py:465-501
+            double ke = pn * pn / ma, dof = 1.0;
+            if (k == 0 && A.global) {
+                const int64_t s = A.idx_m[a];
+                ke = A.tot[RP_NV * s];
+                dof = 3.0 * (double)(A.sys_ptr[s + 1] - A.sys_ptr[s]);
+            }
+            const int L = A.q.chain_length;
+            const int64_t row = (int64_t)k * n_dof + i;
+            pn *= nhc_propagate(ke, dof, A.q, A.chain_v + row * L, A.chain_f + row * L, A.chain_m + row * L);
+        }
+        if (OP == OP_MAIN) mx[j] = xn;
+        mp[j] = pn;
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < PT; j += RP_THREADS) {
+        const int b = j / RP_T, t = j % RP_T;
+        const int64_t i = i0 + t;
+        if (i >= n_dof) continue;
+        double xb = 0.0, pb = 0.0;
+        for (int k = 0; k < P; ++k) {                    // normal_model_transformation.py:93-101 normal2beads
+            const double c = A.C[(int64_t)k * P + b];
+            if (OP == OP_MAIN) xb += c * mx[k * RP_T + t];
+            pb += c * mp[k * RP_T + t];
+        }
+        A.p[b * n_dof + i] = (float)pb;
+        if (OP == OP_MAIN) {
+            const float xf = (float)xb;
+            A.x[b * n_dof + i] = xf;
+            if (A.model_x) A.model_x[b * n_dof + i] = xf * (float)A.pos_conv;
+        }
+    }
+    if (OP == OP_PILE) {   // advance the application index once every CTA has read it (ticket pattern of k_langevin)
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            __threadfence();
+            if (atomicAdd(A.counter + 1, 1ull) == gridDim.x - 1) {
+                A.counter[0] = app + 1;
+                A.counter[1] = 0;
+                __threadfence();
+            }
+        }
+    }
+}
+
+// out = C in (inverse = 0) or C^T in (inverse = 1) over the bead axis, RP_T degrees of freedom per CTA
+__global__ void __launch_bounds__(RP_THREADS) k_rpmd_transform(const float* in, float* out, int64_t n_dof, int P,
+                                                             const double* __restrict__ C, int inverse) {
+    extern __shared__ double smem[];
+    float* bv = reinterpret_cast<float*>(smem);          // [P][RP_T]
+    SPK_PDL_ENTER();
+    const int PT = P * RP_T;
+    const int64_t i0 = (int64_t)blockIdx.x * RP_T;
+    for (int j = threadIdx.x; j < PT; j += RP_THREADS) {
+        const int64_t i = i0 + (j % RP_T);
+        if (i < n_dof) bv[j] = in[(j / RP_T) * n_dof + i];
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < PT; j += RP_THREADS) {
+        const int r = j / RP_T, t = j % RP_T;
+        const int64_t i = i0 + t;
+        if (i >= n_dof) continue;
+        double acc = 0.0;
+        for (int q = 0; q < P; ++q) acc += (inverse ? C[q * P + r] : C[r * P + q]) * (double)bv[q * RP_T + t];
+        out[r * n_dof + i] = (float)acc;
+    }
+}
+
+// per-(system, CTA) partials of sum_a |p~_0,a|^2 / m_a and (with_noise) sum_a |xi_0,a|^2 over the atoms of the base batch
+__global__ void __launch_bounds__(RP_KT) k_rpmd_centroid_partials(const __grid_constant__ RpmdArgs A, int with_noise,
+                                                                  double* __restrict__ sys_part,
+                                                                  double* __restrict__ head) {
+    __shared__ double sv[RP_NV][RP_KT];
+    __shared__ int sf[RP_KT];
+    SPK_PDL_ENTER();
+    const unsigned long long app = with_noise ? *(volatile unsigned long long*)A.counter : 0ull;
+    const int t = threadIdx.x;
+    const int64_t b0 = (int64_t)blockIdx.x * RP_KT;
+    const int64_t a = b0 + t;
+    const int64_t n_dof = 3 * A.n_atoms;
+    double v[RP_NV] = {0.0, 0.0};
+    int f = 1;
+    int64_t s = -1;
+    if (a < A.n_atoms) {
+        const double ma = (double)A.m[a];
+        for (int d = 0; d < 3; ++d) {
+            double pc = 0.0;
+            for (int b = 0; b < A.P; ++b) pc += A.C[b] * (double)A.p[b * n_dof + 3 * a + d];   // row 0 of C
+            v[0] += pc * pc / ma;                                                        // thermostats_rpmd.py:162-165
+        }
+        if (with_noise) {
+            const uint4 r = philox_draw(A.seed, app, a);
+            const double2 z01 = box_muller(r.x, r.y), z23 = box_muller(r.z, r.w);
+            v[1] = z01.x * z01.x + z01.y * z01.y + z23.x * z23.x;                        // :174-176
+        }
+        s = A.idx_m[a];
+        f = (t == 0) || (A.idx_m[a - 1] != s);
+    }
+    seg_scan<RP_KT, RP_NV>(v, f, sv, sf);
+    if (a >= A.n_atoms) return;
+    const bool seg_end = (t == RP_KT - 1) || (a == A.n_atoms - 1) || (A.idx_m[a + 1] != s);
+    if (!seg_end) return;
+    double* dst = A.sys_ptr[s] >= b0 ? sys_part + s * RP_NV : head + (int64_t)blockIdx.x * RP_NV;
+    dst[0] = v[0];
+    dst[1] = v[1];
+}
+
+static bool beads_ok(int P, const double* C) { return P >= 1 && P <= RP_MAX_BEADS && C; }
+
+static int check_modes(const float* momenta, const float* masses, int64_t n_atoms, int P, const double* C) {
+    if (!beads_ok(P, C) || n_atoms < 0 || (int64_t)P * 3 * n_atoms >= (1ll << 31) - 1) return SPK_ERR_ARG;
+    if (n_atoms > 0 && (!momenta || !masses)) return SPK_ERR_ARG;
+    return SPK_OK;
+}
+
+static int check_systems(const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms, int64_t n_sys, void* workspace,
+                         size_t workspace_bytes) {
+    if (n_sys <= 0 || !sys_ptr || (n_atoms > 0 && !idx_m)) return SPK_ERR_ARG;
+    if (!workspace || workspace_bytes < spk_rpmd_workspace_bytes(n_atoms, n_sys)) return SPK_ERR_ARG;
+    return SPK_OK;
+}
+
+template <int OP>
+static void launch_modes(const RpmdArgs& A, cudaStream_t st) {
+    spk_launch(k_rpmd_modes<OP>, (unsigned)spk_cdiv(3 * A.n_atoms, RP_T), RP_THREADS, mode_smem(A.P), st, A);
+}
+
+// the per-system centroid sums of the global variants: partials + ordered per-system finish (2 launches)
+static void centroid_sums(RpmdArgs& A, int with_noise, int64_t n_sys, void* workspace, cudaStream_t st) {
+    Workspace w = carve(workspace, n_sys);
+    spk_launch(k_rpmd_centroid_partials, (unsigned)rp_blocks(A.n_atoms), RP_KT, 0, st, A, with_noise, w.sys_part,
+               w.head);
+    spk_launch(k_seg_finish<RP_KT, RP_NV>, (unsigned)n_sys, SEG_FIN_T, 0, st, A.sys_ptr, (const int32_t*)nullptr,
+               (const double*)w.sys_part, (const double*)w.head, w.tot);
+    A.tot = w.tot;
+}
+
+}  // namespace
+
+extern "C" size_t spk_rpmd_workspace_bytes(int64_t n_atoms, int64_t n_sys) {
+    const int64_t nb = n_atoms > 0 ? rp_blocks(n_atoms) : 0;
+    return sizeof(double) * (size_t)(RP_NV * (2 * (n_sys > 0 ? n_sys : 0) + nb) + 1);
+}
+
+extern "C" int spk_rpmd_normal_modes(const float* in, float* out, int64_t n_atoms, int32_t n_beads,
+                                     const double* c_transform, int32_t inverse, spk_stream_t stream) {
+    if (!beads_ok(n_beads, c_transform) || n_atoms < 0 || (int64_t)n_beads * 3 * n_atoms >= (1ll << 31) - 1)
+        return SPK_ERR_ARG;
+    if (n_atoms == 0) return SPK_OK;
+    if (!in || !out) return SPK_ERR_ARG;
+    spk_launch(k_rpmd_transform, (unsigned)spk_cdiv(3 * n_atoms, RP_T), RP_THREADS,
+               (size_t)n_beads * RP_T * sizeof(float), spk_st(stream), in, out, 3 * n_atoms, (int)n_beads, c_transform,
+               inverse ? 1 : 0);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_rpmd_main_step(float* positions, float* momenta, float* model_positions, const float* masses,
+                                  int64_t n_atoms, int32_t n_beads, const double* c_transform, const double* propagator,
+                                  double position_conversion, spk_stream_t stream) {
+    if (check_modes(momenta, masses, n_atoms, n_beads, c_transform) != SPK_OK || !propagator) return SPK_ERR_ARG;
+    if (n_atoms == 0) return SPK_OK;
+    if (!positions) return SPK_ERR_ARG;
+    RpmdArgs A = {};
+    A.x = positions;
+    A.p = momenta;
+    A.model_x = model_positions;
+    A.m = masses;
+    A.C = c_transform;
+    A.prop = propagator;
+    A.n_atoms = n_atoms;
+    A.pos_conv = position_conversion;
+    A.P = n_beads;
+    launch_modes<OP_MAIN>(A, spk_st(stream));
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_rpmd_pile(float* momenta, const float* masses, const int64_t* idx_m, const int32_t* sys_ptr,
+                             int64_t n_atoms, int64_t n_sys, int32_t n_beads, const double* c_transform, const double* c1,
+                             const double* c2, double kb_temperature, int32_t global, uint64_t seed, uint64_t* counter,
+                             void* workspace, size_t workspace_bytes, spk_stream_t stream) {
+    if (check_modes(momenta, masses, n_atoms, n_beads, c_transform) != SPK_OK) return SPK_ERR_ARG;
+    if (!c1 || !c2 || !counter || !(kb_temperature > 0.0)) return SPK_ERR_ARG;
+    if (global && check_systems(idx_m, sys_ptr, n_atoms, n_sys, workspace, workspace_bytes) != SPK_OK)
+        return SPK_ERR_ARG;
+    if (n_atoms == 0) return SPK_OK;
+    cudaStream_t st = spk_st(stream);
+    RpmdArgs A = {};
+    A.p = momenta;
+    A.m = masses;
+    A.idx_m = idx_m;
+    A.sys_ptr = sys_ptr;
+    A.C = c_transform;
+    A.c1 = c1;
+    A.c2 = c2;
+    A.counter = reinterpret_cast<unsigned long long*>(counter);
+    A.n_atoms = n_atoms;
+    A.kbt_p = kb_temperature;
+    A.seed = seed;
+    A.P = n_beads;
+    A.global = global ? 1 : 0;
+    if (A.global) centroid_sums(A, 1, n_sys, workspace, st);
+    launch_modes<OP_PILE>(A, st);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_rpmd_nhc(float* momenta, const float* masses, const int64_t* idx_m, const int32_t* sys_ptr,
+                            int64_t n_atoms, int64_t n_sys, int32_t n_beads, const double* c_transform,
+                            const spk_nhc_params_t* params, int32_t global, double* chain_v, double* chain_f,
+                            const double* chain_m, void* workspace, size_t workspace_bytes, spk_stream_t stream) {
+    if (check_modes(momenta, masses, n_atoms, n_beads, c_transform) != SPK_OK) return SPK_ERR_ARG;
+    if (!params || params->chain_length < 1 || params->multi_step < 1 ||
+        !(params->order == 3 || params->order == 5 || params->order == 7) || !(params->kb_temperature > 0.0))
+        return SPK_ERR_ARG;
+    if (!chain_v || !chain_f || !chain_m) return SPK_ERR_ARG;
+    if (global && check_systems(idx_m, sys_ptr, n_atoms, n_sys, workspace, workspace_bytes) != SPK_OK)
+        return SPK_ERR_ARG;
+    if (n_atoms == 0) return SPK_OK;
+    cudaStream_t st = spk_st(stream);
+    RpmdArgs A = {};
+    A.p = momenta;
+    A.m = masses;
+    A.idx_m = idx_m;
+    A.sys_ptr = sys_ptr;
+    A.C = c_transform;
+    A.chain_v = chain_v;
+    A.chain_f = chain_f;
+    A.chain_m = chain_m;
+    A.n_atoms = n_atoms;
+    A.P = n_beads;
+    A.global = global ? 1 : 0;
+    A.q = *params;
+    if (A.global) centroid_sums(A, 0, n_sys, workspace, st);
+    launch_modes<OP_NHC>(A, st);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}

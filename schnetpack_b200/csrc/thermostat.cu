@@ -114,38 +114,6 @@ __global__ void k_thermo_system(const int32_t* __restrict__ sys_ptr, int64_t n_s
     scale[s] = sc;
 }
 
-// ---- Philox4x32-10 (Salmon, Moraes, Dror, Shaw, SC'11) + Box-Muller ---------------------------------------------------
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        if (r) {
-            k.x += 0x9E3779B9u;
-            k.y += 0xBB67AE85u;
-        }
-        const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
-        const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
-        c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
-    }
-    return c;
-}
-
-// counter = (element lo, element hi, application lo, application hi), key = seed
-__device__ __forceinline__ uint4 philox_draw(uint64_t seed, uint64_t app, int64_t elem) {
-    const uint64_t e = (uint64_t)elem;
-    return philox4x32_10(make_uint4((uint32_t)e, (uint32_t)(e >> 32), (uint32_t)app, (uint32_t)(app >> 32)),
-                         make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
-}
-
-// u in (0, 1): (x + 1/2) 2^-32; z0 = sqrt(-2 ln u0) cos(2 pi u1), z1 = ... sin(2 pi u1)
-__device__ __forceinline__ double2 box_muller(uint32_t x0, uint32_t x1) {
-    const double u0 = ((double)x0 + 0.5) * 2.3283064365386963e-10;
-    const double u1 = ((double)x1 + 0.5) * 2.3283064365386963e-10;
-    const double r = sqrt(-2.0 * log(u0));
-    double sn, cs;
-    sincospi(2.0 * u1, &sn, &cs);
-    return make_double2(r * cs, r * sn);
-}
-
 // thermostats.py:244-261: p = c1 p + sqrt(m kB T) c2 xi, one thread per atom (xi = the first three normals of its draw).
 // counter[0] is the application index: read by every CTA, advanced by the CTA that finishes last (counter[1] is its
 // ticket, zero between calls), so each replay of a captured step draws fresh noise.

@@ -32,6 +32,12 @@ neighbour list on the new cell, energy + forces + virial, half step, on_step_end
 virial W = sum_e dE/dr_e (x) r_e comes out of the backward of ``PairwiseDistances`` (one fp64 kernel with a fixed summation
 order); the stress in MD units is W / V * energy_conversion / position_conversion^3 (base_calculator.py:97,218-222) with V
 the volume of the model cell.  ``compute_stress=True`` keeps the same virial up to date in NVE / NVT runs.
+
+Ring-polymer MD (DESIGN.md section 9): ``DeviceMD(..., ring_polymer=RingPolymer(...))`` replicates the batch into P beads
+(replica-major, as md/calculators/base_calculator.py:154-221 collates them) and runs the RingPolymer step
+(md/integrators.py:113-229, md/simulator.py:124-150): thermostat, half kick per bead, normal-mode propagation of the free ring
+polymer, neighbour list + energy + forces on all beads, half kick, thermostat -- with the PILE-L / PILE-G / TRPMD and
+ring-polymer NHC thermostats of md/simulation_hooks/thermostats_rpmd.py, all in the same captured graph.
 """
 from __future__ import annotations
 
@@ -46,7 +52,8 @@ from . import properties as P
 from .neighbors import CellListNeighborList
 
 __all__ = ["DeviceMD", "BerendsenThermostat", "LangevinThermostat", "NHCThermostat", "NHCBarostatIsotropic",
-           "NHCBarostatAnisotropic", "KB_MD", "FS_MD", "BAR_MD"]
+           "NHCBarostatAnisotropic", "RingPolymer", "PILELocalThermostat", "PILEGlobalThermostat", "TRPMDThermostat",
+           "NHCRingPolymerThermostat", "KB_MD", "FS_MD", "BAR_MD", "HBAR_MD"]
 
 Tensor = torch.Tensor
 
@@ -61,6 +68,9 @@ KB_MD = (_CODATA_K / _CODATA_E) / _MD_ENERGY                   # units.py:79: ~0
 FS_MD = 1e-15 * 1e10 * math.sqrt(_CODATA_E / _CODATA_AMU) / _MD_TIME   # units.py:59: ~1.0e-3
 # units.py:37-40,64-65: 1 bar = 1e5 Pa = 1e5 J/m^3 = 1e5 N_A / 1e30 kJ/mol/nm^3 (~0.0602214)
 BAR_MD = 1e5 * _CODATA_NA / 1e30
+# units.py:80-82: hbar = h / 2 pi in J s, times ASE's J * s = (1 / e) eV * 1e10 sqrt(e / amu), over energy * time (~0.0635)
+_CODATA_H = 6.626070040e-34
+HBAR_MD = (_CODATA_H / (2.0 * math.pi)) / _CODATA_E * 1e10 * math.sqrt(_CODATA_E / _CODATA_AMU) / (_MD_ENERGY * _MD_TIME)
 
 
 class _Systems:
@@ -352,33 +362,275 @@ class NHCBarostatAnisotropic(_NHCBarostat):
     anisotropic = True
 
 
+# ---- ring-polymer MD ------------------------------------------------------------------------------------------------------
+class RingPolymer:
+    """Ring-polymer integrator (md/integrators.py:113-229) with the reference's keywords: ``n_beads`` replicas (beads) of
+    every molecule at ring-polymer temperature ``temperature`` in K; ``kB`` (MD energy per kelvin) and ``hbar`` (MD energy
+    x MD time) define the caller's MD units.  The time step is ``DeviceMD``'s ``time_step``.  The normal-mode matrix C
+    (md/utils/normal_model_transformation.py:37-68) and the free ring-polymer propagator (integrators.py:154-202) are built
+    on the host in fp64 (the reference builds the propagator in float32)."""
+
+    MAX_BEADS = 64
+
+    def __init__(self, n_beads: int, temperature: float, kB: float = KB_MD, hbar: float = HBAR_MD):
+        if int(n_beads) != n_beads or not 1 <= int(n_beads) <= self.MAX_BEADS:
+            raise ValueError(f"RingPolymer: n_beads must be an integer in [1, {self.MAX_BEADS}], got {n_beads}")
+        if not float(temperature) > 0.0:
+            raise ValueError(f"RingPolymer: temperature must be > 0 K, got {temperature}")
+        self.n_beads = int(n_beads)
+        self.temperature = float(temperature)
+        self.kB = float(kB)
+        self.hbar = float(hbar)
+        self.omega = self.kB * self.n_beads * self.temperature / self.hbar                     # integrators.py:146
+        k = torch.arange(self.n_beads, dtype=torch.float64)
+        self.omega_normal = 2.0 * self.omega * torch.sin(k * math.pi / self.n_beads)            # :175-179
+
+    def transform_matrix(self) -> Tensor:
+        """C [P, P] fp64 (normal_model_transformation.py:37-68): modes = C beads, beads = C^T modes"""
+        P = self.n_beads
+        n = torch.arange(1, P + 1, dtype=torch.float64)
+        c = torch.zeros(P, P, dtype=torch.float64)
+        c[0, :] = 1.0
+        for k in range(1, P // 2 + 1):
+            c[k, :] = math.sqrt(2.0) * torch.cos(2.0 * math.pi * k * n / P)
+        for k in range(P // 2 + 1, P):
+            c[k, :] = math.sqrt(2.0) * torch.sin(2.0 * math.pi * k * n / P)
+        if P % 2 == 0:
+            c[P // 2, :] = (-1.0) ** n
+        return c / math.sqrt(P)
+
+    def propagator(self, time_step: float) -> Tensor:
+        """[P, 2, 2] fp64 (integrators.py:181-200): [[cos, -m-less w sin], [sin / w, cos]] per mode, [0, 1, 0] = dt"""
+        w = self.omega_normal
+        wdt = w * float(time_step)
+        u = torch.zeros(self.n_beads, 2, 2, dtype=torch.float64)
+        u[:, 0, 0] = torch.cos(wdt)
+        u[:, 1, 1] = torch.cos(wdt)
+        u[:, 0, 1] = -torch.sin(wdt) * w
+        u[1:, 1, 0] = torch.sin(wdt[1:]) / w[1:]
+        u[0, 1, 0] = float(time_step)
+        return u
+
+    def bind(self, base: "_Systems", time_step: float):
+        """device copies of C and the propagator for the base batch ``base`` (its masses are one copy of every atom)"""
+        dev = base.masses.device
+        self.base = base
+        self.time_step = float(time_step)
+        self.c_transform = self.transform_matrix().to(dev)
+        self.u = self.propagator(time_step).to(dev)
+
+    def main_step(self, positions: Tensor, momenta: Tensor, model_positions: Optional[Tensor], position_conversion: float):
+        """integrators.py:204-229 on the [P, N, 3] bead state, in place"""
+        b = self.base
+        _lib.call("spk_rpmd_main_step", ops._p(positions), ops._p(momenta), ops._p(model_positions), ops._p(b.masses),
+                  b.n_atoms, self.n_beads, ops._p(self.c_transform), ops._p(self.u), float(position_conversion),
+                  ops._stream())
+
+    def normal_modes(self, x: Tensor, inverse: bool = False) -> Tensor:
+        """beads -> normal modes (or back with ``inverse``) of a [P, N, 3] fp32 tensor, on the device"""
+        x = x.contiguous()
+        out = torch.empty_like(x)
+        _lib.call("spk_rpmd_normal_modes", ops._p(x), ops._p(out), x.numel() // (3 * self.n_beads), self.n_beads,
+                  ops._p(self.c_transform), 1 if inverse else 0, ops._stream())
+        return out
+
+
+class _RingPolymerThermostat(_Thermostat):
+    """Common part of the ring-polymer thermostats (thermostats_rpmd.py): they act on the normal modes of the bead momenta
+    and need the ``RingPolymer`` of the run.  ``systems`` are those of the base batch (one copy of every molecule)."""
+
+    ring_polymer = True
+
+    def bind(self, systems: _Systems, time_step: float, ring_polymer: Optional[RingPolymer] = None):
+        if ring_polymer is None:
+            raise ValueError(f"{type(self).__name__} is a ring-polymer thermostat: pass DeviceMD(ring_polymer=...)")
+        self.rp = ring_polymer
+        super().bind(systems, time_step)
+
+    def _ws(self) -> Tensor:
+        if getattr(self, "_rp_ws", None) is None:
+            s = self.systems
+            nbytes = int(_lib.lib().spk_rpmd_workspace_bytes(s.n_atoms, s.n_sys))
+            self._rp_ws = torch.empty(nbytes, dtype=torch.uint8, device=s.masses.device)
+        return self._rp_ws
+
+
+class PILELocalThermostat(_RingPolymerThermostat):
+    """Local path-integral Langevin thermostat (thermostats_rpmd.py:33-119): in normal-mode space p~_k = c1_k p~_k +
+    c2_k sqrt(m kB P T) xi with gamma_k = 2 omega_k (gamma_0 = 1 / tau when ``thermostat_centroid``), all times
+    ``damping_factor``, c1 = exp(-dt gamma / 2), c2 = sqrt(1 - c1^2).  xi comes from Philox4x32-10 keyed by ``seed`` with the
+    counter (k N + atom, application): mode 0 draws exactly the bits of ``LangevinThermostat`` with the same seed."""
+
+    _global = 0
+
+    def __init__(self, temperature_bath: float, time_constant: float, thermostat_centroid: bool = True,
+                 damping_factor: float = 1.0, seed: int = 0, kB: float = KB_MD, fs: float = FS_MD):
+        super().__init__(temperature_bath, time_constant, kB=kB, fs=fs)
+        self.thermostat_centroid = bool(thermostat_centroid)
+        self.damping_factor = float(damping_factor)
+        self.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self.counter: Optional[Tensor] = None
+
+    def _init_state(self):
+        dev = self.systems.masses.device
+        gamma = 2.0 * self.rp.omega_normal.clone()                            # :75
+        if self.thermostat_centroid:
+            gamma[0] = 1.0 / self.time_constant                               # :78-79
+        gamma = gamma * self.damping_factor                                   # :82
+        c1 = torch.exp(-0.5 * self.time_step * gamma)                         # :85
+        self.c1, self.c2 = c1.to(dev), torch.sqrt(1.0 - c1 ** 2).to(dev)      # :86
+        self.kbt_p = self.kB * self.rp.n_beads * self.temperature_bath        # :92-97
+        self.counter = torch.zeros(2, dtype=torch.int64, device=dev)
+
+    def apply(self, momenta: Tensor):
+        s = self.systems
+        _lib.call("spk_rpmd_pile", ops._p(momenta), ops._p(s.masses), ops._p(s.idx_m), ops._p(s.sys_ptr), s.n_atoms,
+                  s.n_sys, self.rp.n_beads, ops._p(self.rp.c_transform), ops._p(self.c1), ops._p(self.c2), self.kbt_p,
+                  self._global, self.seed, ops._p(self.counter), ops._p(self._ws()), self._ws().numel(), ops._stream(),
+                  launches=3 if self._global else 1)
+
+    def _state(self):
+        return {"counter": self.counter}
+
+
+class PILEGlobalThermostat(PILELocalThermostat):
+    """Global path-integral Langevin thermostat (thermostats_rpmd.py:122-208): stochastic velocity rescaling of the centroid
+    mode of every system, PILE-L on modes 1..P-1.  Per system, K0 = sum_a |p~_0,a|^2 / m_a, factor = K0 / (kB T P),
+    cf = (1 - c) / factor with c = c1_0, S = sum |xi_0|^2 over the system's 3 N centroid noises, alpha^2 = c + S cf +
+    2 R sqrt(c cf), alpha = sqrt(alpha^2) sign(R + sqrt(c / cf)), p~_0 *= alpha.
+
+    Two deliberate differences from the reference:
+      * R is the x-noise of each system's own first atom.  The reference takes the x-noise of the first atom of the whole
+        batch, so all molecules of a batch share one R; for a one-system batch the two agree.
+      * A system whose centroid kinetic energy is zero keeps its centroid as it is (the reference divides by zero and
+        writes NaN there, which happens when a run starts from zero momenta), as ``BerendsenThermostat`` does at T = 0."""
+
+    _global = 1
+
+    def __init__(self, temperature_bath: float, time_constant: float, seed: int = 0, kB: float = KB_MD,
+                 fs: float = FS_MD):
+        super().__init__(temperature_bath, time_constant, thermostat_centroid=True, damping_factor=1.0, seed=seed, kB=kB,
+                         fs=fs)
+
+
+class TRPMDThermostat(PILELocalThermostat):
+    """Thermostatted RPMD (thermostats_rpmd.py:211-234): PILE-L with time_constant = 1 fs, no centroid thermostat (the
+    centroid momenta pass through) and friction ``damping_factor`` x 2 omega_k on the other modes."""
+
+    def __init__(self, temperature_bath: float, damping_factor: float, seed: int = 0, kB: float = KB_MD,
+                 fs: float = FS_MD):
+        super().__init__(temperature_bath, 1.0, thermostat_centroid=False, damping_factor=damping_factor, seed=seed, kB=kB,
+                         fs=fs)
+
+
+class NHCRingPolymerThermostat(_RingPolymerThermostat):
+    """Ring-polymer Nose-Hoover chains (thermostats_rpmd.py:373-501): one chain per normal mode and degree of freedom on
+    p~, kinetic energy p~^2 / m, chain temperature P kB T, every link of mode k of mass P kB T / omega_k^2 with omega_0
+    replaced by 1 / (2 tau).  With ``local=False`` mode 0 of every degree of freedom sees its system's total centroid
+    sum |p~_0|^2 / m, with 3 N_s degrees of freedom and its first link 3 N_s times heavier.  The chain state is fp64 on the
+    device, [P 3 N, chain_length]."""
+
+    YS_WEIGHTS = NHCThermostat.YS_WEIGHTS
+
+    def __init__(self, temperature_bath: float, time_constant: float, local: bool = True, chain_length: int = 3,
+                 multi_step: int = 2, integration_order: int = 3, kB: float = KB_MD, fs: float = FS_MD):
+        super().__init__(temperature_bath, time_constant, kB=kB, fs=fs)
+        if integration_order not in self.YS_WEIGHTS:
+            raise ValueError(f"Order {integration_order:d} not supported for YS integration weights")
+        if int(chain_length) < 1 or int(multi_step) < 1:
+            raise ValueError("chain_length and multi_step must be >= 1")
+        self.local = bool(local)
+        self.chain_length = int(chain_length)
+        self.multi_step = int(multi_step)
+        self.integration_order = int(integration_order)
+        self.velocities = self.forces = self.masses = None
+
+    def _init_state(self):
+        s = self.systems
+        dev = s.masses.device
+        P, L, n_dof = self.rp.n_beads, self.chain_length, 3 * s.n_atoms
+        kbt = self.kB * self.temperature_bath * P                              # :431
+        freq = self.rp.omega_normal.clone()
+        freq[0] = 0.5 / self.time_constant                                     # :434-436
+        masses = (kbt / freq ** 2)[:, None, None].expand(P, n_dof, L).clone()  # :439-445
+        if not self.local:                                                     # :449-458
+            n_s = s.n_atoms_sys.cpu()[s.idx_m.cpu()]
+            masses[0, :, 0] *= (3.0 * n_s).repeat_interleave(3)
+        self.masses = masses.reshape(P * n_dof, L).to(dev)
+        self.velocities = torch.zeros_like(self.masses)
+        self.forces = torch.zeros_like(self.masses)
+        w = self.YS_WEIGHTS[self.integration_order]
+        steps = [self.time_step * wk / self.multi_step for wk in w] + [0.0] * (7 - len(w))
+        self.params = _lib.NHCParams(L, self.multi_step, self.integration_order, 1, kbt, (ctypes.c_double * 7)(*steps))
+
+    def apply(self, momenta: Tensor):
+        s = self.systems
+        g = 0 if self.local else 1
+        _lib.call("spk_rpmd_nhc", ops._p(momenta), ops._p(s.masses), ops._p(s.idx_m), ops._p(s.sys_ptr), s.n_atoms,
+                  s.n_sys, self.rp.n_beads, ops._p(self.rp.c_transform), ctypes.byref(self.params), g,
+                  ops._p(self.velocities), ops._p(self.forces), ops._p(self.masses), ops._p(self._ws()),
+                  self._ws().numel(), ops._stream(), launches=3 if g else 1)
+
+    def _state(self):
+        return {"velocities": self.velocities, "forces": self.forces}
+
+
 class DeviceMD:
     def __init__(self, model: torch.nn.Module, batch: Dict[str, Tensor], masses: Tensor, time_step: float, cutoff: float,
                  capacity: int, momenta: Optional[Tensor] = None, use_graph: bool = True,
                  position_conversion: float = 1.0, energy_conversion: float = 1.0,
                  thermostat: Optional[_Thermostat] = None, barostat: Optional[_NHCBarostat] = None,
-                 compute_stress: bool = False):
+                 compute_stress: bool = False, ring_polymer: Optional[RingPolymer] = None):
         """``batch[_positions]`` (and ``_cell``) are in MODEL units as everywhere in this package; ``self.positions`` is the
         MD-unit state (= model positions / position_conversion).  ``thermostat`` (None = NVE) is bound to the systems of
         the batch and applied around every step.  ``barostat`` (an NHC barostat, which thermostats the particles itself)
         makes the run NPT: every system must be periodic on all three axes.  ``compute_stress`` keeps the virial (and so
-        ``stress`` / ``pressure``) up to date in an NVE / NVT run."""
+        ``stress`` / ``pressure``) up to date in an NVE / NVT run.
+
+        ``ring_polymer`` (a ``RingPolymer``) makes the run ring-polymer MD: the B-system ``batch`` is replicated into P
+        beads, replica-major (P B systems; bead r of system m is system r B + m, positions [P, N, 3] flat as [P N, 3]), all
+        beads start at the batch positions, ``momenta`` may be [N, 3] (copied to every bead) or [P, N, 3], and ``capacity``
+        is the pair capacity of the whole bead batch.  It takes only the ring-polymer thermostats, no barostat and no
+        stress."""
         dev = batch[P.R].device
         if dev.type != "cuda":
             raise ValueError("DeviceMD needs a CUDA batch (no CPU fallback)")
         if barostat is not None and thermostat is not None:
             raise ValueError("DeviceMD: the NHC barostats contain their own thermostat (temperature_control = True); "
                              "pass either a thermostat or a barostat")
+        self._check_ring_polymer(ring_polymer, thermostat, barostat, compute_stress)
+        self.ring_polymer = ring_polymer
         self.model = model
         self.dt = float(time_step)
         self.p_conv = float(position_conversion)
         self.e_conv = float(energy_conversion)
         self.f_conv = self.e_conv / self.p_conv                                   # base_calculator.py:96
         self.static = {k: v.detach().clone() for k, v in batch.items() if k not in (P.idx_i, P.idx_j, P.offsets)}
+        masses = masses.to(dev, torch.float32).reshape(-1).contiguous().clone()
+        self._rp_base: Optional[_Systems] = None
+        if ring_polymer is not None:
+            self._rp_base = self._base_systems(masses)
+            b = self._rp_base
+            self.static.setdefault(P.idx_m, b.idx_m)
+            self.static.setdefault(P.n_atoms, (b.sys_ptr[1:] - b.sys_ptr[:-1]).to(torch.int64))
+            self.static = self._bead_batch(self.static, ring_polymer.n_beads, self._rp_base.n_sys)
+            masses = masses.repeat(ring_polymer.n_beads)
+            ring_polymer.bind(self._rp_base, self.dt)
         self.model_positions = self.static[P.R]                                   # what the model reads
         self.positions = self.model_positions if self.p_conv == 1.0 else self.model_positions / self.p_conv
-        self.masses = masses.to(dev, torch.float32).reshape(-1).contiguous().clone()
-        self.momenta = torch.zeros_like(self.positions) if momenta is None else momenta.to(dev, torch.float32).clone()
+        self.masses = masses
+        if momenta is None:
+            self.momenta = torch.zeros_like(self.positions)
+        elif ring_polymer is None:
+            self.momenta = momenta.to(dev, torch.float32).clone()
+        else:
+            momenta = momenta.to(dev, torch.float32).reshape(-1, 3)
+            if momenta.shape[0] == self._rp_base.n_atoms:
+                momenta = momenta.repeat(ring_polymer.n_beads, 1)                # [N, 3] -> every bead
+            if momenta.shape != self.positions.shape:
+                raise ValueError(f"DeviceMD: ring-polymer momenta must be [N, 3] or [P, N, 3], got "
+                                 f"{momenta.shape[0]} rows for N = {self._rp_base.n_atoms}, P = {ring_polymer.n_beads}")
+            self.momenta = momenta.contiguous().clone()
         self.nl = CellListNeighborList(cutoff, capacity=int(capacity), pad=True)
         self.use_graph = use_graph
         self.energy: Optional[Tensor] = None
@@ -392,8 +644,10 @@ class DeviceMD:
         self.steps_done = 0
         self._systems: Optional[_Systems] = None
         self.thermostat = thermostat
-        if thermostat is not None:
-            thermostat.bind(self.systems, self.dt)                                # on_simulation_start
+        if ring_polymer is not None and thermostat is not None:
+            thermostat.bind(self._rp_base, self.dt, ring_polymer)                # on_simulation_start
+        elif thermostat is not None:
+            thermostat.bind(self.systems, self.dt)
         self.barostat = barostat
         self.cell: Optional[Tensor] = None          # MD-unit cell [n_sys, 3, 3] fp64 (the model reads static[_cell])
         self.virial: Optional[Tensor] = None        # model-unit virial [n_sys, 3, 3] fp64, written by every evaluation
@@ -419,13 +673,65 @@ class DeviceMD:
     @property
     def systems(self) -> _Systems:
         if self._systems is None:
-            n = self.masses.shape[0]
-            idx_m = self.static.get(P.idx_m)
-            if idx_m is None:
-                idx_m = torch.zeros(n, dtype=torch.int64, device=self.masses.device)
-            n_sys = self.static[P.n_atoms].shape[0] if P.n_atoms in self.static else 1
-            self._systems = _Systems(self.masses, idx_m.to(torch.int64).contiguous(), n_sys)
+            self._systems = self._batch_systems(self.static, self.masses)
         return self._systems
+
+    @staticmethod
+    def _batch_systems(static: Dict[str, Tensor], masses: Tensor) -> _Systems:
+        idx_m = static.get(P.idx_m)
+        if idx_m is None:
+            idx_m = torch.zeros(masses.shape[0], dtype=torch.int64, device=masses.device)
+        n_sys = static[P.n_atoms].shape[0] if P.n_atoms in static else 1
+        return _Systems(masses, idx_m.to(torch.int64).contiguous(), n_sys)
+
+    # ---- ring-polymer set-up ------------------------------------------------------------------------------------------------
+    @staticmethod
+    def _check_ring_polymer(ring_polymer, thermostat, barostat, compute_stress):
+        """the combinations the reference refuses (md/cli.py:256-267) or this package does not build"""
+        rp_thermostat = getattr(thermostat, "ring_polymer", False)
+        if ring_polymer is None:
+            if rp_thermostat:
+                raise ValueError(f"DeviceMD: {type(thermostat).__name__} is a ring-polymer thermostat; it needs "
+                                 "ring_polymer=RingPolymer(...)")
+            return
+        if not isinstance(ring_polymer, RingPolymer):
+            raise TypeError("DeviceMD: ring_polymer must be a RingPolymer")
+        if thermostat is not None and not rp_thermostat:
+            raise ValueError(f"DeviceMD: {type(thermostat).__name__} is a classical thermostat; ring-polymer MD takes "
+                             "PILELocalThermostat, PILEGlobalThermostat, TRPMDThermostat or NHCRingPolymerThermostat")
+        if barostat is not None:
+            raise ValueError("DeviceMD: ring-polymer MD with a barostat (the RPMD barostats) is not supported")
+        if compute_stress:
+            raise ValueError("DeviceMD: compute_stress is not supported for ring-polymer MD")
+
+    def _base_systems(self, masses: Tensor) -> _Systems:
+        n = self.static[P.R].shape[0]
+        if masses.shape[0] != n:
+            raise ValueError(f"DeviceMD: {masses.shape[0]} masses for {n} atoms")
+        return self._batch_systems(self.static, masses)
+
+    @staticmethod
+    def _bead_batch(static: Dict[str, Tensor], n_beads: int, n_sys: int) -> Dict[str, Tensor]:
+        """P replicas of the batch, replica-major as the reference's calculator collates them
+        (md/calculators/base_calculator.py:154-221): ``_idx_m`` + r B, every other tensor repeated along its first axis.
+        A ``_cell`` / ``_pbc`` shared by all B systems ([3, 3] or [1, 3, 3] / [3] or [1, 3], which the neighbour list
+        broadcasts) is first expanded to one row per system, so the bead batch has one per bead system."""
+        out = {}
+        for k, v in static.items():
+            if k == P.idx_m:
+                out[k] = torch.cat([v + r * n_sys for r in range(n_beads)])
+                continue
+            if k in (P.cell, P.pbc):
+                width = 9 if k == P.cell else 3
+                rows = v.reshape(-1, width)
+                if rows.shape[0] == 1:
+                    rows = rows.expand(n_sys, width)
+                if rows.shape[0] != n_sys:
+                    raise ValueError(f"DeviceMD: '{k}' of shape {tuple(v.shape)} is neither shared nor one per system "
+                                     f"for {n_sys} systems")
+                v = rows.reshape(n_sys, 3, 3) if k == P.cell else rows.reshape(-1) if v.dim() == 1 else rows
+            out[k] = torch.cat([v] * n_beads).contiguous()
+        return out
 
     # ---- one force evaluation on the current positions (calculator.calculate) ---------------------------------------------
     def _calculate(self):
@@ -466,7 +772,23 @@ class DeviceMD:
         b.kick(self.momenta, self.cell, self.virial, self._virial_scale())        # simulator.py:149-150 on_step_end
         b.apply_thermostat(self.momenta)
 
+    def _rpmd_step(self):
+        """md/simulator.py:124-150 with the RingPolymer integrator (integrators.py:59-70,204-229): thermostat, half kick on
+        every bead, ring-polymer main step, neighbour list + energy + forces on all P B bead systems, half kick,
+        thermostat"""
+        mp = self.model_positions if self.model_positions is not self.positions else None
+        if self.thermostat is not None:
+            self.thermostat.apply(self.momenta)
+        self._verlet(False)
+        self.ring_polymer.main_step(self.positions, self.momenta, mp, self.p_conv)
+        self._calculate()
+        self._verlet(False)
+        if self.thermostat is not None:
+            self.thermostat.apply(self.momenta)
+
     def _step(self):
+        if self.ring_polymer is not None:
+            return self._rpmd_step()
         if self.barostat is not None:
             return self._npt_step()
         if self.thermostat is not None:
@@ -537,9 +859,44 @@ class DeviceMD:
         """Instantaneous temperature of every system in K (system.py:407-421), fp64 on the device; ``kB`` in MD energy per
         kelvin defaults to the thermostat's, else to the reference's MD units."""
         if kB is None:
-            hook = self.thermostat if self.thermostat is not None else self.barostat
-            kB = hook.kB if hook is not None else KB_MD
-        return self.systems.kinetic_energy_and_temperature(self.momenta, kB)[1]
+            kB = self._kB()
+        t = self.systems.kinetic_energy_and_temperature(self.momenta, kB)[1]
+        if self.ring_polymer is not None:                                  # per bead and system (system.py:407-421)
+            t = t.reshape(self.ring_polymer.n_beads, -1)
+        return t
+
+    def _kB(self) -> float:
+        hook = self.thermostat if self.thermostat is not None else self.barostat
+        if hook is not None:
+            return hook.kB
+        return self.ring_polymer.kB if self.ring_polymer is not None else KB_MD
+
+    # ---- centroid accessors of ring-polymer runs (system.py:484-565), MD units, on the device -----------------------------
+    def _need_rp(self) -> RingPolymer:
+        if self.ring_polymer is None:
+            raise RuntimeError("DeviceMD: centroid quantities need a ring-polymer run (ring_polymer=RingPolymer(...))")
+        return self.ring_polymer
+
+    def centroid_positions(self) -> Tensor:
+        """bead average of the positions [N, 3] (system.py:484-495)"""
+        rp = self._need_rp()
+        return self.positions.reshape(rp.n_beads, -1, 3).mean(0)
+
+    def centroid_momenta(self) -> Tensor:
+        """bead average of the momenta [N, 3] (system.py:497-508)"""
+        rp = self._need_rp()
+        return self.momenta.reshape(rp.n_beads, -1, 3).mean(0)
+
+    def centroid_temperature(self, kB: Optional[float] = None) -> Tensor:
+        """2 / (3 N_s kB) * 1/2 sum_a |p_c,a|^2 / m_a per system [B] fp64 (system.py:523-555)"""
+        self._need_rp()
+        pc = self.centroid_momenta().contiguous()
+        return self._rp_base.kinetic_energy_and_temperature(pc, self._kB() if kB is None else kB)[1]
+
+    def centroid_potential_energy(self) -> Tensor:
+        """bead average of the potential energy [B] in MD units (system.py:557-565)"""
+        rp = self._need_rp()
+        return self.potential_energy().reshape(rp.n_beads, -1).mean(0)
 
     def state_dict(self) -> Dict[str, object]:
         """Everything a restarted run needs to continue bitwise: the MD state, the neighbour-list bookkeeping and the
