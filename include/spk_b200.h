@@ -484,6 +484,41 @@ int spk_rpmd_nhc(float* momenta, const float* masses, const int64_t* idx_m, cons
                  double* chain_v, double* chain_f, const double* chain_m, void* workspace, size_t workspace_bytes,
                  spk_stream_t stream);
 
+/* ---- PILE barostat of ring-polymer NPT (csrc/rpmd.cu; md/simulation_hooks/barostats_rpmd.py:21-208 PILEBarostat with
+ * md/integrators.py:266-305 NPTRingPolymer).  One isotropic cell momentum p_c of mass W per system of the base batch
+ * (cell_momenta, cell_mass [n_sys] fp64); bead arrays, masses, idx_m and sys_ptr as for spk_rpmd_pile; cells and virial
+ * [n_beads n_sys, 3, 3] fp64 per bead system, replica-major (bead r of system s is r n_sys + s).  workspace:
+ * spk_rpmd_barostat_workspace_bytes(n_atoms, n_sys) bytes, 8-byte aligned, shared by the half and main step, no
+ * initialisation needed.  Every sum is fixed-order fp64 without atomics.  One NPT-RPMD step (md/simulator.py:124-150)
+ * is: thermostat, barostat_thermostat, half_step + spk_md_velocity_verlet(drift = 0), main_step, forces + virial,
+ * half_step + spk_md_velocity_verlet(drift = 0), barostat_thermostat, thermostat.
+ *   spk_rpmd_barostat_thermostat  p_c = c1 p_c + c2[s] xi (barostats_rpmd.py:101-110): xi is normal 0 of the Philox4x32-10
+ *                                 draw with key seed and counter (s, counter[0]); counter [2] as for spk_rpmd_pile
+ *   spk_rpmd_barostat_half_step   p_c += h c1 + h^2 c2 + h^3 c3, h = time_step / 2 (barostats_rpmd.py:164-205), from the
+ *                                 momenta before the particle kick: c1 = 3 P (V_bar (P_c - target_pressure) +
+ *                                 kb_temperature) with V_bar the bead mean of det(cell), P_c = -tr(bead mean of the stress)
+ *                                 / 3 + 2 K_c / (3 V_bar), stress = virial_scale virial / det(cell), K_c from the bead mean
+ *                                 of the momenta; c2 = sum F~_0 . p~_0 / m, c3 = sum |F~_0|^2 / (3 m) over normal mode 0 of
+ *                                 the momenta and of the forces * force_conversion.  2 launches.
+ *   spk_rpmd_barostat_main_step   a = exp(-dt p_c / W), b = StableSinhDiv(dt p_c / W) per system; p~_0 *= a, then x~_0 =
+ *                                 x~_0 / a + b dt p~_0 / m; modes k >= 1 by the propagator as spk_rpmd_main_step; every
+ *                                 bead copy of the cell divided by a, model_cells (nullable) = cells * position_conversion
+ *                                 in fp32 (barostats_rpmd.py:113-162).  2 launches. */
+size_t spk_rpmd_barostat_workspace_bytes(int64_t n_atoms, int64_t n_sys);
+int spk_rpmd_barostat_thermostat(double* cell_momenta, int64_t n_sys, double c1, const double* c2, uint64_t seed,
+                                 uint64_t* counter, spk_stream_t stream);
+int spk_rpmd_barostat_half_step(const float* momenta, const float* forces, double force_conversion, const float* masses,
+                                const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms, int64_t n_sys,
+                                int32_t n_beads, const double* c_transform, const double* cells, const double* virial,
+                                double virial_scale, double target_pressure, double kb_temperature, double time_step,
+                                const double* cell_mass, double* cell_momenta, void* workspace, size_t workspace_bytes,
+                                spk_stream_t stream);
+int spk_rpmd_barostat_main_step(float* positions, float* momenta, float* model_positions, const float* masses,
+                                const int64_t* idx_m, int64_t n_atoms, int64_t n_sys, int32_t n_beads,
+                                const double* c_transform, const double* propagator, double time_step,
+                                const double* cell_momenta, const double* cell_mass, double* cells, float* model_cells,
+                                double position_conversion, void* workspace, size_t workspace_bytes, spk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

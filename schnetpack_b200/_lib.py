@@ -119,13 +119,20 @@ SIGNATURES = {
     "spk_rpmd_main_step": [P, P, P, P, c_int64, c_int32, P, P, c_double, P],
     "spk_rpmd_pile": [P, P, P, P, c_int64, c_int64, c_int32, P, P, P, c_double, c_int32, c_uint64, P, P, c_size_t, P],
     "spk_rpmd_nhc": [P, P, P, P, c_int64, c_int64, c_int32, P, POINTER(NHCParams), c_int32, P, P, P, P, c_size_t, P],
+    "spk_rpmd_barostat_workspace_bytes": [c_int64, c_int64],
+    "spk_rpmd_barostat_thermostat": [P, c_int64, c_double, P, c_uint64, P, P],
+    "spk_rpmd_barostat_half_step": [P, P, c_double, P, P, P, c_int64, c_int64, c_int32, P, P, P, c_double, c_double,
+                                    c_double, c_double, P, P, P, c_size_t, P],
+    "spk_rpmd_barostat_main_step": [P, P, P, P, P, c_int64, c_int64, c_int32, P, P, c_double, P, P, P, P, c_double, P,
+                                    c_size_t, P],
 }
 _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_size_t,
             "spk_pairwise_virial_workspace_bytes": c_size_t, "spk_md_barostat_workspace_bytes": c_size_t,
             "spk_tc_packed_floats_tn": c_size_t, "spk_atom_chain_workspace_ints": c_size_t,
             "spk_schnet_filter_packed_floats": c_size_t,
             "spk_painn_filter_packed_floats": c_size_t, "spk_neighbor_list_workspace_bytes": c_size_t,
-            "spk_md_thermostat_workspace_bytes": c_size_t, "spk_rpmd_workspace_bytes": c_size_t}
+            "spk_md_thermostat_workspace_bytes": c_size_t, "spk_rpmd_workspace_bytes": c_size_t,
+            "spk_rpmd_barostat_workspace_bytes": c_size_t}
 
 _lib = None
 
@@ -167,7 +174,8 @@ def check(rc: int, name: str):
 LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out": 2, "spk_neighbor_list": 6,
             "spk_md_kinetic_energy": 2, "spk_md_berendsen": 3, "spk_pairwise_virial": 2,
             "spk_md_kinetic_energy_tensor": 3, "spk_md_barostat_thermostat": 4, "spk_md_barostat_kick": 3,
-            "spk_md_barostat_half_step": 2, "spk_md_barostat_main_step": 2}   # spk_rpmd_pile / spk_rpmd_nhc: 3 if global
+            "spk_md_barostat_half_step": 2, "spk_md_barostat_main_step": 2, "spk_rpmd_barostat_half_step": 2,
+            "spk_rpmd_barostat_main_step": 2}   # spk_rpmd_pile / spk_rpmd_nhc: 3 if global
 launch_count = 0
 
 

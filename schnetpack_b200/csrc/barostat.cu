@@ -77,10 +77,6 @@ __device__ __forceinline__ void system_ke(const int32_t* __restrict__ sys_ptr, c
     k2[5] = k2[7] = acc[6];
 }
 
-__device__ __forceinline__ double det3(const double* __restrict__ c) {   // system.py:575-580: c0 . (c1 x c2)
-    return c[0] * (c[4] * c[8] - c[5] * c[7]) + c[1] * (c[5] * c[6] - c[3] * c[8]) + c[2] * (c[3] * c[7] - c[4] * c[6]);
-}
-
 __device__ __forceinline__ spk_nhc_params_t chain_params(const spk_nhc_barostat_t& b) {
     spk_nhc_params_t q;
     q.chain_length = b.chain_length;

@@ -1,6 +1,6 @@
 // Device code shared by the thermostat (thermostat.cu), barostat (barostat.cu) and ring-polymer (rpmd.cu) kernels of the
 // device MD step: the Nose-Hoover chain propagator, the momentum scalings, the Philox4x32-10 generator with Box-Muller, the
-// reference's sinh(x)/x series and a 3x3 symmetric Jacobi eigensolver.
+// reference's sinh(x)/x series, the cell volume and a 3x3 symmetric Jacobi eigensolver.
 #pragma once
 #include "segscan.cuh"
 
@@ -99,6 +99,10 @@ __host__ __device__ __forceinline__ double stable_sinh_div(double x) {
     const double x2 = x * x;
     if (x < eps) return (((e8 * x2 + e6) * x2 + e4) * x + e2) * x2 + e0;
     return sinh(x) / x;
+}
+
+__device__ __forceinline__ double det3(const double* __restrict__ c) {   // system.py:575-580: c0 . (c1 x c2)
+    return c[0] * (c[4] * c[8] - c[5] * c[7]) + c[1] * (c[5] * c[6] - c[3] * c[8]) + c[2] * (c[3] * c[7] - c[4] * c[6]);
 }
 
 // Eigendecomposition of the symmetric 3x3 matrix whose upper triangle is a[0..8] (row-major; the lower triangle is not

@@ -1,7 +1,8 @@
 // Ring-polymer MD of the device MD step: the normal-mode transform (md/utils/normal_model_transformation.py:37-101), the
 // free ring-polymer propagation of the RingPolymer integrator (md/integrators.py:154-229) and the ring-polymer thermostats
-// PILE-L / PILE-G / TRPMD and NHC (md/simulation_hooks/thermostats_rpmd.py:33-234,373-501).  Every entry point only
-// enqueues work, so the whole RPMD step stays one CUDA graph.
+// PILE-L / PILE-G / TRPMD and NHC (md/simulation_hooks/thermostats_rpmd.py:33-234,373-501), and the PILE barostat of
+// ring-polymer NPT (md/simulation_hooks/barostats_rpmd.py:21-208 with md/integrators.py:266-305 NPTRingPolymer).  Every
+// entry point only enqueues work, so the whole RPMD step stays one CUDA graph.
 //
 // Bead arrays are [P, n_atoms, 3] fp32, replica-major, so for a fixed bead a run of consecutive degrees of freedom (atom,
 // component) is contiguous.  The mode kernels give a CTA RP_T = 32 consecutive degrees of freedom across all P beads: the
@@ -11,7 +12,9 @@
 // 48 KB at P = 64.
 //
 // The per-system centroid sums of the global thermostats use the fixed-shape segmented scan of segscan.cuh and one ordered
-// finishing pass per system: no atomics touch a sum, so every call is bitwise reproducible.
+// finishing pass per system: no atomics touch a sum, so every call is bitwise reproducible.  The barostat's half step
+// forms its three per-system sums over the mode-0 forces and momenta the same way; its finishing CTA also averages the
+// P bead volumes and virials of its system and updates the cell momentum.
 #include "md_common.cuh"
 
 namespace {
@@ -21,8 +24,9 @@ constexpr int RP_THREADS = 256;
 constexpr int RP_KT = 256;        // atoms per CTA of the centroid partial pass
 constexpr int RP_NV = 2;          // centroid sums: sum |p~_0|^2 / m, sum |xi_0|^2
 constexpr int RP_MAX_BEADS = 64;
+constexpr int RB_NV = 3;          // barostat sums: sum F~_0 . p~_0 / m, sum |F~_0|^2 / (3 m), sum |p_bar|^2 / m
 
-enum RpmdOp { OP_MAIN = 0, OP_PILE = 1, OP_NHC = 2 };
+enum RpmdOp { OP_MAIN = 0, OP_PILE = 1, OP_NHC = 2, OP_BARO = 3 };
 
 struct RpmdArgs {
     float* x;                     // bead positions (OP_MAIN)
@@ -32,7 +36,8 @@ struct RpmdArgs {
     const int64_t* idx_m;
     const int32_t* sys_ptr;
     const double* C;              // [P, P]
-    const double* prop;           // [P, 2, 2] (OP_MAIN)
+    const double* prop;           // [P, 2, 2] (OP_MAIN, OP_BARO)
+    const double* baro_ab;        // [n_sys, 2] per-system (a, b) of the barostat's centroid propagation (OP_BARO)
     const double* c1;             // [P] (OP_PILE)
     const double* c2;
     const double* tot;            // [n_sys, RP_NV] centroid sums (global variants)
@@ -42,6 +47,7 @@ struct RpmdArgs {
     unsigned long long* counter;  // [2]: application index, ticket (OP_PILE)
     int64_t n_atoms;
     double pos_conv;
+    double dt;                    // time step (OP_BARO)
     double kbt_p;                 // P kB T (OP_PILE)
     uint64_t seed;
     int32_t P;
@@ -89,6 +95,7 @@ __device__ __forceinline__ double pile_alpha(const RpmdArgs& A, uint64_t app, in
 // beads -> normal modes, the per-mode operator OP, normal modes -> beads, for RP_T degrees of freedom per CTA
 template <int OP>
 __global__ void __launch_bounds__(RP_THREADS) k_rpmd_modes(const __grid_constant__ RpmdArgs A) {
+    constexpr bool HAS_X = OP == OP_MAIN || OP == OP_BARO;
     extern __shared__ double smem[];
     const int P = A.P;
     const int PT = P * RP_T;
@@ -105,7 +112,7 @@ __global__ void __launch_bounds__(RP_THREADS) k_rpmd_modes(const __grid_constant
         const int b = j / RP_T;
         const int64_t i = i0 + (j % RP_T);
         if (i < n_dof) {
-            if (OP == OP_MAIN) bx[j] = A.x[b * n_dof + i];
+            if (HAS_X) bx[j] = A.x[b * n_dof + i];
             bp[j] = A.p[b * n_dof + i];
         }
     }
@@ -118,12 +125,16 @@ __global__ void __launch_bounds__(RP_THREADS) k_rpmd_modes(const __grid_constant
         double xn = 0.0, pn = 0.0;
         for (int b = 0; b < P; ++b) {                    // normal_model_transformation.py:78-80 beads2normal
             const double c = Ck[b];
-            if (OP == OP_MAIN) xn += c * (double)bx[b * RP_T + t];
+            if (HAS_X) xn += c * (double)bx[b * RP_T + t];
             pn += c * (double)bp[b * RP_T + t];
         }
         const int64_t a = i / 3;
         const double ma = (double)A.m[a];
-        if (OP == OP_MAIN) {                             // integrators.py:221-230
+        if (OP == OP_BARO && k == 0) {                   // barostats_rpmd.py:136-143: the scaled p~_0 drives x~_0
+            const double* ab = A.baro_ab + 2 * A.idx_m[a];
+            pn = pn * ab[0];
+            xn = xn / ab[0] + ab[1] * (pn / ma) * A.dt;
+        } else if (HAS_X) {                              // integrators.py:221-230, barostats_rpmd.py:152-160
             const double* u = A.prop + 4 * k;
             const double np = u[0] * pn + u[1] * xn * ma;
             xn = u[2] * pn / ma + u[3] * xn;
@@ -146,7 +157,7 @@ __global__ void __launch_bounds__(RP_THREADS) k_rpmd_modes(const __grid_constant
             const int64_t row = (int64_t)k * n_dof + i;
             pn *= nhc_propagate(ke, dof, A.q, A.chain_v + row * L, A.chain_f + row * L, A.chain_m + row * L);
         }
-        if (OP == OP_MAIN) mx[j] = xn;
+        if (HAS_X) mx[j] = xn;
         mp[j] = pn;
     }
     __syncthreads();
@@ -157,11 +168,11 @@ __global__ void __launch_bounds__(RP_THREADS) k_rpmd_modes(const __grid_constant
         double xb = 0.0, pb = 0.0;
         for (int k = 0; k < P; ++k) {                    // normal_model_transformation.py:93-101 normal2beads
             const double c = A.C[(int64_t)k * P + b];
-            if (OP == OP_MAIN) xb += c * mx[k * RP_T + t];
+            if (HAS_X) xb += c * mx[k * RP_T + t];
             pb += c * mp[k * RP_T + t];
         }
         A.p[b * n_dof + i] = (float)pb;
-        if (OP == OP_MAIN) {
+        if (HAS_X) {
             const float xf = (float)xb;
             A.x[b * n_dof + i] = xf;
             if (A.model_x) A.model_x[b * n_dof + i] = xf * (float)A.pos_conv;
@@ -242,6 +253,153 @@ __global__ void __launch_bounds__(RP_KT) k_rpmd_centroid_partials(const __grid_c
     dst[1] = v[1];
 }
 
+// ---- PILE barostat (barostats_rpmd.py) -----------------------------------------------------------------------------------
+struct BaroArgs {
+    const float* p;               // bead momenta [P, n_atoms, 3]
+    const float* f;               // bead forces [P, n_atoms, 3], model units (times f_conv)
+    const float* m;               // [n_atoms]
+    const int64_t* idx_m;         // base batch
+    const int32_t* sys_ptr;
+    const double* C;              // [P, P]
+    const double* cell;           // [P n_sys, 3, 3] MD cells of the bead systems
+    const double* virial;         // [P n_sys, 3, 3] model-unit virials of the bead systems
+    const double* W;              // [n_sys] cell masses
+    double* pc;                   // [n_sys] cell momenta
+    int64_t n_atoms;
+    int64_t n_sys;
+    double f_conv;
+    double virial_scale;          // stress = virial_scale * virial / det(cell)
+    double target_pressure;
+    double kbt;
+    double dt;
+    int32_t P;
+};
+
+struct BaroWorkspace {
+    double* sys_part;  // [n_sys, RB_NV]
+    double* ab;        // [n_sys, 2]
+    double* head;      // [n_blocks, RB_NV]
+};
+
+static inline BaroWorkspace carve_baro(void* ws, int64_t n_sys) {
+    double* d = reinterpret_cast<double*>(ws);
+    return BaroWorkspace{d, d + RB_NV * n_sys, d + (RB_NV + 2) * n_sys};
+}
+
+// _update_barostat (barostats_rpmd.py:101-110): p_c = c1 p_c + c2[s] xi, one thread per system; xi is normal 0 of the
+// Philox draw (seed; counter = system, application), and the application index advances by the ticket of k_langevin
+__global__ void k_rpmd_baro_pile(double* __restrict__ pc, int64_t n_sys, double c1, const double* __restrict__ c2,
+                                 uint64_t seed, unsigned long long* counter) {
+    SPK_PDL_ENTER();
+    const unsigned long long app = *(volatile unsigned long long*)counter;
+    const int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (s < n_sys) {
+        const uint4 r = philox_draw(seed, app, s);
+        pc[s] = c1 * pc[s] + c2[s] * box_muller(r.x, r.y).x;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        if (atomicAdd(counter + 1, 1ull) == gridDim.x - 1) {
+            counter[0] = app + 1;
+            counter[1] = 0;
+            __threadfence();
+        }
+    }
+}
+
+// propagate_half_step (barostats_rpmd.py:173-199), per-(system, CTA) partials over the base atoms: mode 0 of the forces
+// (MD units) and momenta, one row of C across the P beads, and the bead mean of the momenta
+__global__ void __launch_bounds__(RP_KT) k_rpmd_baro_partials(const __grid_constant__ BaroArgs B,
+                                                              double* __restrict__ sys_part, double* __restrict__ head) {
+    __shared__ double sv[RB_NV][RP_KT];
+    __shared__ int sf[RP_KT];
+    SPK_PDL_ENTER();
+    const int t = threadIdx.x;
+    const int64_t b0 = (int64_t)blockIdx.x * RP_KT;
+    const int64_t a = b0 + t;
+    const int64_t n_dof = 3 * B.n_atoms;
+    double v[RB_NV] = {0.0, 0.0, 0.0};
+    int f = 1;
+    int64_t s = -1;
+    if (a < B.n_atoms) {
+        const double ma = (double)B.m[a];
+        double pm2 = 0.0;
+        for (int d = 0; d < 3; ++d) {
+            double p0 = 0.0, f0 = 0.0, ps = 0.0;
+            for (int b = 0; b < B.P; ++b) {
+                const int64_t i = b * n_dof + 3 * a + d;
+                const double pb = (double)B.p[i];
+                p0 += B.C[b] * pb;
+                f0 += B.C[b] * ((double)B.f[i] * B.f_conv);
+                ps += pb;
+            }
+            const double fm = f0 / ma;                   // :180
+            v[0] += fm * p0;                             // :182-184
+            v[1] += fm * f0 / 3.0;                       // :185-187
+            const double pm = ps / (double)B.P;          // system.py:497-508, 524-537
+            pm2 += pm * pm;
+        }
+        v[2] = pm2 / ma;
+        s = B.idx_m[a];
+        f = (t == 0) || (B.idx_m[a - 1] != s);
+    }
+    seg_scan<RP_KT, RB_NV>(v, f, sv, sf);
+    if (a >= B.n_atoms) return;
+    const bool seg_end = (t == RP_KT - 1) || (a == B.n_atoms - 1) || (B.idx_m[a + 1] != s);
+    if (!seg_end) return;
+    double* dst = B.sys_ptr[s] >= b0 ? sys_part + s * RB_NV : head + (int64_t)blockIdx.x * RB_NV;
+    for (int c = 0; c < RB_NV; ++c) dst[c] = v[c];
+}
+
+// one CTA per system: the ordered total of the partials, then (thread 0) the centroid pressure from the bead means of the
+// volume and stress (system.py:616-650) and p_c += h c1 + h^2 c2 + h^3 c3 with h = dt / 2 (barostats_rpmd.py:164-205)
+__global__ void __launch_bounds__(SEG_FIN_T) k_rpmd_baro_finish(const __grid_constant__ BaroArgs B,
+                                                                const double* __restrict__ sys_part,
+                                                                const double* __restrict__ head) {
+    __shared__ double red[RB_NV][SEG_FIN_T];
+    SPK_PDL_ENTER();
+    const int64_t s = blockIdx.x;
+    seg_finish_block<RP_KT, RB_NV>(B.sys_ptr, nullptr, sys_part, head, s, red);
+    if (threadIdx.x != 0) return;
+    double vsum = 0.0, st[3] = {0.0, 0.0, 0.0};
+    for (int r = 0; r < B.P; ++r) {
+        const int64_t bs = (int64_t)r * B.n_sys + s;
+        const double V = det3(B.cell + 9 * bs);
+        vsum += V;
+        for (int k = 0; k < 3; ++k) st[k] += B.virial_scale * B.virial[9 * bs + 4 * k] / V;
+    }
+    const double inv_p = 1.0 / (double)B.P;
+    const double vbar = vsum * inv_p;
+    const double p_vir = ((-st[0] * inv_p) + (-st[1] * inv_p) + (-st[2] * inv_p)) / 3.0;
+    const double p_cent = p_vir + 2.0 * (0.5 * red[2][0]) / vbar / 3.0;
+    const double c1 = 3.0 * (double)B.P * (vbar * (p_cent - B.target_pressure) + B.kbt);
+    const double h = 0.5 * B.dt;
+    B.pc[s] = B.pc[s] + (h * c1 + (h * h) * red[0][0] + (h * h * h) * red[1][0]);
+}
+
+// propagate_main_step (barostats_rpmd.py:119-133), one thread per system: (a, b) = (exp(-dt p_c / W), StableSinhDiv(dt
+// p_c / W)) for the mode kernel, and every bead copy of the cell divided by a (model cell = MD cell * position_conversion)
+__global__ void k_rpmd_baro_cell(const double* __restrict__ pc, const double* __restrict__ W, int64_t n_sys, int P,
+                                 double dt, double* __restrict__ cell, float* __restrict__ model_cell, double pos_conv,
+                                 double* __restrict__ ab) {
+    SPK_PDL_ENTER();
+    const int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (s >= n_sys) return;
+    const double x = dt * (pc[s] / W[s]);
+    const double a = exp(-x);
+    ab[2 * s] = a;
+    ab[2 * s + 1] = stable_sinh_div(x);
+    for (int r = 0; r < P; ++r) {
+        const int64_t bs = (int64_t)r * n_sys + s;
+        for (int k = 0; k < 9; ++k) {
+            const double c = cell[9 * bs + k] / a;
+            cell[9 * bs + k] = c;
+            if (model_cell) model_cell[9 * bs + k] = (float)(c * pos_conv);
+        }
+    }
+}
+
 static bool beads_ok(int P, const double* C) { return P >= 1 && P <= RP_MAX_BEADS && C; }
 
 static int check_modes(const float* momenta, const float* masses, int64_t n_atoms, int P, const double* C) {
@@ -273,6 +431,11 @@ static void centroid_sums(RpmdArgs& A, int with_noise, int64_t n_sys, void* work
 }
 
 }  // namespace
+
+extern "C" size_t spk_rpmd_barostat_workspace_bytes(int64_t n_atoms, int64_t n_sys) {
+    const int64_t nb = n_atoms > 0 ? rp_blocks(n_atoms) : 0;
+    return sizeof(double) * (size_t)((RB_NV + 2) * (n_sys > 0 ? n_sys : 0) + RB_NV * nb + 1);
+}
 
 extern "C" size_t spk_rpmd_workspace_bytes(int64_t n_atoms, int64_t n_sys) {
     const int64_t nb = n_atoms > 0 ? rp_blocks(n_atoms) : 0;
@@ -371,6 +534,89 @@ extern "C" int spk_rpmd_nhc(float* momenta, const float* masses, const int64_t* 
     A.q = *params;
     if (A.global) centroid_sums(A, 0, n_sys, workspace, st);
     launch_modes<OP_NHC>(A, st);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_rpmd_barostat_thermostat(double* cell_momenta, int64_t n_sys, double c1, const double* c2, uint64_t seed,
+                                            uint64_t* counter, spk_stream_t stream) {
+    if (n_sys <= 0 || !cell_momenta || !c2 || !counter) return SPK_ERR_ARG;
+    spk_launch(k_rpmd_baro_pile, (unsigned)spk_cdiv(n_sys, 128), 128, 0, spk_st(stream), cell_momenta, n_sys, c1, c2,
+               seed, reinterpret_cast<unsigned long long*>(counter));
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_rpmd_barostat_half_step(const float* momenta, const float* forces, double force_conversion,
+                                           const float* masses, const int64_t* idx_m, const int32_t* sys_ptr,
+                                           int64_t n_atoms, int64_t n_sys, int32_t n_beads, const double* c_transform,
+                                           const double* cells, const double* virial, double virial_scale,
+                                           double target_pressure, double kb_temperature, double time_step,
+                                           const double* cell_mass, double* cell_momenta, void* workspace,
+                                           size_t workspace_bytes, spk_stream_t stream) {
+    if (check_modes(momenta, masses, n_atoms, n_beads, c_transform) != SPK_OK) return SPK_ERR_ARG;
+    if (n_sys <= 0 || !sys_ptr || (n_atoms > 0 && (!idx_m || !forces))) return SPK_ERR_ARG;
+    if (!cells || !virial || !cell_mass || !cell_momenta || !workspace ||
+        workspace_bytes < spk_rpmd_barostat_workspace_bytes(n_atoms, n_sys))
+        return SPK_ERR_ARG;
+    cudaStream_t st = spk_st(stream);
+    const BaroWorkspace w = carve_baro(workspace, n_sys);
+    BaroArgs B = {};
+    B.p = momenta;
+    B.f = forces;
+    B.m = masses;
+    B.idx_m = idx_m;
+    B.sys_ptr = sys_ptr;
+    B.C = c_transform;
+    B.cell = cells;
+    B.virial = virial;
+    B.W = cell_mass;
+    B.pc = cell_momenta;
+    B.n_atoms = n_atoms;
+    B.n_sys = n_sys;
+    B.f_conv = force_conversion;
+    B.virial_scale = virial_scale;
+    B.target_pressure = target_pressure;
+    B.kbt = kb_temperature;
+    B.dt = time_step;
+    B.P = n_beads;
+    if (n_atoms > 0)
+        spk_launch(k_rpmd_baro_partials, (unsigned)rp_blocks(n_atoms), RP_KT, 0, st, B, w.sys_part, w.head);
+    spk_launch(k_rpmd_baro_finish, (unsigned)n_sys, SEG_FIN_T, 0, st, B, (const double*)w.sys_part,
+               (const double*)w.head);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_rpmd_barostat_main_step(float* positions, float* momenta, float* model_positions, const float* masses,
+                                           const int64_t* idx_m, int64_t n_atoms, int64_t n_sys, int32_t n_beads,
+                                           const double* c_transform, const double* propagator, double time_step,
+                                           const double* cell_momenta, const double* cell_mass, double* cells,
+                                           float* model_cells, double position_conversion, void* workspace,
+                                           size_t workspace_bytes, spk_stream_t stream) {
+    if (check_modes(momenta, masses, n_atoms, n_beads, c_transform) != SPK_OK || !propagator) return SPK_ERR_ARG;
+    if (n_sys <= 0 || !cells || !cell_momenta || !cell_mass || (n_atoms > 0 && (!positions || !idx_m))) return SPK_ERR_ARG;
+    if (!workspace || workspace_bytes < spk_rpmd_barostat_workspace_bytes(n_atoms, n_sys)) return SPK_ERR_ARG;
+    cudaStream_t st = spk_st(stream);
+    const BaroWorkspace w = carve_baro(workspace, n_sys);
+    spk_launch(k_rpmd_baro_cell, (unsigned)spk_cdiv(n_sys, 128), 128, 0, st, cell_momenta, cell_mass, n_sys,
+               (int)n_beads, time_step, cells, model_cells, position_conversion, w.ab);
+    if (n_atoms > 0) {
+        RpmdArgs A = {};
+        A.x = positions;
+        A.p = momenta;
+        A.model_x = model_positions;
+        A.m = masses;
+        A.idx_m = idx_m;
+        A.C = c_transform;
+        A.prop = propagator;
+        A.baro_ab = w.ab;
+        A.n_atoms = n_atoms;
+        A.pos_conv = position_conversion;
+        A.dt = time_step;
+        A.P = n_beads;
+        launch_modes<OP_BARO>(A, st);
+    }
     SPK_LAUNCH_CHECK();
     return SPK_OK;
 }

@@ -44,13 +44,11 @@ __device__ __forceinline__ void seg_scan(double (&v)[NV], int f, double (*sv)[T]
 // i(s) = ptr[outer[s]] (outer given) or ptr[s]; CTAs of the partial pass hold T items.  out[s * NV + c], 0 for no items.
 constexpr int SEG_FIN_T = 128;
 
+// The reduction of k_seg_finish for system s by the SEG_FIN_T threads of a CTA; red[c][0] holds the totals on return.
 template <int T, int NV>
-__global__ void __launch_bounds__(SEG_FIN_T) k_seg_finish(const int32_t* __restrict__ ptr, const int32_t* __restrict__ outer,
-                                                          const double* __restrict__ sys_part,
-                                                          const double* __restrict__ head, double* __restrict__ out) {
-    __shared__ double red[NV][SEG_FIN_T];
-    SPK_PDL_ENTER();
-    const int64_t s = blockIdx.x;
+__device__ __forceinline__ void seg_finish_block(const int32_t* __restrict__ ptr, const int32_t* __restrict__ outer,
+                                                 const double* __restrict__ sys_part, const double* __restrict__ head,
+                                                 int64_t s, double (*red)[SEG_FIN_T]) {
     const int t = threadIdx.x;
     const int64_t i0 = outer ? ptr[outer[s]] : ptr[s];
     const int64_t i1 = outer ? ptr[outer[s + 1]] : ptr[s + 1];
@@ -74,7 +72,17 @@ __global__ void __launch_bounds__(SEG_FIN_T) k_seg_finish(const int32_t* __restr
         }
         __syncthreads();
     }
-    if (t < NV) out[s * NV + t] = red[t][0];
+}
+
+template <int T, int NV>
+__global__ void __launch_bounds__(SEG_FIN_T) k_seg_finish(const int32_t* __restrict__ ptr, const int32_t* __restrict__ outer,
+                                                          const double* __restrict__ sys_part,
+                                                          const double* __restrict__ head, double* __restrict__ out) {
+    __shared__ double red[NV][SEG_FIN_T];
+    SPK_PDL_ENTER();
+    const int64_t s = blockIdx.x;
+    seg_finish_block<T, NV>(ptr, outer, sys_part, head, s, red);
+    if (threadIdx.x < NV) out[s * NV + threadIdx.x] = red[threadIdx.x][0];
 }
 
 }  // namespace

@@ -37,7 +37,10 @@ Ring-polymer MD (DESIGN.md section 9): ``DeviceMD(..., ring_polymer=RingPolymer(
 (replica-major, as md/calculators/base_calculator.py:154-221 collates them) and runs the RingPolymer step
 (md/integrators.py:113-229, md/simulator.py:124-150): thermostat, half kick per bead, normal-mode propagation of the free ring
 polymer, neighbour list + energy + forces on all beads, half kick, thermostat -- with the PILE-L / PILE-G / TRPMD and
-ring-polymer NHC thermostats of md/simulation_hooks/thermostats_rpmd.py, all in the same captured graph.
+ring-polymer NHC thermostats of md/simulation_hooks/thermostats_rpmd.py, all in the same captured graph.  With a
+``PILEBarostat`` (md/simulation_hooks/barostats_rpmd.py) the step is that of NPTRingPolymer (md/integrators.py:266-305):
+the barostat propagates the centroid mode and the cell, the virial of every bead system is kept, and any ring-polymer
+thermostat (or none) runs next to it.
 """
 from __future__ import annotations
 
@@ -53,7 +56,7 @@ from .neighbors import CellListNeighborList
 
 __all__ = ["DeviceMD", "BerendsenThermostat", "LangevinThermostat", "NHCThermostat", "NHCBarostatIsotropic",
            "NHCBarostatAnisotropic", "RingPolymer", "PILELocalThermostat", "PILEGlobalThermostat", "TRPMDThermostat",
-           "NHCRingPolymerThermostat", "KB_MD", "FS_MD", "BAR_MD", "HBAR_MD"]
+           "NHCRingPolymerThermostat", "PILEBarostat", "KB_MD", "FS_MD", "BAR_MD", "HBAR_MD"]
 
 Tensor = torch.Tensor
 
@@ -246,6 +249,8 @@ class _NHCBarostat:
     separate thermostat with it.  State (chains, cell velocities and forces) is fp64 on the device."""
 
     anisotropic = False
+    ring_polymer = False
+    temperature_control = True
     YS_WEIGHTS = NHCThermostat.YS_WEIGHTS
 
     def __init__(self, target_pressure: float, temperature_bath: float, time_constant: float,
@@ -575,11 +580,91 @@ class NHCRingPolymerThermostat(_RingPolymerThermostat):
         return {"velocities": self.velocities, "forces": self.forces}
 
 
+class PILEBarostat:
+    """Isotropic barostat of ring-polymer NPT (barostats_rpmd.py:21-208, after i-PI 2.0, Kapil et al. 2019) with the
+    reference's keywords: target pressure in bar, bath temperature of the cell in K, time constant in fs; ``kB``, ``fs``
+    and ``bar`` define the caller's MD units.  It acts on the centroid mode and the cell only and thermostats the cell
+    momentum with a PILE step, so any ring-polymer thermostat (or none) can run next to it.
+
+    One cell momentum p_c per system of mass W = 3 N_s kB T / omega^2 with omega = 1 / tau (:83-85); the cell thermostat
+    is p_c = c1 p_c + c2 xi with c1 = exp(-dt / (2 tau)) and c2 = sqrt(P W kB T (1 - c1^2)) (:88-99).  xi comes from
+    Philox4x32-10 keyed by ``seed`` with the counter (system, application); the application index lives on the device and
+    advances with every application, also inside a replayed graph.  State (p_c, counter) is on the device."""
+
+    ring_polymer = True
+    temperature_control = False
+
+    def __init__(self, target_pressure: float, temperature_bath: float, time_constant: float, seed: int = 0,
+                 kB: float = KB_MD, fs: float = FS_MD, bar: float = BAR_MD):
+        self.target_pressure = float(target_pressure) * float(bar)               # barostats.py:51-53
+        self.temperature_bath = float(temperature_bath)
+        self.time_constant = float(time_constant) * float(fs)
+        self.frequency = 1.0 / self.time_constant                               # barostats_rpmd.py:53
+        self.kB = float(kB)
+        self.kb_temperature = self.temperature_bath * self.kB                   # :56
+        self.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self.cell_momenta: Optional[Tensor] = None
+        self.counter: Optional[Tensor] = None
+
+    def bind(self, systems: _Systems, time_step: float, ring_polymer: Optional[RingPolymer] = None):
+        """_init_barostat (:66-99) for the base batch ``systems`` (one copy of every molecule)."""
+        if ring_polymer is None:
+            raise ValueError("PILEBarostat is a ring-polymer barostat: pass DeviceMD(ring_polymer=...)")
+        self.rp = ring_polymer
+        self.systems = s = systems
+        self.time_step = float(time_step)
+        dev = s.masses.device
+        kbt = self.kb_temperature
+        self.cell_momenta = torch.zeros(s.n_sys, dtype=torch.float64, device=dev)
+        self.cell_mass = 3.0 * s.n_atoms_sys * kbt / self.frequency ** 2                # :83-85
+        self.c1 = math.exp(-0.5 * self.frequency * self.time_step)                      # :88-93
+        self.c2 = torch.sqrt(ring_polymer.n_beads * self.cell_mass * kbt * (1.0 - self.c1 ** 2))   # :94-99
+        # [0] = application index, [1] = the kernel's internal ticket (zero between calls)
+        self.counter = torch.zeros(2, dtype=torch.int64, device=dev)
+        nbytes = int(_lib.lib().spk_rpmd_barostat_workspace_bytes(s.n_atoms, s.n_sys))
+        self.ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+
+    def apply_thermostat(self):
+        """_update_barostat (:101-110) at on_step_begin and on_step_end"""
+        _lib.call("spk_rpmd_barostat_thermostat", ops._p(self.cell_momenta), self.systems.n_sys, self.c1,
+                  ops._p(self.c2), self.seed, ops._p(self.counter), ops._stream())
+
+    def half_step(self, momenta: Tensor, forces: Tensor, force_conversion: float, cell: Tensor, virial: Tensor,
+                  virial_scale: float):
+        """propagate_half_step (:164-205) up to the particle kick, which DeviceMD enqueues next: p_c from the momenta
+        before the kick, the forces * force_conversion, and the bead systems' cells and virials"""
+        s, rp = self.systems, self.rp
+        _lib.call("spk_rpmd_barostat_half_step", ops._p(momenta), ops._p(forces), float(force_conversion),
+                  ops._p(s.masses), ops._p(s.idx_m), ops._p(s.sys_ptr), s.n_atoms, s.n_sys, rp.n_beads,
+                  ops._p(rp.c_transform), ops._p(cell), ops._p(virial), float(virial_scale), self.target_pressure,
+                  self.kb_temperature, self.time_step, ops._p(self.cell_mass), ops._p(self.cell_momenta),
+                  ops._p(self.ws), self.ws.numel(), ops._stream())
+
+    def main_step(self, positions: Tensor, momenta: Tensor, model_positions: Optional[Tensor], cell: Tensor,
+                  model_cell: Optional[Tensor], position_conversion: float):
+        """propagate_main_step (:113-162): centroid mode and cell scaled by the cell momentum, modes k >= 1 free"""
+        s, rp = self.systems, self.rp
+        _lib.call("spk_rpmd_barostat_main_step", ops._p(positions), ops._p(momenta), ops._p(model_positions),
+                  ops._p(s.masses), ops._p(s.idx_m), s.n_atoms, s.n_sys, rp.n_beads, ops._p(rp.c_transform),
+                  ops._p(rp.u), self.time_step, ops._p(self.cell_momenta), ops._p(self.cell_mass), ops._p(cell),
+                  ops._p(model_cell), float(position_conversion), ops._p(self.ws), self.ws.numel(), ops._stream())
+
+    def _state(self) -> Dict[str, Tensor]:
+        return {"cell_momenta": self.cell_momenta, "counter": self.counter}
+
+    def state_dict(self) -> Dict[str, Tensor]:
+        return {k: v.clone() for k, v in self._state().items()}
+
+    def load_state_dict(self, state: Dict[str, Tensor]):
+        for k, v in self._state().items():
+            v.copy_(state[k])
+
+
 class DeviceMD:
     def __init__(self, model: torch.nn.Module, batch: Dict[str, Tensor], masses: Tensor, time_step: float, cutoff: float,
                  capacity: int, momenta: Optional[Tensor] = None, use_graph: bool = True,
                  position_conversion: float = 1.0, energy_conversion: float = 1.0,
-                 thermostat: Optional[_Thermostat] = None, barostat: Optional[_NHCBarostat] = None,
+                 thermostat: Optional[_Thermostat] = None, barostat: Optional[object] = None,
                  compute_stress: bool = False, ring_polymer: Optional[RingPolymer] = None):
         """``batch[_positions]`` (and ``_cell``) are in MODEL units as everywhere in this package; ``self.positions`` is the
         MD-unit state (= model positions / position_conversion).  ``thermostat`` (None = NVE) is bound to the systems of
@@ -590,12 +675,12 @@ class DeviceMD:
         ``ring_polymer`` (a ``RingPolymer``) makes the run ring-polymer MD: the B-system ``batch`` is replicated into P
         beads, replica-major (P B systems; bead r of system m is system r B + m, positions [P, N, 3] flat as [P N, 3]), all
         beads start at the batch positions, ``momenta`` may be [N, 3] (copied to every bead) or [P, N, 3], and ``capacity``
-        is the pair capacity of the whole bead batch.  It takes only the ring-polymer thermostats, no barostat and no
-        stress."""
+        is the pair capacity of the whole bead batch.  It takes only the ring-polymer thermostats and, for NPT, the
+        ``PILEBarostat`` (next to a ring-polymer thermostat or alone); no NHC barostat and no ``compute_stress``."""
         dev = batch[P.R].device
         if dev.type != "cuda":
             raise ValueError("DeviceMD needs a CUDA batch (no CPU fallback)")
-        if barostat is not None and thermostat is not None:
+        if barostat is not None and thermostat is not None and getattr(barostat, "temperature_control", True):
             raise ValueError("DeviceMD: the NHC barostats contain their own thermostat (temperature_control = True); "
                              "pass either a thermostat or a barostat")
         self._check_ring_polymer(ring_polymer, thermostat, barostat, compute_stress)
@@ -667,7 +752,10 @@ class DeviceMD:
                 raise ValueError("DeviceMD: NPT needs every system periodic on all three axes (system.py:599-602)")
             if bool((self.volume() == 0.0).any()):
                 raise ValueError("DeviceMD: NPT needs a non-zero cell volume for every system (system.py:599-602)")
-            barostat.bind(self.systems, self.dt)                                  # on_simulation_start
+            if ring_polymer is not None:
+                barostat.bind(self._rp_base, self.dt, ring_polymer)               # on_simulation_start
+            else:
+                barostat.bind(self.systems, self.dt)
         self._calculate()                       # forces at t = 0 (simulator.py:118)
 
     @property
@@ -689,9 +777,13 @@ class DeviceMD:
     def _check_ring_polymer(ring_polymer, thermostat, barostat, compute_stress):
         """the combinations the reference refuses (md/cli.py:256-267) or this package does not build"""
         rp_thermostat = getattr(thermostat, "ring_polymer", False)
+        rp_barostat = getattr(barostat, "ring_polymer", False)
         if ring_polymer is None:
             if rp_thermostat:
                 raise ValueError(f"DeviceMD: {type(thermostat).__name__} is a ring-polymer thermostat; it needs "
+                                 "ring_polymer=RingPolymer(...)")
+            if rp_barostat:
+                raise ValueError(f"DeviceMD: {type(barostat).__name__} is a ring-polymer barostat; it needs "
                                  "ring_polymer=RingPolymer(...)")
             return
         if not isinstance(ring_polymer, RingPolymer):
@@ -699,8 +791,9 @@ class DeviceMD:
         if thermostat is not None and not rp_thermostat:
             raise ValueError(f"DeviceMD: {type(thermostat).__name__} is a classical thermostat; ring-polymer MD takes "
                              "PILELocalThermostat, PILEGlobalThermostat, TRPMDThermostat or NHCRingPolymerThermostat")
-        if barostat is not None:
-            raise ValueError("DeviceMD: ring-polymer MD with a barostat (the RPMD barostats) is not supported")
+        if barostat is not None and not rp_barostat:
+            raise ValueError(f"DeviceMD: {type(barostat).__name__} is not a ring-polymer barostat (md/cli.py:267-275); "
+                             "ring-polymer NPT takes PILEBarostat")
         if compute_stress:
             raise ValueError("DeviceMD: compute_stress is not supported for ring-polymer MD")
 
@@ -786,7 +879,28 @@ class DeviceMD:
         if self.thermostat is not None:
             self.thermostat.apply(self.momenta)
 
+    def _rpmd_npt_step(self):
+        """md/simulator.py:124-150 with NPTRingPolymer (integrators.py:266-305) and hooks [thermostat, barostat]:
+        thermostat, cell PILE, barostat half step + kick, centroid / cell / free-mode propagation, neighbour list on the new
+        cells + energy + forces + virial on all P B bead systems, half step + kick, cell PILE, thermostat"""
+        b = self.barostat
+        mp = self.model_positions if self.model_positions is not self.positions else None
+        if self.thermostat is not None:
+            self.thermostat.apply(self.momenta)
+        b.apply_thermostat()
+        b.half_step(self.momenta, self.forces, self.f_conv, self.cell, self.virial, self._virial_scale())
+        self._verlet(False)                                                        # barostats_rpmd.py:207-208
+        b.main_step(self.positions, self.momenta, mp, self.cell, self.model_cell, self.p_conv)
+        self._calculate()
+        b.half_step(self.momenta, self.forces, self.f_conv, self.cell, self.virial, self._virial_scale())
+        self._verlet(False)
+        b.apply_thermostat()
+        if self.thermostat is not None:
+            self.thermostat.apply(self.momenta)
+
     def _step(self):
+        if self.ring_polymer is not None and self.barostat is not None:
+            return self._rpmd_npt_step()
         if self.ring_polymer is not None:
             return self._rpmd_step()
         if self.barostat is not None:
@@ -897,6 +1011,29 @@ class DeviceMD:
         """bead average of the potential energy [B] in MD units (system.py:557-565)"""
         rp = self._need_rp()
         return self.potential_energy().reshape(rp.n_beads, -1).mean(0)
+
+    def centroid_pressure(self, tensor: bool = False, kinetic_component: bool = False) -> Tensor:
+        """system.py:616-650 for a ring-polymer NPT run: -(bead mean of the stress), its trace / 3 ([B]) or the tensor
+        ([B, 3, 3]), optionally plus the kinetic part 2 K_c / (3 V_bar) (2 K_c / V_bar for the tensor) with K_c from the
+        bead mean of the momenta and V_bar the bead mean of the volume.  The tensor's kinetic part uses the kinetic-energy
+        tensor of the centroid momenta (the reference raises there)."""
+        rp = self._need_rp()
+        if self.virial is None:
+            raise RuntimeError("DeviceMD: the centroid pressure needs a ring-polymer NPT run (barostat=PILEBarostat(...))")
+        P_ = rp.n_beads
+        vol = self.volume().reshape(P_, -1).mean(0)
+        p = -self.stress.reshape(P_, -1, 3, 3).mean(0)
+        if tensor:
+            if kinetic_component:
+                pc = self.centroid_momenta().contiguous()
+                p = p + 2.0 * self._rp_base.kinetic_energy_tensor(pc) / vol[:, None, None]
+            return p
+        p = torch.diagonal(p, dim1=1, dim2=2).sum(-1) / 3.0
+        if kinetic_component:
+            pc = self.centroid_momenta().contiguous()
+            ke = self._rp_base.kinetic_energy_and_temperature(pc, KB_MD)[0]
+            p = p + 2.0 * ke / vol / 3.0
+        return p
 
     def state_dict(self) -> Dict[str, object]:
         """Everything a restarted run needs to continue bitwise: the MD state, the neighbour-list bookkeeping and the
