@@ -484,6 +484,22 @@ int spk_rpmd_nhc(float* momenta, const float* masses, const int64_t* idx_m, cons
                  double* chain_v, double* chain_f, const double* chain_m, void* workspace, size_t workspace_bytes,
                  spk_stream_t stream);
 
+/* ---- GLE thermostats (csrc/rpmd.cu; md/simulation_hooks/thermostats.py:527-730 GLEThermostat, thermostats_rpmd.py:
+ * 237-370 RPMDGLEThermostat and PIGLETThermostat).  Bead arrays, masses and c_transform as for spk_rpmd_pile; the
+ * classical GLE is n_beads = 1 with c_transform = [[1.0]], which is exact in fp64.  state [n_beads 3 n_atoms, gle_dim]
+ * fp64 holds the extended momenta of every (normal mode k, degree of freedom i) at row k 3 n_atoms + i;
+ * 1 <= gle_dim <= 16.  c1, c2 [gle_dim, gle_dim] fp64 row-major on the device, or [n_beads, gle_dim, gle_dim] with
+ * per_mode != 0 (PIGLET: mode k uses block k).  Noise column j of row (k, 3 a + d) is normal d of the Philox4x32-10 draw
+ * with key seed and counter ((j n_beads + k) n_atoms + a, counter[0]); counter [2] as for spk_rpmd_pile, advanced by
+ * every call.
+ *   initial != 0   the free-particle-limit start (thermostats.py:687-701): state row = xi^T c2_k, no mass factor;
+ *                  momenta and masses are not read (may be null)
+ *   initial == 0   s[0] = p~; s = c1_k s + sqrt(m_a) c2_k xi (column-vector form of Ceriotti et al. 2010, where the
+ *                  reference propagates s^T c1 = (c1^T s)^T); p~ = s[0] */
+int spk_rpmd_gle(float* momenta, const float* masses, int64_t n_atoms, int32_t n_beads, const double* c_transform,
+                 const double* c1, const double* c2, int32_t gle_dim, int32_t per_mode, double* state, uint64_t seed,
+                 uint64_t* counter, int32_t initial, spk_stream_t stream);
+
 /* ---- PILE barostat of ring-polymer NPT (csrc/rpmd.cu; md/simulation_hooks/barostats_rpmd.py:21-208 PILEBarostat with
  * md/integrators.py:266-305 NPTRingPolymer).  One isotropic cell momentum p_c of mass W per system of the base batch
  * (cell_momenta, cell_mass [n_sys] fp64); bead arrays, masses, idx_m and sys_ptr as for spk_rpmd_pile; cells and virial

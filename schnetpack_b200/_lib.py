@@ -119,6 +119,7 @@ SIGNATURES = {
     "spk_rpmd_main_step": [P, P, P, P, c_int64, c_int32, P, P, c_double, P],
     "spk_rpmd_pile": [P, P, P, P, c_int64, c_int64, c_int32, P, P, P, c_double, c_int32, c_uint64, P, P, c_size_t, P],
     "spk_rpmd_nhc": [P, P, P, P, c_int64, c_int64, c_int32, P, POINTER(NHCParams), c_int32, P, P, P, P, c_size_t, P],
+    "spk_rpmd_gle": [P, P, c_int64, c_int32, P, P, P, c_int32, c_int32, P, c_uint64, P, c_int32, P],
     "spk_rpmd_barostat_workspace_bytes": [c_int64, c_int64],
     "spk_rpmd_barostat_thermostat": [P, c_int64, c_double, P, c_uint64, P, P],
     "spk_rpmd_barostat_half_step": [P, P, c_double, P, P, P, c_int64, c_int64, c_int32, P, P, P, c_double, c_double,

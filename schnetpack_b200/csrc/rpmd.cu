@@ -1,8 +1,10 @@
 // Ring-polymer MD of the device MD step: the normal-mode transform (md/utils/normal_model_transformation.py:37-101), the
 // free ring-polymer propagation of the RingPolymer integrator (md/integrators.py:154-229) and the ring-polymer thermostats
 // PILE-L / PILE-G / TRPMD and NHC (md/simulation_hooks/thermostats_rpmd.py:33-234,373-501), and the PILE barostat of
-// ring-polymer NPT (md/simulation_hooks/barostats_rpmd.py:21-208 with md/integrators.py:266-305 NPTRingPolymer).  Every
-// entry point only enqueues work, so the whole RPMD step stays one CUDA graph.
+// ring-polymer NPT (md/simulation_hooks/barostats_rpmd.py:21-208 with md/integrators.py:266-305 NPTRingPolymer), and the
+// colored-noise GLE / RPMD-GLE / PIGLET thermostats (md/simulation_hooks/thermostats.py:527-730, thermostats_rpmd.py:
+// 237-370; the classical GLE runs as P = 1 with C = [[1]]).  Every entry point only enqueues work, so the whole RPMD step
+// stays one CUDA graph.
 //
 // Bead arrays are [P, n_atoms, 3] fp32, replica-major, so for a fixed bead a run of consecutive degrees of freedom (atom,
 // component) is contiguous.  The mode kernels give a CTA RP_T = 32 consecutive degrees of freedom across all P beads: the
@@ -25,8 +27,9 @@ constexpr int RP_KT = 256;        // atoms per CTA of the centroid partial pass
 constexpr int RP_NV = 2;          // centroid sums: sum |p~_0|^2 / m, sum |xi_0|^2
 constexpr int RP_MAX_BEADS = 64;
 constexpr int RB_NV = 3;          // barostat sums: sum F~_0 . p~_0 / m, sum |F~_0|^2 / (3 m), sum |p_bar|^2 / m
+constexpr int GLE_MAX_D = 16;     // extended momenta per degree of freedom (p~ plus up to 15 auxiliary momenta)
 
-enum RpmdOp { OP_MAIN = 0, OP_PILE = 1, OP_NHC = 2, OP_BARO = 3 };
+enum RpmdOp { OP_MAIN = 0, OP_PILE = 1, OP_NHC = 2, OP_BARO = 3, OP_GLE = 4 };
 
 struct RpmdArgs {
     float* x;                     // bead positions (OP_MAIN)
@@ -44,7 +47,11 @@ struct RpmdArgs {
     double* chain_v;              // [P * 3 n_atoms, L] (OP_NHC)
     double* chain_f;
     const double* chain_m;
-    unsigned long long* counter;  // [2]: application index, ticket (OP_PILE)
+    unsigned long long* counter;  // [2]: application index, ticket (OP_PILE, OP_GLE)
+    double* gle_s;                // [P * 3 n_atoms, D] extended momenta, row k 3 n_atoms + i (OP_GLE)
+    const double* gle_c1;         // [n_mats, D, D] drift propagator exp(-dt/2 A), row-major (OP_GLE)
+    const double* gle_c2;         // [n_mats, D, D] its noise matrix sqrt(C - c1 C c1^T)
+    int64_t gle_stride;           // 0 (one matrix for every mode) or D * D (one per mode)
     int64_t n_atoms;
     double pos_conv;
     double dt;                    // time step (OP_BARO)
@@ -52,6 +59,7 @@ struct RpmdArgs {
     uint64_t seed;
     int32_t P;
     int32_t global;
+    int32_t gle_d;                // D (OP_GLE)
     spk_nhc_params_t q;           // (OP_NHC)
 };
 
@@ -92,10 +100,70 @@ __device__ __forceinline__ double pile_alpha(const RpmdArgs& A, uint64_t app, in
     return sqrt(a2) * (double)((sg > 0.0) - (sg < 0.0));
 }
 
+// noise column c of the GLE row (mode k, dof i of atom a): normal d of the Philox draw of element (c P + k) N + a
+__device__ __forceinline__ double gle_noise(const RpmdArgs& A, uint64_t app, int c, int k, int64_t a, int d) {
+    return mode_noise(A.seed, app, ((int64_t)c * A.P + k) * A.n_atoms + a, d);
+}
+
+// one GLE application to the row (mode k, dof i): s[0] = p~, s <- c1_k s + sqrt(m) c2_k xi (Ceriotti, Bussi, Parrinello
+// 2010, column-vector form; the reference multiplies the row vector s c1 = c1^T s, see DESIGN.md section 9); returns the
+// new p~ = s[0].  D <= GLE_MAX_D is a run-time value: the loops are unrolled to GLE_MAX_D with guards, so s stays in
+// registers, and threads of a warp share k, so the matrix reads are broadcasts.
+__device__ __forceinline__ double gle_step(const RpmdArgs& A, uint64_t app, int k, int64_t i, int64_t a, double ma,
+                                           double pn) {
+    const int D = A.gle_d;
+    const double* c1 = A.gle_c1 + k * A.gle_stride;
+    const double* c2 = A.gle_c2 + k * A.gle_stride;
+    double* row = A.gle_s + ((int64_t)k * 3 * A.n_atoms + i) * D;
+    const int d = (int)(i - 3 * a);
+    double s[GLE_MAX_D], acc[GLE_MAX_D];
+#pragma unroll
+    for (int c = 0; c < GLE_MAX_D; ++c) {
+        s[c] = c == 0 ? pn : (c < D ? row[c] : 0.0);                   // thermostats.py:720
+        acc[c] = 0.0;
+    }
+#pragma unroll
+    for (int c = 0; c < GLE_MAX_D; ++c) {                              // c2 xi, one noise column at a time
+        if (c < D) {
+            const double xi = gle_noise(A, app, c, k, a, d);
+#pragma unroll
+            for (int r = 0; r < GLE_MAX_D; ++r)
+                if (r < D) acc[r] += c2[r * D + c] * xi;
+        }
+    }
+    const double sm = sqrt(ma);
+#pragma unroll
+    for (int r = 0; r < GLE_MAX_D; ++r) {
+        if (r < D) {
+            double v = 0.0;
+#pragma unroll
+            for (int c = 0; c < GLE_MAX_D; ++c)
+                if (c < D) v += c1[r * D + c] * s[c];
+            acc[r] = v + sm * acc[r];
+            row[r] = acc[r];
+        }
+    }
+    return acc[0];
+}
+
+// advance the application index once every CTA of the launch has read it (ticket pattern of k_langevin)
+__device__ __forceinline__ void advance_counter(unsigned long long* counter, unsigned long long app) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        if (atomicAdd(counter + 1, 1ull) == gridDim.x - 1) {
+            counter[0] = app + 1;
+            counter[1] = 0;
+            __threadfence();
+        }
+    }
+}
+
 // beads -> normal modes, the per-mode operator OP, normal modes -> beads, for RP_T degrees of freedom per CTA
 template <int OP>
 __global__ void __launch_bounds__(RP_THREADS) k_rpmd_modes(const __grid_constant__ RpmdArgs A) {
     constexpr bool HAS_X = OP == OP_MAIN || OP == OP_BARO;
+    constexpr bool HAS_NOISE = OP == OP_PILE || OP == OP_GLE;
     extern __shared__ double smem[];
     const int P = A.P;
     const int PT = P * RP_T;
@@ -105,7 +173,7 @@ __global__ void __launch_bounds__(RP_THREADS) k_rpmd_modes(const __grid_constant
     float* bp = bx + PT;
     SPK_PDL_ENTER();
     unsigned long long app = 0;
-    if (OP == OP_PILE) app = *(volatile unsigned long long*)A.counter;
+    if (HAS_NOISE) app = *(volatile unsigned long long*)A.counter;
     const int64_t n_dof = 3 * A.n_atoms;
     const int64_t i0 = (int64_t)blockIdx.x * RP_T;
     for (int j = threadIdx.x; j < PT; j += RP_THREADS) {
@@ -146,6 +214,8 @@ __global__ void __launch_bounds__(RP_THREADS) k_rpmd_modes(const __grid_constant
                 const double xi = mode_noise(A.seed, app, (int64_t)k * A.n_atoms + a, (int)(i - 3 * a));
                 pn = A.c1[k] * pn + sqrt(ma * A.kbt_p) * A.c2[k] * xi;
             }
+        } else if (OP == OP_GLE) {                       // thermostats.py:705-729, thermostats_rpmd.py:271-295
+            pn = gle_step(A, app, k, i, a, ma, pn);
         } else {                                         // thermostats_rpmd.py:465-501
             double ke = pn * pn / ma, dof = 1.0;
             if (k == 0 && A.global) {
@@ -178,17 +248,39 @@ __global__ void __launch_bounds__(RP_THREADS) k_rpmd_modes(const __grid_constant
             if (A.model_x) A.model_x[b * n_dof + i] = xf * (float)A.pos_conv;
         }
     }
-    if (OP == OP_PILE) {   // advance the application index once every CTA has read it (ticket pattern of k_langevin)
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            __threadfence();
-            if (atomicAdd(A.counter + 1, 1ull) == gridDim.x - 1) {
-                A.counter[0] = app + 1;
-                A.counter[1] = 0;
-                __threadfence();
+    if (HAS_NOISE) advance_counter(A.counter, app);
+}
+
+// free-particle-limit start of the GLE state (thermostats.py:687-701): the row vector s = xi c2_k, without a mass factor,
+// one thread per (mode k, dof i); noise as gle_step at the current application
+__global__ void __launch_bounds__(RP_THREADS) k_gle_init(const __grid_constant__ RpmdArgs A) {
+    SPK_PDL_ENTER();
+    const unsigned long long app = *(volatile unsigned long long*)A.counter;
+    const int64_t n_dof = 3 * A.n_atoms;
+    const int64_t rowi = (int64_t)blockIdx.x * RP_THREADS + threadIdx.x;
+    if (rowi < (int64_t)A.P * n_dof) {
+        const int k = (int)(rowi / n_dof);
+        const int64_t i = rowi - (int64_t)k * n_dof, a = i / 3;
+        const int D = A.gle_d;
+        const double* c2 = A.gle_c2 + k * A.gle_stride;
+        double acc[GLE_MAX_D];
+#pragma unroll
+        for (int c = 0; c < GLE_MAX_D; ++c) acc[c] = 0.0;
+#pragma unroll
+        for (int j = 0; j < GLE_MAX_D; ++j) {
+            if (j < D) {
+                const double xi = gle_noise(A, app, j, k, a, (int)(i - 3 * a));
+#pragma unroll
+                for (int c = 0; c < GLE_MAX_D; ++c)
+                    if (c < D) acc[c] += xi * c2[j * D + c];
             }
         }
+        double* row = A.gle_s + rowi * D;
+#pragma unroll
+        for (int c = 0; c < GLE_MAX_D; ++c)
+            if (c < D) row[c] = acc[c];
     }
+    advance_counter(A.counter, app);
 }
 
 // out = C in (inverse = 0) or C^T in (inverse = 1) over the bead axis, RP_T degrees of freedom per CTA
@@ -534,6 +626,37 @@ extern "C" int spk_rpmd_nhc(float* momenta, const float* masses, const int64_t* 
     A.q = *params;
     if (A.global) centroid_sums(A, 0, n_sys, workspace, st);
     launch_modes<OP_NHC>(A, st);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_rpmd_gle(float* momenta, const float* masses, int64_t n_atoms, int32_t n_beads,
+                            const double* c_transform, const double* c1, const double* c2, int32_t gle_dim,
+                            int32_t per_mode, double* state, uint64_t seed, uint64_t* counter, int32_t initial,
+                            spk_stream_t stream) {
+    if (!beads_ok(n_beads, c_transform) || n_atoms < 0 || (int64_t)n_beads * 3 * n_atoms >= (1ll << 31) - 1)
+        return SPK_ERR_ARG;
+    if (n_atoms > 0 && !initial && (!momenta || !masses)) return SPK_ERR_ARG;   // the initial draw reads neither
+    if (gle_dim < 1 || gle_dim > GLE_MAX_D || !c1 || !c2 || !state || !counter) return SPK_ERR_ARG;
+    if (n_atoms == 0) return SPK_OK;
+    RpmdArgs A = {};
+    A.p = momenta;
+    A.m = masses;
+    A.C = c_transform;
+    A.gle_s = state;
+    A.gle_c1 = c1;
+    A.gle_c2 = c2;
+    A.gle_stride = per_mode ? (int64_t)gle_dim * gle_dim : 0;
+    A.gle_d = gle_dim;
+    A.counter = reinterpret_cast<unsigned long long*>(counter);
+    A.n_atoms = n_atoms;
+    A.seed = seed;
+    A.P = n_beads;
+    cudaStream_t st = spk_st(stream);
+    if (initial)
+        spk_launch(k_gle_init, (unsigned)spk_cdiv((int64_t)n_beads * 3 * n_atoms, RP_THREADS), RP_THREADS, 0, st, A);
+    else
+        launch_modes<OP_GLE>(A, st);
     SPK_LAUNCH_CHECK();
     return SPK_OK;
 }

@@ -41,6 +41,14 @@ ring-polymer NHC thermostats of md/simulation_hooks/thermostats_rpmd.py, all in 
 ``PILEBarostat`` (md/simulation_hooks/barostats_rpmd.py) the step is that of NPTRingPolymer (md/integrators.py:266-305):
 the barostat propagates the centroid mode and the cell, the virial of every bead system is kept, and any ring-polymer
 thermostat (or none) runs next to it.
+
+Colored-noise runs (DESIGN.md section 9): ``GLEThermostat`` (classical), ``RPMDGLEThermostat`` (one GLE on every normal mode)
+and ``PIGLETThermostat`` (one GLE per normal mode) of md/simulation_hooks/thermostats.py:527-730 and thermostats_rpmd.py:
+237-370 read gle4md matrix files with ``load_gle_matrices`` and keep D extended momenta per (normal mode, degree of
+freedom) in fp64 on the device.  One kernel (``spk_rpmd_gle``) transforms to normal modes, propagates s = c1 s + sqrt(m)
+c2 xi and transforms back; the classical thermostat is the same kernel at P = 1.  It uses the propagator of the GLE
+papers, where the reference multiplies by the transpose of c1, which samples a wrong distribution for a non-normal drift
+matrix.  RPMD-GLE and PIGLET also run next to ``PILEBarostat``.
 """
 from __future__ import annotations
 
@@ -56,7 +64,8 @@ from .neighbors import CellListNeighborList
 
 __all__ = ["DeviceMD", "BerendsenThermostat", "LangevinThermostat", "NHCThermostat", "NHCBarostatIsotropic",
            "NHCBarostatAnisotropic", "RingPolymer", "PILELocalThermostat", "PILEGlobalThermostat", "TRPMDThermostat",
-           "NHCRingPolymerThermostat", "PILEBarostat", "KB_MD", "FS_MD", "BAR_MD", "HBAR_MD"]
+           "NHCRingPolymerThermostat", "PILEBarostat", "GLEThermostat", "RPMDGLEThermostat", "PIGLETThermostat",
+           "load_gle_matrices", "KB_MD", "FS_MD", "BAR_MD", "HBAR_MD"]
 
 Tensor = torch.Tensor
 
@@ -74,6 +83,12 @@ BAR_MD = 1e5 * _CODATA_NA / 1e30
 # units.py:80-82: hbar = h / 2 pi in J s, times ASE's J * s = (1 / e) eV * 1e10 sqrt(e / amu), over energy * time (~0.0635)
 _CODATA_H = 6.626070040e-34
 HBAR_MD = (_CODATA_H / (2.0 * math.pi)) / _CODATA_E * 1e10 * math.sqrt(_CODATA_E / _CODATA_AMU) / (_MD_ENERGY * _MD_TIME)
+# units of gle4md matrix files (thermostat_utils.py:78-86), CODATA 2014: Hartree energy in J, atomic unit of time in s;
+# energies go through kelvin (x kB) and times through femtoseconds (x fs), so custom MD units need no further constant
+_CODATA_HARTREE, _CODATA_AUT = 4.359744650e-18, 2.418884326509e-17
+_EV_K = _CODATA_E / _CODATA_K                                   # 1 eV in K (~11604.5)
+_HARTREE_K = _CODATA_HARTREE / _CODATA_K                        # 1 Hartree in K (~315775)
+_AUT_FS = _CODATA_AUT * 1e15                                    # 1 atomic time unit in fs (~0.0241888)
 
 
 class _Systems:
@@ -580,6 +595,185 @@ class NHCRingPolymerThermostat(_RingPolymerThermostat):
         return {"velocities": self.velocities, "forces": self.forces}
 
 
+# ---- generalized-Langevin (colored-noise) thermostats ------------------------------------------------------------------------
+GLE_MAX_DIM = 16      # extended momenta per degree of freedom the kernel keeps in registers
+
+
+def _gle_unit(name: str, kB: float, fs: float) -> Optional[float]:
+    """the factor that turns a gle4md unit into MD units (thermostat_utils.py:78-86), or None if the unit is unknown"""
+    return {"femtoseconds^-1": 1.0 / fs, "picoseconds^-1": 1e-3 / fs, "seconds^-1": 1e-15 / fs,
+            "atomic time units^-1": 1.0 / (_AUT_FS * fs), "K": kB, "eV": _EV_K * kB,
+            "atomic energy units": _HARTREE_K * kB}.get(name)
+
+
+def load_gle_matrices(path: str, kB: float = KB_MD, fs: float = FS_MD):
+    """Read a gle4md matrix file in raw format (GLEMatrixParser, thermostat_utils.py:64-178): the drift matrix A between
+    ``A MATRIX:`` and ``C MATRIX:``, the covariance C after ``C MATRIX:``, blocks split at ``# Matrix for normal mode``
+    comment lines, the unit taken from the ``(...)`` of each header line.  Returns (A [n_blocks, D, D], C [n_blocks, D, D]
+    or None) fp64 in the MD units given by ``kB`` (energy per kelvin) and ``fs`` (one femtosecond in MD time).  Raises
+    ``ValueError`` for an unknown unit, a file without A, blocks that are not square or do not match, and D > 16."""
+    heads = {"A": ("A MATRIX:", "C MATRIX:"), "C": ("C MATRIX:", None)}
+    reading = {"A": False, "C": False}
+    units: Dict[str, float] = {}
+    blocks = {"A": [], "C": []}
+    current = {"A": [], "C": []}
+    with open(path) as f:
+        for line in f:
+            line = line.strip()
+            if not line:
+                continue
+            for key, (start, stop) in heads.items():
+                if start in line:                                           # thermostat_utils.py:108-112
+                    unit = line.split("(")[-1].replace(")", "")
+                    factor = _gle_unit(unit, kB, fs)
+                    if factor is None:
+                        raise ValueError(f"load_gle_matrices: unknown unit {unit!r} in the {key} header of {path}")
+                    reading[key], units[key] = True, factor
+                elif reading[key]:
+                    if line.startswith("#"):                                # :114-121
+                        if stop is not None and stop in line:
+                            reading[key] = False
+                        if "Matrix for normal mode" in line and current[key]:
+                            blocks[key].append(current[key])
+                            current[key] = []
+                    else:
+                        try:
+                            current[key].append([float(x) for x in line.split()])
+                        except ValueError:
+                            raise ValueError(f"load_gle_matrices: cannot read the {key} row {line!r} of {path}") from None
+    out = {}
+    for key in ("A", "C"):
+        if current[key]:
+            blocks[key].append(current[key])
+        if key not in units:
+            out[key] = None
+            continue
+        if not blocks[key]:
+            raise ValueError(f"load_gle_matrices: the {key} MATRIX section of {path} has no rows")
+        for n, b in enumerate(blocks[key]):
+            if any(len(row) != len(b) for row in b):
+                raise ValueError(f"load_gle_matrices: {key} block {n} of {path} is not square ({len(b)} rows of "
+                                 f"{sorted({len(row) for row in b})} columns)")
+        if len({len(b) for b in blocks[key]}) != 1:
+            raise ValueError(f"load_gle_matrices: the {key} blocks of {path} differ in size")
+        out[key] = torch.tensor(blocks[key], dtype=torch.float64) * units[key]     # :140-145
+    A, C = out["A"], out["C"]
+    if A is None:
+        raise ValueError(f"load_gle_matrices: no 'A MATRIX:' section in {path} (not a gle4md matrix file)")
+    if C is not None and C.shape != A.shape:
+        raise ValueError(f"load_gle_matrices: A {tuple(A.shape)} and C {tuple(C.shape)} of {path} do not match")
+    if A.shape[-1] > GLE_MAX_DIM:
+        raise ValueError(f"load_gle_matrices: D = {A.shape[-1]} extended momenta in {path}; at most {GLE_MAX_DIM} "
+                         "are supported")
+    return A, C
+
+
+def _gle_propagators(A: Tensor, C: Tensor, time_step: float):
+    """_init_single_gle_matrix (thermostats.py:653-657) in fp64 on the host: c1 = exp(-dt/2 A) and c2 the symmetric square
+    root of C - c1 C c1^T, from its eigendecomposition.  Eigenvalues that are negative by rounding only are clamped to
+    zero; a clearly negative one means C is not a stationary covariance of A, and no GLE has these matrices."""
+    c1 = torch.linalg.matrix_exp(-0.5 * float(time_step) * A)
+    m = C - c1 @ C @ c1.T
+    m = 0.5 * (m + m.T)
+    w, v = torch.linalg.eigh(m)
+    tol = 1e3 * torch.finfo(torch.float64).eps * float(torch.linalg.matrix_norm(C, 2))
+    if float(w.min()) < -tol:
+        raise ValueError(f"GLE: C - c1 C c1^T has the eigenvalue {float(w.min()):.3e} < 0; A and C are not a valid "
+                         "GLE (C must be a stationary covariance of the drift A)")
+    c2 = (v * torch.sqrt(w.clamp_min(0.0))) @ v.T
+    return c1, 0.5 * (c2 + c2.T)
+
+
+class _GLE:
+    """State and kernel call shared by the GLE thermostats: D extended momenta per (normal mode, degree of freedom) in fp64
+    on the device, [P 3 N, D], row k 3 N + i (P = 1 for the classical thermostat), and the Philox application counter.
+
+    The extended momenta s (s[0] = p, or the normal-mode momentum p~_k) follow s <- c1 s + sqrt(m) c2 xi with c1 =
+    exp(-dt/2 A) and c2 = sqrt(C - c1 C c1^T), the propagator of Ceriotti, Bussi, Parrinello (JCTC 6, 1170, 2010).  The
+    reference multiplies the row vector s by c1, which is c1^T s: for a non-normal A that chain does not keep C as its
+    stationary covariance, so this thermostat departs from it there on purpose (DESIGN.md section 9).  For a symmetric A
+    both are the same.  xi comes from Philox4x32-10 keyed by ``seed``: normal d of the draw of element (j P + k) N + a for
+    column j; the free-particle-limit start s = xi c2 (no mass factor, thermostats.py:687-701) is application 0."""
+
+    _per_mode = False
+
+    def __init__(self, temperature_bath: float, gle_file: str, free_particle_limit: bool = True, seed: int = 0,
+                 kB: float = KB_MD, fs: float = FS_MD):
+        super().__init__(temperature_bath, 0.0, kB=kB, fs=fs)          # thermostats.py:557-559
+        self.gle_file = str(gle_file)
+        self.free_particle_limit = bool(free_particle_limit)
+        self.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self.A, self.C = load_gle_matrices(self.gle_file, kB=kB, fs=fs)
+        if not self._per_mode and self.A.shape[0] > 1:                    # thermostats.py:603-606
+            raise ValueError(f"{type(self).__name__}: more than one A matrix found in {self.gle_file}. Could be PIGLET "
+                             "input (PIGLETThermostat).")
+        self.state: Optional[Tensor] = None
+        self.counter: Optional[Tensor] = None
+
+    def _n_beads(self) -> int:
+        return self.rp.n_beads if self.ring_polymer else 1
+
+    def _init_state(self):
+        s = self.systems
+        dev = s.masses.device
+        P = self._n_beads()
+        A, C, D = self.A, self.C, int(self.A.shape[-1])
+        if self._per_mode and A.shape[0] != P:                            # thermostats_rpmd.py:348-352
+            raise ValueError(f"{type(self).__name__}: expected {P} A matrices, one per normal mode, but found "
+                             f"{A.shape[0]} in {self.gle_file}")
+        if C is None:                                                     # thermostats.py:639-648
+            C = torch.eye(D, dtype=torch.float64).expand_as(A) * (self.temperature_bath * self.kB)
+            if self.ring_polymer:
+                C = C * P
+        c1, c2 = zip(*(_gle_propagators(A[b], C[b], self.time_step) for b in range(A.shape[0])))
+        self.c1, self.c2 = torch.stack(c1).to(dev), torch.stack(c2).to(dev)
+        self.c_transform = self.rp.c_transform if self.ring_polymer else torch.ones(1, 1, dtype=torch.float64,
+                                                                                    device=dev)
+        self.state = torch.zeros(P * 3 * s.n_atoms, D, dtype=torch.float64, device=dev)
+        # [0] = application index, [1] = the kernel's internal ticket (zero between calls)
+        self.counter = torch.zeros(2, dtype=torch.int64, device=dev)
+        if self.free_particle_limit:
+            self._call(None, 1)
+
+    def _call(self, momenta: Optional[Tensor], initial: int):
+        s = self.systems
+        _lib.call("spk_rpmd_gle", ops._p(momenta), ops._p(s.masses), s.n_atoms, self._n_beads(),
+                  ops._p(self.c_transform), ops._p(self.c1), ops._p(self.c2), int(self.A.shape[-1]),
+                  1 if self._per_mode else 0, ops._p(self.state), self.seed, ops._p(self.counter), initial, ops._stream())
+
+    def apply(self, momenta: Tensor):
+        self._call(momenta, 0)
+
+    def _state(self):
+        return {"state": self.state, "counter": self.counter}
+
+
+class GLEThermostat(_GLE, _Thermostat):
+    """Generalized-Langevin (colored-noise) thermostat (thermostats.py:527-730) with the reference's keywords plus ``seed``,
+    ``kB`` and ``fs``: the matrices come from the gle4md file ``gle_file`` (one A block; with no C, C = kB T I), and with
+    ``free_particle_limit`` the extended momenta start as xi c2, else at zero.  See ``_GLE`` for the propagator, which is
+    that of the GLE papers and not the reference's transpose."""
+
+    ring_polymer = False
+
+
+class RPMDGLEThermostat(_GLE, _RingPolymerThermostat):
+    """GLE thermostat on every normal mode of the bead momenta (thermostats_rpmd.py:237-295): one A for all modes, with
+    no C in the file C = P kB T I.  It runs the classical thermostat's kernel on p~_k, so at P = 1 it equals
+    ``GLEThermostat`` bitwise.  The reference notes that its version "does not seem to give the proper temperature
+    average"; its transposed propagator is the cause for a non-normal A (see ``_GLE``)."""
+
+
+class PIGLETThermostat(RPMDGLEThermostat):
+    """PIGLET (Ceriotti and Manolopoulos 2012; thermostats_rpmd.py:298-370): one GLE per normal mode, block k of the file
+    on mode k, so the file needs exactly ``n_beads`` blocks.  Always starts in the free-particle limit."""
+
+    _per_mode = True
+
+    def __init__(self, temperature_bath: float, gle_file: str, seed: int = 0, kB: float = KB_MD, fs: float = FS_MD):
+        super().__init__(temperature_bath, gle_file, free_particle_limit=True, seed=seed, kB=kB, fs=fs)
+
+
 class PILEBarostat:
     """Isotropic barostat of ring-polymer NPT (barostats_rpmd.py:21-208, after i-PI 2.0, Kapil et al. 2019) with the
     reference's keywords: target pressure in bar, bath temperature of the cell in K, time constant in fs; ``kB``, ``fs``
@@ -790,7 +984,8 @@ class DeviceMD:
             raise TypeError("DeviceMD: ring_polymer must be a RingPolymer")
         if thermostat is not None and not rp_thermostat:
             raise ValueError(f"DeviceMD: {type(thermostat).__name__} is a classical thermostat; ring-polymer MD takes "
-                             "PILELocalThermostat, PILEGlobalThermostat, TRPMDThermostat or NHCRingPolymerThermostat")
+                             "PILELocalThermostat, PILEGlobalThermostat, TRPMDThermostat, NHCRingPolymerThermostat, "
+                             "RPMDGLEThermostat or PIGLETThermostat")
         if barostat is not None and not rp_barostat:
             raise ValueError(f"DeviceMD: {type(barostat).__name__} is not a ring-polymer barostat (md/cli.py:267-275); "
                              "ring-polymer NPT takes PILEBarostat")
