@@ -535,6 +535,35 @@ int spk_rpmd_barostat_main_step(float* positions, float* momenta, float* model_p
                                 const double* cell_momenta, const double* cell_mass, double* cells, float* model_cells,
                                 double position_conversion, void* workspace, size_t workspace_bytes, spk_stream_t stream);
 
+/* ---- SO3net (representation/so3net.py, nn/so3.py) -------------------------------------------------------------------
+ * Features are [N, S, F] with S = (lmax+1)^2 rows s = l^2 + l + m per atom.  lmax <= 3, F % 4 == 0, F <= 256, any n_rbf;
+ * otherwise SPK_ERR_UNSUPPORTED.  Clebsch-Gordan table and harmonics: csrc/so3_tables.cuh.
+ *
+ * Convolution of one interaction block over the receiver CSR (rowptr, slot_j) and the spk_edge_geometry records:
+ *   y[i, so, f] = sum_{e -> i} sum_nz C * W[l(s1), f] * Y[s1](u_e) * x[j_e, s2, f],
+ *   W[l, f] = fc_e * (phi_e . wf[l*F + f, :] + bf[l*F + f])                        (filter never stored) */
+int spk_so3_conv_fwd(const float* x, const float* phi, const float* geo, const int32_t* rowptr, const int32_t* slot_j,
+                     const float* wf, const float* bf, int64_t n_atoms, int64_t n_edges, int lmax, int F, int n_rbf,
+                     float* y, spk_stream_t stream);
+/* Reverse, grouped by sender (sptr, pos_slot, pos_i): g_x[j] = g_res[j] + sum_{e: j_e = j} dy/dx[j]^T g_y[i_e]
+ * (g_x may be NULL: only g_rij; g_res may be NULL: no residual), g_rij[eid] (+)= dE/dr_ij through d and u. */
+int spk_so3_conv_bwd(const float* x, const float* g_y, const float* phi, const float* dphi, const float* geo,
+                     const int32_t* sptr, const int32_t* pos_slot, const int32_t* pos_i, const int32_t* slot_eid,
+                     const float* wf, const float* bf, int64_t n_atoms, int64_t n_edges, int lmax, int F, int n_rbf,
+                     const float* g_res, float* g_x, float* g_rij, int accumulate, spk_stream_t stream);
+/* out = dx + SO3TensorProduct(dx, ddx), and its reverse (g_dx includes the identity term) */
+int spk_so3_tp_fwd(const float* dx, const float* ddx, int64_t n_atoms, int lmax, int F, float* out, spk_stream_t stream);
+int spk_so3_tp_bwd(const float* g, const float* dx, const float* ddx, int64_t n_atoms, int lmax, int F, float* g_dx,
+                   float* g_ddx, spk_stream_t stream);
+/* gate y[n, s, f] = x[n, s, f] * sigmoid(h[n, l(s)*F + f]); reverse: g_x for rows s >= 1, g_x0 [N,F] for row 0 (the
+ * caller adds the gate layer's input gradient), g_h [N, (lmax+1) F] */
+int spk_so3_gate_fwd(const float* x, const float* h, int64_t n_atoms, int lmax, int F, float* y, spk_stream_t stream);
+int spk_so3_gate_bwd(const float* g_y, const float* x, const float* h, int64_t n_atoms, int lmax, int F, float* g_x,
+                     float* g_x0, float* g_h, spk_stream_t stream);
+/* out[n, s, f] = (src ? src[n, s, f] : 0) + (s == 0 ? v[n, f] : 0);  q[n, f] = x[n, 0, f] */
+int spk_so3_put_l0(const float* src, const float* v, int64_t n_atoms, int lmax, int F, float* out, spk_stream_t stream);
+int spk_so3_take_l0(const float* x, int64_t n_atoms, int lmax, int F, float* q, spk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

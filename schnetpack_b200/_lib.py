@@ -121,6 +121,14 @@ SIGNATURES = {
     "spk_rpmd_nhc": [P, P, P, P, c_int64, c_int64, c_int32, P, POINTER(NHCParams), c_int32, P, P, P, P, c_size_t, P],
     "spk_rpmd_gle": [P, P, c_int64, c_int32, P, P, P, c_int32, c_int32, P, c_uint64, P, c_int32, P],
     "spk_rpmd_barostat_workspace_bytes": [c_int64, c_int64],
+    "spk_so3_conv_fwd": [P, P, P, P, P, P, P, c_int64, c_int64, c_int, c_int, c_int, P, P],
+    "spk_so3_conv_bwd": [P, P, P, P, P, P, P, P, P, P, P, c_int64, c_int64, c_int, c_int, c_int, P, P, P, c_int, P],
+    "spk_so3_tp_fwd": [P, P, c_int64, c_int, c_int, P, P],
+    "spk_so3_tp_bwd": [P, P, P, c_int64, c_int, c_int, P, P, P],
+    "spk_so3_gate_fwd": [P, P, c_int64, c_int, c_int, P, P],
+    "spk_so3_gate_bwd": [P, P, P, c_int64, c_int, c_int, P, P, P, P],
+    "spk_so3_put_l0": [P, P, c_int64, c_int, c_int, P, P],
+    "spk_so3_take_l0": [P, c_int64, c_int, c_int, P, P],
     "spk_rpmd_barostat_thermostat": [P, c_int64, c_double, P, c_uint64, P, P],
     "spk_rpmd_barostat_half_step": [P, P, c_double, P, P, P, c_int64, c_int64, c_int32, P, P, P, c_double, c_double,
                                     c_double, c_double, P, P, P, c_size_t, P],

@@ -430,6 +430,94 @@ class PaiNNMixingFunction(torch.autograd.Function):
 
 
 # =====================================================================================================================
+# SO3net  (representation/so3net.py:103-155)
+# =====================================================================================================================
+class SO3netPack(ParamPack):
+    def build(self, mod):
+        self.F, self.T, self.L = mod.n_atom_basis, mod.n_interactions, mod.lmax
+        self.blocks = []
+        for t in range(self.T):
+            conv, gate = mod.so3convs[t], mod.gatings[t]
+            self.blocks.append(dict(
+                wf=_c(conv.filternet.weight), bf=_c(conv.filternet.bias), m1=ops.Lin(mod.mixings1[t].weight),
+                m2=ops.Lin(mod.mixings2[t].weight), m3=ops.Lin(mod.mixings3[t].weight),
+                sc=ops.Lin(gate.scaling.weight, gate.scaling.bias)))
+
+
+def so3net_forward(pk: SO3netPack, x0: Tensor, r_ij: Tensor, graph: ops.EdgeGraph, rbf_kind: int, n_rbf: int,
+                   rbf_p0: Tensor, rbf_p1: Optional[Tensor], cutoff: float, need_grad: bool):
+    """Returns the multipole features x [N,S,F] and the tape needed by so3net_backward."""
+    F, L = pk.F, pk.L
+    N, S = x0.shape[0], (pk.L + 1) ** 2
+    phi, dphi, geo = ops.edge_geometry(r_ij, graph, rbf_kind, n_rbf, rbf_p0, rbf_p1, cutoff, need_grad)
+    x = ops.so3_put_l0(None, x0, N, L, F, x0.device)                                          # scalar2rsh (:136)
+    tape = []
+    for b in pk.blocks:
+        dx = ops.so3_conv_fwd(x, phi, geo, graph, b["wf"], b["bf"], L, F, n_rbf)              # :140
+        ddx = b["m1"].fwd(dx.view(N * S, F)).view(N, S, F)                                    # :141
+        tp = ops.so3_tp_fwd(dx, ddx, L, F)                                                    # :142
+        m2 = b["m2"].fwd(tp.view(N * S, F)).view(N, S, F)                                     # :143
+        h = b["sc"].fwd(m2.view(N, S * F), k=F)                                               # :144, so3.py:330-332
+        g = ops.so3_gate_fwd(m2, h, L, F)                                                     # so3.py:333
+        x_new = b["m3"].fwd(g.view(N * S, F), addend=x.view(N * S, F)).view(N, S, F)          # :145-146
+        if need_grad:
+            tape.append((x, dx, ddx, m2, h))
+        x = x_new
+    return x, (phi, dphi, geo, tape)
+
+
+def so3net_backward(pk: SO3netPack, saved, graph: ops.EdgeGraph, n_rbf: int, g_x: Tensor, n_edges_total: int) -> Tensor:
+    """dE/dr_ij [E,3] (in the caller's edge order) from dE/dx [N,S,F]."""
+    F, L = pk.F, pk.L
+    phi, dphi, geo, tape = saved
+    N, S = g_x.shape[0], (L + 1) ** 2
+    g_rij = torch.empty((n_edges_total, 3), dtype=torch.float32, device=g_x.device)
+    for t in reversed(range(pk.T)):
+        b = pk.blocks[t]
+        x, dx, ddx, m2, h = tape[t]
+        g_g = b["m3"].bwd(g_x.view(N * S, F)).view(N, S, F)
+        g_m2, g_m2_row0, g_h = ops.so3_gate_bwd(g_g, m2, h, L, F)
+        b["sc"].bwd(g_h, addend=g_m2_row0, out=g_m2.view(N, S * F))                          # row 0 += scaling^T g_h
+        g_tp = b["m2"].bwd(g_m2.view(N * S, F)).view(N, S, F)
+        g_dx, g_ddx = ops.so3_tp_bwd(g_tp, dx, ddx, L, F)
+        g_dx = b["m1"].bwd(g_ddx.view(N * S, F), addend=g_dx.view(N * S, F)).view(N, S, F)
+        # dE/dx_in = residual + convolution reverse; block 0's would only reach the (position-independent) embedding
+        g_x = ops.so3_conv_bwd(x, g_dx, phi, dphi, geo, graph, b["wf"], b["bf"], L, F, n_rbf, g_x, g_rij,
+                               accumulate=(t != pk.T - 1), need_gx=(t > 0))
+    return g_rij
+
+
+class SO3netFunction(torch.autograd.Function):
+    """(r_ij [E,3], x0 [N,F]) -> (scalar rows [N,F], multipoles [N,S,F]); the scalar rows are returned contiguous so that
+    the Atomwise gradient arrives without a copy.  Backward gives dE/dr_ij (x0 = embedding output is treated as constant)."""
+
+    @staticmethod
+    def forward(ctx, r_ij, x0, holder):
+        mod, graph = holder["module"], holder["graph"]
+        pk = mod._pack()
+        need = r_ij.requires_grad
+        with ops.device_of(r_ij, x0):
+            x, saved = so3net_forward(pk, x0, r_ij.detach(), graph, mod._rbf_kind, mod._n_rbf, mod._rbf_p0, mod._rbf_p1,
+                                      mod._cutoff_value, need)
+            q = ops.so3_take_l0(x, pk.L, pk.F)
+        ctx.holder = dict(pk=pk, saved=saved, graph=graph, n_rbf=mod._n_rbf, E=r_ij.shape[0], N=x0.shape[0])
+        ctx.set_materialize_grads(False)
+        return q, x
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_q, g_x):
+        h = ctx.holder
+        pk = h["pk"]
+        some = g_q if g_q is not None else g_x
+        with ops.device_of(some):
+            g = ops.so3_put_l0(g_x.contiguous() if g_x is not None else None,
+                               g_q.contiguous() if g_q is not None else None, h["N"], pk.L, pk.F, some.device)
+            g_rij = so3net_backward(pk, h["saved"], h["graph"], h["n_rbf"], g, h["E"])
+        return g_rij, None, None
+
+
+# =====================================================================================================================
 # SchNet  (representation/schnet.py:147-173)
 # =====================================================================================================================
 class SchNetPack(ParamPack):

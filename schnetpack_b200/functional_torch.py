@@ -130,6 +130,27 @@ def schnet(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
     return inputs
 
 
+def so3net(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
+    """representation/so3net.py:103-155 with the nn.so3 modules' own ATen formulas."""
+    from .nn import so3
+
+    r_ij, idx_i, idx_j = inputs[properties.Rij], inputs[properties.idx_i], inputs[properties.idx_j]
+    d = torch.norm(r_ij, dim=1, keepdim=True)                                # :122
+    Y = mod.sphharm(r_ij / d)                                                # :123-125
+    phi = radial(mod.radial_basis, d)                                        # :126
+    fc = cutoff(mod.cutoff_fn, d)[..., None]                                 # :127
+    x = so3.scalar2rsh(_embed(mod, inputs)[:, None], int(mod.lmax))          # :130-136
+    for conv, m1, m2, gate, m3 in zip(mod.so3convs, mod.mixings1, mod.mixings2, mod.gatings, mod.mixings3):
+        dx = conv(x, phi, Y, fc, idx_i, idx_j)                               # :140
+        dx = dx + mod.so3product(dx, m1(dx))                                 # :141-142
+        x = x + m3(gate(m2(dx)))                                             # :143-146
+    inputs["scalar_representation"] = x[:, 0]
+    inputs["multipole_representation"] = x
+    if mod.return_vector_representation:
+        inputs["vector_representation"] = torch.roll(x[:, 1:4], 1, 1)
+    return inputs
+
+
 def atomwise(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
     """atomistic/atomwise.py:69-88."""
     act = _activation(mod.activation)

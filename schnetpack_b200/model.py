@@ -136,6 +136,12 @@ def _convert_representation(rep):
         new = representation.SchNet(rep.n_atom_basis, len(rep.interactions), rbf, cut, n_filters=rep.n_filters,
                                     shared_interactions=shared, activation=_map_act(act), nuclear_embedding=emb,
                                     electronic_embeddings=eemb)
+    elif name == "SO3net":
+        shared = len(rep.so3convs) > 1 and rep.so3convs[0] is rep.so3convs[1]
+        new = representation.SO3net(rep.n_atom_basis, rep.n_interactions, int(rep.lmax), rbf, cut,
+                                    shared_interactions=shared,
+                                    return_vector_representation=rep.return_vector_representation,
+                                    activation=rep.activation, nuclear_embedding=emb, electronic_embeddings=eemb)
     else:
         raise NotImplementedError(f"representation {name} is outside the CUDA hot path")
     new.load_state_dict(rep.state_dict())
@@ -181,8 +187,12 @@ def convert_model(model: nn.Module) -> NeuralNetworkPotential:
     return new
 
 
+# module lists of the representations that ``shared_interactions`` replicates (one module under every index)
+SHARED_BLOCK_KEYS = r"\.(interactions|mixing|so3convs|mixings1|mixings2|mixings3|gatings)\.\d+\."
+
+
 def from_spec(spec: dict, params: Optional[dict] = None, device=None) -> NeuralNetworkPotential:
-    """Assemble [PairwiseDistances] -> {PaiNN|SchNet} -> [Atomwise(energy), Forces] from a ``synthetic.model_spec``
+    """Assemble [PairwiseDistances] -> {PaiNN|SchNet|SO3net} -> [Atomwise(energy), Forces] from a ``synthetic.model_spec``
     dictionary and (optionally) a flat weight dictionary with the reference ``state_dict`` keys."""
     import numpy as np
 
@@ -195,6 +205,10 @@ def from_spec(spec: dict, params: Optional[dict] = None, device=None) -> NeuralN
         rep = representation.PaiNN(spec["n_atom_basis"], spec["n_interactions"], rbf, cut,
                                    shared_interactions=spec["shared_interactions"],
                                    shared_filters=spec["shared_filters"], epsilon=spec["epsilon"])
+    elif spec["kind"] == "so3net":
+        rep = representation.SO3net(spec["n_atom_basis"], spec["n_interactions"], spec["lmax"], rbf, cut,
+                                    shared_interactions=spec["shared_interactions"],
+                                    return_vector_representation=bool(spec.get("return_vector_representation", False)))
     else:
         rep = representation.SchNet(spec["n_atom_basis"], spec["n_interactions"], rbf, cut,
                                     n_filters=spec["n_filters"], shared_interactions=spec["shared_interactions"])
@@ -212,7 +226,7 @@ def from_spec(spec: dict, params: Optional[dict] = None, device=None) -> NeuralN
         for k in sd:
             kk = k
             if k not in params and spec["shared_interactions"]:
-                kk = re.sub(r"\.(interactions|mixing)\.\d+\.", r".\1.0.", k)
+                kk = re.sub(SHARED_BLOCK_KEYS, r".\1.0.", k)
             new[k] = torch.as_tensor(np.asarray(params[kk])).to(sd[k].dtype)
         model.load_state_dict(new)
     model.eval()

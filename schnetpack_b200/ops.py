@@ -684,3 +684,65 @@ def atomwise_out_bwd(g_energy: Optional[Tensor], idx_m: Optional[Tensor], w1, n_
     g_hid = torch.empty((n_atoms, H), dtype=torch.float32, device=w1.device)
     _lib.call("spk_atomwise_out_bwd", _p(g_energy), _p(idx_m), _p(w1), n_atoms, H, _p(g_hid), _stream())
     return g_hid
+
+
+# ------------------------------------------------------------------------------------------------------------ SO3net
+def so3_conv_fwd(x, phi, geo, graph: EdgeGraph, wf, bf, lmax: int, F: int, n_rbf: int):
+    """SO3Convolution of one interaction block: x [N,S,F] -> y [N,S,F], filter evaluated in-kernel."""
+    N, S = graph.n_atoms, (lmax + 1) ** 2
+    y = torch.empty((N, S, F), dtype=torch.float32, device=x.device)
+    _lib.call("spk_so3_conv_fwd", _p(x), _p(phi), _p(geo), _p(graph.rowptr), _p(graph.slot_j), _p(wf), _p(bf), N,
+              graph.n_edges, lmax, F, n_rbf, _p(y), _stream())
+    return y
+
+
+def so3_conv_bwd(x, g_y, phi, dphi, geo, graph: EdgeGraph, wf, bf, lmax: int, F: int, n_rbf: int,
+                 g_res: Optional[Tensor], g_rij: Tensor, accumulate: bool, need_gx: bool = True):
+    """(dE/dy, residual dE/dx) -> dE/dx_in [N,S,F] (None unless ``need_gx``); dE/dr_ij written or added to ``g_rij``."""
+    N, S = graph.n_atoms, (lmax + 1) ** 2
+    g_x = torch.empty((N, S, F), dtype=torch.float32, device=x.device) if need_gx else None
+    _lib.call("spk_so3_conv_bwd", _p(x), _p(g_y), _p(phi), _p(dphi), _p(geo), _p(graph.sptr), _p(graph.pos_slot),
+              _p(graph.pos_i), _p(graph.slot_eid), _p(wf), _p(bf), N, graph.n_edges, lmax, F, n_rbf, _p(g_res), _p(g_x),
+              _p(g_rij), 1 if accumulate else 0, _stream())
+    return g_x
+
+
+def so3_tp_fwd(dx, ddx, lmax: int, F: int):
+    out = torch.empty_like(dx)
+    _lib.call("spk_so3_tp_fwd", _p(dx), _p(ddx), dx.shape[0], lmax, F, _p(out), _stream())
+    return out
+
+
+def so3_tp_bwd(g, dx, ddx, lmax: int, F: int):
+    g_dx = torch.empty_like(dx)
+    g_ddx = torch.empty_like(dx)
+    _lib.call("spk_so3_tp_bwd", _p(g), _p(dx), _p(ddx), dx.shape[0], lmax, F, _p(g_dx), _p(g_ddx), _stream())
+    return g_dx, g_ddx
+
+
+def so3_gate_fwd(x, h, lmax: int, F: int):
+    y = torch.empty_like(x)
+    _lib.call("spk_so3_gate_fwd", _p(x), _p(h), x.shape[0], lmax, F, _p(y), _stream())
+    return y
+
+
+def so3_gate_bwd(g_y, x, h, lmax: int, F: int):
+    """-> (dE/dx [N,S,F] with row 0 left for the caller, dE/dx row 0 through the gate [N,F], dE/dh [N,(lmax+1)F])"""
+    N = x.shape[0]
+    g_x = torch.empty_like(x)
+    g_x0 = torch.empty((N, F), dtype=torch.float32, device=x.device)
+    g_h = torch.empty_like(h)
+    _lib.call("spk_so3_gate_bwd", _p(g_y), _p(x), _p(h), N, lmax, F, _p(g_x), _p(g_x0), _p(g_h), _stream())
+    return g_x, g_x0, g_h
+
+
+def so3_put_l0(src: Optional[Tensor], v: Optional[Tensor], n_atoms: int, lmax: int, F: int, device):
+    out = torch.empty((n_atoms, (lmax + 1) ** 2, F), dtype=torch.float32, device=device)
+    _lib.call("spk_so3_put_l0", _p(src), _p(v), n_atoms, lmax, F, _p(out), _stream())
+    return out
+
+
+def so3_take_l0(x, lmax: int, F: int):
+    q = torch.empty((x.shape[0], F), dtype=torch.float32, device=x.device)
+    _lib.call("spk_so3_take_l0", _p(x), x.shape[0], lmax, F, _p(q), _stream())
+    return q

@@ -242,6 +242,9 @@ class ScriptRepresentation(nn.Module):
 
     def __init__(self, rep: nn.Module):
         super().__init__()
+        if not isinstance(rep, (representation.PaiNN, representation.SchNet)):
+            raise NotImplementedError(f"to_scriptable: {type(rep).__name__} has no TorchScript deployment (PaiNN and "
+                                      "SchNet only)")
         self.kind = "painn" if isinstance(rep, representation.PaiNN) else "schnet"
         if not isinstance(rep.embedding, nn.Embedding) or len(rep.electronic_embeddings) > 0:
             raise NotImplementedError("to_scriptable: plain nn.Embedding representations")

@@ -303,10 +303,13 @@ def periodic_box(n_atoms_total: int = 8192, density: float = 0.1002, cutoff: flo
 def model_spec(kind: str = "painn", n_atom_basis: int = 128, n_interactions: int = 3, n_rbf: int = 20,
                cutoff: float = 5.0, rbf: str = "gaussian", shared_interactions: bool = False,
                shared_filters: bool = False, epsilon: float = 1e-8, n_filters: Optional[int] = None,
-               forces: bool = True):
-    return dict(kind=kind, n_atom_basis=n_atom_basis, n_interactions=n_interactions, n_rbf=n_rbf, cutoff=cutoff,
+               forces: bool = True, lmax: int = 2):
+    spec = dict(kind=kind, n_atom_basis=n_atom_basis, n_interactions=n_interactions, n_rbf=n_rbf, cutoff=cutoff,
                 rbf=rbf, shared_interactions=shared_interactions, shared_filters=shared_filters, epsilon=epsilon,
                 n_filters=n_filters or n_atom_basis, forces=forces)
+    if kind == "so3net":
+        spec["lmax"] = lmax
+    return spec
 
 
 def _xavier(rng, out_f, in_f):
@@ -366,6 +369,21 @@ def init_params(spec: dict, seed: int = 0, bias_scale: float = 0.1) -> Dict[str,
             p[b + "filter_network.0.bias"] = bias(nfil)
             p[b + "filter_network.1.weight"] = _xavier(rng, nfil, nfil)
             p[b + "filter_network.1.bias"] = bias(nfil)
+    elif spec["kind"] == "so3net":
+        L = spec["lmax"]
+        from .nn.so3 import sh_indices, sparse_clebsch_gordan
+
+        widx = sh_indices(L)[0][sparse_clebsch_gordan(L)[1]].numpy()     # SO3Convolution.Widx (a persistent buffer)
+        for t in range(nblocks):
+            c = f"{pre}so3convs.{t}."
+            p[c + "Widx"] = widx
+            p[c + "filternet.weight"] = _xavier(rng, (L + 1) * F, nr)
+            p[c + "filternet.bias"] = bias((L + 1) * F)
+            for k in ("mixings1", "mixings2", "mixings3"):
+                p[f"{pre}{k}.{t}.weight"] = _xavier(rng, F, F)
+            g = f"{pre}gatings.{t}.scaling."
+            p[g + "weight"] = _xavier(rng, (L + 1) * F, F)
+            p[g + "bias"] = bias((L + 1) * F)
     else:
         raise ValueError(spec["kind"])
     # Atomwise head F -> F//2 -> 1 (atomistic/atomwise.py:60-66, nn/blocks.py:38-76)
