@@ -564,6 +564,68 @@ int spk_so3_gate_bwd(const float* g_y, const float* x, const float* h, int64_t n
 int spk_so3_put_l0(const float* src, const float* v, int64_t n_atoms, int lmax, int F, float* out, spk_stream_t stream);
 int spk_so3_take_l0(const float* x, int64_t n_atoms, int lmax, int F, float* q, spk_stream_t stream);
 
+/* ---- per-step model properties of DeviceMD (md/calculators/base_calculator.py:113-141) -------------------------------
+ * dst[i] = src[i] * conversion.  Time series: counter (int64[2], device) = (steps completed, records stored); step
+ * s = counter[0] + 1 is recorded when s % every == 0: buf[counter[1] * n + i] = src[i] (nothing once counter[1] reaches
+ * capacity).  spk_md_record_advance then advances both counters; call it once per step after every spk_md_record. */
+int spk_md_property(const float* src, int64_t n, float conversion, float* dst, spk_stream_t stream);
+int spk_md_record(const float* src, int64_t n, const int64_t* counter, int64_t every, int64_t capacity, float* buf,
+                  spk_stream_t stream);
+int spk_md_record_advance(int64_t* counter, int64_t every, int64_t capacity, spk_stream_t stream);
+
+/* ---- gated equivariant output heads (csrc/equivariant.cu) -------------------------------------------------------------
+ * nn/equivariant.py:57-71 (GatedEquivariantBlock), atomistic/atomwise.py:172-213 (DipoleMoment), :267-293
+ * (Polarizability).  Vectors are [N, 3, F]; VW = mix_vectors(V) is [N, 3, 2Fo] with V = VW[..., :Fo], W = VW[..., Fo:].
+ *
+ * Hidden-block glue (the three Dense layers run on spk_dense_tc / spk_dense):
+ *   ctx = [s | ||V||] [N, Fi+Fo] (no epsilon);  reverse: g_s = g_ctx[:, :Fi], g_VW[V columns] = g_ctx[:, Fi:] V / ||V||
+ *   (0 where ||V|| = 0; the W columns are left to spk_geq_gate_bwd)
+ *   s_out = act(x[:, :Fo]), v_out = x[:, Fo:] * W;  reverse: g_x [N, 2Fo], g_VW[W columns]  (g_s / g_v may be NULL) */
+int spk_geq_ctx(const float* s, const float* VW, int64_t n_atoms, int Fi, int Fo, float* ctx, spk_stream_t stream);
+int spk_geq_ctx_bwd(const float* g_ctx, const float* VW, int64_t n_atoms, int Fi, int Fo, float* g_s, float* g_VW,
+                    spk_stream_t stream);
+int spk_geq_gate(const float* x, const float* VW, int64_t n_atoms, int Fo, int act, float* s_out, float* v_out,
+                 spk_stream_t stream);
+int spk_geq_gate_bwd(const float* g_s, const float* g_v, const float* x, const float* VW, int64_t n_atoms, int Fo,
+                     int act, float* g_x, float* g_VW, spk_stream_t stream);
+
+#define SPK_HEAD_DIPOLE 0
+#define SPK_HEAD_POLAR 1
+/* weights of the last block (n_sout = n_vout = 1): Fi inputs, H gating hidden units (both <= 256) */
+typedef struct {
+    const float* wmix; /* [2, Fi]    mix_vectors.weight     */
+    const float* w0;   /* [H, Fi+1]  scalar_net.0.weight    */
+    const float* w0t;  /* [Fi+1, H]  its transpose          */
+    const float* b0;   /* [H]                               */
+    const float* w1;   /* [2, H]     scalar_net.1.weight    */
+    const float* b1;   /* [2]                               */
+    int32_t Fi, H, act, reserved;
+} spk_head_tail_t;
+size_t spk_head_workspace_bytes(int64_t n_atoms, int64_t n_sys);
+/* Per-system head outputs.  With `tail` the last block runs per atom on (s [N,Fi], V [N,3,Fi]); without it (scalar
+ * DipoleMoment) the charges q [N] are given.  Atoms of system m are [sys_ptr[m], sys_ptr[m+1]) (idx_m sorted).
+ *   dipole:  q' = q + c_m, c_m = correct ? (Q_m - sum_m q) / n_m : 0 (0 for an empty system, Q = total_charge or 0),
+ *            y_m = sum q' R + sum mu_atomic;  out [B, 3], or |y_m| [B] with `magnitude`
+ *   polar:   out [B, 3, 3] = sum alpha I + sum (nu (x) R + R (x) nu)
+ * Sums in fp64 through a fixed-shape segmented reduction: bitwise reproducible, no atomics.  q_atom [N] (may be NULL)
+ * receives the tail's charges; saved [B, 8] fp64 keeps (c, mean R, y, n) of the dipole for spk_head_charges and the
+ * reverse (zeros for the polarizability, whose reverse needs none of them). */
+int spk_head_fwd(int kind, const spk_head_tail_t* tail, const float* s, const float* V, const float* q, const float* R,
+                 const int64_t* idx_m, const int32_t* sys_ptr, const float* total_charge, int64_t n_atoms, int64_t n_sys,
+                 int correct, int magnitude, float* out, float* q_atom, double* saved, void* workspace,
+                 size_t workspace_bytes, spk_stream_t stream);
+/* charges[i] = q_atom[i] + c_{m(i)} */
+int spk_head_charges(const float* q_atom, const int64_t* idx_m, const double* saved, int64_t n_atoms, float* charges,
+                     spk_stream_t stream);
+/* Reverse of the tail head for g_out (the shape of out): g_s [N,Fi], g_V [N,3,Fi], g_R [N,3] (the direct position term) */
+int spk_head_bwd(int kind, const spk_head_tail_t* tail, const float* s, const float* V, const float* R,
+                 const int64_t* idx_m, const double* saved, const float* g_out, int64_t n_atoms, int correct,
+                 int magnitude, float* g_s, float* g_V, float* g_R, spk_stream_t stream);
+/* Reverse of the scalar dipole: g_hid[i, :] = g_q_i w1 (w1 [H] = the last Dense H -> 1) and g_R [N,3] */
+int spk_head_scalar_bwd(const float* q, const float* R, const int64_t* idx_m, const double* saved, const float* g_out,
+                        int correct, int magnitude, const float* w1, int64_t n_atoms, int H, float* g_hid, float* g_R,
+                        spk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -49,6 +49,12 @@ class NHCBarostat(Structure):
                 ("c_m", c_void_p), ("b_v", c_void_p), ("b_f", c_void_p), ("b_m", c_void_p)]
 
 
+class HeadTail(Structure):
+    """spk_head_tail_t of include/spk_b200.h."""
+    _fields_ = [("wmix", c_void_p), ("w0", c_void_p), ("w0t", c_void_p), ("b0", c_void_p), ("w1", c_void_p),
+                ("b1", c_void_p), ("Fi", c_int32), ("H", c_int32), ("act", c_int32), ("reserved", c_int32)]
+
+
 # name -> argument ctypes (return type is int unless listed in _RESTYPE)
 SIGNATURES = {
     "spk_version": [],
@@ -129,6 +135,19 @@ SIGNATURES = {
     "spk_so3_gate_bwd": [P, P, P, c_int64, c_int, c_int, P, P, P, P],
     "spk_so3_put_l0": [P, P, c_int64, c_int, c_int, P, P],
     "spk_so3_take_l0": [P, c_int64, c_int, c_int, P, P],
+    "spk_md_property": [P, c_int64, c_float, P, P],
+    "spk_md_record": [P, c_int64, P, c_int64, c_int64, P, P],
+    "spk_md_record_advance": [P, c_int64, c_int64, P],
+    "spk_geq_ctx": [P, P, c_int64, c_int, c_int, P, P],
+    "spk_geq_ctx_bwd": [P, P, c_int64, c_int, c_int, P, P, P],
+    "spk_geq_gate": [P, P, c_int64, c_int, c_int, P, P, P],
+    "spk_geq_gate_bwd": [P, P, P, P, c_int64, c_int, c_int, P, P, P],
+    "spk_head_workspace_bytes": [c_int64, c_int64],
+    "spk_head_fwd": [c_int, POINTER(HeadTail), P, P, P, P, P, P, P, c_int64, c_int64, c_int, c_int, P, P, P, P, c_size_t,
+                     P],
+    "spk_head_charges": [P, P, P, c_int64, P, P],
+    "spk_head_bwd": [c_int, POINTER(HeadTail), P, P, P, P, P, P, c_int64, c_int, c_int, P, P, P, P],
+    "spk_head_scalar_bwd": [P, P, P, P, P, c_int, c_int, P, c_int64, c_int, P, P, P],
     "spk_rpmd_barostat_thermostat": [P, c_int64, c_double, P, c_uint64, P, P],
     "spk_rpmd_barostat_half_step": [P, P, c_double, P, P, P, c_int64, c_int64, c_int32, P, P, P, c_double, c_double,
                                     c_double, c_double, P, P, P, c_size_t, P],
@@ -141,7 +160,7 @@ _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_siz
             "spk_schnet_filter_packed_floats": c_size_t,
             "spk_painn_filter_packed_floats": c_size_t, "spk_neighbor_list_workspace_bytes": c_size_t,
             "spk_md_thermostat_workspace_bytes": c_size_t, "spk_rpmd_workspace_bytes": c_size_t,
-            "spk_rpmd_barostat_workspace_bytes": c_size_t}
+            "spk_rpmd_barostat_workspace_bytes": c_size_t, "spk_head_workspace_bytes": c_size_t}
 
 _lib = None
 
@@ -184,7 +203,7 @@ LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out
             "spk_md_kinetic_energy": 2, "spk_md_berendsen": 3, "spk_pairwise_virial": 2,
             "spk_md_kinetic_energy_tensor": 3, "spk_md_barostat_thermostat": 4, "spk_md_barostat_kick": 3,
             "spk_md_barostat_half_step": 2, "spk_md_barostat_main_step": 2, "spk_rpmd_barostat_half_step": 2,
-            "spk_rpmd_barostat_main_step": 2}   # spk_rpmd_pile / spk_rpmd_nhc: 3 if global
+            "spk_rpmd_barostat_main_step": 2, "spk_head_fwd": 2}   # spk_rpmd_pile / spk_rpmd_nhc: 3 if global
 launch_count = 0
 
 

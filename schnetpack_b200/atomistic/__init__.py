@@ -1,6 +1,7 @@
 """Mirror of the hot-path output/input modules of ``schnetpack.atomistic`` on the CUDA kernels:
 ``PairwiseDistances`` (atomistic/distances.py:9-26), ``Atomwise`` (atomistic/atomwise.py:14-88) and ``Forces``
-(atomistic/response.py:18-92)."""
+(atomistic/response.py:18-92), and the gated equivariant heads ``DipoleMoment`` / ``Polarizability``
+(atomistic/atomwise.py:91-293)."""
 from __future__ import annotations
 
 from typing import Callable, Dict, List, Optional, Sequence, Union
@@ -15,7 +16,7 @@ from .. import nn as snn
 from .. import ops
 from .. import properties
 
-__all__ = ["PairwiseDistances", "Atomwise", "Forces", "Strain"]
+__all__ = ["PairwiseDistances", "Atomwise", "Forces", "Strain", "DipoleMoment", "Polarizability"]
 
 
 class PairwiseDistances(nn.Module):
@@ -186,4 +187,134 @@ class Forces(nn.Module):
             volume = torch.sum(cell[:, 0, :] * torch.cross(cell[:, 1, :], cell[:, 2, :], dim=1), dim=1,
                                keepdim=True)[:, :, None]
             inputs[self.stress_key] = stress / volume
+        return inputs
+
+
+class _GatedHead(nn.Module):
+    """Kernel plumbing shared by DipoleMoment and Polarizability: weight packing, the limits of the tail kernel and the
+    per-system index arrays (the number of systems comes from ``_n_atoms``, so there is no host read)."""
+
+    MAX_F = 256     # Fi and gating width of the last block (csrc/equivariant.cu HT_MAXF)
+
+    def _pack(self) -> K.HeadPack:
+        params = list(self.outnet.parameters())
+        if self._pk.stale(params):
+            self._pk.build(self)
+            self._pk.mark(params)
+        return self._pk
+
+    def _apply(self, fn, *a, **k):  # .to()/.cuda()/.float(): drop the cached kernel-side weights
+        self._pk = K.HeadPack()
+        return super()._apply(fn, *a, **k)
+
+    def _check_kernel_shape(self):
+        for m in self.modules():
+            if isinstance(m, snn.Dense):
+                snn.activation_code(m.activation)
+        if self._vector:
+            last = self.outnet[-1]
+            if last.n_sin > self.MAX_F or last.n_hidden > self.MAX_F:
+                raise NotImplementedError(f"{type(self).__name__}: the last gated block's input width ({last.n_sin}) and "
+                                          f"gating width ({last.n_hidden}) must be <= {self.MAX_F} for the CUDA kernels")
+            for blk in self.outnet:
+                snn.activation_code(blk.sactivation)
+
+    def _holder(self, inputs, kind, correct=False, magnitude=False, want_charges=False):
+        if properties.n_atoms not in inputs:
+            raise KeyError(f"{type(self).__name__} needs '{properties.n_atoms}' (the number of systems, without a host read)")
+        n_sys = int(inputs[properties.n_atoms].shape[0])
+        idx_m = inputs[properties.idx_m]
+        idx_m = (idx_m if idx_m.dtype == torch.int64 else idx_m.long()).contiguous()
+        tq = None
+        if correct and properties.total_charge in inputs:
+            tq = inputs[properties.total_charge].detach().to(torch.float32).contiguous()
+        return dict(pack=self._pack(), kind=kind, idx_m=idx_m, sys_ptr=ops.segment_ptr(idx_m, n_sys), n_sys=n_sys,
+                    total_charge=tq, correct=bool(correct), magnitude=bool(magnitude), want_charges=bool(want_charges))
+
+
+class DipoleMoment(_GatedHead):
+    """atomistic/atomwise.py:91-213 -- dipole moments from latent partial charges and, with
+    ``use_vector_representation``, atomic dipoles from the vector features.  Output [B, 3] ([B] with
+    ``predict_magnitude``), charges [N, 1] with ``return_charges``.
+
+    ``eval()``: the gated blocks / the charge MLP and the per-system assembly run on the kernels of csrc/equivariant.cu
+    (fp64 segmented sums, no atomics, no host read), differentiable with respect to positions and the representation
+    (dipole derivatives through ``torch.autograd.grad``).  The charges output is not differentiable on that path.
+    ``train()`` with trainable parameters under grad mode: the ATen formula of ``functional_torch``."""
+
+    def __init__(self, n_in: int, n_hidden: Optional[Union[int, Sequence[int]]] = None, n_layers: int = 2,
+                 activation: Callable = F.silu, predict_magnitude: bool = False, return_charges: bool = False,
+                 dipole_key: str = properties.dipole_moment, charges_key: str = properties.partial_charges,
+                 correct_charges: bool = True, use_vector_representation: bool = False):
+        super().__init__()
+        self.dipole_key = dipole_key
+        self.charges_key = charges_key
+        self.return_charges = return_charges
+        self.model_outputs = [dipole_key]
+        if self.return_charges:
+            self.model_outputs.append(charges_key)
+        self.predict_magnitude = predict_magnitude
+        self.use_vector_representation = use_vector_representation
+        self.correct_charges = correct_charges
+        if use_vector_representation:
+            self.outnet = snn.build_gated_equivariant_mlp(n_in=n_in, n_out=1, n_hidden=n_hidden, n_layers=n_layers,
+                                                          activation=activation, sactivation=activation)
+        else:
+            self.outnet = snn.build_mlp(n_in=n_in, n_out=1, n_hidden=n_hidden, n_layers=n_layers, activation=activation)
+        self._pk = K.HeadPack()
+
+    @property
+    def _vector(self) -> bool:
+        return self.use_vector_representation
+
+    @ops.on_tensor_device
+    def forward(self, inputs: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        if snn.use_training_path(self):
+            from .. import functional_torch as T
+
+            return T.dipole_moment(self, inputs)
+        self._check_kernel_shape()
+        h = self._holder(inputs, ops.HEAD_DIPOLE, self.correct_charges, self.predict_magnitude, self.return_charges)
+        s, R = inputs["scalar_representation"], inputs[properties.R]
+        if self.use_vector_representation:
+            y, charges = K.GatedHeadFunction.apply(s, inputs["vector_representation"], R, h)
+        else:
+            y, charges = K.ScalarDipoleFunction.apply(s, R, h)
+        if self.return_charges:
+            inputs[self.charges_key] = charges.unsqueeze(-1)
+        inputs[self.dipole_key] = y
+        return inputs
+
+
+class Polarizability(_GatedHead):
+    """atomistic/atomwise.py:216-293 -- rank-factorised polarizability alpha_m = sum alpha_i I + sum (nu_i (x) R_i +
+    R_i (x) nu_i), output [B, 3, 3]; needs scalar and vector features.  Kernel and training paths as ``DipoleMoment``."""
+
+    def __init__(self, n_in: int, n_hidden: Optional[Union[int, Sequence[int]]] = None, n_layers: int = 2,
+                 activation: Callable = F.silu, polarizability_key: str = properties.polarizability):
+        super().__init__()
+        self.n_in = n_in
+        self.n_layers = n_layers
+        self.n_hidden = n_hidden
+        self.polarizability_key = polarizability_key
+        self.model_outputs = [polarizability_key]
+        self.outnet = snn.build_gated_equivariant_mlp(n_in=n_in, n_out=1, n_hidden=n_hidden, n_layers=n_layers,
+                                                      activation=activation, sactivation=activation)
+        self.requires_dr = False
+        self.requires_stress = False
+        self._pk = K.HeadPack()
+
+    _vector = True
+
+    @ops.on_tensor_device
+    def forward(self, inputs: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        if snn.use_training_path(self):
+            from .. import functional_torch as T
+
+            return T.polarizability(self, inputs)
+        self._check_kernel_shape()
+        h = self._holder(inputs, ops.HEAD_POLAR)
+        alpha, _ = K.GatedHeadFunction.apply(inputs["scalar_representation"], inputs["vector_representation"],
+                                             inputs[properties.R], h)
+        inputs[self.polarizability_key] = alpha
         return inputs

@@ -252,6 +252,33 @@ __global__ void __launch_bounds__(VIR_T) k_virial_partials(const float* __restri
     for (int c = 0; c < 9; ++c) dst[c] = v[c];
 }
 
+// Per-step model properties of DeviceMD (md/calculators/base_calculator.py:113-141): dst = src * conversion, and the
+// device-side time series.  counter[0] = steps completed, counter[1] = records stored; both live in device memory and
+// advance in stream order, so a captured step records at the right slot on every replay.  Step s (1-based) is recorded
+// when s % every == 0.
+__global__ void k_md_property(const float* __restrict__ src, int64_t n, float conversion, float* __restrict__ dst) {
+    SPK_PDL_ENTER();
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i < n) dst[i] = src[i] * conversion;
+}
+
+__global__ void k_md_record(const float* __restrict__ src, int64_t n, const int64_t* __restrict__ counter, int64_t every,
+                            int64_t capacity, float* __restrict__ buf) {
+    SPK_PDL_ENTER();
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const int64_t step = counter[0] + 1, slot = counter[1];
+    if (i >= n || step % every != 0 || slot >= capacity) return;
+    buf[slot * n + i] = src[i];
+}
+
+__global__ void k_md_record_advance(int64_t* __restrict__ counter, int64_t every, int64_t capacity) {
+    SPK_PDL_ENTER();
+    if (threadIdx.x != 0) return;
+    const int64_t step = counter[0] + 1;
+    counter[0] = step;
+    if (step % every == 0 && counter[1] < capacity) counter[1] += 1;
+}
+
 }  // namespace
 
 #define GRID1D(n, T) (unsigned)spk_cdiv((n), (T)), (T), 0, spk_st(stream)
@@ -382,6 +409,32 @@ extern "C" int spk_pairwise_virial(const float* g_rij, const float* r_ij, const 
                    slot_eid, sys_ptr, n_sys, sys_part, head);
     spk_launch(k_seg_finish<VIR_T, 9>, (unsigned)n_sys, SEG_FIN_T, 0, spk_st(stream), rowptr, sys_ptr, sys_part, head,
                virial);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_md_property(const float* src, int64_t n, float conversion, float* dst, spk_stream_t stream) {
+    if (n < 0) return SPK_ERR_ARG;
+    if (n == 0) return SPK_OK;
+    if (!src || !dst) return SPK_ERR_ARG;
+    spk_launch(k_md_property, GRID1D(n, 256), src, n, conversion, dst);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_md_record(const float* src, int64_t n, const int64_t* counter, int64_t every, int64_t capacity,
+                             float* buf, spk_stream_t stream) {
+    if (n < 0 || every <= 0 || capacity <= 0) return SPK_ERR_ARG;
+    if (n == 0) return SPK_OK;
+    if (!src || !counter || !buf) return SPK_ERR_ARG;
+    spk_launch(k_md_record, GRID1D(n, 256), src, n, counter, every, capacity, buf);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_md_record_advance(int64_t* counter, int64_t every, int64_t capacity, spk_stream_t stream) {
+    if (!counter || every <= 0 || capacity <= 0) return SPK_ERR_ARG;
+    spk_launch(k_md_record_advance, 1, 32, 0, spk_st(stream), counter, every, capacity);
     SPK_LAUNCH_CHECK();
     return SPK_OK;
 }

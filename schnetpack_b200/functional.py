@@ -741,3 +741,121 @@ class PairwiseDistancesFunction(torch.autograd.Function):
                 (r_ij,) = ctx.saved_tensors
                 ops.pairwise_virial(g_rij, r_ij, graph, h["sys_ptr"], h["virial"])
         return g_R, (g_rij if ctx.off_grad else None), None
+
+
+# =====================================================================================================================
+# DipoleMoment / Polarizability (atomistic/atomwise.py:172-213, 267-293) with the gated equivariant MLP
+# (nn/equivariant.py:57-71, nn/blocks.py:79-156)
+# =====================================================================================================================
+class HeadPack(ParamPack):
+    """Kernel-ready weights of a head's outnet: hidden gated blocks as Lin triples, the last block as an
+    ``spk_head_tail_t``; for the scalar dipole, the hidden Dense layers and the last layer's weight row."""
+
+    def build(self, mod):
+        from .nn import activation_code
+
+        net = mod.outnet
+        self.blocks = []
+        if mod._vector:
+            for blk in list(net)[:-1]:
+                self.blocks.append(dict(mix=ops.Lin(blk.mix_vectors.weight), l0=ops.Lin(blk.scalar_net[0].weight,
+                                        blk.scalar_net[0].bias), l1=ops.Lin(blk.scalar_net[1].weight, blk.scalar_net[1].bias),
+                                        Fi=blk.n_sin, Fo=blk.n_vout, act=activation_code(blk.scalar_net[0].activation),
+                                        sact=activation_code(blk.sactivation)))
+            last = net[-1]
+            self.tail, self._keep = ops.head_tail(last.mix_vectors.weight, last.scalar_net[0].weight,
+                                                  last.scalar_net[0].bias, last.scalar_net[1].weight,
+                                                  last.scalar_net[1].bias, activation_code(last.scalar_net[0].activation))
+        else:
+            for lin in list(net)[:-1]:
+                self.blocks.append(dict(lin=ops.Lin(lin.weight, lin.bias), act=activation_code(lin.activation)))
+            self.w1 = _c(net[-1].weight).reshape(-1)
+            self.b1 = _c(net[-1].bias)
+            self.tail = None
+
+
+class GatedHeadFunction(torch.autograd.Function):
+    """(s [N,Fi], V [N,3,Fi], R [N,3]) -> (dipole [B,3] / |dipole| [B] / polarizability [B,3,3], charges [N]).  The
+    charges output is not differentiable; the head output is, with respect to s, V and R."""
+
+    @staticmethod
+    def forward(ctx, s, V, R, holder):
+        pk, kind = holder["pack"], holder["kind"]
+        s, V, Rd = _c(s), _c(V), _c(R)
+        N = s.shape[0]
+        tape = []
+        with ops.device_of(s, V, Rd):
+            for b in pk.blocks:
+                Fi, Fo = b["Fi"], b["Fo"]
+                VW = b["mix"].fwd(V.view(3 * N, Fi)).view(N, 3, 2 * Fo)
+                c = ops.geq_ctx(s, VW, Fi, Fo)
+                h, d0 = b["l0"].fwd(c, b["act"], save_deriv=True)
+                x = b["l1"].fwd(h)
+                tape.append((VW, d0, x))
+                s, V = ops.geq_gate(x, VW, Fo, b["sact"])
+            out, q_atom, saved = ops.head_fwd(kind, pk.tail, s, V, None, Rd, holder["idx_m"], holder["sys_ptr"],
+                                              holder["total_charge"], holder["n_sys"], holder["correct"],
+                                              holder["magnitude"], holder["want_charges"])
+            charges = ops.head_charges(q_atom, holder["idx_m"], saved) if q_atom is not None else s.new_zeros((0,))
+        ctx.holder = dict(holder, tape=tape, s=s, V=V, R=Rd, saved=saved)
+        ctx.mark_non_differentiable(charges)
+        ctx.set_materialize_grads(False)
+        return out, charges
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_out, _g_charges):
+        h = ctx.holder
+        if g_out is None:
+            return None, None, None, None
+        pk = h["pack"]
+        with ops.device_of(g_out):
+            g_s, g_V, g_R = ops.head_bwd(h["kind"], pk.tail, h["s"], h["V"], h["R"], h["idx_m"], h["saved"],
+                                         g_out.contiguous(), h["correct"], h["magnitude"])
+            N = g_s.shape[0]
+            for b, (VW, d0, x) in zip(reversed(pk.blocks), reversed(h["tape"])):
+                Fi, Fo = b["Fi"], b["Fo"]
+                g_x, g_VW = ops.geq_gate_bwd(g_s, g_V, x, VW, Fo, b["sact"])
+                g_h = b["l1"].bwd(g_x)
+                g_c = b["l0"].bwd(g_h, a_pre=d0, a_act=ops.ACT_GIVEN)
+                g_s = ops.geq_ctx_bwd(g_c, VW, g_VW, Fi, Fo)
+                g_V = b["mix"].bwd(g_VW.view(3 * N, 2 * Fo)).view(N, 3, Fi)
+        return g_s, g_V, g_R, None
+
+
+class ScalarDipoleFunction(torch.autograd.Function):
+    """(s [N,F], R [N,3]) -> (dipole [B,3] / |dipole| [B], charges [N]) for charges from a plain MLP (Lin layers, then
+    ``spk_atomwise_out`` without aggregation for the last Dense H -> 1)."""
+
+    @staticmethod
+    def forward(ctx, s, R, holder):
+        pk = holder["pack"]
+        h, Rd = _c(s), _c(R)
+        tape = []
+        with ops.device_of(h, Rd):
+            for b in pk.blocks:
+                h, d = b["lin"].fwd(h, b["act"], save_deriv=True)
+                tape.append(d)
+            q, _ = ops.atomwise_out(h, pk.w1, pk.b1, None, 0)
+            out, _, saved = ops.head_fwd(ops.HEAD_DIPOLE, None, None, None, q, Rd, holder["idx_m"], holder["sys_ptr"],
+                                         holder["total_charge"], holder["n_sys"], holder["correct"],
+                                         holder["magnitude"], False)
+            charges = ops.head_charges(q, holder["idx_m"], saved) if holder["want_charges"] else q.new_zeros((0,))
+        ctx.holder = dict(holder, tape=tape, q=q, R=Rd, saved=saved)
+        ctx.mark_non_differentiable(charges)
+        ctx.set_materialize_grads(False)
+        return out, charges
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_out, _g_charges):
+        h = ctx.holder
+        if g_out is None:
+            return None, None, None
+        pk = h["pack"]
+        with ops.device_of(g_out):
+            g_h, g_R = ops.head_scalar_bwd(h["q"], h["R"], h["idx_m"], h["saved"], g_out.contiguous(), h["correct"],
+                                           h["magnitude"], pk.w1)
+            for b, d in zip(reversed(pk.blocks), reversed(h["tape"])):
+                g_h = b["lin"].bwd(g_h, a_pre=d, a_act=ops.ACT_GIVEN)
+        return g_h, g_R, None

@@ -169,3 +169,64 @@ def atomwise(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
             y = y / inputs[properties.n_atoms]
     inputs[mod.output_key] = y
     return inputs
+
+
+def gated_block(blk, s: Tensor, v: Tensor):
+    """nn/equivariant.py:57-71."""
+    vmix = F_.linear(v, blk.mix_vectors.weight)
+    vV, vW = torch.split(vmix, blk.n_vout, dim=-1)
+    ctx = torch.cat([s, torch.norm(vV, dim=-2)], dim=-1)
+    x = dense(ctx, blk.scalar_net[0], _activation(blk.scalar_net[0].activation))
+    x = dense(x, blk.scalar_net[1])
+    s_out, x = torch.split(x, [blk.n_sout, blk.n_vout], dim=-1)
+    v_out = x.unsqueeze(-2) * vW
+    if blk.sactivation:
+        s_out = _act(_activation(blk.sactivation), s_out)
+    return s_out, v_out
+
+
+def _n_sys(inputs: Dict[str, Tensor]) -> int:
+    return int(inputs[properties.n_atoms].shape[0])
+
+
+def dipole_moment(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
+    """atomistic/atomwise.py:172-213."""
+    R, idx_m = inputs[properties.R], inputs[properties.idx_m]
+    n_sys = _n_sys(inputs)
+    s = inputs["scalar_representation"]
+    if mod.use_vector_representation:
+        v = inputs["vector_representation"]
+        for blk in mod.outnet:
+            s, v = gated_block(blk, s, v)
+        charges, atomic_dipoles = s, v.squeeze(-1)
+    else:
+        for lin in mod.outnet:
+            s = dense(s, lin, _activation(lin.activation))
+        charges, atomic_dipoles = s, None
+    if mod.correct_charges:
+        sum_charge = scatter_add(charges, idx_m, n_sys)
+        total = inputs[properties.total_charge][:, None] if properties.total_charge in inputs else torch.zeros_like(sum_charge)
+        charges = charges + ((total - sum_charge) / inputs[properties.n_atoms].unsqueeze(-1))[idx_m]
+    if mod.return_charges:
+        inputs[mod.charges_key] = charges
+    y = R * charges
+    if atomic_dipoles is not None:
+        y = y + atomic_dipoles
+    y = scatter_add(y, idx_m, n_sys)
+    if mod.predict_magnitude:
+        y = torch.norm(y, dim=1, keepdim=False)
+    inputs[mod.dipole_key] = y
+    return inputs
+
+
+def polarizability(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
+    """atomistic/atomwise.py:267-293."""
+    R = inputs[properties.R]
+    s, v = inputs["scalar_representation"], inputs["vector_representation"]
+    for blk in mod.outnet:
+        s, v = gated_block(blk, s, v)
+    alpha = torch.diag_embed(s[..., 0:1].expand(-1, 3))
+    mur = v[..., None, 0] * R[..., None, :]
+    alpha = alpha + mur + mur.transpose(-2, -1)
+    inputs[mod.polarizability_key] = scatter_add(alpha, inputs[properties.idx_m], _n_sys(inputs))
+    return inputs

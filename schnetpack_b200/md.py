@@ -54,7 +54,7 @@ from __future__ import annotations
 
 import ctypes
 import math
-from typing import Dict, Optional
+from typing import Dict, List, Optional
 
 import torch
 
@@ -859,7 +859,10 @@ class DeviceMD:
                  capacity: int, momenta: Optional[Tensor] = None, use_graph: bool = True,
                  position_conversion: float = 1.0, energy_conversion: float = 1.0,
                  thermostat: Optional[_Thermostat] = None, barostat: Optional[object] = None,
-                 compute_stress: bool = False, ring_polymer: Optional[RingPolymer] = None):
+                 compute_stress: bool = False, ring_polymer: Optional[RingPolymer] = None,
+                 required_properties: Optional[List[str]] = None,
+                 property_conversion: Optional[Dict[str, float]] = None, record_every: int = 1,
+                 record_capacity: int = 0):
         """``batch[_positions]`` (and ``_cell``) are in MODEL units as everywhere in this package; ``self.positions`` is the
         MD-unit state (= model positions / position_conversion).  ``thermostat`` (None = NVE) is bound to the systems of
         the batch and applied around every step.  ``barostat`` (an NHC barostat, which thermostats the particles itself)
@@ -870,7 +873,16 @@ class DeviceMD:
         beads, replica-major (P B systems; bead r of system m is system r B + m, positions [P, N, 3] flat as [P N, 3]), all
         beads start at the batch positions, ``momenta`` may be [N, 3] (copied to every bead) or [P, N, 3], and ``capacity``
         is the pair capacity of the whole bead batch.  It takes only the ring-polymer thermostats and, for NPT, the
-        ``PILEBarostat`` (next to a ring-polymer thermostat or alone); no NHC barostat and no ``compute_stress``."""
+        ``PILEBarostat`` (next to a ring-polymer thermostat or alone); no NHC barostat and no ``compute_stress``.
+
+        ``required_properties`` (model output keys such as ``dipole_moment`` or ``polarizability``) are kept in
+        ``self.properties[name]`` after every evaluation, shaped ``[n_replicas, B, ...]`` (n_replicas = number of beads,
+        1 without a ring polymer) and multiplied by ``property_conversion[name]`` (default 1.0), as the reference's
+        calculator does (md/calculators/base_calculator.py:50-141).  The conversion is a number: unit strings would need
+        ASE's unit tables.  With ``record_capacity`` > 0 the step also appends them to a device-side time series every
+        ``record_every`` steps (steps s with s % record_every == 0, counted from the start), written inside the captured
+        step; ``recorded(name)`` returns the series, ``drain()`` empties it, and ``run`` refuses a call that would store
+        more than ``record_capacity`` records since the last drain."""
         dev = batch[P.R].device
         if dev.type != "cuda":
             raise ValueError("DeviceMD needs a CUDA batch (no CPU fallback)")
@@ -950,6 +962,7 @@ class DeviceMD:
                 barostat.bind(self._rp_base, self.dt, ring_polymer)               # on_simulation_start
             else:
                 barostat.bind(self.systems, self.dt)
+        self._setup_properties(required_properties, property_conversion, record_every, record_capacity)
         self._calculate()                       # forces at t = 0 (simulator.py:118)
 
     @property
@@ -1021,6 +1034,81 @@ class DeviceMD:
             out[k] = torch.cat([v] * n_beads).contiguous()
         return out
 
+    # ---- per-step model properties and their device-side time series ------------------------------------------------------
+    def _setup_properties(self, required, conversion, every, capacity):
+        self.required_properties = list(dict.fromkeys(required or []))
+        conversion = dict(conversion or {})
+        unknown = sorted(set(conversion) - set(self.required_properties))
+        if unknown:
+            raise ValueError(f"DeviceMD: property_conversion names properties that are not required: {unknown}")
+        for k, v in conversion.items():
+            if isinstance(v, str):
+                raise NotImplementedError(f"DeviceMD: property_conversion['{k}'] = {v!r}: give the conversion factor as a "
+                                          "number (unit strings need ASE's unit tables)")
+        self.property_conversion = {p: float(conversion.get(p, 1.0)) for p in self.required_properties}
+        outputs = getattr(self.model, "model_outputs", None)
+        if outputs is not None:
+            missing = [p for p in self.required_properties if p not in outputs]
+            if missing:
+                raise ValueError(f"DeviceMD: required properties {missing} are not model outputs ({sorted(outputs)})")
+        if int(every) < 1 or int(capacity) < 0:
+            raise ValueError("DeviceMD: record_every must be >= 1 and record_capacity >= 0")
+        if int(capacity) > 0 and not self.required_properties:
+            raise ValueError("DeviceMD: record_capacity needs required_properties")
+        self.record_every, self.record_capacity = int(every), int(capacity)
+        self.properties: Dict[str, Tensor] = {}
+        self._records: Dict[str, Tensor] = {}
+        self._n_records = 0                      # host mirror of the device count: the record count is deterministic
+        self._rec_counter = torch.zeros(2, dtype=torch.int64, device=self.positions.device)
+
+    def _n_replicas(self) -> int:
+        return self.ring_polymer.n_beads if self.ring_polymer is not None else 1
+
+    def _refresh_properties(self, out: Dict[str, Tensor]):
+        """properties[p] = out[p] viewed [n_replicas, B, ...] times the conversion (base_calculator.py:132-137)"""
+        for p in self.required_properties:
+            v = out[p].detach()
+            if v.dtype != torch.float32 or not v.is_contiguous():
+                raise TypeError(f"DeviceMD: property '{p}' must be a contiguous float32 model output")
+            buf = self.properties.get(p)
+            if buf is None:
+                buf = torch.empty(v.reshape(self._n_replicas(), -1, *v.shape[1:]).shape, dtype=torch.float32,
+                                  device=v.device)
+                self.properties[p] = buf
+                if self.record_capacity:
+                    self._records[p] = torch.zeros((self.record_capacity,) + tuple(buf.shape), dtype=torch.float32,
+                                                   device=v.device)
+            _lib.call("spk_md_property", ops._p(v), v.numel(), self.property_conversion[p], ops._p(buf), ops._stream())
+
+    def _record(self):
+        if not self.record_capacity:
+            return
+        for p in self.required_properties:
+            buf = self.properties[p]
+            _lib.call("spk_md_record", ops._p(buf), buf.numel(), ops._p(self._rec_counter), self.record_every,
+                      self.record_capacity, ops._p(self._records[p]), ops._stream())
+        _lib.call("spk_md_record_advance", ops._p(self._rec_counter), self.record_every, self.record_capacity,
+                  ops._stream())
+
+    def _records_in(self, n_steps: int) -> int:
+        k = self.record_every
+        return (self.steps_done + n_steps) // k - self.steps_done // k
+
+    def recorded(self, name: str) -> Tensor:
+        """The time series of ``name`` since the last ``drain`` in step order, [n_records, n_replicas, B, ...] on the host
+        (one device-to-host copy)."""
+        if name not in self._records:
+            raise KeyError(f"DeviceMD: '{name}' is not recorded (required_properties={self.required_properties}, "
+                           f"record_capacity={self.record_capacity})")
+        return self._records[name][:self._n_records].cpu()
+
+    def drain(self) -> Dict[str, Tensor]:
+        """Return every recorded series (as ``recorded``) and empty the recorder."""
+        out = {p: self.recorded(p) for p in self._records}
+        self._rec_counter[1].zero_()
+        self._n_records = 0
+        return out
+
     # ---- one force evaluation on the current positions (calculator.calculate) ---------------------------------------------
     def _calculate(self):
         ops._GRAPH_CACHE.clear()
@@ -1037,6 +1125,8 @@ class DeviceMD:
             self.forces.copy_(f)
             self.n_pairs.copy_(x["_n_pairs"])
         torch.maximum(self.nl_watch, x["_n_pairs"], out=self.nl_watch)
+        if self.required_properties:
+            self._refresh_properties(out)
 
     def _verlet(self, drift: bool):
         n = self.positions.shape[0]
@@ -1094,6 +1184,10 @@ class DeviceMD:
             self.thermostat.apply(self.momenta)
 
     def _step(self):
+        self._dynamics()
+        self._record()
+
+    def _dynamics(self):
         if self.ring_polymer is not None and self.barostat is not None:
             return self._rpmd_npt_step()
         if self.ring_polymer is not None:
@@ -1120,6 +1214,9 @@ class DeviceMD:
             state.extend([self.virial, self.cell, self.model_cell])
         if self.barostat is not None:
             state.extend(self.barostat._state().values())
+        state.extend(self.properties.values())
+        if self.record_capacity:
+            state.extend([self._rec_counter] + list(self._records.values()))
         saved = [t.clone() for t in state]
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
@@ -1135,7 +1232,15 @@ class DeviceMD:
         self._graph = graph
 
     def run(self, n_steps: int):
-        """Advance ``n_steps`` velocity-Verlet steps; returns (energy, forces) buffers of the last step (device)."""
+        """Advance ``n_steps`` velocity-Verlet steps; returns (energy, forces) buffers of the last step (device).  With a
+        recorder, a call that would store more than ``record_capacity`` records since the last ``drain`` is refused before
+        anything is launched."""
+        if self.record_capacity:
+            new = self._records_in(int(n_steps))
+            if self._n_records + new > self.record_capacity:
+                raise RuntimeError(f"DeviceMD: run({int(n_steps)}) would store {new} records on top of the "
+                                   f"{self._n_records} held, more than record_capacity = {self.record_capacity}; "
+                                   "call drain() first")
         if self.use_graph and self._graph is None:
             self._capture()
         for _ in range(int(n_steps)):
@@ -1143,6 +1248,8 @@ class DeviceMD:
                 self._graph.replay()
             else:
                 self._step()
+        if self.record_capacity:
+            self._n_records += self._records_in(int(n_steps))
         self.steps_done += int(n_steps)
         self.check_neighbor_list()
         return self.energy, self.forces
@@ -1244,6 +1351,11 @@ class DeviceMD:
             sd.update(cell=self.cell.clone(), model_cell=self.model_cell.clone(), virial=self.virial.clone())
         if self.barostat is not None:
             sd["barostat"] = self.barostat.state_dict()
+        if self.required_properties:
+            sd["properties"] = {p: v.clone() for p, v in self.properties.items()}
+        if self.record_capacity:
+            sd["recorder"] = {"counter": self._rec_counter.clone(), "n_records": self._n_records,
+                              "records": {p: v[:self._n_records].clone() for p, v in self._records.items()}}
         return sd
 
     def load_state_dict(self, state: Dict[str, object]):
@@ -1259,6 +1371,18 @@ class DeviceMD:
                 getattr(self, k).copy_(state[k])
         if self.barostat is not None:
             self.barostat.load_state_dict(state["barostat"])
+        for p, v in state.get("properties", {}).items():
+            self.properties[p].copy_(v)
+        if self.record_capacity:
+            rec = state["recorder"]
+            n = int(rec["n_records"])
+            if n > self.record_capacity:
+                raise ValueError(f"DeviceMD: the state holds {n} records, more than record_capacity = "
+                                 f"{self.record_capacity}")
+            self._rec_counter.copy_(rec["counter"])
+            for p, v in rec["records"].items():
+                self._records[p][:n].copy_(v)
+            self._n_records = n
         self.steps_done = int(state["steps_done"])
 
     # ---- cell, stress and pressure (system.py:567-614), MD units, per system, fp64 on the device ----------------------------

@@ -154,10 +154,39 @@ def _map_act(act):
     return {0: None, 1: F.silu, 2: snn.shifted_softplus}[code]
 
 
+def _gated_layout(outnet):
+    """(n_hidden as a list of block output widths, activation) of a reference gated equivariant MLP"""
+    blocks = list(outnet)
+    return [b.n_sout for b in blocks[:-1]], _map_act(blocks[0].scalar_net[0].activation)
+
+
+def _convert_head(m):
+    n = type(m).__name__
+    if n == "Polarizability" or m.use_vector_representation:
+        hidden, act = _gated_layout(m.outnet)
+        for b in m.outnet:
+            if b.n_hidden != b.n_sin:
+                raise NotImplementedError(f"{n}: gating widths other than the block input width")
+    else:
+        hidden, act = [l.out_features for l in list(m.outnet)[:-1]], _map_act(m.outnet[0].activation)
+    n_in = m.outnet[0].n_sin if (n == "Polarizability" or m.use_vector_representation) else m.outnet[0].in_features
+    kw = dict(n_in=n_in, n_hidden=hidden, n_layers=len(m.outnet), activation=act)
+    if n == "Polarizability":
+        new = atomistic.Polarizability(**kw, polarizability_key=m.polarizability_key)
+    else:
+        new = atomistic.DipoleMoment(**kw, predict_magnitude=m.predict_magnitude, return_charges=m.return_charges,
+                                     dipole_key=m.dipole_key, charges_key=m.charges_key,
+                                     correct_charges=m.correct_charges,
+                                     use_vector_representation=m.use_vector_representation)
+    new.load_state_dict(m.state_dict())
+    return new
+
+
 def convert_model(model: nn.Module) -> NeuralNetworkPotential:
     """Build a CUDA ``NeuralNetworkPotential`` from a loaded reference model (duck-typed on class names; weights are
-    copied through ``state_dict`` whose keys are identical).  Modules outside the hot path (postprocessors, custom
-    embeddings, other output heads) are reused as they are."""
+    copied through ``state_dict`` whose keys are identical).  ``Atomwise`` (n_out=1, n_layers=2), ``Forces``,
+    ``DipoleMoment`` and ``Polarizability`` heads are swapped for the CUDA modules; modules outside the hot path
+    (postprocessors, custom embeddings, other output heads) are reused as they are."""
     in_mods = []
     for m in model.input_modules:
         in_mods.append(atomistic.PairwiseDistances() if type(m).__name__ == "PairwiseDistances" else m)
@@ -173,6 +202,8 @@ def convert_model(model: nn.Module) -> NeuralNetworkPotential:
             out_mods.append(new)
         elif n == "Forces":
             out_mods.append(atomistic.Forces(m.calc_forces, m.calc_stress, m.energy_key, m.force_key, m.stress_key))
+        elif n in ("DipoleMoment", "Polarizability"):
+            out_mods.append(_convert_head(m))
         else:
             out_mods.append(m)
     new = NeuralNetworkPotential(_convert_representation(model.representation), in_mods, out_mods,

@@ -18,7 +18,8 @@ from torch.nn.init import xavier_uniform_, zeros_
 from .. import ops
 
 __all__ = ["GaussianRBF", "BesselRBF", "CosineCutoff", "cosine_cutoff", "gaussian_rbf", "Dense", "shifted_softplus",
-           "scatter_add", "build_mlp", "replicate_module", "activation_code", "use_training_path"]
+           "scatter_add", "build_mlp", "replicate_module", "activation_code", "use_training_path", "GatedEquivariantBlock",
+           "build_gated_equivariant_mlp"]
 
 
 def use_training_path(module: nn.Module) -> bool:
@@ -239,6 +240,60 @@ def build_mlp(n_in: int, n_out: int, n_hidden: Optional[Union[int, Sequence[int]
                             bias=last_bias))
     else:
         layers.append(Dense(n_neurons[-2], n_neurons[-1], activation=None, bias=last_bias))
+    return nn.Sequential(*layers)
+
+
+class GatedEquivariantBlock(nn.Module):
+    """nn/equivariant.py:11-71 -- gated mixing of scalar [N, n_sin] and vector [N, 3, n_vin] features.  Called on its own
+    it evaluates the ATen formula on any device; inside ``atomistic.DipoleMoment`` / ``Polarizability`` in ``eval()`` mode
+    its weights run on the kernels of ``csrc/equivariant.cu``."""
+
+    def __init__(self, n_sin: int, n_vin: int, n_sout: int, n_vout: int, n_hidden: int, activation=F.silu,
+                 sactivation=None):
+        super().__init__()
+        self.n_sin = n_sin
+        self.n_vin = n_vin
+        self.n_sout = n_sout
+        self.n_vout = n_vout
+        self.n_hidden = n_hidden
+        self.mix_vectors = Dense(n_vin, 2 * n_vout, activation=None, bias=False)
+        self.scalar_net = nn.Sequential(Dense(n_sin + n_vout, n_hidden, activation=activation),
+                                        Dense(n_hidden, n_sout + n_vout, activation=None))
+        self.sactivation = sactivation
+
+    def forward(self, inputs):
+        from .. import functional_torch as T
+
+        return T.gated_block(self, *inputs)
+
+
+def build_gated_equivariant_mlp(n_in: int, n_out: int, n_hidden: Optional[Union[int, Sequence[int]]] = None,
+                                n_gating_hidden: Optional[Union[int, Sequence[int]]] = None, n_layers: int = 2,
+                                activation: Callable = F.silu, sactivation: Callable = F.silu) -> nn.Module:
+    """nn/blocks.py:79-156 -- MLP of GatedEquivariantBlocks; the last block has no scalar activation."""
+    if n_hidden is None:
+        c_neurons = n_in
+        n_neurons = []
+        for _ in range(n_layers):
+            n_neurons.append(c_neurons)
+            c_neurons = max(n_out, c_neurons // 2)
+        n_neurons.append(n_out)
+    else:
+        if type(n_hidden) is int:
+            n_hidden = [n_hidden] * (n_layers - 1)
+        else:
+            n_hidden = list(n_hidden)
+        n_neurons = [n_in] + n_hidden + [n_out]
+    if n_gating_hidden is None:
+        n_gating_hidden = n_neurons[:-1]
+    elif type(n_gating_hidden) is int:
+        n_gating_hidden = [n_gating_hidden] * n_layers
+    else:
+        n_gating_hidden = list(n_gating_hidden)
+    layers = [GatedEquivariantBlock(n_neurons[i], n_neurons[i], n_neurons[i + 1], n_neurons[i + 1], n_gating_hidden[i],
+                                    activation=activation, sactivation=sactivation) for i in range(n_layers - 1)]
+    layers.append(GatedEquivariantBlock(n_neurons[-2], n_neurons[-2], n_neurons[-1], n_neurons[-1], n_gating_hidden[-1],
+                                        activation=activation, sactivation=None))
     return nn.Sequential(*layers)
 
 

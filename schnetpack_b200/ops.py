@@ -746,3 +746,95 @@ def so3_take_l0(x, lmax: int, F: int):
     q = torch.empty((x.shape[0], F), dtype=torch.float32, device=x.device)
     _lib.call("spk_so3_take_l0", _p(x), x.shape[0], lmax, F, _p(q), _stream())
     return q
+
+
+# ------------------------------------------------------------------------------------------------------------ output heads
+HEAD_DIPOLE, HEAD_POLAR = 0, 1
+
+
+def geq_ctx(s: Tensor, VW: Tensor, Fi: int, Fo: int) -> Tensor:
+    """[s | ||V||] of a GatedEquivariantBlock (VW = mix_vectors(V) [N,3,2Fo])."""
+    N = s.shape[0]
+    ctx = torch.empty((N, Fi + Fo), dtype=torch.float32, device=s.device)
+    _lib.call("spk_geq_ctx", _p(f32(s, "s")), _p(f32(VW, "VW")), N, Fi, Fo, _p(ctx), _stream())
+    return ctx
+
+
+def geq_ctx_bwd(g_ctx: Tensor, VW: Tensor, g_VW: Tensor, Fi: int, Fo: int) -> Tensor:
+    """-> g_s [N,Fi]; writes the V columns of g_VW"""
+    N = g_ctx.shape[0]
+    g_s = torch.empty((N, Fi), dtype=torch.float32, device=g_ctx.device)
+    _lib.call("spk_geq_ctx_bwd", _p(f32(g_ctx, "g_ctx")), _p(VW), N, Fi, Fo, _p(g_s), _p(g_VW), _stream())
+    return g_s
+
+
+def geq_gate(x: Tensor, VW: Tensor, Fo: int, act: int):
+    N = x.shape[0]
+    s_out = torch.empty((N, Fo), dtype=torch.float32, device=x.device)
+    v_out = torch.empty((N, 3, Fo), dtype=torch.float32, device=x.device)
+    _lib.call("spk_geq_gate", _p(f32(x, "x")), _p(f32(VW, "VW")), N, Fo, act, _p(s_out), _p(v_out), _stream())
+    return s_out, v_out
+
+
+def geq_gate_bwd(g_s: Optional[Tensor], g_v: Optional[Tensor], x: Tensor, VW: Tensor, Fo: int, act: int):
+    """-> (g_x [N,2Fo], g_VW [N,3,2Fo] with the W columns written)"""
+    N = x.shape[0]
+    g_x = torch.empty((N, 2 * Fo), dtype=torch.float32, device=x.device)
+    g_VW = torch.empty((N, 3, 2 * Fo), dtype=torch.float32, device=x.device)
+    _lib.call("spk_geq_gate_bwd", _p(g_s), _p(g_v), _p(x), _p(VW), N, Fo, act, _p(g_x), _p(g_VW), _stream())
+    return g_x, g_VW
+
+
+def head_tail(wmix: Tensor, w0: Tensor, b0: Tensor, w1: Tensor, b1: Tensor, act: int):
+    """Kernel-ready weights of the last gated block (n_sout = n_vout = 1); returns (struct, tensors kept alive)."""
+    keep = [f32(t.detach().contiguous(), "weight") for t in (wmix, w0, w0.t(), b0, w1, b1)]
+    st = _lib.HeadTail()
+    st.wmix, st.w0, st.w0t, st.b0, st.w1, st.b1 = (t.data_ptr() for t in keep)
+    st.Fi, st.H, st.act = int(wmix.shape[1]), int(w0.shape[0]), int(act)
+    return st, keep
+
+
+def head_fwd(kind: int, tail, s: Optional[Tensor], V: Optional[Tensor], q: Optional[Tensor], R: Tensor, idx_m: Tensor,
+             sys_ptr: Tensor, total_charge: Optional[Tensor], n_sys: int, correct: bool, magnitude: bool,
+             want_q: bool):
+    """-> (out [B,3] / [B] / [B,3,3], q_atom [N] or None, saved [B,8] fp64)"""
+    N = R.shape[0]
+    dev = R.device
+    shape = (n_sys, 3, 3) if kind == HEAD_POLAR else ((n_sys,) if magnitude else (n_sys, 3))
+    out = torch.empty(shape, dtype=torch.float32, device=dev)
+    saved = torch.empty((n_sys, 8), dtype=torch.float64, device=dev)
+    q_atom = torch.empty((N,), dtype=torch.float32, device=dev) if want_q and tail is not None else None
+    nbytes = int(_lib.lib().spk_head_workspace_bytes(N, n_sys))
+    ws = torch.empty(max(nbytes, 8), dtype=torch.uint8, device=dev)
+    _lib.call("spk_head_fwd", kind, tail, _p(s), _p(V), _p(q), _p(f32(R, "_positions")), _p(i64(idx_m, "_idx_m")),
+              _p(sys_ptr), _p(total_charge), N, n_sys, int(correct), int(magnitude), _p(out), _p(q_atom), _p(saved),
+              _p(ws), nbytes, _stream(), launches=2 if N > 0 else 1)
+    return out, q_atom, saved
+
+
+def head_charges(q_atom: Tensor, idx_m: Tensor, saved: Tensor) -> Tensor:
+    charges = torch.empty_like(q_atom)
+    _lib.call("spk_head_charges", _p(q_atom), _p(idx_m), _p(saved), q_atom.shape[0], _p(charges), _stream())
+    return charges
+
+
+def head_bwd(kind: int, tail, s: Tensor, V: Tensor, R: Tensor, idx_m: Tensor, saved: Tensor, g_out: Tensor,
+             correct: bool, magnitude: bool):
+    N, Fi = s.shape
+    dev = s.device
+    g_s = torch.empty((N, Fi), dtype=torch.float32, device=dev)
+    g_V = torch.empty((N, 3, Fi), dtype=torch.float32, device=dev)
+    g_R = torch.empty((N, 3), dtype=torch.float32, device=dev)
+    _lib.call("spk_head_bwd", kind, tail, _p(s), _p(V), _p(R), _p(idx_m), _p(saved), _p(f32(g_out, "g_out")), N,
+              int(correct), int(magnitude), _p(g_s), _p(g_V), _p(g_R), _stream())
+    return g_s, g_V, g_R
+
+
+def head_scalar_bwd(q: Tensor, R: Tensor, idx_m: Tensor, saved: Tensor, g_out: Tensor, correct: bool, magnitude: bool,
+                    w1: Tensor):
+    N, H = q.shape[0], w1.numel()
+    g_hid = torch.empty((N, H), dtype=torch.float32, device=q.device)
+    g_R = torch.empty((N, 3), dtype=torch.float32, device=q.device)
+    _lib.call("spk_head_scalar_bwd", _p(q), _p(R), _p(idx_m), _p(saved), _p(f32(g_out, "g_out")), int(correct),
+              int(magnitude), _p(w1), N, H, _p(g_hid), _p(g_R), _stream())
+    return g_hid, g_R

@@ -381,6 +381,9 @@ def to_scriptable(model: NeuralNetworkPotential) -> ScriptedPotential:
             outs.append(ScriptAtomwise(m))
         elif n == "Forces":
             outs.append(ScriptForces(m))
+        elif n in ("DipoleMoment", "Polarizability"):
+            raise NotImplementedError(f"to_scriptable: {n} has no TorchScript twin (its kernels run through "
+                                      "torch.autograd.Function); evaluate the model in Python")
         else:
             outs.append(m)                         # other heads must be scriptable themselves (as in the reference)
     return ScriptedPotential(ins, ScriptRepresentation(model.representation), outs, list(model.postprocessors),
