@@ -626,6 +626,49 @@ int spk_head_scalar_bwd(const float* q, const float* R, const int64_t* idx_m, co
                         int correct, int magnitude, const float* w1, int64_t n_atoms, int H, float* g_hid, float* g_R,
                         spk_stream_t stream);
 
+/* ---- batchwise L-BFGS relaxation (csrc/relax.cu; interfaces/batchwise_optimization.py:613-917) ----------------------
+ * One optimizer per system (atoms [sys_ptr[m], sys_ptr[m+1])), state fp64 on the device, positions in optimizer units
+ * (model positions x position_conversion).  order [n_sys] lists the systems of at most SPK_RELAX_WARP_ATOMS atoms first
+ * (n_warp of them, one warp each), then the larger ones (one thread-block cluster each).  counter (int64[2]) = (steps
+ * taken as the next step reads it, steps taken as the last step wrote it); spk_relax_converged must run between two
+ * steps, on the forces the next step uses.
+ *
+ * spk_relax_step, with f = forces x force_conversion (0 on fixed atoms) and it = counter[0]:
+ *   if it > 0: slot (it-1) % memory of s / y [memory, 3N] = r - r0, f0 - f; rho [memory, n_sys] = 1 / (y.s) if
+ *              y.s > 1e-8, else 1;
+ *   two-loop recursion over the last min(memory, it) entries with H0 = h0; p = 0 for a converged system;
+ *   per system, p *= maxstep / longest if the longest per-atom step >= maxstep;
+ *   r0 = r, f0 = f, r += damping p, model_positions = float(r / position_conversion), counter[1] = it + 1.
+ * spk_relax_converged: fmax_sys[m] = max_a |f_a|, converged[m] = fmax_sys[m]^2 < fmax[0]^2, steps[m] = the counter[1]
+ *   at which the system became converged (kept while it stays converged, -1 otherwise), n_unconverged[0] = count of
+ *   unconverged systems, counter[0] = counter[1].
+ * All sums run in a fixed order (bitwise reproducible), without atomics. */
+#define SPK_RELAX_WARP_ATOMS 256
+#define SPK_RELAX_MAX_MEMORY 4096
+typedef struct {
+    double* r;                 /* [N, 3] */
+    double* r0;                /* [N, 3] */
+    double* f0;                /* [N, 3] */
+    double* s;                 /* [memory, N, 3] */
+    double* y;                 /* [memory, N, 3] */
+    double* rho;               /* [memory, n_sys] */
+    double* p;                 /* [N, 3] step direction after masking and capping */
+    int64_t* counter;          /* [2] */
+    const double* fmax;        /* [1] convergence threshold */
+    double* fmax_sys;          /* [n_sys] */
+    int32_t* converged;        /* [n_sys] */
+    int64_t* steps;            /* [n_sys] */
+    int32_t* n_unconverged;    /* [1] */
+    const uint8_t* fixed;      /* [N] or NULL */
+    float* model_positions;    /* [N, 3] */
+    const int32_t* sys_ptr;    /* [n_sys + 1] */
+    const int32_t* order;      /* [n_sys] */
+    int64_t n_atoms, n_sys, n_warp, memory;
+    double force_conversion, position_conversion, maxstep, damping, h0;
+} spk_lbfgs_t;
+int spk_relax_step(const spk_lbfgs_t* state, const float* forces, spk_stream_t stream);
+int spk_relax_converged(const spk_lbfgs_t* state, const float* forces, spk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

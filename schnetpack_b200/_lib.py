@@ -55,6 +55,20 @@ class HeadTail(Structure):
                 ("b1", c_void_p), ("Fi", c_int32), ("H", c_int32), ("act", c_int32), ("reserved", c_int32)]
 
 
+class LBFGSState(Structure):
+    """spk_lbfgs_t of include/spk_b200.h (device pointers of the optimizer state and its parameters)."""
+    _fields_ = [("r", c_void_p), ("r0", c_void_p), ("f0", c_void_p), ("s", c_void_p), ("y", c_void_p),
+                ("rho", c_void_p), ("p", c_void_p), ("counter", c_void_p), ("fmax", c_void_p), ("fmax_sys", c_void_p),
+                ("converged", c_void_p), ("steps", c_void_p), ("n_unconverged", c_void_p), ("fixed", c_void_p),
+                ("model_positions", c_void_p), ("sys_ptr", c_void_p), ("order", c_void_p), ("n_atoms", c_int64),
+                ("n_sys", c_int64), ("n_warp", c_int64), ("memory", c_int64), ("force_conversion", c_double),
+                ("position_conversion", c_double), ("maxstep", c_double), ("damping", c_double), ("h0", c_double)]
+
+
+RELAX_WARP_ATOMS = 256      # SPK_RELAX_WARP_ATOMS
+RELAX_MAX_MEMORY = 4096     # SPK_RELAX_MAX_MEMORY
+
+
 # name -> argument ctypes (return type is int unless listed in _RESTYPE)
 SIGNATURES = {
     "spk_version": [],
@@ -153,6 +167,8 @@ SIGNATURES = {
                                     c_double, c_double, P, P, P, c_size_t, P],
     "spk_rpmd_barostat_main_step": [P, P, P, P, P, c_int64, c_int64, c_int32, P, P, c_double, P, P, P, P, c_double, P,
                                     c_size_t, P],
+    "spk_relax_step": [POINTER(LBFGSState), P, P],
+    "spk_relax_converged": [POINTER(LBFGSState), P, P],
 }
 _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_size_t,
             "spk_pairwise_virial_workspace_bytes": c_size_t, "spk_md_barostat_workspace_bytes": c_size_t,
@@ -203,7 +219,8 @@ LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out
             "spk_md_kinetic_energy": 2, "spk_md_berendsen": 3, "spk_pairwise_virial": 2,
             "spk_md_kinetic_energy_tensor": 3, "spk_md_barostat_thermostat": 4, "spk_md_barostat_kick": 3,
             "spk_md_barostat_half_step": 2, "spk_md_barostat_main_step": 2, "spk_rpmd_barostat_half_step": 2,
-            "spk_rpmd_barostat_main_step": 2, "spk_head_fwd": 2}   # spk_rpmd_pile / spk_rpmd_nhc: 3 if global
+            "spk_rpmd_barostat_main_step": 2, "spk_head_fwd": 2,
+            "spk_relax_converged": 2}   # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global
 launch_count = 0
 
 

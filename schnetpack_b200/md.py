@@ -854,7 +854,67 @@ class PILEBarostat:
             v.copy_(state[k])
 
 
-class DeviceMD:
+class _CapturedEvaluation:
+    """The force evaluation of a device-resident loop (calculator.calculate) and the capture of one whole step with it:
+    neighbour list on the fixed-capacity ``self.nl``, ``self.model`` on ``self.static`` and copies of the outputs into
+    ``self.energy`` / ``self.forces``, with the sticky overflow watch ``self.nl_watch``.  ``DeviceMD`` and
+    ``relax.DeviceLBFGS`` build their steps around it."""
+
+    energy_key = P.energy
+    force_key = P.forces
+    virial: Optional[Tensor] = None
+    required_properties: List[str] = []
+
+    # ---- one force evaluation on the current positions (calculator.calculate) ---------------------------------------------
+    def _calculate(self):
+        ops._GRAPH_CACHE.clear()
+        x = {k: (v.detach() if v.is_floating_point() else v) for k, v in self.static.items()}
+        if self.virial is not None:
+            x[P.virial] = self.virial
+        x = self.nl(x)
+        out = self.model(x)
+        e, f = out[self.energy_key].detach(), out[self.force_key].detach()
+        if self.energy is None:
+            self.energy, self.forces, self.n_pairs = e.clone(), f.clone(), x["_n_pairs"].clone()
+        else:
+            self.energy.copy_(e)
+            self.forces.copy_(f)
+            self.n_pairs.copy_(x["_n_pairs"])
+        torch.maximum(self.nl_watch, x["_n_pairs"], out=self.nl_watch)
+        if self.required_properties:
+            self._refresh_properties(out)
+
+    def _capture_step(self, state: List[Tensor]) -> "torch.cuda.CUDAGraph":
+        """Capture ``self._step()`` into a CUDA graph.  Capture works on copies of ``state`` (every tensor the step writes)
+        so that the warm-up iteration does not advance the run."""
+        dev = self.static[P.R].device
+        saved = [t.clone() for t in state]
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with self._chain_ws:
+            with torch.cuda.stream(side):
+                self._step()
+            torch.cuda.current_stream(dev).wait_stream(side)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                self._step()
+        for dst, src in zip(state, saved):
+            dst.copy_(src)
+        return graph
+
+    def check_neighbor_list(self):
+        """One host read per ``run``: raise if ANY step since the start overflowed the list capacity (the search then
+        dropped pairs and the trajectory is wrong from that step on).  ``peak_pairs`` tells how much head-room is left."""
+        peak, over = (int(v) for v in self.nl_watch.tolist())
+        self.peak_pairs = peak
+        if over:
+            name = type(self).__name__
+            raise RuntimeError(
+                f"{name}: the neighbour list overflowed its capacity of {self.nl.capacity} pairs during the run (peak "
+                f"{peak}); the trajectory is invalid from that step on -- re-create {name} with a larger capacity")
+
+
+class DeviceMD(_CapturedEvaluation):
     def __init__(self, model: torch.nn.Module, batch: Dict[str, Tensor], masses: Tensor, time_step: float, cutoff: float,
                  capacity: int, momenta: Optional[Tensor] = None, use_graph: bool = True,
                  position_conversion: float = 1.0, energy_conversion: float = 1.0,
@@ -1109,25 +1169,6 @@ class DeviceMD:
         self._n_records = 0
         return out
 
-    # ---- one force evaluation on the current positions (calculator.calculate) ---------------------------------------------
-    def _calculate(self):
-        ops._GRAPH_CACHE.clear()
-        x = {k: (v.detach() if v.is_floating_point() else v) for k, v in self.static.items()}
-        if self.virial is not None:
-            x[P.virial] = self.virial
-        x = self.nl(x)
-        out = self.model(x)
-        e, f = out["energy"].detach(), out["forces"].detach()
-        if self.energy is None:
-            self.energy, self.forces, self.n_pairs = e.clone(), f.clone(), x["_n_pairs"].clone()
-        else:
-            self.energy.copy_(e)
-            self.forces.copy_(f)
-            self.n_pairs.copy_(x["_n_pairs"])
-        torch.maximum(self.nl_watch, x["_n_pairs"], out=self.nl_watch)
-        if self.required_properties:
-            self._refresh_properties(out)
-
     def _verlet(self, drift: bool):
         n = self.positions.shape[0]
         mp = self.model_positions if self.model_positions is not self.positions else None
@@ -1203,8 +1244,6 @@ class DeviceMD:
             self.thermostat.apply(self.momenta)   # simulator.py:149-150 on_step_end
 
     def _capture(self):
-        dev = self.positions.device
-        # capture works on copies of the state so that warm-up iterations do not advance the trajectory
         state = [self.positions, self.momenta, self.forces, self.energy]
         if self.model_positions is not self.positions:
             state.append(self.model_positions)
@@ -1217,19 +1256,7 @@ class DeviceMD:
         state.extend(self.properties.values())
         if self.record_capacity:
             state.extend([self._rec_counter] + list(self._records.values()))
-        saved = [t.clone() for t in state]
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with self._chain_ws:
-            with torch.cuda.stream(side):
-                self._step()
-            torch.cuda.current_stream(dev).wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                self._step()
-        for dst, src in zip(state, saved):
-            dst.copy_(src)
-        self._graph = graph
+        self._graph = self._capture_step(state)
 
     def run(self, n_steps: int):
         """Advance ``n_steps`` velocity-Verlet steps; returns (energy, forces) buffers of the last step (device).  With a
@@ -1253,16 +1280,6 @@ class DeviceMD:
         self.steps_done += int(n_steps)
         self.check_neighbor_list()
         return self.energy, self.forces
-
-    def check_neighbor_list(self):
-        """One host read per ``run``: raise if ANY step since the start overflowed the list capacity (the search then
-        dropped pairs and the trajectory is wrong from that step on).  ``peak_pairs`` tells how much head-room is left."""
-        peak, over = (int(v) for v in self.nl_watch.tolist())
-        self.peak_pairs = peak
-        if over:
-            raise RuntimeError(
-                f"DeviceMD: the neighbour list overflowed its capacity of {self.nl.capacity} pairs during the run (peak "
-                f"{peak}); the trajectory is invalid from that step on -- re-create DeviceMD with a larger capacity")
 
     def kinetic_energy(self) -> Tensor:
         return 0.5 * (self.momenta ** 2 / self.masses[:, None]).sum()

@@ -1,0 +1,279 @@
+"""Batchwise structure relaxation on the device: the L-BFGS of the reference's ``ASEBatchwiseLBFGS``
+(interfaces/batchwise_optimization.py:613-917) with one optimizer per system of a collated batch, its state and history
+in fp64 on the device, and the whole step -- optimizer, neighbour list, energy + forces, convergence test -- captured
+once as a CUDA graph (DESIGN.md section 12).
+
+The reference copies positions and forces to the host on every step and runs the two-loop recursion in numpy.  Here the
+step is two kinds of kernels of ``csrc/relax.cu``: ``spk_relax_step`` (history update, two-loop recursion, masking of
+converged systems, step capping, position update) and ``spk_relax_converged`` (per-system largest force and the count of
+unconverged systems), and ``DeviceLBFGS.run`` reads that count once per ``check_every`` steps.
+
+Systems may differ in size (the reference needs equal atom counts).  The fp64 recursion departs on purpose from the
+reference, whose float32 forces keep ``q`` and ``z`` in float32 through numpy's in-place updates.
+"""
+from __future__ import annotations
+
+import ctypes
+from typing import Dict, Optional
+
+import torch
+
+from . import _lib, ops
+from . import properties as P
+from .md import _CapturedEvaluation
+from .neighbors import CellListNeighborList
+
+__all__ = ["DeviceLBFGS", "LBFGSState"]
+
+Tensor = torch.Tensor
+DEFAULT_MAX_STEPS = 100_000_000          # ASE's Dynamics default, which the reference's run loop inherits
+
+
+def _fixed_mask(fixed_atoms_mask, n_atoms: int, dev) -> Optional[Tensor]:
+    """uint8 [N] from a boolean mask of length N or a list of atom indices (both index ``f[mask] = 0`` in the
+    reference's get_forces)"""
+    if fixed_atoms_mask is None:
+        return None
+    m = torch.as_tensor(fixed_atoms_mask).reshape(-1).cpu()
+    if m.dtype == torch.bool:
+        if m.numel() != n_atoms:
+            raise ValueError(f"fixed_atoms_mask: a boolean mask needs {n_atoms} entries, got {m.numel()}")
+        out = m
+    else:
+        idx = m.to(torch.int64)
+        if idx.numel() and (int(idx.min()) < -n_atoms or int(idx.max()) >= n_atoms):
+            raise ValueError(f"fixed_atoms_mask: atom index out of range for {n_atoms} atoms")
+        out = torch.zeros(n_atoms, dtype=torch.bool)
+        out[idx] = True
+    return out.to(torch.uint8).to(dev)
+
+
+class LBFGSState:
+    """Optimizer state of a batch and the launches of its kernels (the step and the convergence test), given a forces
+    tensor.  ``positions`` [N, 3] are the starting positions in optimizer units (model positions x
+    ``position_conversion``); forces are model forces, multiplied by ``force_conversion`` in the kernels.  Systems are
+    the ``idx_m`` segments.  ``check(forces)`` must run on the forces of the current positions before every ``step``
+    with the same forces.  ``model_positions`` (fp32 [N, 3], allocated if not given) receives r / position_conversion
+    at every step."""
+
+    def __init__(self, positions: Tensor, idx_m: Tensor, n_sys: int, memory: int = 100, maxstep: float = 0.2,
+                 damping: float = 1.0, alpha: float = 70.0, fixed_atoms_mask=None, position_conversion: float = 1.0,
+                 force_conversion: float = 1.0, model_positions: Optional[Tensor] = None, fmax: float = 0.05):
+        dev = positions.device
+        if dev.type != "cuda":
+            raise ValueError("LBFGSState needs CUDA tensors (no CPU fallback)")
+        if not 1 <= int(memory) <= _lib.RELAX_MAX_MEMORY:
+            raise ValueError(f"LBFGSState: memory must be in [1, {_lib.RELAX_MAX_MEMORY}], got {memory}")
+        n, n_sys = int(positions.shape[0]), int(n_sys)
+        if n_sys < 1:
+            raise ValueError("LBFGSState: the batch has no system")
+        f64 = dict(dtype=torch.float64, device=dev)
+        self.n_atoms, self.n_sys, self.memory = n, n_sys, int(memory)
+        self.r = positions.detach().to(**f64).reshape(n, 3).contiguous().clone()
+        self.r0 = torch.zeros_like(self.r)
+        self.f0 = torch.zeros_like(self.r)
+        self.s = torch.zeros(self.memory, n, 3, **f64)
+        self.y = torch.zeros_like(self.s)
+        self.rho = torch.ones(self.memory, n_sys, **f64)
+        self.p = torch.zeros_like(self.r)
+        self.counter = torch.zeros(2, dtype=torch.int64, device=dev)
+        self.fmax_target = torch.full((1,), float(fmax), **f64)
+        self.fmax = torch.zeros(n_sys, **f64)
+        self.converged = torch.zeros(n_sys, dtype=torch.int32, device=dev)
+        self.steps_to_converge = torch.full((n_sys,), -1, dtype=torch.int64, device=dev)
+        self.n_unconverged = torch.full((1,), n_sys, dtype=torch.int32, device=dev)
+        self.fixed = _fixed_mask(fixed_atoms_mask, n, dev)
+        p_conv = float(position_conversion)
+        if model_positions is None:
+            model_positions = (self.r / p_conv).float()
+        self.model_positions = ops.f32(model_positions, "model_positions")
+        self.idx_m = idx_m.to(dev, torch.int64).contiguous()
+        self.sys_ptr = ops.segment_ptr(self.idx_m, n_sys)
+        # size path of every system (one host read, here only): warp systems first, then the cluster systems
+        sizes = (self.sys_ptr[1:] - self.sys_ptr[:-1]).cpu()
+        small = sizes <= _lib.RELAX_WARP_ATOMS
+        self.n_warp = int(small.sum())
+        ids = torch.arange(n_sys)
+        self.order = torch.cat([ids[small], ids[~small]]).to(dev, torch.int32)
+        p = ops._p
+        self._params = _lib.LBFGSState(
+            p(self.r), p(self.r0), p(self.f0), p(self.s), p(self.y), p(self.rho), p(self.p), p(self.counter),
+            p(self.fmax_target), p(self.fmax), p(self.converged), p(self.steps_to_converge), p(self.n_unconverged),
+            p(self.fixed), p(self.model_positions), p(self.sys_ptr), p(self.order), n, n_sys, self.n_warp,
+            self.memory, float(force_conversion), p_conv, float(maxstep), float(damping), 1.0 / float(alpha))
+
+    def _forces(self, forces: Tensor) -> Tensor:
+        f = ops.f32(forces, "forces")
+        if f.numel() != 3 * self.n_atoms:
+            raise ValueError(f"LBFGSState: forces of {f.numel()} values for {self.n_atoms} atoms")
+        return f
+
+    def check(self, forces: Tensor):
+        """the convergence test of the forces at the current positions (fmax, converged, steps_to_converge and the
+        unconverged count, on the device)"""
+        _lib.call("spk_relax_converged", ctypes.byref(self._params), ops._p(self._forces(forces)), ops._stream())
+
+    def step(self, forces: Tensor):
+        """one L-BFGS step with the forces at the current positions"""
+        _lib.call("spk_relax_step", ctypes.byref(self._params), ops._p(self._forces(forces)), ops._stream(),
+                  launches=int(self.n_warp > 0) + int(self.n_warp < self.n_sys))
+
+    def set_fmax(self, fmax: float):
+        self.fmax_target.fill_(float(fmax))
+
+    def tensors(self) -> Dict[str, Tensor]:
+        """every buffer the step writes"""
+        return {"r": self.r, "r0": self.r0, "f0": self.f0, "s": self.s, "y": self.y, "rho": self.rho, "p": self.p,
+                "counter": self.counter, "fmax_target": self.fmax_target, "fmax": self.fmax,
+                "converged": self.converged, "steps_to_converge": self.steps_to_converge,
+                "n_unconverged": self.n_unconverged, "model_positions": self.model_positions}
+
+    def state_dict(self) -> Dict[str, Tensor]:
+        return {k: v.clone() for k, v in self.tensors().items()}
+
+    def load_state_dict(self, state: Dict[str, Tensor]):
+        for k, v in self.tensors().items():
+            v.copy_(state[k])
+
+
+class DeviceLBFGS(_CapturedEvaluation):
+    """Relax every system of ``batch`` with the reference's batchwise L-BFGS (keywords and defaults of
+    ASEBatchwiseLBFGS; ``alpha`` gives H0 = 1 / alpha).  ``batch[_positions]`` is in model units;
+    ``position_conversion`` and ``energy_conversion`` turn model lengths and energies into the optimizer's units (Angstrom
+    and eV in the reference), so ``maxstep`` and ``fmax`` are in those.  ``fixed_atoms_mask`` (boolean mask or atom
+    indices) zeroes the forces of atoms that must not move.  ``cutoff`` and ``capacity`` size the device neighbour list,
+    which is rebuilt at every step.
+
+    One step is the optimizer kernels, the neighbour list, the model and the convergence test, captured once as a CUDA
+    graph (``use_graph``).  ``run`` replays it in chunks of ``check_every`` steps and reads the count of unconverged
+    systems once per chunk; steps replayed after every system has converged leave the positions bitwise unchanged."""
+
+    def __init__(self, model: torch.nn.Module, batch: Dict[str, Tensor], cutoff: float, capacity: int,
+                 maxstep: float = 0.2, memory: int = 100, damping: float = 1.0, alpha: float = 70.0,
+                 fixed_atoms_mask=None, position_conversion: float = 1.0, energy_conversion: float = 1.0,
+                 energy_key: str = P.energy, force_key: str = P.forces, use_graph: bool = True):
+        dev = batch[P.R].device
+        if dev.type != "cuda":
+            raise ValueError("DeviceLBFGS needs a CUDA batch (no CPU fallback)")
+        if float(maxstep) > 1.0:                                                 # batchwise_optimization.py:711-715
+            raise ValueError("You are using a much too large value for the maximum step size: %.1f Angstrom"
+                             % float(maxstep))
+        outputs = getattr(model, "model_outputs", None)
+        if outputs is not None and (force_key not in outputs or energy_key not in outputs):
+            raise ValueError(f"DeviceLBFGS: the model must output '{energy_key}' and '{force_key}' (it outputs "
+                             f"{sorted(outputs)})")
+        self.model = model
+        self.energy_key, self.force_key = energy_key, force_key
+        self.p_conv = float(position_conversion)
+        self.e_conv = float(energy_conversion)
+        self.f_conv = self.e_conv / self.p_conv
+        self.static = {k: v.detach().clone() for k, v in batch.items() if k not in (P.idx_i, P.idx_j, P.offsets)}
+        mp = self.static[P.R]
+        if mp.dtype != torch.float32 or not mp.is_contiguous():
+            raise ValueError("DeviceLBFGS: '_positions' must be a contiguous float32 tensor")
+        n = mp.shape[0]
+        idx_m = self.static.get(P.idx_m)
+        if idx_m is None:
+            idx_m = torch.zeros(n, dtype=torch.int64, device=dev)
+        n_sys = self.static[P.n_atoms].shape[0] if P.n_atoms in self.static else 1
+        self.nl = CellListNeighborList(cutoff, capacity=int(capacity), pad=True)
+        self.use_graph = use_graph
+        self.energy: Optional[Tensor] = None
+        self.forces: Optional[Tensor] = None
+        self.n_pairs: Optional[Tensor] = None
+        # [0] = largest pair count seen, [1] = 1 if any evaluation overflowed ``capacity``
+        self.nl_watch = torch.zeros(2, dtype=torch.int64, device=dev)
+        self._graph = None
+        self._chain_ws = ops.ChainWorkspace()
+        self.opt = LBFGSState(mp.double() * self.p_conv, idx_m, n_sys, memory=memory, maxstep=maxstep,
+                              damping=damping, alpha=alpha, fixed_atoms_mask=fixed_atoms_mask,
+                              position_conversion=self.p_conv, force_conversion=self.f_conv, model_positions=mp)
+        self.iterations = 0                      # steps taken (host mirror of the device counter)
+        self.nsteps = 0
+        self._calculate()                        # forces of the starting positions (irun, :417)
+        self.opt.check(self.forces)
+
+    def _step(self):
+        self.opt.step(self.forces)
+        self._calculate()
+        self.opt.check(self.forces)
+
+    def _state_tensors(self):
+        return list(self.opt.tensors().values()) + [self.energy, self.forces, self.n_pairs, self.nl_watch]
+
+    def run(self, fmax: float = 0.05, steps: Optional[int] = None, check_every: int = 10) -> bool:
+        """Relax until every system's largest force is below ``fmax`` or ``steps`` steps (default: unlimited) were taken
+        in this call; returns whether every system converged.  ``nsteps`` is then the step count at which the reference's
+        loop would have stopped."""
+        if int(check_every) < 1:
+            raise ValueError("DeviceLBFGS: check_every must be >= 1")
+        budget = DEFAULT_MAX_STEPS if not steps else int(steps)
+        self.opt.set_fmax(fmax)
+        self.opt.check(self.forces)              # the convergence test under this fmax
+        if self.use_graph and self._graph is None:
+            self._graph = self._capture_step(self._state_tensors())
+        done = 0
+        left = int(self.opt.n_unconverged.item())
+        while left and done < budget:
+            k = min(int(check_every), budget - done)
+            for _ in range(k):
+                if self.use_graph:
+                    self._graph.replay()
+                else:
+                    self._step()
+            done += k
+            self.iterations += k
+            left = int(self.opt.n_unconverged.item())
+        self.check_neighbor_list()
+        self.nsteps = int(self.opt.steps_to_converge.max().item()) if left == 0 else self.iterations
+        return left == 0
+
+    # ---- results ------------------------------------------------------------------------------------------------------
+    @property
+    def positions(self) -> Tensor:
+        """[N, 3] fp64 positions in optimizer units (Angstrom in the reference)"""
+        return self.opt.r
+
+    @property
+    def model_positions(self) -> Tensor:
+        """[N, 3] fp32 positions the model reads (positions / position_conversion)"""
+        return self.static[P.R]
+
+    def get_energy(self) -> Tensor:
+        """energies of the current positions [n_sys] in optimizer units"""
+        return self.energy * self.e_conv
+
+    def get_forces(self) -> Tensor:
+        """forces of the current positions [N, 3] fp64 in optimizer units, zero on fixed atoms (get_forces, :182-198)"""
+        f = self.forces.double() * self.f_conv
+        if self.opt.fixed is not None:
+            f = f * (1 - self.opt.fixed.double())[:, None]
+        return f
+
+    @property
+    def fmax(self) -> Tensor:
+        """largest force per system [n_sys] fp64 (the quantity the convergence test compares with ``fmax``)"""
+        return self.opt.fmax
+
+    @property
+    def converged(self) -> Tensor:
+        return self.opt.converged.bool()
+
+    @property
+    def steps_to_converge(self) -> Tensor:
+        """[n_sys] the step count at which each system met the criterion (-1 while it has not)"""
+        return self.opt.steps_to_converge
+
+    def state_dict(self) -> Dict[str, object]:
+        """Everything a restart needs to continue bitwise (it replaces the reference's pickle restart file)."""
+        return {"opt": self.opt.state_dict(), "energy": self.energy.clone(), "forces": self.forces.clone(),
+                "n_pairs": self.n_pairs.clone(), "nl_watch": self.nl_watch.clone(), "iterations": self.iterations,
+                "nsteps": self.nsteps}
+
+    def load_state_dict(self, state: Dict[str, object]):
+        """Copy a ``state_dict`` into the existing buffers (a captured graph stays valid)."""
+        self.opt.load_state_dict(state["opt"])
+        for k in ("energy", "forces", "n_pairs", "nl_watch"):
+            getattr(self, k).copy_(state[k])
+        self.iterations = int(state["iterations"])
+        self.nsteps = int(state["nsteps"])
