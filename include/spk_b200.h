@@ -135,17 +135,6 @@ int spk_dense_tc(const float* A, int64_t M, int K, int64_t lda, const float* a_p
                  int N, const float* bias, int act, const float* addend, int64_t ld_add, float* Y, int64_t ldy,
                  float* y_pre, spk_stream_t stream);
 
-/* Two Dense layers as ONE launch (csrc/mlp2_tc.cu): H = act(A W0^T + b0) [M,128] stays in shared memory as the tensor-core
- * operand of Y = H W1^T + b1 [+ addend] [M,N2]; h_deriv (or NULL) receives act'(pre) of the hidden layer [M,128] (what
- * spk_dense_tc returns with SPK_SAVE_DERIV) for the reverse pass.  Replaces nn.Sequential(Dense(K1, 128, activation),
- * Dense(128, N2)) of /root/reference/src/schnetpack/representation/painn.py:39-44, 84-91 (PaiNN's context networks).
- * W0_packed / W1_packed = the 128-column-tile section of spk_tc_pack_weight's output (offset
- * spk_tc_packed_floats_tn(N, K, 64) floats) for W0 [128,K1] and W1 [N2,128].  Requirements: hidden width 128, N2 % 128 == 0,
- * K1 % 4 == 0, leading dimensions % 4 == 0, 16 B-aligned pointers; otherwise SPK_ERR_UNSUPPORTED (run two spk_dense_tc). */
-int spk_mlp2_tc(const float* A, int64_t M, int K1, int64_t lda, const float* W0_packed, const float* b0, int act,
-                const float* W1_packed, int N2, const float* b1, const float* addend, int64_t ld_add, float* Y, int64_t ldy,
-                float* h_deriv, spk_stream_t stream);
-
 /* ---------------------------------------------------------------------------------------------------------------
  * PaiNN.  representation/painn.py:31-67 (PaiNNInteraction.forward) and :92-117 (PaiNNMixing.forward).
  * ------------------------------------------------------------------------------------------------------------- */
@@ -169,11 +158,12 @@ int spk_painn_edge_bwd(const float* x, const float* mu, const float* g_q, const 
                        int64_t n_atoms, int64_t n_edges, int F, int n_rbf, float* g_x, float* g_mu_in, float* g_rij,
                        int accumulate, spk_stream_t stream);
 /* Tensor-core variant of spk_painn_edge_fwd (csrc/painn_tc.cu): the filter W = fc * (phi . w^T + b) of a chunk of edges is
- * one 3xTF32 tcgen05 GEMM per filter third with the channels on the TMEM lanes, so the gather/accumulate threads read their
- * channel's filter values with tcgen05.ld instead of recomputing them from warp-broadcast shared-memory loads (the
- * streaming kernel is bound by the load/store unit).  wf_packed = spk_painn_pack_filter(wf, bf) (hi/lo operand tiles,
- * spk_painn_filter_packed_floats() floats).  Same results as spk_painn_edge_fwd to fp32 rounding.  Returns
- * SPK_ERR_UNSUPPORTED unless F == 128, n_rbf <= 31 and n_edges > 0 (the caller then uses spk_painn_edge_fwd). */
+ * computed by a producer warpgroup with 3xTF32 wgmma (channels on the M side) and handed to the gather/accumulate warps as
+ * a filter tile in shared memory, so they read their channel's filter values instead of recomputing them from
+ * warp-broadcast shared-memory loads (the streaming kernel is bound by the load/store unit).
+ * wf_packed = spk_painn_pack_filter(wf, bf) (hi/lo operand tiles, spk_painn_filter_packed_floats() floats).  Same results
+ * as spk_painn_edge_fwd to fp32 rounding.  Returns SPK_ERR_UNSUPPORTED unless F == 128, n_rbf <= 31 and n_edges > 0
+ * (the caller then uses spk_painn_edge_fwd). */
 size_t spk_painn_filter_packed_floats(void);
 int spk_painn_pack_filter(const float* wf, const float* bf, int F, int n_rbf, float* packed, spk_stream_t stream);
 int spk_painn_edge_fwd_tc(const float* x, const float* mu, const float* q, const float* phi, const float* geo,
@@ -211,47 +201,6 @@ int spk_painn_mix_update_bwd(const float* g_q, const float* g_mu, const float* s
 /* reverse of mix_ctx: g_q_out = g_q + g_ctx[:, :F]; g_VW[:, d, :F] += g_ctx[:, F:] * V_d / n */
 int spk_painn_mix_ctx_bwd(const float* g_ctx, const float* g_q, const float* VW, int64_t n_atoms, int F, float eps,
                           float* g_q_out, float* g_VW, spk_stream_t stream);
-
-/* ---------------------------------------------------------------------------------------------------------------
- * Persistent per-atom stage (csrc/atom_chain.cu): all per-atom work between two edge kernels -- PaiNNMixing
- * (painn.py:103-116) followed by the next block's interatomic_context_net (painn.py:54), or their reverses -- as ONE
- * launch.  The caller describes the stage as up to SPK_CHAIN_MAX_STEPS steps executed in order for every 128-atom tile
- * (step k of a tile starts when step k-1 of the SAME tile is complete; tiles are independent because every step is
- * row-local):
- *   SPK_CHAIN_GEMM   Y[rows, N] = act( (A[rows, K] .* a_pre) * W^T + bias ) + addend over rows_per_atom * n_atoms rows
- *                    (the spk_dense_tc operation; a_pre != NULL multiplies A by the saved act'(pre) = SPK_ACT_GIVEN; with an
- *                    activation, y_pre != NULL receives act'(pre)).  Wp = spk_tc_pack_weight output advanced to the
- *                    128-column tiles: Wp + spk_tc_packed_floats_tn(N, K, 64).  Requires N % 128 == 0, K % 16 == 0.
- *   SPK_CHAIN_MIX_CTX / MIX_UPDATE / MIX_UPDATE_BWD / MIX_CTX_BWD   the elementwise glue of spk_painn_mix_* with operands
- *                    (g0, g1, g2, g3) -> (o0, o1) as listed in csrc/atom_chain.cu.
- * workspace: spk_atom_chain_workspace_ints(n_steps, n_atoms) int32, zero before the FIRST use (the kernel leaves it zero);
- * one workspace per concurrently running stream.
- * ------------------------------------------------------------------------------------------------------------- */
-#define SPK_CHAIN_MAX_STEPS 8
-#define SPK_CHAIN_GEMM 0
-#define SPK_CHAIN_MIX_CTX 1        /* g0 = q [N,F], g1 = VW [N,3,2F]                      -> o0 = ctx [N,2F]                  */
-#define SPK_CHAIN_MIX_UPDATE 2     /* g0 = q, g1 = VW, g2 = mu [N,3,F], g3 = s [N,3F]     -> o0 = q', o1 = mu'               */
-#define SPK_CHAIN_MIX_UPDATE_BWD 3 /* g0 = g_q, g1 = VW, g2 = g_mu, g3 = s               -> o0 = g_s [N,3F], o1 = g_VW      */
-#define SPK_CHAIN_MIX_CTX_BWD 4    /* g0 = g_ctx [N,2F], g1 = VW, g2 = g_q               -> o0 = g_q', o1 = g_VW (V part +=) */
-typedef struct {
-    int32_t kind, rows_per_atom, K, N, act, F;
-    float eps;
-    int32_t reserved;
-    int64_t lda, ldy, ld_add;
-    const float *A, *a_pre, *Wp, *bias, *addend;
-    float *Y, *y_pre;
-    const float *g0, *g1, *g2, *g3;
-    float *o0, *o1;
-} spk_chain_step_t;
-size_t spk_tc_packed_floats_tn(int N, int K, int tile_n); /* floats of the tile_n-wide (64 | 128) packing of W [N,K] */
-size_t spk_atom_chain_workspace_ints(int n_steps, int64_t n_atoms);
-#define SPK_CHAIN_FLAG_NFOLD 1 /* 2 MMAs per k-step: [W_hi ; W_lo] as one 256-row operand (see csrc/atom_chain.cu) */
-int spk_atom_chain(const spk_chain_step_t* steps /* host array */, int n_steps, int64_t n_atoms, int32_t* workspace,
-                   size_t workspace_ints, int flags, spk_stream_t stream);
-/* development aid: the same launch writing 8 int64 stamps per work item (claimed, dependencies satisfied, K-loop done,
- * published in ns of %globaltimer; CTA; step; atom tile; unused) to trace[8 * items] */
-int spk_atom_chain_debug(const spk_chain_step_t* steps, int n_steps, int64_t n_atoms, int32_t* workspace,
-                         size_t workspace_ints, int flags, long long* trace, spk_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * SchNet.  representation/schnet.py:41-70 (SchNetInteraction.forward).

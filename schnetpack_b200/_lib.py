@@ -21,19 +21,6 @@ GEO_STRIDE = 8
 
 P = c_void_p  # device pointers and the stream travel as void*
 
-CHAIN_MAX_STEPS = 8
-CHAIN_GEMM, CHAIN_MIX_CTX, CHAIN_MIX_UPDATE, CHAIN_MIX_UPDATE_BWD, CHAIN_MIX_CTX_BWD = 0, 1, 2, 3, 4
-
-
-class ChainStep(Structure):
-    """spk_chain_step_t of include/spk_b200.h."""
-    _fields_ = [("kind", c_int32), ("rows_per_atom", c_int32), ("K", c_int32), ("N", c_int32), ("act", c_int32),
-                ("F", c_int32), ("eps", c_float), ("reserved", c_int32), ("lda", c_int64), ("ldy", c_int64),
-                ("ld_add", c_int64), ("A", c_void_p), ("a_pre", c_void_p), ("Wp", c_void_p), ("bias", c_void_p),
-                ("addend", c_void_p), ("Y", c_void_p), ("y_pre", c_void_p), ("g0", c_void_p), ("g1", c_void_p),
-                ("g2", c_void_p), ("g3", c_void_p), ("o0", c_void_p), ("o1", c_void_p)]
-
-
 class NHCParams(Structure):
     """spk_nhc_params_t of include/spk_b200.h."""
     _fields_ = [("chain_length", c_int32), ("multi_step", c_int32), ("order", c_int32), ("massive", c_int32),
@@ -86,13 +73,8 @@ SIGNATURES = {
     "spk_segment_sum": [P, P, P, c_int64, c_int, P, P],
     "spk_dense": [P, c_int64, c_int, c_int64, P, c_int, P, c_int, P, c_int, P, c_int64, P, c_int64, P, P],
     "spk_tc_packed_floats": [c_int, c_int],
-    "spk_tc_packed_floats_tn": [c_int, c_int, c_int],
-    "spk_atom_chain_workspace_ints": [c_int, c_int64],
-    "spk_atom_chain": [POINTER(ChainStep), c_int, c_int64, P, c_size_t, c_int, P],
-    "spk_atom_chain_debug": [POINTER(ChainStep), c_int, c_int64, P, c_size_t, c_int, P, P],
     "spk_tc_pack_weight": [P, c_int, c_int, P, P],
     "spk_dense_tc": [P, c_int64, c_int, c_int64, P, c_int, P, c_int, P, c_int, P, c_int64, P, c_int64, P, P],
-    "spk_mlp2_tc": [P, c_int64, c_int, c_int64, P, P, c_int, P, c_int, P, P, c_int64, P, c_int64, P, P],
     "spk_painn_edge_fwd": [P, P, P, P, P, P, P, P, P, c_int64, c_int64, c_int, c_int, P, P, P],
     "spk_painn_edge_bwd": [P, P, P, P, P, P, P, P, P, P, P, P, P, c_int64, c_int64, c_int, c_int, P, P, P, c_int, P],
     "spk_painn_filter_packed_floats": [],
@@ -172,7 +154,6 @@ SIGNATURES = {
 }
 _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_size_t,
             "spk_pairwise_virial_workspace_bytes": c_size_t, "spk_md_barostat_workspace_bytes": c_size_t,
-            "spk_tc_packed_floats_tn": c_size_t, "spk_atom_chain_workspace_ints": c_size_t,
             "spk_schnet_filter_packed_floats": c_size_t,
             "spk_painn_filter_packed_floats": c_size_t, "spk_neighbor_list_workspace_bytes": c_size_t,
             "spk_md_thermostat_workspace_bytes": c_size_t, "spk_rpmd_workspace_bytes": c_size_t,

@@ -354,12 +354,6 @@ static int dispatch_tc(const TcArgs& g, cudaStream_t st) {
                                     : launch_tc<TN, 3, 0>(g, st);
 }
 
-extern "C" size_t spk_tc_packed_floats_tn(int N, int K, int tile_n) {
-    if (tile_n != 64 && tile_n != 128) return 0;
-    if (tile_n == 128 && !has_wide(N)) return 0;
-    return packed_floats_tn(N, K, tile_n);
-}
-
 extern "C" size_t spk_tc_packed_floats(int N, int K) {
     return packed_floats_tn(N, K, 64) + (has_wide(N) ? packed_floats_tn(N, K, 128) : 0);
 }

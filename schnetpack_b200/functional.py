@@ -86,8 +86,6 @@ def _packed_filter(pk: "PaiNNPack", t: int, n_rbf: int, n_edges: int):
 # ---- per-block pipelines (pure functions over detached fp32 CUDA tensors) -------------------------------------------
 def painn_context_fwd(b, q: Tensor, act: int):
     """x = interatomic_context_net(q) [N,3F] (painn.py:54) and the saved act'(pre) of its first layer."""
-    if ops.mlp2_ok(b["c0"], b["c1"], q):
-        return ops.mlp2(q, b["c0"], b["c1"], act)
     a, hpre = b["c0"].fwd(q, act, save_deriv=True)
     return b["c1"].fwd(a), hpre
 
@@ -103,11 +101,8 @@ def painn_mixing_fwd(b, q1: Tensor, mu1: Tensor, F: int, eps: float, act: int):
     N = q1.shape[0]
     VW = b["mix"].fwd(mu1.view(3 * N, F))                                                    # :103  [3N,2F]
     ctx = ops.painn_mix_ctx(q1, VW, F, eps)                                                  # :104-107
-    if ops.mlp2_ok(b["m0"], b["m1"], ctx):
-        s, cpre = ops.mlp2(ctx, b["m0"], b["m1"], act)                                       # :108 as one launch
-    else:
-        c, cpre = b["m0"].fwd(ctx, act, save_deriv=True)                                     # :108
-        s = b["m1"].fwd(c)
+    c, cpre = b["m0"].fwd(ctx, act, save_deriv=True)                                         # :108
+    s = b["m1"].fwd(c)
     q2, mu2 = ops.painn_mix_update(q1, mu1, s, VW, F)                                        # :110-116
     return q2, mu2, (VW, cpre, s)
 
@@ -124,120 +119,9 @@ def painn_mixing_bwd(b, g_q: Tensor, g_mu: Tensor, tape, F: int, eps: float):
     return g_q1, g_mu1
 
 
-# ---- fused per-atom stages (csrc/atom_chain.cu): the same operations as the per-block pipelines above, one launch per stage ----
-def _chain_ok(pk: PaiNNPack) -> bool:
-    if not ops.CHAIN_IMPL or pk.F != 128:
-        return False
-    b = pk.blocks[0]
-    return all(b[k].w_pk is not None and b[k].wt_pk is not None for k in ("c0", "c1", "mix", "m0", "m1"))
-
-
-def _context_steps(b, q: Tensor, act: int, F: int):
-    N, dev = q.shape[0], q.device
-    a = torch.empty((N, F), dtype=torch.float32, device=dev)
-    hpre = torch.empty((N, F), dtype=torch.float32, device=dev)
-    x = torch.empty((N, 3 * F), dtype=torch.float32, device=dev)
-    steps = [ops.chain_gemm(q, b["c0"].fwd_wide(), F, F, a, bias=b["c0"].b, act=act, y_pre=hpre),       # painn.py:54
-             ops.chain_gemm(a, b["c1"].fwd_wide(), 3 * F, F, x, bias=b["c1"].b)]
-    return steps, x, hpre, (a,)
-
-
-def _mixing_steps(b, q1: Tensor, mu1: Tensor, F: int, eps: float, act: int):
-    N, dev = q1.shape[0], q1.device
-    f32 = dict(dtype=torch.float32, device=dev)
-    VW = torch.empty((N, 3, 2 * F), **f32)
-    ctx = torch.empty((N, 2 * F), **f32)
-    c = torch.empty((N, F), **f32)
-    cpre = torch.empty((N, F), **f32)
-    s = torch.empty((N, 3 * F), **f32)
-    q2 = torch.empty((N, F), **f32)
-    mu2 = torch.empty((N, 3, F), **f32)
-    L = _lib_consts()
-    steps = [ops.chain_gemm(mu1, b["mix"].fwd_wide(), 2 * F, F, VW, rows_per_atom=3),                  # :103
-             ops.chain_glue(L.CHAIN_MIX_CTX, F, eps, q1, VW, None, None, ctx, None),                    # :104-107
-             ops.chain_gemm(ctx, b["m0"].fwd_wide(), F, 2 * F, c, bias=b["m0"].b, act=act, y_pre=cpre),  # :108
-             ops.chain_gemm(c, b["m1"].fwd_wide(), 3 * F, F, s, bias=b["m1"].b),
-             ops.chain_glue(L.CHAIN_MIX_UPDATE, F, eps, q1, VW, mu1, s, q2, mu2)]                       # :110-116
-    return steps, q2, mu2, (VW, cpre, s), (ctx, c)
-
-
-def _lib_consts():
-    from . import _lib
-    return _lib
-
-
-def painn_forward_chain(pk: PaiNNPack, q0, r_ij, graph, rbf_kind, n_rbf, rbf_p0, rbf_p1, cutoff, act, need_grad):
-    """painn_forward with the per-atom work of every stage in one persistent launch: context(0) | edge(0) | mixing(0) +
-    context(1) | edge(1) | ... | mixing(T-1)."""
-    F, N, dev = pk.F, q0.shape[0], q0.device
-    phi, dphi, geo = ops.edge_geometry(r_ij, graph, rbf_kind, n_rbf, rbf_p0, rbf_p1, cutoff, need_grad)
-    steps, x, hpre, keep = _context_steps(pk.blocks[0], q0, act, F)
-    ops.atom_chain(steps, N, dev)
-    q, mu = q0, None
-    tape = []
-    for t in range(pk.T):
-        b = pk.blocks[t]
-        q1, mu1 = ops.painn_edge_fwd(x, mu, q, phi, geo, graph, pk.wf[t], pk.bf[t], F, n_rbf,
-                                     wf_packed=_packed_filter(pk, t, n_rbf, graph.n_edges))
-        steps, q2, mu2, mtape, keep = _mixing_steps(b, q1, mu1, F, pk.eps, act)
-        if t + 1 < pk.T:
-            more, x_next, hpre_next, keep2 = _context_steps(pk.blocks[t + 1], q2, act, F)
-            steps += more
-        ops.atom_chain(steps, N, dev)
-        if need_grad:
-            tape.append((hpre, x, mu, mtape))
-        q, mu = q2, mu2
-        if t + 1 < pk.T:
-            x, hpre = x_next, hpre_next
-    return q, mu, (phi, dphi, geo, tape)
-
-
-def painn_backward_chain(pk: PaiNNPack, saved, graph, n_rbf, act, g_q, g_mu, n_edges_total) -> Tensor:
-    """painn_backward with one persistent launch per stage: [context(t+1) reversed + mixing(t) reversed] | edge(t) reversed."""
-    F = pk.F
-    phi, dphi, geo, tape = saved
-    N, dev = g_q.shape[0], g_q.device
-    f32 = dict(dtype=torch.float32, device=dev)
-    L = _lib_consts()
-    g_rij = torch.empty((n_edges_total, 3), **f32)
-    if g_mu is None:
-        g_mu = torch.zeros((N, 3, F), **f32)
-    pre = []                       # reverse of the NEXT block's context net, prepended to this block's mixing reverse
-    for t in reversed(range(pk.T)):
-        b = pk.blocks[t]
-        hpre, x, mu_in, (VW, cpre, s) = tape[t]
-        g_s = torch.empty((N, 3 * F), **f32)
-        g_VW = torch.empty((N, 3, 2 * F), **f32)
-        g_c = torch.empty((N, F), **f32)
-        g_ctx = torch.empty((N, 2 * F), **f32)
-        g_q1 = torch.empty((N, F), **f32)
-        g_mu1 = torch.empty((N, 3, F), **f32)
-        steps = pre + [
-            ops.chain_glue(L.CHAIN_MIX_UPDATE_BWD, F, pk.eps, g_q, VW, g_mu, s, g_s, g_VW),
-            ops.chain_gemm(g_s, b["m1"].bwd_wide(), F, 3 * F, g_c),
-            ops.chain_gemm(g_c, b["m0"].bwd_wide(), 2 * F, F, g_ctx, a_pre=cpre),
-            ops.chain_glue(L.CHAIN_MIX_CTX_BWD, F, pk.eps, g_ctx, VW, g_q, None, g_q1, g_VW),
-            ops.chain_gemm(g_VW, b["mix"].bwd_wide(), F, 2 * F, g_mu1, rows_per_atom=3, addend=g_mu)]
-        ops.atom_chain(steps, N, dev)
-        g_x, g_mu0 = ops.painn_edge_bwd(x, mu_in, g_q1, g_mu1, phi, dphi, geo, graph, pk.wf[t], pk.bf[t], F, n_rbf,
-                                        g_rij, accumulate=(t != pk.T - 1),
-                                        wf_packed=_packed_filter(pk, t, n_rbf, graph.n_edges))
-        if t == 0:
-            break   # dE/dq0 would only reach the (position-independent) embedding
-        g_a = torch.empty((N, F), **f32)
-        g_q_new = torch.empty((N, F), **f32)
-        pre = [ops.chain_gemm(g_x, b["c1"].bwd_wide(), F, 3 * F, g_a),
-               ops.chain_gemm(g_a, b["c0"].bwd_wide(), F, F, g_q_new, a_pre=hpre, addend=g_q1)]
-        keep = (g_x, g_a, g_q1)   # noqa: F841  (alive until the next stage has been enqueued)
-        g_q, g_mu = g_q_new, g_mu0
-    return g_rij
-
-
 def painn_forward(pk: PaiNNPack, q0: Tensor, r_ij: Tensor, graph: ops.EdgeGraph, rbf_kind: int, n_rbf: int,
                   rbf_p0: Tensor, rbf_p1: Optional[Tensor], cutoff: float, act: int, need_grad: bool):
     """Returns q [N,F], mu [N,3,F] and the tape needed by painn_backward."""
-    if _chain_ok(pk):
-        return painn_forward_chain(pk, q0, r_ij, graph, rbf_kind, n_rbf, rbf_p0, rbf_p1, cutoff, act, need_grad)
     F = pk.F
     phi, dphi, geo = ops.edge_geometry(r_ij, graph, rbf_kind, n_rbf, rbf_p0, rbf_p1, cutoff, need_grad)
     q, mu = q0, None
@@ -257,8 +141,6 @@ def painn_forward(pk: PaiNNPack, q0: Tensor, r_ij: Tensor, graph: ops.EdgeGraph,
 def painn_backward(pk: PaiNNPack, saved, graph: ops.EdgeGraph, n_rbf: int, act: int, g_q: Tensor,
                    g_mu: Optional[Tensor], n_edges_total: int) -> Tensor:
     """dE/dr_ij [E,3] (in the caller's edge order) from dE/dq [N,F], dE/dmu [N,3,F]."""
-    if _chain_ok(pk):
-        return painn_backward_chain(pk, saved, graph, n_rbf, act, g_q, g_mu, n_edges_total)
     F = pk.F
     phi, dphi, geo, tape = saved
     N = g_q.shape[0]
@@ -543,36 +425,19 @@ def schnet_forward_fused(pk: SchNetPack, x0: Tensor, r_ij: Tensor, idx_i: Tensor
                          rbf_p0, rbf_p1, cutoff: float, act: int) -> Tensor:
     """Inference forward (no tape) with ONE fused edge kernel per interaction block (filter network on the tensor cores inside it,
     csrc/schnet_tc.cu) over the ACTIVE edges only (d < cutoff: padding slots of a padded neighbour list are dropped when the
-    receiver CSR is built), and the per-atom layers f2out + residual + the next block's in2f as one persistent launch
-    (csrc/atom_chain.cu).  schnet.py:56-70,160-171."""
-    F, N, dev = pk.F, x0.shape[0], x0.device
+    receiver CSR is built).  schnet.py:56-70,160-171."""
+    N = x0.shape[0]
     graph = ops.EdgeGraph(idx_i, idx_j, N, r_ij=r_ij, cutoff=cutoff)
     phi, _, geo = ops.edge_geometry(r_ij, graph, rbf_kind, n_rbf, rbf_p0, rbf_p1, cutoff, False, active_only=True)
-    f32 = dict(dtype=torch.float32, device=dev)
-    use_chain = ops.CHAIN_IMPL and all(b[k].w_pk is not None for b in pk.blocks for k in ("in2f", "o0", "o1"))
     x = x0
     h = pk.blocks[0]["in2f"].fwd(x)                                                          # schnet.py:60
     for t in range(pk.T):
         b = pk.blocks[t]
         m = ops.schnet_cfconv_fwd_tc(h, phi, geo, graph, _schnet_filter_packed(b, n_rbf), b["f1"].b, act, n_rbf)   # :61-67
-        if use_chain:
-            v0 = torch.empty((N, F), **f32)
-            x_new = torch.empty((N, F), **f32)
-            steps = [ops.chain_gemm(m, b["o0"].fwd_wide(), F, pk.NF, v0, bias=b["o0"].b, act=act),      # :69
-                     ops.chain_gemm(v0, b["o1"].fwd_wide(), F, F, x_new, bias=b["o1"].b, addend=x)]     # :69 + :168
-            if t + 1 < pk.T:
-                h_next = torch.empty((N, pk.NF), **f32)
-                steps.append(ops.chain_gemm(x_new, pk.blocks[t + 1]["in2f"].fwd_wide(), pk.NF, F, h_next))
-            ops.atom_chain(steps, N, dev)
-            keep = (m, v0, x)   # noqa: F841
-            x = x_new
-            if t + 1 < pk.T:
-                h = h_next
-        else:
-            v0 = b["o0"].fwd(m, act)
-            x = b["o1"].fwd(v0, addend=x)
-            if t + 1 < pk.T:
-                h = pk.blocks[t + 1]["in2f"].fwd(x)
+        v0 = b["o0"].fwd(m, act)
+        x = b["o1"].fwd(v0, addend=x)
+        if t + 1 < pk.T:
+            h = pk.blocks[t + 1]["in2f"].fwd(x)
     return x
 
 

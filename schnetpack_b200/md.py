@@ -891,13 +891,12 @@ class _CapturedEvaluation:
         saved = [t.clone() for t in state]
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
-        with self._chain_ws:
-            with torch.cuda.stream(side):
-                self._step()
-            torch.cuda.current_stream(dev).wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                self._step()
+        with torch.cuda.stream(side):
+            self._step()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            self._step()
         for dst, src in zip(state, saved):
             dst.copy_(src)
         return graph
@@ -991,7 +990,6 @@ class DeviceMD(_CapturedEvaluation):
         # count seen so far, [1] = 1 if any step overflowed ``capacity`` (its list was then truncated)
         self.nl_watch = torch.zeros(2, dtype=torch.int64, device=dev)
         self._graph = None
-        self._chain_ws = ops.ChainWorkspace()      # dependency counters of the persistent per-atom stages, owned here
         self.steps_done = 0
         self._systems: Optional[_Systems] = None
         self.thermostat = thermostat

@@ -295,9 +295,6 @@ class GraphedPotential:
         self.warmup = warmup
         self._cache = {}
         self._last = None
-        from . import ops
-
-        self._chain_ws = ops.ChainWorkspace()      # dependency counters of the persistent per-atom stages, owned here
 
     @staticmethod
     def _signature(inputs: Dict[str, torch.Tensor]):
@@ -317,14 +314,13 @@ class GraphedPotential:
 
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
-        with self._chain_ws:
-            with torch.cuda.stream(side):
-                for _ in range(self.warmup):
-                    run()
-            torch.cuda.current_stream(dev).wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                out = run()
+        with torch.cuda.stream(side):
+            for _ in range(self.warmup):
+                run()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            out = run()
         static_out = {k: v.detach() for k, v in out.items()}
         return graph, static_in, static_out
 

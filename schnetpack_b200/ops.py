@@ -360,19 +360,6 @@ class Lin:
 
     __slots__ = ("w", "wt", "b", "w_pk", "wt_pk")
 
-    @staticmethod
-    def _wide(pk: Optional[Tensor], n: int, k: int) -> Optional[Tensor]:
-        """the 128-column tiles of a packed weight ([64-wide tiles | 128-wide tiles]); None if it has none"""
-        if pk is None or n % 128:
-            return None
-        return pk[_lib.lib().spk_tc_packed_floats_tn(n, k, 64):]
-
-    def fwd_wide(self):
-        return self._wide(self.w_pk, self.w.shape[0], self.w.shape[1])
-
-    def bwd_wide(self):
-        return self._wide(self.wt_pk, self.wt.shape[0], self.wt.shape[1])
-
     def __init__(self, weight: Tensor, bias: Optional[Tensor] = None):
         self.w = weight.detach().contiguous()
         self.wt = weight.detach().t().contiguous()
@@ -408,110 +395,8 @@ class Lin:
         return dense(G, self.w, None, ACT_NONE, **kw)
 
 
-# Dense -> Dense pairs as one launch with the hidden tile resident in shared memory (csrc/mlp2_tc.cu).  SPK_B200_MLP2=0 runs the
-# two layers as separate spk_dense_tc launches (A/B measurements; also the path for shapes outside the fused kernel's).
-MLP2_IMPL = os.environ.get("SPK_B200_MLP2", "0") != "0"
-
-
-def mlp2_ok(l0: "Lin", l1: "Lin", A: Tensor) -> bool:
-    return (MLP2_IMPL and l0.w_pk is not None and l1.w_pk is not None and l0.w.shape[0] == 128 and l1.w.shape[1] == 128
-            and l1.w.shape[0] % 128 == 0 and A.shape[1] % 4 == 0 and A.shape[1] == l0.w.shape[1])
-
-
-def mlp2(A: Tensor, l0: "Lin", l1: "Lin", act: int, addend: Optional[Tensor] = None):
-    """(act(A W0^T + b0) W1^T + b1 [+ addend], act'(pre) of the hidden layer) in one launch."""
-    f32(A, "A")
-    M, K1 = A.shape
-    N2 = l1.w.shape[0]
-    Y = torch.empty((M, N2), dtype=torch.float32, device=A.device)
-    deriv = torch.empty((M, 128), dtype=torch.float32, device=A.device)
-    _lib.call("spk_mlp2_tc", _p(A), M, K1, K1, _p(l0.fwd_wide()), _p(l0.b), act, _p(l1.fwd_wide()), N2, _p(l1.b),
-              _p(addend), N2, _p(Y), N2, _p(deriv), _stream())
-    return Y, deriv
-
-
-# ------------------------------------------------------------------------------------------------------------ atom chain
-# persistent per-atom stage (csrc/atom_chain.cu): one launch for mixing(t) + context(t+1) (or their reverses) instead of
-# seven.  Opt-in (SPK_B200_CHAIN=1); the default is the launch-per-layer pipeline.
-CHAIN_IMPL = os.environ.get("SPK_B200_CHAIN", "0") != "0"
-CHAIN_NFOLD = os.environ.get("SPK_B200_CHAIN_NFOLD", "0") != "0"    # SPK_CHAIN_FLAG_NFOLD; the sm_90a kernel has one scheme
-CHAIN_TRACE = None          # set to a list to collect (stamps, program) of every stage launch
-_CHAIN_WS: "dict[tuple, Tensor]" = {}
-
-
-def chain_gemm(A: Tensor, w_wide: Tensor, n_out: int, k: int, Y: Tensor, rows_per_atom: int = 1, bias=None, act=ACT_NONE,
-               a_pre=None, addend=None, y_pre=None) -> _lib.ChainStep:
-    st = _lib.ChainStep()
-    st.kind, st.rows_per_atom, st.K, st.N, st.act = _lib.CHAIN_GEMM, rows_per_atom, int(k), int(n_out), int(act)
-    st.lda, st.ldy = int(A.shape[-1]), int(Y.shape[-1])
-    st.ld_add = int(addend.shape[-1]) if addend is not None else 0
-    st.A, st.Wp, st.Y = A.data_ptr(), w_wide.data_ptr(), Y.data_ptr()
-    st.a_pre = a_pre.data_ptr() if a_pre is not None else None
-    st.bias = bias.data_ptr() if bias is not None else None
-    st.addend = addend.data_ptr() if addend is not None else None
-    st.y_pre = y_pre.data_ptr() if y_pre is not None else None
-    return st
-
-
-def chain_glue(kind: int, F: int, eps: float, g0, g1, g2, g3, o0, o1) -> _lib.ChainStep:
-    st = _lib.ChainStep()
-    st.kind, st.F, st.eps = kind, int(F), float(eps)
-    for name, t in (("g0", g0), ("g1", g1), ("g2", g2), ("g3", g3), ("o0", o0), ("o1", o1)):
-        setattr(st, name, t.data_ptr() if t is not None else None)
-    return st
-
-
-class ChainWorkspace:
-    """Dependency-counter workspace owned by a caller that captures evaluations into CUDA graphs (``GraphedPotential``,
-    ``DeviceMD``): allocated OUTSIDE the capture (during the eager warm-up) and alive as long as its owner, so a captured
-    graph never refers to memory of the allocator's per-stream cache or of another graph's private pool."""
-
-    def __init__(self):
-        self.ws: Optional[Tensor] = None
-        self.retired = []          # outgrown workspaces stay alive: graphs captured earlier still write to them
-
-    def __enter__(self):
-        self._prev = _CHAIN_OWNER[0]
-        _CHAIN_OWNER[0] = self
-        return self
-
-    def __exit__(self, *exc):
-        _CHAIN_OWNER[0] = self._prev
-        return False
-
-
-_CHAIN_OWNER = [None]
-
-
-def atom_chain(steps, n_atoms: int, device):
-    """Run a stage program (list of ChainStep) over all 128-atom tiles in ONE persistent launch."""
-    n = len(steps)
-    arr = (_lib.ChainStep * n)(*steps)
-    need = _lib.lib().spk_atom_chain_workspace_ints(n, n_atoms)
-    stream = torch.cuda.current_stream()
-    owner = _CHAIN_OWNER[0]
-    if owner is not None:
-        if owner.ws is None or owner.ws.numel() < need or owner.ws.device != device:
-            if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError("atom_chain: the owner's workspace must be sized by an eager warm-up before graph capture")
-            if owner.ws is not None:
-                owner.retired.append(owner.ws)
-            owner.ws = torch.zeros(max(need, 4096), dtype=torch.int32, device=device)
-        ws = owner.ws
-    else:
-        key = (device.index if device.index is not None else torch.cuda.current_device(), stream.cuda_stream)
-        ws = _CHAIN_WS.get(key)
-        if ws is None or ws.numel() < need:
-            ws = torch.zeros(max(need, 4096), dtype=torch.int32, device=device)   # zero once; the kernel leaves it zero
-            _CHAIN_WS[key] = ws
-    if CHAIN_TRACE is not None:      # development: per-item time stamps of every stage launch (spk_atom_chain_debug)
-        items = sum((s.rows_per_atom * (s.N // 128) if s.kind == _lib.CHAIN_GEMM else 1) for s in steps) * ((n_atoms + 127) // 128)
-        tr = torch.zeros((items, 8), dtype=torch.int64, device=device)
-        CHAIN_TRACE.append((tr, [(s.kind, s.K, s.N, s.rows_per_atom) for s in steps]))
-        _lib.call("spk_atom_chain_debug", arr, n, n_atoms, _p(ws), ws.numel(), 1 if CHAIN_NFOLD else 0, _p(tr),
-                  c_void_p(stream.cuda_stream))
-        return
-    _lib.call("spk_atom_chain", arr, n, n_atoms, _p(ws), ws.numel(), 1 if CHAIN_NFOLD else 0, c_void_p(stream.cuda_stream))
+# bench.py reports this in impl_switches; there is no chain path, so it is always False.
+CHAIN_IMPL = False
 
 
 # ------------------------------------------------------------------------------------------------------------ PaiNN

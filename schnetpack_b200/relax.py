@@ -184,7 +184,6 @@ class DeviceLBFGS(_CapturedEvaluation):
         # [0] = largest pair count seen, [1] = 1 if any evaluation overflowed ``capacity``
         self.nl_watch = torch.zeros(2, dtype=torch.int64, device=dev)
         self._graph = None
-        self._chain_ws = ops.ChainWorkspace()
         self.opt = LBFGSState(mp.double() * self.p_conv, idx_m, n_sys, memory=memory, maxstep=maxstep,
                               damping=damping, alpha=alpha, fixed_atoms_mask=fixed_atoms_mask,
                               position_conversion=self.p_conv, force_conversion=self.f_conv, model_positions=mp)

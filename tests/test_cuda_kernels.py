@@ -197,44 +197,6 @@ def test_dense_tcgen05_3xtf32(M, K, N, lda):
     assert rel(out[:, :N], ref_lin) < 3e-6 and bool((out[:, N:] == -1.0).all())
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("M,K1,N2", [(300, 128, 384), (5376, 128, 384), (1000, 256, 384), (77, 64, 128), (129, 20, 256)])
-def test_mlp2_one_launch_matches_fp64_and_two_launches(M, K1, N2):
-    """Dense(K1,128,act) -> Dense(128,N2) as one wgmma launch with the hidden tile resident in shared memory
-    (csrc/mlp2_tc.cu) against the fp64 restatement and against two spk_dense_tc launches: values, saved act'(pre), addend,
-    ragged last row tile, K1 not a multiple of the 16-float K-tile."""
-    from schnetpack_b200 import ops
-
-    torch.manual_seed(11)
-    A = torch.randn(M, K1, device=DEV)
-    W0 = torch.randn(128, K1, device=DEV) / math.sqrt(K1)
-    b0 = torch.randn(128, device=DEV)
-    W1 = torch.randn(N2, 128, device=DEV) / math.sqrt(128)
-    b1 = torch.randn(N2, device=DEV)
-    add = torch.randn(M, N2, device=DEV)
-    l0, l1 = ops.Lin(W0, b0), ops.Lin(W1, b1)
-    old = ops.MLP2_IMPL
-    ops.MLP2_IMPL = True
-    try:
-        assert ops.mlp2_ok(l0, l1, A)
-        for act, f in ((ops.ACT_SILU, torch.nn.functional.silu), (ops.ACT_NONE, lambda v: v),
-                       (ops.ACT_SSP, lambda v: torch.nn.functional.softplus(v) - math.log(2.0))):
-            pre = (A.double() @ W0.double().t() + b0.double()).requires_grad_()
-            h = f(pre)
-            dact = torch.autograd.grad(h.sum(), pre)[0]
-            ref = h.detach() @ W1.double().t() + b1.double()
-            Y, deriv = ops.mlp2(A, l0, l1, act)
-            assert rel(Y, ref) < 3e-6, rel(Y, ref)
-            assert rel(deriv, dact) < 3e-6, rel(deriv, dact)
-            Y2, _ = ops.mlp2(A, l0, l1, act, addend=add)
-            assert rel(Y2, ref + add.double()) < 3e-6
-            a, d2 = l0.fwd(A, act, save_deriv=True)
-            Y3 = l1.fwd(a)
-            assert rel(Y, Y3.double()) < 2e-6 and rel(deriv, d2.double()) < 2e-6
-    finally:
-        ops.MLP2_IMPL = old
-
-
 def _painn_layer_ref(x, mu, q, r, ii, jj, wf, bf, rc, p0, p1):
     d = r.norm(dim=1, keepdim=True)
     u = r / d
@@ -587,36 +549,6 @@ def test_bad_neighbor_indices_raise_and_never_gather_out_of_bounds():
     Z = torch.tensor([1, 6, 250, -1], device=DEV)
     out = ops.embedding(torch.randn(100, 32, device=DEV), Z)
     assert not bool(torch.isnan(out[:2]).any()) and bool(torch.isnan(out[2:]).all())
-
-
-@pytest.mark.parametrize("nfold", [False, True])
-@pytest.mark.parametrize("batch", [1, 7, 40])
-def test_atom_chain_matches_per_layer_pipeline(batch, nfold):
-    """Persistent per-atom stage (csrc/atom_chain.cu: mixing + next context net, and their reverses, as one launch with
-    tile-level dependency counters) == the launch-per-layer pipeline of the same kernels, for atom counts below one tile
-    (21), with a partial last tile (147) and several tiles (840); energies / forces also against the fp64 oracle.  Repeated
-    calls reuse the self-resetting dependency workspace."""
-    from oracle import spk_oracle as O
-    from schnetpack_b200 import ops
-    from schnetpack_b200 import synthetic as S
-    from schnetpack_b200.model import batch_to_device, from_spec
-
-    spec, data = S.make_config("cfg2", batch=batch)
-    params = S.init_params(spec, seed=17)
-    model = from_spec(spec, params, DEV)
-    old = ops.CHAIN_IMPL, ops.CHAIN_NFOLD
-    try:
-        ops.CHAIN_IMPL = False
-        ref = model(batch_to_device(data, DEV))
-        ops.CHAIN_IMPL, ops.CHAIN_NFOLD = True, nfold          # both accumulation schemes of the 3xTF32 K-tiles
-        for _ in range(3):
-            out = model(batch_to_device(data, DEV))
-        torch.cuda.synchronize()
-    finally:
-        ops.CHAIN_IMPL, ops.CHAIN_NFOLD = old
-    assert rel(out["energy"], ref["energy"]) < 2e-6 and rel(out["forces"], ref["forces"]) < 2e-6
-    o = O.energy_forces(spec, params, data, dtype=torch.float64)
-    assert rel(out["energy"].cpu(), o["energy"]) < 1e-5 and rel(out["forces"].cpu(), o["forces"]) < 1e-5
 
 
 @pytest.mark.parametrize("case", ["qm9", "qm9_padded", "box", "bessel18"])
