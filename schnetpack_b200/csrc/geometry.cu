@@ -306,8 +306,8 @@ extern "C" int spk_pairwise_bwd(const float* g_rij, const int32_t* rowptr, const
 extern "C" int spk_edge_geometry(const float* r_ij, const int32_t* slot_eid, int64_t n_edges, int rbf_kind, int n_rbf,
                                  const float* rbf_p0, const float* rbf_p1, float cutoff, const int32_t* n_active,
                                  float* phi, float* dphi, float* geo, spk_stream_t stream) {
+    // any n_rbf: the edge kernels that consume phi check their own limits (SO3net's convolution takes n_rbf > 32)
     if (n_edges < 0 || n_rbf <= 0) return SPK_ERR_ARG;
-    if (n_rbf > 32) return SPK_ERR_UNSUPPORTED;
     if (rbf_kind != SPK_RBF_GAUSSIAN && rbf_kind != SPK_RBF_BESSEL) return SPK_ERR_ARG;
     if (n_edges == 0) return SPK_OK;
     if (!r_ij || !rbf_p0 || !phi || !geo) return SPK_ERR_ARG;

@@ -214,7 +214,8 @@ extern "C" int spk_cfconv_bwd(const float* h, const float* w_raw, const float* g
 extern "C" int spk_radial_bwd(const float* g_phi, const float* g_fc, const float* dphi, const float* geo,
                               const int32_t* slot_eid, int64_t n_edges, int n_rbf, float* g_rij, int accumulate,
                               spk_stream_t stream) {
-    if (n_edges < 0 || n_rbf <= 0 || n_rbf > 32) return SPK_ERR_ARG;
+    if (n_edges < 0 || n_rbf <= 0) return SPK_ERR_ARG;
+    if (n_rbf > 32) return SPK_ERR_UNSUPPORTED;
     if (n_edges == 0) return SPK_OK;
     if (!geo || !g_rij || (g_phi && !dphi)) return SPK_ERR_ARG;
     spk_launch(k_radial_bwd, GRID1D(n_edges, 256), g_phi, g_fc, dphi, geo, slot_eid, n_edges, n_rbf, spk_kp(n_rbf), g_rij,

@@ -7,6 +7,8 @@ import numpy as np
 import pytest
 import torch
 
+from edge_oracle import _check_graph, _painn_layer_ref
+
 pytestmark = pytest.mark.gpu
 
 DEV = "cuda:0"
@@ -23,29 +25,6 @@ def _graph_inputs(seed=0, batch=6):
 
     b = S.aspirin_batch(batch, seed=seed)
     return b, torch.as_tensor(b["_idx_i"], device=DEV), torch.as_tensor(b["_idx_j"], device=DEV), b["_atomic_numbers"].shape[0]
-
-
-def _check_graph(g, ii, jj, n):
-    ii = np.asarray(ii)
-    jj = np.asarray(jj)
-    E = ii.shape[0]
-    rowptr = g.rowptr.cpu().numpy()
-    sptr = g.sptr.cpu().numpy()
-    slot_j = g.slot_j.cpu().numpy()[:E]
-    slot_eid = g.slot_eid.cpu().numpy()[:E]
-    pos_slot = g.pos_slot.cpu().numpy()[:E]
-    pos_i = g.pos_i.cpu().numpy()[:E]
-    # CSR: stable grouping by receiver
-    order = np.argsort(ii, kind="stable")
-    np.testing.assert_array_equal(rowptr, np.concatenate([[0], np.cumsum(np.bincount(ii, minlength=n))]))
-    np.testing.assert_array_equal(slot_eid, order)
-    np.testing.assert_array_equal(slot_j, jj[order])
-    # sender grouping: stable by slot
-    sj = jj[order]
-    order2 = np.argsort(sj, kind="stable")
-    np.testing.assert_array_equal(sptr, np.concatenate([[0], np.cumsum(np.bincount(jj, minlength=n))]))
-    np.testing.assert_array_equal(pos_slot, order2)
-    np.testing.assert_array_equal(pos_i, ii[order][order2])
 
 
 def test_graph_build_sorted_and_unsorted_bit_exact():
@@ -195,22 +174,6 @@ def test_dense_tcgen05_3xtf32(M, K, N, lda):
     out = torch.full((M, N + 4), -1.0, device=DEV)
     ops.dense_tc(Afull, wp, N, bias, k=K, out=out)
     assert rel(out[:, :N], ref_lin) < 3e-6 and bool((out[:, N:] == -1.0).all())
-
-
-def _painn_layer_ref(x, mu, q, r, ii, jj, wf, bf, rc, p0, p1):
-    d = r.norm(dim=1, keepdim=True)
-    u = r / d
-    phi = torch.exp(-0.5 / p1 ** 2 * (d - p0) ** 2)
-    fc = 0.5 * (torch.cos(d * math.pi / rc) + 1) * (d < rc)
-    W = (phi @ wf.t() + bf) * fc
-    F = q.shape[1]
-    y = W * x[jj]
-    dq, dmuR, dmumu = y.split(F, dim=-1)
-    N = q.shape[0]
-    qo = q + torch.zeros_like(q).index_add(0, ii, dq)
-    dmu = dmuR[:, None, :] * u[:, :, None] + dmumu[:, None, :] * mu[jj]
-    muo = mu + torch.zeros_like(mu).index_add(0, ii, dmu)
-    return qo, muo
 
 
 @pytest.mark.parametrize("F,n_rbf,has_mu", [(128, 20, True), (128, 20, False), (64, 16, True), (256, 32, True)])
