@@ -227,9 +227,8 @@ extern "C" int spk_radial_bwd(const float* g_phi, const float* g_fc, const float
 extern "C" int spk_atomwise_out(const float* hid, const float* w1, const float* b1, const int32_t* mol_ptr,
                                 int64_t n_atoms, int64_t n_mol, int H, float* y, float* energy, spk_stream_t stream) {
     if (n_atoms < 0 || n_mol < 0 || H <= 0) return SPK_ERR_ARG;
-    if (!y) return SPK_ERR_ARG;
     if (n_atoms > 0) {
-        if (!hid || !w1) return SPK_ERR_ARG;
+        if (!hid || !w1 || !y) return SPK_ERR_ARG;
         spk_launch(k_atom_dot, GRID1D(n_atoms * 32, 256), hid, w1, b1, n_atoms, H, y);
     }
     if (energy && n_mol > 0) {

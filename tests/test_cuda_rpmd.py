@@ -23,11 +23,11 @@ def _np(t):
     return t.detach().cpu().numpy()
 
 
-def _mixed_batch(P, seed=3):
-    """a 1-atom system, small molecules and one 20 000-atom system, with bead positions and momenta near 300 K.  Positions
-    stay near the origin: the fp32 state resolves them to ~1e-8 there, which the stiff high modes (omega_k m up to 4e4)
-    turn into momentum errors"""
-    n_atoms = [1, 3, 9, 20_000, 20, 1, 5]
+def _mixed_batch(P, seed=3, n_atoms=(1, 3, 9, 20_000, 20, 1, 5)):
+    """by default a 1-atom system, small molecules and one 20 000-atom system, with bead positions and momenta near 300 K.
+    Positions stay near the origin: the fp32 state resolves them to ~1e-8 there, which the stiff high modes (omega_k m up
+    to 4e4) turn into momentum errors"""
+    n_atoms = [int(n) for n in n_atoms]
     rng = np.random.default_rng(seed + P)
     n = sum(n_atoms)
     masses = rng.choice([1.0, 12.0, 16.0], size=n).astype(np.float32)

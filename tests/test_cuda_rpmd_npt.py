@@ -27,10 +27,10 @@ def _np(t):
 
 
 # ---- 1. kernels against the oracle ----------------------------------------------------------------------------------------
-def _mixed_batch(P, seed=3):
-    """a 1-atom system next to a 20 000-atom one and small molecules, with bead state near 300 K, forces, cells (one
-    triclinic) and virials of every bead system"""
-    n_atoms = [1, 20_000, 3, 9]
+def _mixed_batch(P, seed=3, n_atoms=(1, 20_000, 3, 9)):
+    """by default a 1-atom system next to a 20 000-atom one and small molecules, with bead state near 300 K, forces, cells
+    (the third one triclinic) and virials of every bead system"""
+    n_atoms = [int(n) for n in n_atoms]
     B = len(n_atoms)
     rng = np.random.default_rng(seed + P)
     n = sum(n_atoms)
@@ -62,7 +62,12 @@ def test_barostat_kernels_follow_the_oracle(P):
     """two rounds of cell PILE, half step (p_c only: the particle kick is spk_md_velocity_verlet) and main step; each round
     starts the oracle from the device's state, so p_c and the cells are held to 1e-9 and the fp32 bead state to its
     rounding.  All P bead copies of a cell stay bitwise equal and the model cell is the MD cell * position_conversion."""
-    n_atoms, masses, x, p, f, cells, virial = _mixed_batch(P)
+    barostat_follows_the_oracle(P, _mixed_batch(P))
+
+
+def barostat_follows_the_oracle(P, batch):
+    """the checks of test_barostat_kernels_follow_the_oracle on ``batch`` (as _mixed_batch returns it)"""
+    n_atoms, masses, x, p, f, cells, virial = batch
     B = len(n_atoms)
     base, rp, baro = _bind(P, n_atoms, masses)
     f_conv, v_scale, p_conv = 0.5, 0.25, 10.0
