@@ -34,17 +34,12 @@ __global__ void __launch_bounds__(KT) k_ke7_partials(const float* __restrict__ p
                                                      const int64_t* __restrict__ idx_m, const int32_t* __restrict__ sys_ptr,
                                                      int64_t n_atoms, double* __restrict__ sys_part,
                                                      double* __restrict__ head) {
-    __shared__ double sv[NK][KT];
-    __shared__ int sf[KT];
     SPK_PDL_ENTER();
-    const int t = threadIdx.x;
-    const int64_t b0 = (int64_t)blockIdx.x * KT;
-    const int64_t a = b0 + t;
+    const int64_t a = (int64_t)blockIdx.x * KT + threadIdx.x;
     double v[NK];
 #pragma unroll
     for (int c = 0; c < NK; ++c) v[c] = 0.0;
-    int f = 1;
-    int64_t s = -1;
+    int64_t s = 0, first = 0, end = 0;
     if (a < n_atoms) {
         const double px = p[3 * a], py = p[3 * a + 1], pz = p[3 * a + 2], ma = (double)m[a];
         v[0] = (px * px + py * py + pz * pz) / ma;             // system.py:383-385
@@ -55,15 +50,10 @@ __global__ void __launch_bounds__(KT) k_ke7_partials(const float* __restrict__ p
         v[5] = px * pz / ma;
         v[6] = py * pz / ma;
         s = idx_m[a];
-        f = (t == 0) || (idx_m[a - 1] != s);
+        first = sys_ptr[s];
+        end = sys_ptr[s + 1];
     }
-    seg_scan<KT, NK>(v, f, sv, sf);
-    if (a >= n_atoms) return;
-    const bool seg_end = (t == KT - 1) || (a == n_atoms - 1) || (idx_m[a + 1] != s);
-    if (!seg_end) return;
-    double* dst = sys_ptr[s] >= b0 ? sys_part + s * NK : head + (int64_t)blockIdx.x * NK;
-#pragma unroll
-    for (int c = 0; c < NK; ++c) dst[c] = v[c];
+    seg_partials<KT, NK>(v, n_atoms, s, first, end, sys_part, head);
 }
 
 // 2 KE (= sum |p|^2/m) and 2 K (= sum p p^T / m, row-major 3x3) of system s

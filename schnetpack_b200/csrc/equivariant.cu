@@ -12,8 +12,8 @@
 // read coalesced), the H -> 2 layer (warp per atom), the gate; then the atoms' contributions
 //     dipole          [q, q R, R, mu_atomic]          (10 fp64)
 //     polarizability  [alpha, nu (x) R]               (10 fp64)
-// go through a segmented scan over warp 0 (the addition tree of segscan.cuh's seg_scan, by shuffles), and k_head_finish
-// adds each system's CTA partials in a fixed order (bitwise reproducible, no atomics).  With q' = q + c_m, c_m = (Q_m - sum_m q) / n_m the dipole is
+// go through the partial pass of segscan.cuh (seg_partials, which scans a tile of 8 atoms over warp 0 by shuffles), and
+// k_head_finish adds each system's CTA partials in a fixed order (bitwise reproducible, no atomics).  With q' = q + c_m, c_m = (Q_m - sum_m q) / n_m the dipole is
 //     mu_m = sum q R + c_m sum R + sum mu_atomic,      alpha_m = sum alpha I + S + S^T,  S = sum nu (x) R.
 // The reverse kernel recomputes the tail per atom and writes dE/ds, dE/dV and dE/dR directly.
 #include "segscan.cuh"
@@ -192,58 +192,6 @@ __device__ __forceinline__ void tail_eval(const float* __restrict__ s, const flo
     __syncthreads();
 }
 
-// Inclusive segmented scan (Hillis-Steele) of NV fp64 values over the 32 lanes of warp 0 by shuffles: the same addition
-// tree as seg_scan for a tile of at most 32 items, without shared memory or block barriers.
-template <int NV>
-__device__ __forceinline__ void seg_scan_warp(double (&v)[NV], int f) {
-    const int lane = threadIdx.x & 31;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        const int fu = __shfl_up_sync(0xffffffffu, f, d);
-        double up[NV];
-#pragma unroll
-        for (int c = 0; c < NV; ++c) up[c] = __shfl_up_sync(0xffffffffu, v[c], d);
-        if (lane >= d) {
-            if (!f) {
-#pragma unroll
-                for (int c = 0; c < NV; ++c) v[c] += up[c];
-            }
-            f |= fu;
-        }
-    }
-}
-
-// One CTA-tile of atoms [b0, b0 + tile) contributes v (thread t = atom b0 + t, t < tile) to the segmented sums of its system;
-// leaves one partial per (system, CTA) in sys_part (the CTA the system starts in) or head (later CTAs), as geometry.cu's
-// virial does.  WARP: tile <= 32 and only warp 0 takes part (the other warps return).
-template <bool WARP>
-__device__ __forceinline__ void seg_partials(double (&v)[HT_NV], int64_t b0, int tile, int64_t n_atoms,
-                                             const int64_t* __restrict__ idx_m, const int32_t* __restrict__ sys_ptr,
-                                             double* __restrict__ sys_part, double* __restrict__ head,
-                                             double (*sv)[HT_THREADS], int* sf) {
-    const int t = threadIdx.x;
-    const int64_t a = b0 + t;
-    const bool item = t < tile && a < n_atoms;
-    int64_t m = 0;
-    int f = 1;
-    if (item) {
-        m = idx_m[a];
-        f = (t == 0) || (a == sys_ptr[m]);
-    }
-    if (WARP) {
-        if (threadIdx.x >= 32) return;
-        seg_scan_warp<HT_NV>(v, f);
-    } else {
-        seg_scan<HT_THREADS, HT_NV>(v, f, sv, sf);
-    }
-    if (!item) return;
-    const bool seg_end = (t == tile - 1) || (a == n_atoms - 1) || (a + 1 == sys_ptr[m + 1]);
-    if (!seg_end) return;
-    double* dst = sys_ptr[m] >= b0 ? sys_part + m * HT_NV : head + (int64_t)blockIdx.x * HT_NV;
-#pragma unroll
-    for (int c = 0; c < HT_NV; ++c) dst[c] = v[c];
-}
-
 __device__ __forceinline__ void atom_terms(int mode, float q, const float* nu, const float* R, double (&v)[HT_NV]) {
     const double rx = R[0], ry = R[1], rz = R[2];
     v[0] = q;
@@ -287,12 +235,16 @@ __global__ void __launch_bounds__(HT_THREADS) k_head_tail(const float* __restric
     double v[HT_NV];
 #pragma unroll
     for (int c = 0; c < HT_NV; ++c) v[c] = 0.0;
+    int64_t m = 0, first = 0, end = 0;
     if (t < HT_TILE && a < n_atoms) {
         atom_terms(MODE, res[t][0], &res[t][1], R + 3 * a, v);
         if (q_atom) q_atom[a] = res[t][0];
+        m = idx_m[a];
+        first = sys_ptr[m];
+        end = sys_ptr[m + 1];
     }
     if (threadIdx.x >= 32) return;
-    seg_partials<true>(v, b0, HT_TILE, n_atoms, idx_m, sys_ptr, sys_part, head, nullptr, nullptr);
+    seg_partials<HT_TILE, HT_NV>(v, n_atoms, m, first, end, sys_part, head);
 }
 
 // charges from the scalar MLP (use_vector_representation=False): the same assembly without atomic dipoles
@@ -302,19 +254,20 @@ __global__ void __launch_bounds__(HT_THREADS) k_head_scalar(const float* __restr
                                                             const int64_t* __restrict__ idx_m,
                                                             const int32_t* __restrict__ sys_ptr, int64_t n_atoms,
                                                             double* __restrict__ sys_part, double* __restrict__ head) {
-    __shared__ double sv[HT_NV][HT_THREADS];
-    __shared__ int sf[HT_THREADS];
     SPK_PDL_ENTER();
-    const int64_t b0 = (int64_t)blockIdx.x * HS_TILE;
-    const int64_t a = b0 + threadIdx.x;
+    const int64_t a = (int64_t)blockIdx.x * HS_TILE + threadIdx.x;
     double v[HT_NV];
 #pragma unroll
     for (int c = 0; c < HT_NV; ++c) v[c] = 0.0;
+    int64_t m = 0, first = 0, end = 0;
     if (a < n_atoms) {
         const float zero[3] = {0.f, 0.f, 0.f};
         atom_terms(HEAD_DIPOLE, q[a], zero, R + 3 * a, v);
+        m = idx_m[a];
+        first = sys_ptr[m];
+        end = sys_ptr[m + 1];
     }
-    seg_partials<false>(v, b0, HS_TILE, n_atoms, idx_m, sys_ptr, sys_part, head, sv, sf);
+    seg_partials<HS_TILE, HT_NV>(v, n_atoms, m, first, end, sys_part, head);
 }
 
 // Per system: the totals, the outputs and what the reverse needs (saved[m] = c, R_mean, y, n).

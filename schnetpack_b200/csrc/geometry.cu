@@ -202,9 +202,9 @@ __global__ void k_velocity_verlet(float* __restrict__ momenta, float* __restrict
 
 // Per-system virial W_m[b][a] = sum_{e in m} g_e[b] r_e[a] (the strain derivative of atomistic/response.py:78-90 without the
 // 1/V).  The edges of system m are the receiver slots [rowptr[sys_ptr[m]], rowptr[sys_ptr[m+1]]); CTAs take VIR_T
-// consecutive slots, reduce them with a fixed-shape segmented scan in fp64 and leave one partial per (system, CTA) pair, which
-// k_seg_finish adds in a fixed order -- the scheme of the kinetic-energy sums in thermostat.cu, so the result is bitwise the
-// same on every call for any mix of system sizes.  Padding pairs (distance 2 cutoff) have g_e = 0 and add nothing.
+// consecutive slots and the two passes of segscan.cuh sum them in fp64 (seg_partials, then k_seg_finish), so the result is
+// bitwise the same on every call for any mix of system sizes.  Padding pairs (distance 2 cutoff) have g_e = 0 and add
+// nothing.
 constexpr int VIR_T = 256;
 
 __device__ __forceinline__ int64_t slot_of_sys(const int* __restrict__ rowptr, const int* __restrict__ sys_ptr, int64_t m) {
@@ -215,16 +215,11 @@ __global__ void __launch_bounds__(VIR_T) k_virial_partials(const float* __restri
                                                            const int* __restrict__ rowptr, const int* __restrict__ slot_eid,
                                                            const int* __restrict__ sys_ptr, int64_t n_sys,
                                                            double* __restrict__ sys_part, double* __restrict__ head) {
-    __shared__ double sv[9][VIR_T];
-    __shared__ int sf[VIR_T];
     SPK_PDL_ENTER();
-    const int t = threadIdx.x;
-    const int64_t b0 = (int64_t)blockIdx.x * VIR_T;
-    const int64_t s = b0 + t;
+    const int64_t s = (int64_t)blockIdx.x * VIR_T + threadIdx.x;
     const int64_t n_slots = slot_of_sys(rowptr, sys_ptr, n_sys);
     double v[9];
-    int f = 1;
-    int64_t m = -1;
+    int64_t m = 0, first = 0, end = 0;
 #pragma unroll
     for (int c = 0; c < 9; ++c) v[c] = 0.0;
     if (s < n_slots) {
@@ -241,15 +236,10 @@ __global__ void __launch_bounds__(VIR_T) k_virial_partials(const float* __restri
         v[0] = gx * rx; v[1] = gx * ry; v[2] = gx * rz;
         v[3] = gy * rx; v[4] = gy * ry; v[5] = gy * rz;
         v[6] = gz * rx; v[7] = gz * ry; v[8] = gz * rz;
-        f = (t == 0) || (s == slot_of_sys(rowptr, sys_ptr, m));
+        first = slot_of_sys(rowptr, sys_ptr, m);
+        end = slot_of_sys(rowptr, sys_ptr, m + 1);
     }
-    seg_scan<VIR_T, 9>(v, f, sv, sf);
-    if (s >= n_slots) return;
-    const bool seg_end = (t == VIR_T - 1) || (s == n_slots - 1) || (s + 1 == slot_of_sys(rowptr, sys_ptr, m + 1));
-    if (!seg_end) return;
-    double* dst = slot_of_sys(rowptr, sys_ptr, m) >= b0 ? sys_part + m * 9 : head + (int64_t)blockIdx.x * 9;
-#pragma unroll
-    for (int c = 0; c < 9; ++c) dst[c] = v[c];
+    seg_partials<VIR_T, 9>(v, n_slots, m, first, end, sys_part, head);
 }
 
 // Per-step model properties of DeviceMD (md/calculators/base_calculator.py:113-141): dst = src * conversion, and the

@@ -1,6 +1,7 @@
 // Device code shared by the thermostat (thermostat.cu), barostat (barostat.cu) and ring-polymer (rpmd.cu) kernels of the
-// device MD step: the Nose-Hoover chain propagator, the momentum scalings, the Philox4x32-10 generator with Box-Muller, the
-// reference's sinh(x)/x series, the cell volume and a 3x3 symmetric Jacobi eigensolver.
+// device MD step: the Nose-Hoover chain propagator, the momentum scalings, the Philox4x32-10 generator with its
+// application-counter ticket and Box-Muller, the reference's sinh(x)/x series, the cell volume and a 3x3 symmetric Jacobi
+// eigensolver.
 #pragma once
 #include "segscan.cuh"
 
@@ -78,6 +79,21 @@ __device__ __forceinline__ uint4 philox_draw(uint64_t seed, uint64_t app, int64_
     const uint64_t e = (uint64_t)elem;
     return philox4x32_10(make_uint4((uint32_t)e, (uint32_t)(e >> 32), (uint32_t)app, (uint32_t)(app >> 32)),
                          make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
+}
+
+// The application-counter ticket of the noise kernels: counter[0] is the application index every CTA reads at entry,
+// counter[1] a ticket, zero between launches.  The CTA that finishes last advances the index, so each replay of a captured
+// step draws fresh noise.  Every thread of the CTA calls it after its last use of app.
+__device__ __forceinline__ void advance_counter(unsigned long long* counter, unsigned long long app) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        if (atomicAdd(counter + 1, 1ull) == gridDim.x - 1) {
+            counter[0] = app + 1;
+            counter[1] = 0;
+            __threadfence();
+        }
+    }
 }
 
 // u in (0, 1): (x + 1/2) 2^-32; z0 = sqrt(-2 ln u0) cos(2 pi u1), z1 = ... sin(2 pi u1)

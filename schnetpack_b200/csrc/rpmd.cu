@@ -146,19 +146,6 @@ __device__ __forceinline__ double gle_step(const RpmdArgs& A, uint64_t app, int 
     return acc[0];
 }
 
-// advance the application index once every CTA of the launch has read it (ticket pattern of k_langevin)
-__device__ __forceinline__ void advance_counter(unsigned long long* counter, unsigned long long app) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        if (atomicAdd(counter + 1, 1ull) == gridDim.x - 1) {
-            counter[0] = app + 1;
-            counter[1] = 0;
-            __threadfence();
-        }
-    }
-}
-
 // beads -> normal modes, the per-mode operator OP, normal modes -> beads, for RP_T degrees of freedom per CTA
 template <int OP>
 __global__ void __launch_bounds__(RP_THREADS) k_rpmd_modes(const __grid_constant__ RpmdArgs A) {
@@ -310,17 +297,12 @@ __global__ void __launch_bounds__(RP_THREADS) k_rpmd_transform(const float* in, 
 __global__ void __launch_bounds__(RP_KT) k_rpmd_centroid_partials(const __grid_constant__ RpmdArgs A, int with_noise,
                                                                   double* __restrict__ sys_part,
                                                                   double* __restrict__ head) {
-    __shared__ double sv[RP_NV][RP_KT];
-    __shared__ int sf[RP_KT];
     SPK_PDL_ENTER();
     const unsigned long long app = with_noise ? *(volatile unsigned long long*)A.counter : 0ull;
-    const int t = threadIdx.x;
-    const int64_t b0 = (int64_t)blockIdx.x * RP_KT;
-    const int64_t a = b0 + t;
+    const int64_t a = (int64_t)blockIdx.x * RP_KT + threadIdx.x;
     const int64_t n_dof = 3 * A.n_atoms;
     double v[RP_NV] = {0.0, 0.0};
-    int f = 1;
-    int64_t s = -1;
+    int64_t s = 0, first = 0, end = 0;
     if (a < A.n_atoms) {
         const double ma = (double)A.m[a];
         for (int d = 0; d < 3; ++d) {
@@ -334,15 +316,10 @@ __global__ void __launch_bounds__(RP_KT) k_rpmd_centroid_partials(const __grid_c
             v[1] = z01.x * z01.x + z01.y * z01.y + z23.x * z23.x;                        // :174-176
         }
         s = A.idx_m[a];
-        f = (t == 0) || (A.idx_m[a - 1] != s);
+        first = A.sys_ptr[s];
+        end = A.sys_ptr[s + 1];
     }
-    seg_scan<RP_KT, RP_NV>(v, f, sv, sf);
-    if (a >= A.n_atoms) return;
-    const bool seg_end = (t == RP_KT - 1) || (a == A.n_atoms - 1) || (A.idx_m[a + 1] != s);
-    if (!seg_end) return;
-    double* dst = A.sys_ptr[s] >= b0 ? sys_part + s * RP_NV : head + (int64_t)blockIdx.x * RP_NV;
-    dst[0] = v[0];
-    dst[1] = v[1];
+    seg_partials<RP_KT, RP_NV>(v, A.n_atoms, s, first, end, sys_part, head);
 }
 
 // ---- PILE barostat (barostats_rpmd.py) -----------------------------------------------------------------------------------
@@ -379,7 +356,7 @@ static inline BaroWorkspace carve_baro(void* ws, int64_t n_sys) {
 }
 
 // _update_barostat (barostats_rpmd.py:101-110): p_c = c1 p_c + c2[s] xi, one thread per system; xi is normal 0 of the
-// Philox draw (seed; counter = system, application), and the application index advances by the ticket of k_langevin
+// Philox draw (seed; counter = system, application), and the application index advances by advance_counter
 __global__ void k_rpmd_baro_pile(double* __restrict__ pc, int64_t n_sys, double c1, const double* __restrict__ c2,
                                  uint64_t seed, unsigned long long* counter) {
     SPK_PDL_ENTER();
@@ -389,31 +366,18 @@ __global__ void k_rpmd_baro_pile(double* __restrict__ pc, int64_t n_sys, double 
         const uint4 r = philox_draw(seed, app, s);
         pc[s] = c1 * pc[s] + c2[s] * box_muller(r.x, r.y).x;
     }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        if (atomicAdd(counter + 1, 1ull) == gridDim.x - 1) {
-            counter[0] = app + 1;
-            counter[1] = 0;
-            __threadfence();
-        }
-    }
+    advance_counter(counter, app);
 }
 
 // propagate_half_step (barostats_rpmd.py:173-199), per-(system, CTA) partials over the base atoms: mode 0 of the forces
 // (MD units) and momenta, one row of C across the P beads, and the bead mean of the momenta
 __global__ void __launch_bounds__(RP_KT) k_rpmd_baro_partials(const __grid_constant__ BaroArgs B,
                                                               double* __restrict__ sys_part, double* __restrict__ head) {
-    __shared__ double sv[RB_NV][RP_KT];
-    __shared__ int sf[RP_KT];
     SPK_PDL_ENTER();
-    const int t = threadIdx.x;
-    const int64_t b0 = (int64_t)blockIdx.x * RP_KT;
-    const int64_t a = b0 + t;
+    const int64_t a = (int64_t)blockIdx.x * RP_KT + threadIdx.x;
     const int64_t n_dof = 3 * B.n_atoms;
     double v[RB_NV] = {0.0, 0.0, 0.0};
-    int f = 1;
-    int64_t s = -1;
+    int64_t s = 0, first = 0, end = 0;
     if (a < B.n_atoms) {
         const double ma = (double)B.m[a];
         double pm2 = 0.0;
@@ -434,14 +398,10 @@ __global__ void __launch_bounds__(RP_KT) k_rpmd_baro_partials(const __grid_const
         }
         v[2] = pm2 / ma;
         s = B.idx_m[a];
-        f = (t == 0) || (B.idx_m[a - 1] != s);
+        first = B.sys_ptr[s];
+        end = B.sys_ptr[s + 1];
     }
-    seg_scan<RP_KT, RB_NV>(v, f, sv, sf);
-    if (a >= B.n_atoms) return;
-    const bool seg_end = (t == RP_KT - 1) || (a == B.n_atoms - 1) || (B.idx_m[a + 1] != s);
-    if (!seg_end) return;
-    double* dst = B.sys_ptr[s] >= b0 ? sys_part + s * RB_NV : head + (int64_t)blockIdx.x * RB_NV;
-    for (int c = 0; c < RB_NV; ++c) dst[c] = v[c];
+    seg_partials<RP_KT, RB_NV>(v, B.n_atoms, s, first, end, sys_part, head);
 }
 
 // one CTA per system: the ordered total of the partials, then (thread 0) the centroid pressure from the bead means of the

@@ -1,6 +1,8 @@
-// Fixed-shape segmented reduction for deterministic per-system fp64 sums without atomics (used by the per-system virial in
-// geometry.cu and the kinetic-energy sums of barostat.cu): CTAs of T consecutive items scan their items segment by segment
-// and leave one partial per (system, CTA) pair; a per-system pass adds a system's partials in CTA order.
+// Fixed-shape segmented reduction for deterministic per-system fp64 sums without atomics, used by every per-system sum of
+// the library: the kinetic energies of thermostat.cu, the kinetic-energy sums of barostat.cu, the centroid and barostat
+// sums of rpmd.cu, the virial of geometry.cu and the dipole / polarizability assembly of equivariant.cu.  CTAs of T
+// consecutive items scan their items segment by segment and leave one partial per (system, CTA) pair (seg_partials); a
+// per-system pass adds a system's partials in CTA order (seg_finish_block, k_seg_finish).
 #pragma once
 #include "common.cuh"
 
@@ -34,6 +36,56 @@ __device__ __forceinline__ void seg_scan(double (&v)[NV], int f, double (*sv)[T]
         sf[t] = f = nf;
         __syncthreads();
     }
+}
+
+// The same scan over the 32 lanes of warp 0 by shuffles: the addition tree of seg_scan for T <= 32 items, without shared
+// memory or block barriers.
+template <int NV>
+__device__ __forceinline__ void seg_scan_warp(double (&v)[NV], int f) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const int fu = __shfl_up_sync(0xffffffffu, f, d);
+        double up[NV];
+#pragma unroll
+        for (int c = 0; c < NV; ++c) up[c] = __shfl_up_sync(0xffffffffu, v[c], d);
+        if (lane >= d) {
+            if (!f) {
+#pragma unroll
+                for (int c = 0; c < NV; ++c) v[c] += up[c];
+            }
+            f |= fu;
+        }
+    }
+}
+
+// The partial pass for the CTA of items [b0, b0 + T), b0 = blockIdx.x * T.  Thread t holds the NV terms v of item
+// i = b0 + t (zeros if i >= n_items) and, for a valid item, its system m with items [first, end).  Each segment's total is
+// the (system, CTA) partial: it goes to sys_part + m * NV if the system starts in this CTA, else to head + blockIdx.x * NV
+// (only a CTA's first segment can continue a system).  Every thread of the CTA calls it (blockDim.x == T), or for T <= 32
+// the 32 threads of warp 0 only.
+template <int T, int NV>
+__device__ __forceinline__ void seg_partials(double (&v)[NV], int64_t n_items, int64_t m, int64_t first, int64_t end,
+                                             double* __restrict__ sys_part, double* __restrict__ head) {
+    const int t = threadIdx.x;
+    const int64_t b0 = (int64_t)blockIdx.x * T;
+    const int64_t i = b0 + t;
+    const bool item = t < T && i < n_items;
+    const int f = !item || t == 0 || i == first;
+    // the segment's last item writes its total; both are decided before the scan, so that m, first and end are not live
+    // across it
+    const bool last = item && (t == T - 1 || i == n_items - 1 || i + 1 == end);
+    double* dst = first >= b0 ? sys_part + m * NV : head + (int64_t)blockIdx.x * NV;
+    if constexpr (T <= 32) {
+        seg_scan_warp<NV>(v, f);
+    } else {
+        __shared__ double sv[NV][T];
+        __shared__ int sf[T];
+        seg_scan<T, NV>(v, f, sv, sf);
+    }
+    if (!last) return;
+#pragma unroll
+    for (int c = 0; c < NV; ++c) dst[c] = v[c];
 }
 
 // Per-system totals of NV-wide CTA partials, one CTA of SEG_FIN_T threads per system: the system's partials -- item 0 is

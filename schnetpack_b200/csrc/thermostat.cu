@@ -2,12 +2,10 @@
 // Berendsen rescaling, Nose-Hoover-chain propagation (per system or massive) and the Langevin kick with a counter-based
 // Philox4x32-10 generator.  Every entry point only enqueues work, so a whole NVT step can be captured into one CUDA graph.
 //
-// Per-system sums are deterministic: the atoms are cut into CTAs of KE_T consecutive atoms; a CTA reduces its atoms with a
-// segmented scan of fixed shape and writes one fp64 partial per (system, CTA) pair -- into sys_part[s] for the CTA in which
-// system s starts, into head[b] for a CTA b that a system entered before b (only the first segment of a CTA can be such a
-// continuation).  The per-system pass then adds a system's partials in CTA order.  No atomics touch a sum, so the result is
-// bitwise the same on every call, whatever the size mix of the batch (one 262 144-atom box spans 1024 CTAs, a 1-atom system
-// one).
+// Per-system sums are deterministic: the atoms are cut into CTAs of KE_T consecutive atoms, and the partial pass of
+// segscan.cuh leaves one fp64 partial per (system, CTA) pair.  k_thermo_system then adds a system's partials in CTA order,
+// one thread per system.  No atomics touch a sum, so the result is bitwise the same on every call, whatever the size mix of
+// the batch (one 262 144-atom box spans 1024 CTAs, a 1-atom system one).
 #include "md_common.cuh"
 
 namespace {
@@ -34,45 +32,18 @@ __global__ void __launch_bounds__(KE_T) k_ke_partials(const float* __restrict__ 
                                                       const int64_t* __restrict__ idx_m,
                                                       const int32_t* __restrict__ sys_ptr, int64_t n_atoms,
                                                       double* __restrict__ sys_part, double* __restrict__ head) {
-    __shared__ double sv[KE_T];
-    __shared__ int sf[KE_T];
     SPK_PDL_ENTER();
-    const int t = threadIdx.x;
-    const int64_t b0 = (int64_t)blockIdx.x * KE_T;
-    const int64_t a = b0 + t;
-    double v = 0.0;
-    int f = 1;  // segment head
-    int64_t s = -1;
+    const int64_t a = (int64_t)blockIdx.x * KE_T + threadIdx.x;
+    double v[1] = {0.0};
+    int64_t s = 0, first = 0, end = 0;
     if (a < n_atoms) {
         const double px = p[3 * a], py = p[3 * a + 1], pz = p[3 * a + 2];
-        v = (px * px + py * py + pz * pz) / (double)m[a];
+        v[0] = (px * px + py * py + pz * pz) / (double)m[a];
         s = idx_m[a];
-        f = (t == 0) || (idx_m[a - 1] != s);
+        first = sys_ptr[s];
+        end = sys_ptr[s + 1];
     }
-    // inclusive segmented scan (Hillis-Steele): the addition tree depends only on the segment layout
-    sv[t] = v;
-    sf[t] = f;
-    __syncthreads();
-#pragma unroll
-    for (int d = 1; d < KE_T; d <<= 1) {
-        double nv = v;
-        int nf = f;
-        if (t >= d) {
-            if (!f) nv = sv[t - d] + v;
-            nf = f | sf[t - d];
-        }
-        __syncthreads();
-        sv[t] = nv;
-        sf[t] = nf;
-        v = nv;
-        f = nf;
-        __syncthreads();
-    }
-    if (a >= n_atoms) return;
-    const bool seg_end = (t == KE_T - 1) || (a == n_atoms - 1) || (idx_m[a + 1] != s);
-    if (!seg_end) return;
-    if (sys_ptr[s] >= b0) sys_part[s] = v;   // the system starts in this CTA
-    else head[blockIdx.x] = v;               // continuation of a system begun in an earlier CTA
+    seg_partials<KE_T, 1>(v, n_atoms, s, first, end, sys_part, head);
 }
 
 // sum_{a in s} p_a^2 / m_a in CTA order (0 for an empty system)
@@ -115,8 +86,7 @@ __global__ void k_thermo_system(const int32_t* __restrict__ sys_ptr, int64_t n_s
 }
 
 // thermostats.py:244-261: p = c1 p + sqrt(m kB T) c2 xi, one thread per atom (xi = the first three normals of its draw).
-// counter[0] is the application index: read by every CTA, advanced by the CTA that finishes last (counter[1] is its
-// ticket, zero between calls), so each replay of a captured step draws fresh noise.
+// counter: the application index and its ticket (advance_counter).
 __global__ void k_langevin(float* __restrict__ p, const float* __restrict__ m, int64_t n_atoms, double c1, double c2,
                            double kbt, uint64_t seed, unsigned long long* counter) {
     SPK_PDL_ENTER();
@@ -130,15 +100,7 @@ __global__ void k_langevin(float* __restrict__ p, const float* __restrict__ m, i
         p[3 * a + 1] = (float)(c1 * (double)p[3 * a + 1] + fac * z01.y);
         p[3 * a + 2] = (float)(c1 * (double)p[3 * a + 2] + fac * z23.x);
     }
-    __syncthreads();   // every thread of this CTA has consumed `app`
-    if (threadIdx.x == 0) {
-        __threadfence();
-        if (atomicAdd(counter + 1, 1ull) == gridDim.x - 1) {
-            counter[0] = app + 1;
-            counter[1] = 0;
-            __threadfence();
-        }
-    }
+    advance_counter(counter, app);
 }
 
 __global__ void k_philox_bits(uint64_t seed, const unsigned long long* __restrict__ counter, int64_t n,
