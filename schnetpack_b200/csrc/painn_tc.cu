@@ -9,8 +9,9 @@
 //   * orientation: channels on the M side.  For each filter third t the A operand is W_t = [w | b] (128 channels x 32,
 //     static, packed once by spk_painn_pack_filter in the shared-memory operand layout and fetched by ONE TMA bulk copy),
 //     the B operand is a chunk of NR = 32 operand rows  Phi' = fc * [phi | 1]  (K-major, 64 B swizzle, hi/lo split of 3xTF32);
-//   * one persistent CTA per SM: 4 consumer warpgroups (a group owns 128 channels of its own edge-balanced receiver range,
-//     as a CTA of painn.cu did) and one producer warpgroup.  The producer stages the Phi' rows of a whole chunk (every
+//   * one persistent CTA per SM: 4 consumer warpgroups forward (a group owns 128 channels of its own edge-balanced
+//     receiver range, as a CTA of painn.cu did), 8 consumer warps reverse (a warp owns its own edge-balanced sender range,
+//     a lane 4 channels), and one producer warpgroup.  The producer stages the Phi' rows of a whole chunk (every
 //     group's rows), multiplies them with wide wgmma (m64n32k8: 3 thirds x 2 m-halves x 3 k-steps x 3 products = 54
 //     instructions per chunk) and stores the fragments straight into a [operand row][third * 128 + channel] fp32 tile;
 //     the consumers read their rows of it with thread = channel, the mapping of the gather/accumulate code.  They never
@@ -45,6 +46,8 @@ extern "C" int spk_debug_edge_trace(long long* host) {
 #endif
 // Stamp slots (consumer warp 0, chunks k < 16): 64+k the wait for the chunk starts, 176+k it returns, 80+k the filter
 // values are in registers, 96+k the chunk is done; 16+k (producer warp 0): the chunk's filter tile is published.
+// Reverse: 64+k the chunk starts, 80+k the gathers of chunk k+1 are issued and the wait starts, 176+k it returns, 96+k
+// the chunk is done (its g_rij included).
 
 namespace {
 
@@ -378,18 +381,84 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_fwd_tc(
 
 
 // ------------------------------------------------------------------------------------------------------------------
-// reverse pass, grouped by sender (same structure; reference: autograd of painn.py:55-65)
+// reverse pass, grouped by sender (reference: autograd of painn.py:55-65)
 // ------------------------------------------------------------------------------------------------------------------
-// A chunk is 4 groups x 4 edges.  Its operand has NR = 32 rows: rows 0..15 = fc [phi | 1] (-> W) and rows 16..31 =
+// One persistent CTA per SM of 8 consumer warps and the producer warpgroup (384 threads, up to 168 registers each).  Each
+// consumer WARP owns an edge-balanced sender range and 2 edges of every chunk; a lane owns 4 channels and reads them as
+// float4.  A chunk is 8 warps x 2 edges; its operand has NR = 32 rows: rows 0..15 = fc [phi | 1] (-> W) and rows 16..31 =
 // dfc [phi | 1] + fc [dphi | 0] (-> dW/dd), so one m64n32 product yields both the filter and its radial derivative.
-constexpr int EGB = NR / 2 / NG;               // 4 edges per group and chunk
-constexpr int NEB = EGB * NG;                  // 16 edges per chunk (x 2 operand rows each)
-constexpr int META_B = NEB * 4 + NEB * 4 + NEB * 16;   // receiver index, edge id, (ux, uy, uz, 1/d) per edge
+// A warp finds the receivers of its own edges (pos_i over its contiguous range), so the g_q / g_mu gathers of chunk k+1
+// are in flight before it waits for the filter tile of chunk k.  The four per-edge channel sums (dE/dd, dE/du) end
+// inside the warp, and the warp writes its edges' g_rij: no barrier between the consumer warps.
+constexpr int NCW_B = 8;                       // consumer warps
+constexpr int W_PROD0_B = NCW_B;               // the producer warpgroup: warps NCW_B .. NCW_B + 3
+constexpr int NTHREADS_B = (NCW_B + 4) * 32;
+constexpr int PROD_BAR_B = 1;                  // named barrier of the producer warpgroup
+constexpr int EGB = NR / 2 / NCW_B;            // 2 edges per warp and chunk
+constexpr int NEB = EGB * NCW_B;               // 16 edges per chunk (x 2 operand rows each)
+constexpr int WIN = 32 / EGB;                  // chunks per index window (one edge per lane)
+constexpr int META_B = NEB * 16;               // (ux, uy, uz, 1/d) per edge
 constexpr int SMEM_BYTES_B = A_BYTES + B_BYTES + NBUF * (T_BYTES + META_B) + 1024;
 
+__device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
+__device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
+
+// Sum over the 32 lanes of 8 values per lane (2 edges x 4 scalars) with a transposing butterfly: 9 shuffles.  Afterwards
+// lane l holds the complete sum of value index 4*bit4 + 2*bit3 + bit2 (all four lanes of a quad).
+__device__ __forceinline__ float butterfly8(float (&v)[8], int lane) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const bool up = lane & 16;
+        const float send = up ? v[i] : v[i + 4];
+        const float keep = up ? v[i + 4] : v[i];
+        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const bool up = lane & 8;
+        const float send = up ? v[i] : v[i + 2];
+        const float keep = up ? v[i + 2] : v[i];
+        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
+    }
+    {
+        const bool up = lane & 4;
+        const float send = up ? v[0] : v[1];
+        const float keep = up ? v[1] : v[0];
+        v[0] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
+    }
+    v[0] += __shfl_xor_sync(0xffffffffu, v[0], 2);
+    return v[0] + __shfl_xor_sync(0xffffffffu, v[0], 1);
+}
+
+// One channel of one edge: the sender accumulators (the expressions of the one-thread-per-channel kernel, so g_x and
+// g_mu_in do not depend on how channels map to lanes) and this channel's share of the four per-edge scalars in s.
+template <bool HAS_MU>
+__device__ __forceinline__ void bwd_channel(float gq, float g0, float g1, float g2, float4 ge, float w0, float w1,
+                                            float w2, float d0, float d1, float d2, float xa, float xb, float xc,
+                                            float m0, float m1, float m2, float& gxa, float& gxb, float& gxc,
+                                            float& gm0, float& gm1, float& gm2, float (&s)[4]) {
+    const float gu = g0 * ge.x + g1 * ge.y + g2 * ge.z;
+    gxa = fmaf(w0, gq, gxa);
+    gxb = fmaf(w1, gu, gxb);
+    float part_d = gq * xa * d0 + gu * xb * d1;
+    const float wbx = w1 * xb;
+    if (HAS_MU) {
+        const float gm = g0 * m0 + g1 * m1 + g2 * m2;
+        gxc = fmaf(w2, gm, gxc);
+        const float wcx = w2 * xc;
+        gm0 = fmaf(wcx, g0, gm0);
+        gm1 = fmaf(wcx, g1, gm1);
+        gm2 = fmaf(wcx, g2, gm2);
+        part_d = fmaf(gm * xc, d2, part_d);
+    }
+    s[0] += part_d;
+    s[1] += g0 * wbx;
+    s[2] += g1 * wbx;
+    s[3] += g2 * wbx;
+}
 
 template <bool HAS_MU>
-__global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
+__global__ void __launch_bounds__(NTHREADS_B, 1) k_painn_edge_bwd_tc(
     const float* __restrict__ x, const float* __restrict__ mu, const float* __restrict__ g_q,
     const float* __restrict__ g_mu, const float* __restrict__ phi, const float* __restrict__ dphi,
     const float* __restrict__ geo, const int* __restrict__ sptr, const int* __restrict__ pos_slot,
@@ -405,8 +474,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
     float* sT = reinterpret_cast<float*>(sB + B_BYTES);
     uint8_t* sMeta = sB + B_BYTES + NBUF * T_BYTES;
     __shared__ __align__(8) uint64_t a_full, full_bar[NBUF], empty_bar[NBUF];
-    __shared__ int s_rlo[NG], s_rhi[NG], s_sb[NG], s_se[NG];
-    __shared__ float s_red[2][NG][EGB][4][4];      // [chunk parity][group][edge][warp][scalar]
+    __shared__ int s_rlo[NCW_B], s_rhi[NCW_B], s_sb[NCW_B], s_se[NCW_B];
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // broadcast: the compiler may treat the role index as warp-uniform
@@ -416,7 +484,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
 #pragma unroll
         for (int b = 0; b < NBUF; ++b) {
             mbar_init(&full_bar[b], 4);
-            mbar_init(&empty_bar[b], NCW);
+            mbar_init(&empty_bar[b], NCW_B);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         mbar_expect_tx(&a_full, A_BYTES);          // static operand: fetched BEFORE griddepcontrol.wait (pack kernels never trigger their dependents early, common.cuh)
@@ -425,11 +493,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
     if (tid == 0) BTRACE(0);
     SPK_PDL_WAIT();
     if (tid == 0) BTRACE(1);
-    if (warp <= NG) {                              // warp w finds boundary w of this CTA's NG group ranges (warp-wide search)
-        const int bnd = spk_block_row_begin_warp(sptr, n_atoms, n_edges, gridDim.x * NG, blockIdx.x * NG + warp);
+    if (warp <= NCW_B) {                           // warp w finds boundary w of this CTA's NCW_B warp ranges (warp-wide search)
+        const int bnd = spk_block_row_begin_warp(sptr, n_atoms, n_edges, gridDim.x * NCW_B, blockIdx.x * NCW_B + warp);
         if (lane == 0) {
             const int e = sptr[bnd];
-            if (warp < NG) {
+            if (warp < NCW_B) {
                 s_rlo[warp] = bnd;
                 s_sb[warp] = e;
             }
@@ -442,44 +510,51 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
     __syncthreads();
     int n_chunks = 0;
 #pragma unroll
-    for (int g = 0; g < NG; ++g) n_chunks = max(n_chunks, (s_se[g] - s_sb[g] + EGB - 1) / EGB);
+    for (int w = 0; w < NCW_B; ++w) n_chunks = max(n_chunks, (s_se[w] - s_sb[w] + EGB - 1) / EGB);
     const int KP = spk_kp(n_rbf);
 
-    if (warp >= W_PROD0) {
+    if (warp >= W_PROD0_B) {
         // =========================================== producers ===========================================
-        const int pt = tid - W_PROD0 * 32;
+        const int pt = tid - W_PROD0_B * 32;
         const int qc = pt & 7, e = pt >> 3;                    // 8 x 16 B K-chunks per row, one edge per 8 threads
         const bool q_in = qc * 4 < KP;
-        float4 pv, dv;
-        float fc = 0.f, dfc = 0.f;
-        int m_i = 0, m_e = 0;                                  // metadata: threads pt < NEB, edge = pt
-        float4 m_u = make_float4(0.f, 0.f, 0.f, 0.f);
-        auto load = [&](int k) {
-            {
-                const int g = e / EGB;
-                const int pp = s_sb[g] + k * EGB + (e % EGB);
-                const bool ok = pp < s_se[g];
-                const int sl = pos_slot[ok ? pp : 0];
-                const float2 f2 = *reinterpret_cast<const float2*>(geo + (int64_t)sl * SPK_GEO_STRIDE + 4);   // fc, dfc
-                fc = ok ? f2.x : 0.f;
-                dfc = ok ? f2.y : 0.f;
-                pv = *reinterpret_cast<const float4*>(phi + (int64_t)sl * KP + (q_in ? qc * 4 : 0));
-                dv = *reinterpret_cast<const float4*>(dphi + (int64_t)sl * KP + (q_in ? qc * 4 : 0));
-            }
+        // Edge ed of chunk k: its position in the sender grouping (0 past the warp's range), ok = inside the range.
+        auto edge_pos = [&](int k, int ed, bool& ok) {
+            const int w = ed / EGB;
+            const int pp = s_sb[w] + k * EGB + (ed % EGB);
+            ok = pp < s_se[w];
+            return ok ? pp : 0;
+        };
+        // The global loads run two chunks ahead of the MMAs, in two register sets that alternate with the chunk's parity:
+        // set k % 2 holds the rows of chunk k until they are staged, then those of chunk k+2, and the slots of chunk
+        // k+2, then those of chunk k+4.  A load then has two chunk periods to land, and no load waits for its slot.
+        struct Rows {
+            float4 pv, dv;                                     // phi, dphi of the row edge (16 B K-chunk qc)
+            float2 fcd;                                        // fc, dfc of the row edge
+            float4 m_u;                                        // metadata: threads pt < NEB, edge = pt
+            bool ok;                                           // the row edge lies inside its warp's range
+            int sl, sl_m;                                      // slots of the chunk loaded next into this set
+        };
+        auto load_slots = [&](Rows& r, int k) {
+            bool ok;
+            r.sl = pos_slot[edge_pos(k, e, ok)];
+            if (pt < NEB) r.sl_m = pos_slot[edge_pos(k, pt, ok)];
+        };
+        // Nothing here reads the loaded values; stage() is the first (masking fc, dfc of rows past a range included).
+        auto load = [&](Rows& r, int k) {                      // the slots of chunk k are in r.sl, r.sl_m
+            edge_pos(k, e, r.ok);
+            r.fcd = *reinterpret_cast<const float2*>(geo + (int64_t)r.sl * SPK_GEO_STRIDE + 4);
+            r.pv = *reinterpret_cast<const float4*>(phi + (int64_t)r.sl * KP + (q_in ? qc * 4 : 0));
+            r.dv = *reinterpret_cast<const float4*>(dphi + (int64_t)r.sl * KP + (q_in ? qc * 4 : 0));
             if (pt < NEB) {
-                const int g = pt / EGB;
-                const int pp = s_sb[g] + k * EGB + (pt % EGB);
-                const bool ok = pp < s_se[g];
-                const int sl = pos_slot[ok ? pp : 0];
-                m_i = pos_i[ok ? pp : 0];
-                m_e = slot_eid[sl];
-                const float4 g0 = *reinterpret_cast<const float4*>(geo + (int64_t)sl * SPK_GEO_STRIDE);
-                m_u = make_float4(g0.x, g0.y, g0.z, geo[(int64_t)sl * SPK_GEO_STRIDE + 6]);
+                const float4 g0 = *reinterpret_cast<const float4*>(geo + (int64_t)r.sl_m * SPK_GEO_STRIDE);
+                r.m_u = make_float4(g0.x, g0.y, g0.z, geo[(int64_t)r.sl_m * SPK_GEO_STRIDE + 6]);
             }
         };
-        auto stage = [&](int k) {                              // rows of the W and dW/dd operands
-            const float4 v = with_bias(pv, q_in, qc, n_rbf);   // [phi | 1]
-            float4 d = q_in ? dv : make_float4(0.f, 0.f, 0.f, 0.f);
+        auto stage = [&](const Rows& r, int k) {               // rows of the W and dW/dd operands
+            const float fc = r.ok ? r.fcd.x : 0.f, dfc = r.ok ? r.fcd.y : 0.f;
+            const float4 v = with_bias(r.pv, q_in, qc, n_rbf); // [phi | 1]
+            float4 d = q_in ? r.dv : make_float4(0.f, 0.f, 0.f, 0.f);
             if (qc == (n_rbf >> 2)) {                          // bias column of [dphi | 0]
                 const int kb = n_rbf & 3;
                 if (kb == 0) d.x = 0.f; else if (kb == 1) d.y = 0.f; else if (kb == 2) d.z = 0.f; else d.w = 0.f;
@@ -490,173 +565,230 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_painn_edge_bwd_tc(
             dw.z = fmaf(dfc, v.z, fc * d.z); dw.w = fmaf(dfc, v.w, fc * d.w);
             put_row(sB, e, qc, w);
             put_row(sB, NEB + e, qc, dw);
-            if (pt < NEB) {
-                uint8_t* m = sMeta + (k % NBUF) * META_B;
-                reinterpret_cast<int*>(m)[pt] = m_i;
-                reinterpret_cast<int*>(m)[NEB + pt] = m_e;
-                reinterpret_cast<float4*>(m + 2 * NEB * 4)[pt] = m_u;
-            }
+            if (pt < NEB) reinterpret_cast<float4*>(sMeta + (k % NBUF) * META_B)[pt] = r.m_u;
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            wg_bar(PROD_BAR);
+            wg_bar(PROD_BAR_B);
         };
         const uint32_t aB = smem_u32(sA), bB = smem_u32(sB);
+        Rows ra{}, rb{};
         if (n_chunks > 0) {
-            load(0);
-            stage(0);
+            load_slots(ra, 0);
+            if (n_chunks > 1) load_slots(rb, 1);
+            load(ra, 0);
+            if (n_chunks > 1) load(rb, 1);
+            if (n_chunks > 2) load_slots(ra, 2);
+            if (n_chunks > 3) load_slots(rb, 3);
+            stage(ra, 0);
         }
         mbar_wait(&a_full, 0);
-        for (int k = 0; k < n_chunks; ++k) {
+        auto step = [&](int k, Rows& cur, Rows& nxt) {         // cur: chunk k, staged; nxt: chunk k+1
             const int b = k % NBUF;
-            const bool more = k + 1 < n_chunks;
-            if (more) load(k + 1);
+            if (k + 2 < n_chunks) {
+                load(cur, k + 2);
+                if (k + 4 < n_chunks) load_slots(cur, k + 4);
+            }
             filter_to_tile<NT>(aB, bB, sT + b * T_FLOATS, pt);
             __syncwarp();
             if (lane == 0) mbar_arrive(&full_bar[b]);
-            if (warp == W_PROD0 && k < 16) BTRACE(16 + k);
-            if (more) {
+            if (warp == W_PROD0_B && k < 16) BTRACE(16 + k);
+            if (k + 1 < n_chunks) {
                 const int nb = (k + 1) % NBUF, use = (k + 1) / NBUF;
                 if (use >= 1) mbar_wait(&empty_bar[nb], (use - 1) & 1);
-                wg_bar(PROD_BAR);
-                stage(k + 1);
+                wg_bar(PROD_BAR_B);
+                stage(nxt, k + 1);
             }
+        };
+        for (int k = 0; k < n_chunks; k += 2) {                // the two register sets stay in fixed registers
+            step(k, ra, rb);
+            if (k + 1 < n_chunks) step(k + 1, rb, ra);
         }
     } else {
         // =========================================== consumers ===========================================
-        const int g = warp >> 2, qd = warp & 3;
-        const int c = qd * 32 + lane;
-        const int j_hi = s_rhi[g], p_begin = s_sb[g], p_end = s_se[g];
-        int j = s_rlo[g];
+        const int c = lane * 4;                                // this lane's four channels
+        const int j_hi = s_rhi[warp], p_begin = s_sb[warp], p_end = s_se[warp];
+        const int n_mine = (p_end - p_begin + EGB - 1) / EGB;  // chunks with edges of this warp
+        const int n_win = (p_end - p_begin + 31) / 32;
+        int j = s_rlo[warp];
         int next_boundary = j < j_hi ? sptr[j + 1] : 0x7fffffff;
-        float xa = 0.f, xb = 0.f, xc = 0.f, m0 = 0.f, m1 = 0.f, m2 = 0.f;
-        float gxa = 0.f, gxb = 0.f, gxc = 0.f, gm0 = 0.f, gm1 = 0.f, gm2 = 0.f;
+        int boundary2 = j + 1 < j_hi ? sptr[j + 2] : 0x7fffffff;
+        const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        float4 xa = z4, xb = z4, xc = z4, m0 = z4, m1 = z4, m2 = z4;
+        float4 gxa = z4, gxb = z4, gxc = z4, gm0 = z4, gm1 = z4, gm2 = z4;
         auto load_own = [&](int row) {
             const float* __restrict__ xr = x + (size_t)row * (3 * F) + c;
-            xa = xr[0];
-            xb = xr[F];
+            xa = ld4(xr);
+            xb = ld4(xr + F);
             if (HAS_MU) {
-                xc = xr[2 * F];
+                xc = ld4(xr + 2 * F);
                 const float* __restrict__ mr = mu + (size_t)row * (3 * F) + c;
-                m0 = mr[0];
-                m1 = mr[F];
-                m2 = mr[2 * F];
+                m0 = ld4(mr);
+                m1 = ld4(mr + F);
+                m2 = ld4(mr + 2 * F);
             }
         };
         auto flush = [&](int row) {
             const size_t o = (size_t)row * 3 * F + c;
-            g_x[o] = gxa;
-            g_x[o + F] = gxb;
-            g_x[o + 2 * F] = gxc;
-            if (HAS_MU) {
-                g_mu_in[o] = g_mu[o] + gm0;
-                g_mu_in[o + F] = g_mu[o + F] + gm1;
-                g_mu_in[o + 2 * F] = g_mu[o + 2 * F] + gm2;
+            float4 r0, r1, r2;
+            if (HAS_MU) {                                      // residual: issued before the stores
+                r0 = ld4(g_mu + o);
+                r1 = ld4(g_mu + o + F);
+                r2 = ld4(g_mu + o + 2 * F);
             }
-            gxa = gxb = gxc = gm0 = gm1 = gm2 = 0.f;
+            st4(g_x + o, gxa);
+            st4(g_x + o + F, gxb);
+            st4(g_x + o + 2 * F, gxc);
+            if (HAS_MU) {
+                st4(g_mu_in + o, make_float4(r0.x + gm0.x, r0.y + gm0.y, r0.z + gm0.z, r0.w + gm0.w));
+                st4(g_mu_in + o + F, make_float4(r1.x + gm1.x, r1.y + gm1.y, r1.z + gm1.z, r1.w + gm1.w));
+                st4(g_mu_in + o + 2 * F, make_float4(r2.x + gm2.x, r2.y + gm2.y, r2.z + gm2.z, r2.w + gm2.w));
+            }
+            gxa = gxb = gxc = gm0 = gm1 = gm2 = z4;
+        };
+        // Edge p is past the current row: flush it and any edge-free rows after it, and move to the row of p.  The own
+        // rows of the new sender are loaded before the flush, so their latency and that of the residual overlap.
+        auto next_row = [&](int p) {
+            int j2 = j + 1, nbd = boundary2;
+            while (p >= nbd) nbd = sptr[++j2 + 1];
+            load_own(j2);
+            flush(j);
+            for (int r = j + 1; r < j2; ++r) flush(r);
+            j = j2;
+            next_boundary = nbd;
+            boundary2 = j + 1 < j_hi ? sptr[j + 2] : 0x7fffffff;
         };
         if (j < j_hi) load_own(j);
-        const int my_idx = ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
-        for (int k = 0; k < n_chunks; ++k) {
+
+        // Index windows: lane l holds receiver, edge id and (accumulate) the old g_rij of edge p_begin + 32 w + l, the
+        // edges of chunks WIN w .. WIN w + WIN-1.  The next window is filled in three steps spread over the current
+        // one (pos_i + pos_slot, slot_eid, g_rij), so no chunk waits on that chain.
+        int wi = 0, we = 0, ni = 0, ne = 0;
+        float wr0 = 0.f, wr1 = 0.f, wr2 = 0.f, nr0 = 0.f, nr1 = 0.f, nr2 = 0.f;
+        auto win_idx = [&](int w, int& i_, int& e_) {          // e_: the slot until win_eid
+            const int p = p_begin + 32 * w + lane;
+            if (p < p_end) {
+                i_ = pos_i[p];
+                e_ = pos_slot[p];
+            }
+        };
+        auto win_eid = [&](int w, int& e_) {
+            if (p_begin + 32 * w + lane < p_end) e_ = slot_eid[e_];
+        };
+        auto win_old = [&](int w, int e_, float& a, float& b_, float& c_) {
+            if (accumulate && p_begin + 32 * w + lane < p_end) {
+                const float* o = g_rij + (int64_t)e_ * 3;
+                a = o[0];
+                b_ = o[1];
+                c_ = o[2];
+            }
+        };
+        // g_q and g_mu rows of the receivers of chunk q's edges, [edge][g_q, g_mu x, y, z]
+        auto gather = [&](float4 (&G)[EGB][4], int q, int src_i) {
+#pragma unroll
+            for (int u = 0; u < EGB; ++u) {
+                const int i = __shfl_sync(0xffffffffu, src_i, (q * EGB + u) & 31);
+                if (p_begin + q * EGB + u < p_end) {
+                    G[u][0] = ld4(g_q + (size_t)i * F + c);
+                    const float* __restrict__ gmi = g_mu + (size_t)i * (3 * F) + c;
+                    G[u][1] = ld4(gmi);
+                    G[u][2] = ld4(gmi + F);
+                    G[u][3] = ld4(gmi + 2 * F);
+                }
+            }
+        };
+        float4 ga[EGB][4], gb[EGB][4];
+        if (n_mine > 0) {
+            win_idx(0, wi, we);
+            if (n_win > 1) win_idx(1, ni, ne);
+            gather(ga, 0, wi);
+            win_eid(0, we);
+            win_old(0, we, wr0, wr1, wr2);
+        }
+
+        auto step = [&](int k, float4 (&G)[EGB][4], float4 (&Gn)[EGB][4]) {
             const int b = k % NBUF;
-            if (warp == 0 && k < 16) BTRACE(64 + k);           // consumer 0: starts waiting
+            if (warp == 0 && k < 16) BTRACE(64 + k);           // consumer 0: the chunk starts
+            if (k + 1 < n_mine) gather(Gn, k + 1, (k + 1) % WIN == 0 ? ni : wi);
+            if (warp == 0 && k < 16) BTRACE(80 + k);           // gathers of the next chunk issued, starts waiting
             mbar_wait(&full_bar[b], (k / NBUF) & 1);           // filter tile and metadata of the chunk
             if (warp == 0 && k < 16) BTRACE(176 + k);
-            const float* tg = sT + b * T_FLOATS + g * EGB * T_LD + c;   // W rows of the group; dW/dd rows NEB further
-            float Wv[3][EGB], Dv[3][EGB];
-#pragma unroll
-            for (int t = 0; t < NT; ++t)
-#pragma unroll
-                for (int u = 0; u < EGB; ++u) {
-                    Wv[t][u] = tg[u * T_LD + t * F];
-                    Dv[t][u] = tg[(NEB + u) * T_LD + t * F];
-                }
-            if (warp == 0 && k < 16) BTRACE(80 + k);           // filter values ready
             if (warp == 0 && lane == 0 && k == 0) SPK_TL_PHASE(2);
-            const int* st_i = reinterpret_cast<const int*>(sMeta + b * META_B) + g * EGB;
-            const int* st_e = reinterpret_cast<const int*>(sMeta + b * META_B) + NEB + g * EGB;
-            const float4* st_u = reinterpret_cast<const float4*>(sMeta + b * META_B + 2 * NEB * 4) + g * EGB;
-            const int base = p_begin + k * EGB;
-            {
-                float gq[EGB], g0[EGB], g1[EGB], g2[EGB];
-#pragma unroll
-                for (int u = 0; u < EGB; ++u) {                // rows past the range gather receiver 0; their W, dW are 0
-                    const int i = st_i[u];
-                    gq[u] = g_q[(size_t)i * F + c];
-                    const float* __restrict__ gmi = g_mu + (size_t)i * (3 * F) + c;
-                    g0[u] = gmi[0];
-                    g1[u] = gmi[F];
-                    g2[u] = gmi[2 * F];
-                }
-                float red[16];
+            const float4* st_u = reinterpret_cast<const float4*>(sMeta + b * META_B) + warp * EGB;
+            if (k < n_mine) {
+                // this warp's rows of the filter tile, read where they are used; dW/dd rows NEB further
+                const float* tw = sT + b * T_FLOATS + warp * EGB * T_LD + c;
+                const int base = p_begin + k * EGB;
+                float red[4 * EGB];
 #pragma unroll
                 for (int u = 0; u < EGB; ++u) {
-                    const int p = base + u;
-                    float part_d = 0.f, pu0 = 0.f, pu1 = 0.f, pu2 = 0.f;
-                    if (p < p_end) {
-                        if (p >= next_boundary) {
-                            do {
-                                flush(j);
-                                ++j;
-                                next_boundary = sptr[j + 1];
-                            } while (p >= next_boundary);
-                            load_own(j);
-                        }
-                        const float4 ge = st_u[u];                 // ux uy uz 1/d
-                        const float gu = g0[u] * ge.x + g1[u] * ge.y + g2[u] * ge.z;
-                        gxa = fmaf(Wv[0][u], gq[u], gxa);
-                        gxb = fmaf(Wv[1][u], gu, gxb);
-                        part_d = gq[u] * xa * Dv[0][u] + gu * xb * Dv[1][u];
-                        const float wbx = Wv[1][u] * xb;
-                        pu0 = g0[u] * wbx;
-                        pu1 = g1[u] * wbx;
-                        pu2 = g2[u] * wbx;
-                        if (HAS_MU) {
-                            const float gm = g0[u] * m0 + g1[u] * m1 + g2[u] * m2;
-                            gxc = fmaf(Wv[2][u], gm, gxc);
-                            const float wcx = Wv[2][u] * xc;
-                            gm0 = fmaf(wcx, g0[u], gm0);
-                            gm1 = fmaf(wcx, g1[u], gm1);
-                            gm2 = fmaf(wcx, g2[u], gm2);
-                            part_d = fmaf(gm * xc, Dv[2][u], part_d);
-                        }
+                    float s[4] = {0.f, 0.f, 0.f, 0.f};
+                    if (base + u < p_end) {
+                        if (base + u >= next_boundary) next_row(base + u);
+                        const float4 ge = st_u[u];             // ux uy uz 1/d
+                        const float4 w0 = ld4(tw + u * T_LD), w1 = ld4(tw + u * T_LD + F);
+                        const float4 d0 = ld4(tw + (NEB + u) * T_LD), d1 = ld4(tw + (NEB + u) * T_LD + F);
+                        const float4 w2 = HAS_MU ? ld4(tw + u * T_LD + 2 * F) : z4;
+                        const float4 d2 = HAS_MU ? ld4(tw + (NEB + u) * T_LD + 2 * F) : z4;
+                        const float4 gq = G[u][0], g0 = G[u][1], g1 = G[u][2], g2 = G[u][3];
+                        bwd_channel<HAS_MU>(gq.x, g0.x, g1.x, g2.x, ge, w0.x, w1.x, w2.x, d0.x, d1.x, d2.x, xa.x, xb.x,
+                                            xc.x, m0.x, m1.x, m2.x, gxa.x, gxb.x, gxc.x, gm0.x, gm1.x, gm2.x, s);
+                        bwd_channel<HAS_MU>(gq.y, g0.y, g1.y, g2.y, ge, w0.y, w1.y, w2.y, d0.y, d1.y, d2.y, xa.y, xb.y,
+                                            xc.y, m0.y, m1.y, m2.y, gxa.y, gxb.y, gxc.y, gm0.y, gm1.y, gm2.y, s);
+                        bwd_channel<HAS_MU>(gq.z, g0.z, g1.z, g2.z, ge, w0.z, w1.z, w2.z, d0.z, d1.z, d2.z, xa.z, xb.z,
+                                            xc.z, m0.z, m1.z, m2.z, gxa.z, gxb.z, gxc.z, gm0.z, gm1.z, gm2.z, s);
+                        bwd_channel<HAS_MU>(gq.w, g0.w, g1.w, g2.w, ge, w0.w, w1.w, w2.w, d0.w, d1.w, d2.w, xa.w, xb.w,
+                                            xc.w, m0.w, m1.w, m2.w, gxa.w, gxb.w, gxc.w, gm0.w, gm1.w, gm2.w, s);
                     }
-                    red[4 * u + 0] = part_d;
-                    red[4 * u + 1] = pu0;
-                    red[4 * u + 2] = pu1;
-                    red[4 * u + 3] = pu2;
-                }
-                const float tot = butterfly16(red, lane);
-                if (!(lane & 1)) s_red[k & 1][g][my_idx >> 2][qd][my_idx & 3] = tot;
-            }
-            // the four warps of the group have published their partial sums of this chunk's edges
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");
-            if (qd == 0 && lane < EGB && base + lane < p_end) {
-                const int t = lane;
-                float gd = 0.f, u0 = 0.f, u1 = 0.f, u2 = 0.f;
 #pragma unroll
-                for (int wv = 0; wv < 4; ++wv) {
-                    gd += s_red[k & 1][g][t][wv][0];
-                    u0 += s_red[k & 1][g][t][wv][1];
-                    u1 += s_red[k & 1][g][t][wv][2];
-                    u2 += s_red[k & 1][g][t][wv][3];
+                    for (int t = 0; t < 4; ++t) red[4 * u + t] = s[t];
                 }
-                const float4 ge = st_u[t];
-                const float dot = u0 * ge.x + u1 * ge.y + u2 * ge.z;
-                float r0 = gd * ge.x + (u0 - dot * ge.x) * ge.w;
-                float r1 = gd * ge.y + (u1 - dot * ge.y) * ge.w;
-                float r2 = gd * ge.z + (u2 - dot * ge.z) * ge.w;
-                float* out = g_rij + (int64_t)st_e[t] * 3;
-                if (accumulate) {
-                    r0 += out[0];
-                    r1 += out[1];
-                    r2 += out[2];
+                // lane 16 u + 4 t holds scalar t (dE/dd, dE/du x, y, z) of edge u; lane 16 u writes the edge's g_rij
+                const float v = butterfly8(red, lane);
+                const float u0 = __shfl_down_sync(0xffffffffu, v, 4);
+                const float u1 = __shfl_down_sync(0xffffffffu, v, 8);
+                const float u2 = __shfl_down_sync(0xffffffffu, v, 12);
+                const int src = (k * EGB + (lane >> 4)) & 31;  // the edge's lane in the index window
+                const int eid = __shfl_sync(0xffffffffu, we, src);
+                const float o0 = __shfl_sync(0xffffffffu, wr0, src);
+                const float o1 = __shfl_sync(0xffffffffu, wr1, src);
+                const float o2 = __shfl_sync(0xffffffffu, wr2, src);
+                if ((lane & 15) == 0 && base + (lane >> 4) < p_end) {
+                    const float4 ge = st_u[lane >> 4];
+                    const float dot = u0 * ge.x + u1 * ge.y + u2 * ge.z;
+                    float r0 = v * ge.x + (u0 - dot * ge.x) * ge.w;
+                    float r1 = v * ge.y + (u1 - dot * ge.y) * ge.w;
+                    float r2 = v * ge.z + (u2 - dot * ge.z) * ge.w;
+                    if (accumulate) {
+                        r0 += o0;
+                        r1 += o1;
+                        r2 += o2;
+                    }
+                    float* out = g_rij + (int64_t)eid * 3;
+                    out[0] = r0;
+                    out[1] = r1;
+                    out[2] = r2;
                 }
-                out[0] = r0;
-                out[1] = r1;
-                out[2] = r2;
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty_bar[b]);
-            if (warp == 0 && k < 16) BTRACE(96 + k);           // chunk done (incl. the g_rij tail of warp qd == 0)
+            if (warp == 0 && k < 16) BTRACE(96 + k);           // chunk done (incl. its g_rij)
+            // the next window's steps; at the window's end it becomes the current one
+            const int kw = k / WIN, kk = k % WIN;
+            if (kw + 1 < n_win) {
+                if (kk == 4) win_eid(kw + 1, ne);
+                if (kk == 8) win_old(kw + 1, ne, nr0, nr1, nr2);
+                if (kk == WIN - 1) {
+                    wi = ni;
+                    we = ne;
+                    wr0 = nr0;
+                    wr1 = nr1;
+                    wr2 = nr2;
+                    if (kw + 2 < n_win) win_idx(kw + 2, ni, ne);
+                }
+            }
+        };
+        for (int k = 0; k < n_chunks; k += 2) {                // two gather buffers in fixed registers
+            step(k, ga, gb);
+            if (k + 1 < n_chunks) step(k + 1, gb, ga);
         }
         if (warp == 0 && lane == 0) SPK_TL_PHASE(3);           // main loop done
         if (warp == 0) BTRACE(2);
@@ -720,7 +852,9 @@ extern "C" int spk_painn_edge_bwd_tc(const float* x, const float* mu, const floa
         return SPK_ERR_ARG;
     if (mu && !g_mu_in) return SPK_ERR_ARG;
     if ((reinterpret_cast<uintptr_t>(phi) | reinterpret_cast<uintptr_t>(dphi) | reinterpret_cast<uintptr_t>(geo) |
-         reinterpret_cast<uintptr_t>(wf_packed)) & 15)
+         reinterpret_cast<uintptr_t>(wf_packed) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(mu) |
+         reinterpret_cast<uintptr_t>(g_q) | reinterpret_cast<uintptr_t>(g_mu) | reinterpret_cast<uintptr_t>(g_x) |
+         reinterpret_cast<uintptr_t>(g_mu_in)) & 15)                               // float4 rows
         return SPK_ERR_UNSUPPORTED;
     static SpkSmemOnce once_mu, once_nomu;
     if (cudaError_t e = once_mu.set(k_painn_edge_bwd_tc<true>, SMEM_BYTES_B); e != cudaSuccess) return SPK_CUDA_ERR(e);
@@ -731,10 +865,10 @@ extern "C" int spk_painn_edge_bwd_tc(const float* x, const float* mu, const floa
     if (nb < 1) nb = 1;
     cudaStream_t st = spk_st(stream);
     if (mu)
-        spk_launch(k_painn_edge_bwd_tc<true>, (unsigned)nb, NTHREADS, SMEM_BYTES_B, st, x, mu, g_q, g_mu, phi, dphi, geo, sptr,
+        spk_launch(k_painn_edge_bwd_tc<true>, (unsigned)nb, NTHREADS_B, SMEM_BYTES_B, st, x, mu, g_q, g_mu, phi, dphi, geo, sptr,
                    pos_slot, pos_i, slot_eid, wf_packed, (int)n_atoms, (int)n_edges, n_rbf, g_x, g_mu_in, g_rij, accumulate);
     else
-        spk_launch(k_painn_edge_bwd_tc<false>, (unsigned)nb, NTHREADS, SMEM_BYTES_B, st, x, mu, g_q, g_mu, phi, dphi, geo, sptr,
+        spk_launch(k_painn_edge_bwd_tc<false>, (unsigned)nb, NTHREADS_B, SMEM_BYTES_B, st, x, mu, g_q, g_mu, phi, dphi, geo, sptr,
                    pos_slot, pos_i, slot_eid, wf_packed, (int)n_atoms, (int)n_edges, n_rbf, g_x, g_mu_in, g_rij, accumulate);
     SPK_LAUNCH_CHECK();
     return SPK_OK;
