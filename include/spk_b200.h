@@ -574,6 +574,60 @@ int spk_head_bwd(int kind, const spk_head_tail_t* tail, const float* s, const fl
 int spk_head_scalar_bwd(const float* q, const float* R, const int64_t* idx_m, const double* saved, const float* g_out,
                         int correct, int magnitude, const float* w1, int64_t n_atoms, int H, float* g_hid, float* g_R,
                         spk_stream_t stream);
+/* Reverse of spk_head_charges for the charge gradient g_charges [N]: g_q [N] = g_charges - mean_m(g_charges) with
+ * `correct` (the per-system mean as an fp64 segmented sum, bitwise reproducible, no atomics), else g_charges. */
+size_t spk_head_charges_bwd_workspace_bytes(int64_t n_atoms, int64_t n_sys);
+int spk_head_charges_bwd(const float* g_charges, const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms,
+                         int64_t n_sys, int correct, float* g_q, void* workspace, size_t workspace_bytes,
+                         spk_stream_t stream);
+/* spk_head_bwd / spk_head_scalar_bwd with the gradient g_q [N] of the tail's charges (from spk_head_charges_bwd) added
+ * to the one the dipole sends to them; kind = SPK_HEAD_DIPOLE only. */
+int spk_head_bwd_q(int kind, const spk_head_tail_t* tail, const float* s, const float* V, const float* R,
+                   const int64_t* idx_m, const double* saved, const float* g_out, const float* g_q, int64_t n_atoms,
+                   int correct, int magnitude, float* g_s, float* g_V, float* g_R, spk_stream_t stream);
+int spk_head_scalar_bwd_q(const float* q, const float* R, const int64_t* idx_m, const double* saved, const float* g_out,
+                          const float* g_q, int correct, int magnitude, const float* w1, int64_t n_atoms, int H,
+                          float* g_hid, float* g_R, spk_stream_t stream);
+
+/* ---- pair energies (csrc/pair_energy.cu; atomistic/nuclear_repulsion.py:81-104, atomistic/electrostatic.py:14-152) ---
+ * Per edge e = (i, j), d = |r_ij| (an edge with d > d_max when d_max > 0 contributes nothing):
+ *   ZBL:     a_k = Z_k^softplus(a_pow), a_ij = (a_i + a_j) softplus(a_div), c = normalize_L1(softplus(coefficients)),
+ *            e = Z_i Z_j / d sum_k c_k exp(-a_ij softplus(exponents_k) d), times the cosine cutoff if cutoff > 0
+ *   Coulomb: e = q_i q_j V(d), V = 1/d or (damped) f_sw / sqrt(d^2 + 1) + (1 - f_sw) / d with the switch function of
+ *            (switch_on, switch_off); with cutoff > 0, V + shift^2 / V - 2 shift for d <= cutoff and 0 beyond
+ * The ZBL parameters are read raw from device memory (softplus and normalisation on the device). */
+#define SPK_PAIR_ZBL 0
+#define SPK_PAIR_COULOMB 1
+#define SPK_PAIR_DAMPED_COULOMB 2
+#define SPK_PAIR_MAX_TERMS 16
+typedef struct {
+    int32_t kind;
+    int32_t n_terms;           /* ZBL: number of screening terms (length of coefficients / exponents) */
+    const float* a_pow;        /* ZBL: [1] */
+    const float* a_div;        /* ZBL: [1] */
+    const float* coefficients; /* ZBL: [n_terms] */
+    const float* exponents;    /* ZBL: [n_terms] */
+    double ke;
+    double cutoff;             /* ZBL: cosine cutoff radius; Coulomb: shift cutoff; <= 0: none */
+    double shift;              /* Coulomb with cutoff: V(cutoff) */
+    double switch_on, switch_off;
+    double d_max;              /* distance mask d <= d_max; <= 0: none */
+} spk_pair_t;
+size_t spk_pair_energy_workspace_bytes(int64_t n_edges, int64_t n_sys);
+/* energy [B] = 0.5 ke sum_{e in m} e_ij over the receiver slots [rowptr[sys_ptr[m]], rowptr[sys_ptr[m+1]]), summed in fp64
+ * by the segmented-partial pass (bitwise reproducible, no atomics).  Z [N] for ZBL, q [N] for Coulomb. */
+int spk_pair_energy_fwd(const spk_pair_t* p, const float* r_ij, const int64_t* idx_i, const int64_t* idx_j,
+                        const int64_t* Z, const float* q, const int64_t* idx_m, const int32_t* rowptr,
+                        const int32_t* slot_eid, const int32_t* sys_ptr, int64_t n_edges, int64_t n_sys, float* energy,
+                        void* workspace, size_t workspace_bytes, spk_stream_t stream);
+/* Reverse for g_E [B]: g_rij [E,3] = 0.5 ke g_E[m(e)] de/dd r_ij / d in edge order; for Coulomb and g_q != NULL also
+ * g_q [N] = 0.5 ke g_E[m(a)] (sum over the receiver slots of a of q_j V + sum over its sender slots of q_i V) in the fixed
+ * order of the two graph views. */
+int spk_pair_energy_bwd(const spk_pair_t* p, const float* r_ij, const int64_t* idx_i, const int64_t* idx_j,
+                        const int64_t* Z, const float* q, const int64_t* idx_m, const float* g_E, const int32_t* rowptr,
+                        const int32_t* slot_j, const int32_t* slot_eid, const int32_t* sptr, const int32_t* pos_slot,
+                        const int32_t* pos_i, int64_t n_atoms, int64_t n_edges, float* g_rij, float* g_q,
+                        spk_stream_t stream);
 
 /* ---- batchwise L-BFGS relaxation (csrc/relax.cu; interfaces/batchwise_optimization.py:613-917) ----------------------
  * One optimizer per system (atoms [sys_ptr[m], sys_ptr[m+1])), state fp64 on the device, positions in optimizer units

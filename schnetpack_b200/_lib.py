@@ -52,6 +52,16 @@ class LBFGSState(Structure):
                 ("position_conversion", c_double), ("maxstep", c_double), ("damping", c_double), ("h0", c_double)]
 
 
+class PairParams(Structure):
+    """spk_pair_t of include/spk_b200.h."""
+    _fields_ = [("kind", c_int32), ("n_terms", c_int32), ("a_pow", c_void_p), ("a_div", c_void_p),
+                ("coefficients", c_void_p), ("exponents", c_void_p), ("ke", c_double), ("cutoff", c_double),
+                ("shift", c_double), ("switch_on", c_double), ("switch_off", c_double), ("d_max", c_double)]
+
+
+PAIR_ZBL, PAIR_COULOMB, PAIR_DAMPED_COULOMB = 0, 1, 2     # SPK_PAIR_*
+PAIR_MAX_TERMS = 16                                       # SPK_PAIR_MAX_TERMS
+
 RELAX_WARP_ATOMS = 256      # SPK_RELAX_WARP_ATOMS
 RELAX_MAX_MEMORY = 4096     # SPK_RELAX_MAX_MEMORY
 
@@ -149,6 +159,13 @@ SIGNATURES = {
                                     c_double, c_double, P, P, P, c_size_t, P],
     "spk_rpmd_barostat_main_step": [P, P, P, P, P, c_int64, c_int64, c_int32, P, P, c_double, P, P, P, P, c_double, P,
                                     c_size_t, P],
+    "spk_head_charges_bwd_workspace_bytes": [c_int64, c_int64],
+    "spk_head_charges_bwd": [P, P, P, c_int64, c_int64, c_int, P, P, c_size_t, P],
+    "spk_head_bwd_q": [c_int, POINTER(HeadTail), P, P, P, P, P, P, P, c_int64, c_int, c_int, P, P, P, P],
+    "spk_head_scalar_bwd_q": [P, P, P, P, P, P, c_int, c_int, P, c_int64, c_int, P, P, P],
+    "spk_pair_energy_workspace_bytes": [c_int64, c_int64],
+    "spk_pair_energy_fwd": [POINTER(PairParams), P, P, P, P, P, P, P, P, P, c_int64, c_int64, P, P, c_size_t, P],
+    "spk_pair_energy_bwd": [POINTER(PairParams), P, P, P, P, P, P, P, P, P, P, P, P, P, c_int64, c_int64, P, P, P],
     "spk_relax_step": [POINTER(LBFGSState), P, P],
     "spk_relax_converged": [POINTER(LBFGSState), P, P],
 }
@@ -157,7 +174,8 @@ _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_siz
             "spk_schnet_filter_packed_floats": c_size_t,
             "spk_painn_filter_packed_floats": c_size_t, "spk_neighbor_list_workspace_bytes": c_size_t,
             "spk_md_thermostat_workspace_bytes": c_size_t, "spk_rpmd_workspace_bytes": c_size_t,
-            "spk_rpmd_barostat_workspace_bytes": c_size_t, "spk_head_workspace_bytes": c_size_t}
+            "spk_rpmd_barostat_workspace_bytes": c_size_t, "spk_head_workspace_bytes": c_size_t,
+            "spk_head_charges_bwd_workspace_bytes": c_size_t, "spk_pair_energy_workspace_bytes": c_size_t}
 
 _lib = None
 
@@ -201,7 +219,7 @@ LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out
             "spk_md_kinetic_energy_tensor": 3, "spk_md_barostat_thermostat": 4, "spk_md_barostat_kick": 3,
             "spk_md_barostat_half_step": 2, "spk_md_barostat_main_step": 2, "spk_rpmd_barostat_half_step": 2,
             "spk_rpmd_barostat_main_step": 2, "spk_head_fwd": 2,
-            "spk_relax_converged": 2}   # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global
+            "spk_relax_converged": 2, "spk_pair_energy_fwd": 2, "spk_head_charges_bwd": 3}   # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global
 launch_count = 0
 
 

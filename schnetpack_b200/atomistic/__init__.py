@@ -16,7 +16,8 @@ from .. import nn as snn
 from .. import ops
 from .. import properties
 
-__all__ = ["PairwiseDistances", "Atomwise", "Forces", "Strain", "DipoleMoment", "Polarizability"]
+__all__ = ["PairwiseDistances", "Atomwise", "Forces", "Strain", "DipoleMoment", "Polarizability", "ZBLRepulsionEnergy",
+           "CoulombPotential", "DampedCoulombPotential", "EnergyCoulomb", "Aggregation", "FilterShortRange"]
 
 
 class PairwiseDistances(nn.Module):
@@ -239,7 +240,10 @@ class DipoleMoment(_GatedHead):
 
     ``eval()``: the gated blocks / the charge MLP and the per-system assembly run on the kernels of csrc/equivariant.cu
     (fp64 segmented sums, no atomics, no host read), differentiable with respect to positions and the representation
-    (dipole derivatives through ``torch.autograd.grad``).  The charges output is not differentiable on that path.
+    (dipole derivatives through ``torch.autograd.grad``).  The charges output is differentiable when
+    ``differentiable_charges`` is set -- ``NeuralNetworkPotential`` sets it when an ``EnergyCoulomb`` of the model reads
+    these charges, so that its energy has the ``dE/dq dq/dR`` force term; otherwise the charges are a plain output and the
+    reverse is exactly that of the dipole.
     ``train()`` with trainable parameters under grad mode: the ATen formula of ``functional_torch``."""
 
     def __init__(self, n_in: int, n_hidden: Optional[Union[int, Sequence[int]]] = None, n_layers: int = 2,
@@ -256,6 +260,7 @@ class DipoleMoment(_GatedHead):
         self.predict_magnitude = predict_magnitude
         self.use_vector_representation = use_vector_representation
         self.correct_charges = correct_charges
+        self.differentiable_charges = False
         if use_vector_representation:
             self.outnet = snn.build_gated_equivariant_mlp(n_in=n_in, n_out=1, n_hidden=n_hidden, n_layers=n_layers,
                                                           activation=activation, sactivation=activation)
@@ -275,6 +280,7 @@ class DipoleMoment(_GatedHead):
             return T.dipole_moment(self, inputs)
         self._check_kernel_shape()
         h = self._holder(inputs, ops.HEAD_DIPOLE, self.correct_charges, self.predict_magnitude, self.return_charges)
+        h["diff_charges"] = self.return_charges and self.differentiable_charges
         s, R = inputs["scalar_representation"], inputs[properties.R]
         if self.use_vector_representation:
             y, charges = K.GatedHeadFunction.apply(s, inputs["vector_representation"], R, h)
@@ -318,3 +324,7 @@ class Polarizability(_GatedHead):
                                              inputs[properties.R], h)
         inputs[self.polarizability_key] = alpha
         return inputs
+
+
+from .pair_terms import (Aggregation, CoulombPotential, DampedCoulombPotential, EnergyCoulomb,  # noqa: E402
+                         FilterShortRange, ZBLRepulsionEnergy)

@@ -1,0 +1,294 @@
+"""Physics add-ons of PhysNet-style potentials on the kernels of csrc/pair_energy.cu: ZBL repulsion
+(atomistic/nuclear_repulsion.py:13-108), the Coulomb energy of point charges with its potentials
+(atomistic/electrostatic.py:14-152), ``Aggregation`` (atomistic/aggregation.py) and a capture-safe ``FilterShortRange``
+(atomistic/distances.py:29-57).  Constructor signatures, parameters, buffers and ``state_dict`` keys are the
+reference's.
+
+``eval()``: every pair term is one ``spk_pair_energy_fwd`` (fp64 per-system sums in a fixed order, no atomics, no host
+read: the number of systems comes from ``_n_atoms``) and its reverse gives dE/dr_ij and, for Coulomb, dE/dq -- which
+reaches the charge head through the differentiable ``charges`` output of ``DipoleMoment``.  ``train()`` with trainable
+parameters under grad mode: the ATen formulas of ``functional_torch``."""
+from __future__ import annotations
+
+from typing import Callable, Dict, List, Optional, Union
+
+import torch
+import torch.nn as nn
+
+from .. import functional as K
+from .. import nn as snn
+from .. import ops
+from .. import properties
+from ..units import convert_units
+
+__all__ = ["ZBLRepulsionEnergy", "CoulombPotential", "DampedCoulombPotential", "EnergyCoulomb", "Aggregation",
+           "FilterShortRange", "check_padded_pair_terms", "check_short_range_cutoff", "link_charges"]
+
+
+def _softplus_inverse(x: torch.Tensor) -> torch.Tensor:
+    """nn/utils.py softplus_inverse: x + log(-expm1(-x))."""
+    x = torch.as_tensor(x)
+    return x + torch.log(-torch.expm1(-x))
+
+
+class _HostScalars:
+    """Python floats of small buffers (ke, cutoff, shift, switch limits): one host read per change of a buffer (loading a
+    state dict), none on the evaluation path."""
+
+    def __init__(self):
+        self._key, self._vals = None, None
+
+    def get(self, *bufs: Optional[torch.Tensor]):
+        key = tuple((b.data_ptr(), b._version) if b is not None else None for b in bufs)
+        if key != self._key:
+            self._vals = tuple(float(b.reshape(-1)[0]) if b is not None else None for b in bufs)
+            self._key = key
+        return self._vals
+
+
+def _systems(inputs: Dict[str, torch.Tensor], who: str):
+    if properties.n_atoms not in inputs:
+        raise KeyError(f"{who} needs '{properties.n_atoms}' (the number of systems, without a host read)")
+    n_sys = int(inputs[properties.n_atoms].shape[0])
+    idx_m = inputs[properties.idx_m]
+    idx_m = (idx_m if idx_m.dtype == torch.int64 else idx_m.long()).contiguous()
+    return idx_m, n_sys, ops.segment_ptr(idx_m, n_sys)
+
+
+def _edges(inputs: Dict[str, torch.Tensor], key_r: str, key_i: str, key_j: str, n_atoms: int):
+    idx_i, idx_j = inputs[key_i], inputs[key_j]
+    idx_i = (idx_i if idx_i.dtype == torch.int64 else idx_i.long()).contiguous()
+    idx_j = (idx_j if idx_j.dtype == torch.int64 else idx_j.long()).contiguous()
+    return inputs[key_r], idx_i, idx_j, ops.get_graph(idx_i, idx_j, n_atoms)
+
+
+def _short_range_d_max(inputs: Dict[str, torch.Tensor]) -> Optional[float]:
+    src = inputs.get(properties.short_range_cutoff)
+    return None if src is None else float(src)
+
+
+def _cosine_cutoff_radius(cutoff_fn, who: str) -> Optional[float]:
+    if cutoff_fn is None:
+        return None
+    if type(cutoff_fn).__name__ != "CosineCutoff":
+        raise NotImplementedError(f"{who}: cutoff {type(cutoff_fn).__name__} has no CUDA kernel (CosineCutoff or None)")
+    return cutoff_fn.value() if isinstance(cutoff_fn, snn.CosineCutoff) else float(cutoff_fn.cutoff)
+
+
+class ZBLRepulsionEnergy(nn.Module):
+    """nuclear_repulsion.py:13-108.  The kernel reads the raw parameters from device memory and applies softplus and the
+    L1 normalisation there, so a captured graph sees parameter updates.  ``cutoff_fn`` in {None, CosineCutoff}."""
+
+    def __init__(self, energy_unit: Union[str, float], position_unit: Union[str, float], output_key: str,
+                 trainable: bool = True, cutoff_fn: Optional[Callable] = None):
+        super().__init__()
+        energy_units = convert_units("Ha", energy_unit)
+        position_units = convert_units("Bohr", position_unit)
+        ke = energy_units * position_units
+        self.register_buffer("ke", torch.tensor(ke))
+        self.cutoff_fn = cutoff_fn
+        self.output_key = output_key
+        a_div = _softplus_inverse(torch.tensor([1.0 / (position_units * 0.8854)]))
+        a_pow = _softplus_inverse(torch.tensor([0.23]))
+        exponents = _softplus_inverse(torch.tensor([3.19980, 0.94229, 0.40290, 0.20162]))
+        coefficients = _softplus_inverse(torch.tensor([0.18175, 0.50986, 0.28022, 0.02817]))
+        self.a_pow = nn.Parameter(a_pow, requires_grad=trainable)
+        self.a_div = nn.Parameter(a_div, requires_grad=trainable)
+        self.coefficients = nn.Parameter(coefficients, requires_grad=trainable)
+        self.exponents = nn.Parameter(exponents, requires_grad=trainable)
+        self._host = _HostScalars()
+
+    @ops.on_tensor_device
+    def forward(self, inputs: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        if snn.use_training_path(self):
+            from .. import functional_torch as T
+
+            return T.zbl_repulsion(self, inputs)
+        rc = _cosine_cutoff_radius(self.cutoff_fn, "ZBLRepulsionEnergy")
+        (ke,) = self._host.get(self.ke)
+        Z = inputs[properties.Z]
+        Z = (Z if Z.dtype == torch.int64 else Z.long()).contiguous()
+        idx_m, n_sys, sys_ptr = _systems(inputs, "ZBLRepulsionEnergy")
+        r_ij, idx_i, idx_j, graph = _edges(inputs, properties.Rij, properties.idx_i, properties.idx_j, Z.shape[0])
+        params, keep = ops.pair_params(ops.PAIR_ZBL, ke, cutoff=rc, d_max=_short_range_d_max(inputs),
+                                       zbl=(self.a_pow, self.a_div, self.coefficients, self.exponents))
+        holder = dict(params=params, keep=keep, idx_i=idx_i, idx_j=idx_j, Z=Z, idx_m=idx_m, graph=graph,
+                      sys_ptr=sys_ptr, n_sys=n_sys)
+        inputs[self.output_key] = K.PairEnergyFunction.apply(r_ij, None, holder)
+        return inputs
+
+
+class CoulombPotential(nn.Module):
+    """electrostatic.py:14-23: 1 / d."""
+
+    def forward(self, d_ij: torch.Tensor) -> torch.Tensor:
+        return 1.0 / d_ij
+
+
+class DampedCoulombPotential(nn.Module):
+    """electrostatic.py:26-57: f_sw / sqrt(d^2 + 1) + (1 - f_sw) / d with ``switch_fn`` a ``SwitchFunction``."""
+
+    def __init__(self, switch_fn: nn.Module):
+        super().__init__()
+        self.switch_fn = switch_fn
+
+    def forward(self, d_ij: torch.Tensor) -> torch.Tensor:
+        potential = 1.0 / d_ij
+        damped = 1.0 / torch.sqrt(d_ij ** 2 + 1)
+        f_switch = self.switch_fn(d_ij)
+        return f_switch * damped + (1 - f_switch) * potential
+
+
+class EnergyCoulomb(nn.Module):
+    """electrostatic.py:60-152: Coulomb energy of the charges under ``charges_key`` by direct summation over the
+    long-range (``use_neighbors_lr``) or the standard neighbour list, shifted to zero at ``cutoff`` when given.  The
+    potential is ``CoulombPotential`` or ``DampedCoulombPotential`` with a ``SwitchFunction``."""
+
+    def __init__(self, energy_unit: Union[str, float], position_unit: Union[str, float], coulomb_potential: nn.Module,
+                 output_key: str, charges_key: str = properties.partial_charges, use_neighbors_lr: bool = True,
+                 cutoff: Optional[float] = None):
+        super().__init__()
+        ke = convert_units("Ha", energy_unit) * convert_units("Bohr", position_unit)
+        self.register_buffer("ke", torch.Tensor([ke]))
+        self.coulomb_potential = coulomb_potential
+        self.charges_key = charges_key
+        self.output_key = output_key
+        self.model_outputs = [output_key]
+        self.use_neighbors_lr = use_neighbors_lr
+        if cutoff is not None:
+            cutoff = torch.tensor(cutoff)
+            shift = self.coulomb_potential(cutoff).detach()
+            self.register_buffer("cutoff", cutoff)
+            self.register_buffer("shift", shift)
+        else:
+            self.cutoff = None
+            self.shift = None
+        self._host = _HostScalars()
+
+    def _kind(self):
+        name = type(self.coulomb_potential).__name__
+        if name == "CoulombPotential":
+            return ops.PAIR_COULOMB, None
+        if name == "DampedCoulombPotential":
+            sw = self.coulomb_potential.switch_fn
+            if type(sw).__name__ != "SwitchFunction":
+                raise NotImplementedError(f"EnergyCoulomb: switch {type(sw).__name__} has no CUDA kernel")
+            return ops.PAIR_DAMPED_COULOMB, sw
+        raise NotImplementedError(f"EnergyCoulomb: potential {name} has no CUDA kernel "
+                                  "(CoulombPotential, DampedCoulombPotential)")
+
+    @ops.on_tensor_device
+    def forward(self, inputs: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        if self.training and torch.is_grad_enabled():      # no parameters: the charges carry the training graph
+            from .. import functional_torch as T
+
+            return T.energy_coulomb(self, inputs)
+        kind, sw = self._kind()
+        ke, rc, shift, s_on, s_off = self._host.get(self.ke, self.cutoff, self.shift,
+                                                    sw.switch_on if sw is not None else None,
+                                                    sw.switch_off if sw is not None else None)
+        q = inputs[self.charges_key].reshape(-1)
+        if q.dtype != torch.float32:
+            raise TypeError("EnergyCoulomb: the charges must be float32 on the kernel path")
+        idx_m, n_sys, sys_ptr = _systems(inputs, "EnergyCoulomb")
+        if self.use_neighbors_lr:
+            r_ij, idx_i, idx_j, graph = _edges(inputs, properties.Rij_lr, properties.idx_i_lr, properties.idx_j_lr,
+                                               q.shape[0])
+            d_max = None
+        else:
+            r_ij, idx_i, idx_j, graph = _edges(inputs, properties.Rij, properties.idx_i, properties.idx_j, q.shape[0])
+            d_max = _short_range_d_max(inputs)
+        params, keep = ops.pair_params(kind, ke, cutoff=rc, shift=shift or 0.0, switch_on=s_on or 0.0,
+                                       switch_off=s_off or 0.0, d_max=d_max)
+        holder = dict(params=params, keep=keep, idx_i=idx_i, idx_j=idx_j, idx_m=idx_m, graph=graph, sys_ptr=sys_ptr,
+                      n_sys=n_sys)
+        inputs[self.output_key] = K.PairEnergyFunction.apply(r_ij, q, holder)
+        return inputs
+
+
+class Aggregation(nn.Module):
+    """aggregation.py: the sum of several per-system outputs."""
+
+    def __init__(self, keys: List[str], output_key: str = "y"):
+        super().__init__()
+        self.keys: List[str] = list(keys)
+        self.output_key = output_key
+        self.model_outputs = [output_key]
+
+    def forward(self, inputs: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        inputs[self.output_key] = torch.stack([inputs[key] for key in self.keys]).sum(0)
+        return inputs
+
+
+class FilterShortRange(nn.Module):
+    """distances.py:29-57 without the compaction.  The long-range keys (``_Rij_lr``, ``_idx_i_lr``, ``_idx_j_lr``) alias
+    the full list (no copy); the short-range keys keep the full list too, and ``short_range_cutoff`` is recorded in the
+    batch (``properties.short_range_cutoff``).  Pair terms that read the short list apply it as a distance mask
+    d <= short_range_cutoff, and the representation gives exactly zero for edges beyond its own cutoff, which
+    ``NeuralNetworkPotential`` checks is at most ``short_range_cutoff``.  So the result is the reference's, without a
+    host sync or a data-dependent shape; the price is that the representation iterates over the long-range edges too.
+
+    ``train()`` under grad mode: the reference's exact compaction (``torch.nonzero``)."""
+
+    def __init__(self, short_range_cutoff: float):
+        super().__init__()
+        self.short_range_cutoff = short_range_cutoff
+
+    def forward(self, inputs: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        if self.training and torch.is_grad_enabled():
+            from .. import functional_torch as T
+
+            return T.filter_short_range(self, inputs)
+        inputs[properties.Rij_lr] = inputs[properties.Rij]
+        inputs[properties.idx_i_lr] = inputs[properties.idx_i]
+        inputs[properties.idx_j_lr] = inputs[properties.idx_j]
+        inputs[properties.short_range_cutoff] = torch.tensor(float(self.short_range_cutoff), dtype=torch.float64)
+        return inputs
+
+
+def _representation_cutoff(rep) -> Optional[float]:
+    cf = getattr(rep, "cutoff_fn", None)
+    if cf is None:
+        return None
+    return cf.value() if isinstance(cf, snn.CosineCutoff) else float(cf.cutoff)
+
+
+def check_short_range_cutoff(representation: nn.Module, input_modules) -> None:
+    """A ``FilterShortRange`` keeps the full list under the short-range keys; that is exact only when the
+    representation's own cutoff removes every edge beyond ``short_range_cutoff``."""
+    rc = _representation_cutoff(representation)
+    for m in input_modules:
+        if type(m).__name__ == "FilterShortRange" and rc is not None and rc > float(m.short_range_cutoff):
+            raise ValueError(f"FilterShortRange: the representation's cutoff ({rc}) exceeds short_range_cutoff "
+                             f"({m.short_range_cutoff}); the short-range list keeps every edge, so the representation "
+                             "would see pairs the reference filters out")
+
+
+def check_padded_pair_terms(model: nn.Module, list_cutoff: float, who: str) -> None:
+    """The padded fixed-capacity neighbour list of the device drivers puts inert self pairs at distance 2 list_cutoff.
+    They are inert only for terms that vanish beyond a cutoff no larger than the list's."""
+    for m in model.modules():
+        name = type(m).__name__
+        if name == "ZBLRepulsionEnergy":
+            rc = _cosine_cutoff_radius(m.cutoff_fn, who) if m.cutoff_fn is not None else None
+            if rc is None:
+                raise ValueError(f"{who}: ZBLRepulsionEnergy without cutoff_fn would add the padding pairs of the "
+                                 "fixed-capacity neighbour list; give it a CosineCutoff")
+            if rc > list_cutoff:
+                raise ValueError(f"{who}: ZBLRepulsionEnergy cutoff {rc} exceeds the neighbour-list cutoff {list_cutoff}")
+        elif name == "EnergyCoulomb":
+            if m.cutoff is None:
+                raise ValueError(f"{who}: EnergyCoulomb without a cutoff would add the padding pairs of the "
+                                 "fixed-capacity neighbour list; give it a cutoff")
+            rc = float(m.cutoff)
+            if rc > list_cutoff:
+                raise ValueError(f"{who}: EnergyCoulomb cutoff {rc} exceeds the neighbour-list cutoff {list_cutoff}")
+
+
+def link_charges(output_modules) -> None:
+    """Make the charges of a ``DipoleMoment`` differentiable when an ``EnergyCoulomb`` of the same model reads them (the
+    kernel head returns plain charges otherwise, so models that only output charges are unchanged)."""
+    keys = {m.charges_key for m in output_modules if type(m).__name__ == "EnergyCoulomb"}
+    for m in output_modules:
+        if hasattr(m, "differentiable_charges") and m.return_charges and m.charges_key in keys:
+            m.differentiable_charges = True

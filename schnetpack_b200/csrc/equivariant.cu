@@ -361,8 +361,9 @@ __device__ __forceinline__ void head_atom_grad(int mode, const float* __restrict
 template <int MODE>
 __global__ void __launch_bounds__(HT_THREADS) k_head_tail_bwd(
     const float* __restrict__ s, const float* __restrict__ V, const float* __restrict__ R,
-    const int64_t* __restrict__ idx_m, const double* __restrict__ saved, const float* __restrict__ g_out, int correct,
-    int magnitude, int64_t n_atoms, TailW w, float* __restrict__ g_s, float* __restrict__ g_V, float* __restrict__ g_R) {
+    const int64_t* __restrict__ idx_m, const double* __restrict__ saved, const float* __restrict__ g_out,
+    const float* __restrict__ g_qx, int correct, int magnitude, int64_t n_atoms, TailW w, float* __restrict__ g_s,
+    float* __restrict__ g_V, float* __restrict__ g_R) {
     __shared__ TailSmem sm;
     __shared__ float go[HT_AB][2];
     __shared__ float gvm[HT_AB][6];
@@ -381,6 +382,7 @@ __global__ void __launch_bounds__(HT_THREADS) k_head_tail_bwd(
             const float nu[3] = {sm.o[r][1] * sm.vm[r][3], sm.o[r][1] * sm.vm[r][4], sm.o[r][1] * sm.vm[r][5]};
             head_atom_grad(MODE, g_out + m * no, saved + m * HT_SAVED, correct, magnitude, sm.o[r][0], nu, R + 3 * a, gq,
                            gnu, gR);
+            if (g_qx) gq += g_qx[a];     // gradient of the charges output (spk_head_bwd_q)
             for (int d = 0; d < 3; ++d) g_R[3 * a + d] = gR[d];
         }
         // nu = o1 * vm1  ->  g_o1 = g_nu . vm1,  g_vm1 = g_nu * o1
@@ -434,8 +436,9 @@ __global__ void __launch_bounds__(HT_THREADS) k_head_tail_bwd(
 // reverse of the scalar-charge assembly: g_hid = g_q (x) w1 (the last Dense H -> 1) and g_R, thread per (atom, hidden unit)
 __global__ void k_head_scalar_bwd(const float* __restrict__ q, const float* __restrict__ R,
                                   const int64_t* __restrict__ idx_m, const double* __restrict__ saved,
-                                  const float* __restrict__ g_out, int correct, int magnitude, const float* __restrict__ w1,
-                                  int64_t n_atoms, int H, float* __restrict__ g_hid, float* __restrict__ g_R) {
+                                  const float* __restrict__ g_out, const float* __restrict__ g_qx, int correct,
+                                  int magnitude, const float* __restrict__ w1, int64_t n_atoms, int H,
+                                  float* __restrict__ g_hid, float* __restrict__ g_R) {
     SPK_PDL_ENTER();
     const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (t >= n_atoms * H) return;
@@ -446,9 +449,52 @@ __global__ void k_head_scalar_bwd(const float* __restrict__ q, const float* __re
     const float zero[3] = {0.f, 0.f, 0.f};
     head_atom_grad(HEAD_DIPOLE, g_out + m * (magnitude ? 1 : 3), saved + m * HT_SAVED, correct, magnitude, q[a], zero,
                    R + 3 * a, gq, gnu, gR);
+    if (g_qx) gq += g_qx[a];             // gradient of the charges output (spk_head_scalar_bwd_q)
     g_hid[t] = gq * w1[j];
     if (j == 0)
         for (int d = 0; d < 3; ++d) g_R[3 * a + d] = gR[d];
+}
+
+// Reverse of the charge correction q' = q + (Q_m - sum_m q) / n_m: g_q = g_q' - mean_m(g_q').  The per-system sums of g_q'
+// run through the segmented-partial pass of segscan.cuh (CTAs of HC_T atoms), so they are bitwise reproducible.
+constexpr int HC_T = 256;
+
+__global__ void __launch_bounds__(HC_T) k_charges_bwd_partials(const float* __restrict__ g_c,
+                                                               const int64_t* __restrict__ idx_m,
+                                                               const int32_t* __restrict__ sys_ptr, int64_t n_atoms,
+                                                               double* __restrict__ sys_part, double* __restrict__ head) {
+    SPK_PDL_ENTER();
+    const int64_t a = (int64_t)blockIdx.x * HC_T + threadIdx.x;
+    double v[1] = {0.0};
+    int64_t m = 0, first = 0, end = 0;
+    if (a < n_atoms) {
+        v[0] = g_c[a];
+        m = idx_m[a];
+        first = sys_ptr[m];
+        end = sys_ptr[m + 1];
+    }
+    seg_partials<HC_T, 1>(v, n_atoms, m, first, end, sys_part, head);
+}
+
+__global__ void __launch_bounds__(SEG_FIN_T) k_charges_bwd_mean(const int32_t* __restrict__ sys_ptr,
+                                                                const double* __restrict__ sys_part,
+                                                                const double* __restrict__ head,
+                                                                double* __restrict__ mean) {
+    __shared__ double red[1][SEG_FIN_T];
+    SPK_PDL_ENTER();
+    const int64_t m = blockIdx.x;
+    seg_finish_block<HC_T, 1>(sys_ptr, nullptr, sys_part, head, m, red);
+    if (threadIdx.x != 0) return;
+    const int64_t n = sys_ptr[m + 1] - sys_ptr[m];
+    mean[m] = n > 0 ? red[0][0] / (double)n : 0.0;
+}
+
+__global__ void k_charges_bwd_apply(const float* __restrict__ g_c, const int64_t* __restrict__ idx_m,
+                                    const double* __restrict__ mean, int64_t n_atoms, float* __restrict__ g_q) {
+    SPK_PDL_ENTER();
+    const int64_t a = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (a >= n_atoms) return;
+    g_q[a] = mean ? (float)((double)g_c[a] - mean[idx_m[a]]) : g_c[a];
 }
 
 }  // namespace
@@ -582,11 +628,11 @@ extern "C" int spk_head_bwd(int kind, const spk_head_tail_t* tail, const float* 
     const TailW w = tail_of(tail);
     const unsigned nb = (unsigned)spk_cdiv(n_atoms, HT_AB);
     if (kind == SPK_HEAD_DIPOLE)
-        spk_launch(k_head_tail_bwd<HEAD_DIPOLE>, nb, HT_THREADS, 0, spk_st(stream), s, V, R, idx_m, saved, g_out, correct,
-                   magnitude, n_atoms, w, g_s, g_V, g_R);
+        spk_launch(k_head_tail_bwd<HEAD_DIPOLE>, nb, HT_THREADS, 0, spk_st(stream), s, V, R, idx_m, saved, g_out,
+                   (const float*)nullptr, correct, magnitude, n_atoms, w, g_s, g_V, g_R);
     else
-        spk_launch(k_head_tail_bwd<HEAD_POLAR>, nb, HT_THREADS, 0, spk_st(stream), s, V, R, idx_m, saved, g_out, correct,
-                   magnitude, n_atoms, w, g_s, g_V, g_R);
+        spk_launch(k_head_tail_bwd<HEAD_POLAR>, nb, HT_THREADS, 0, spk_st(stream), s, V, R, idx_m, saved, g_out,
+                   (const float*)nullptr, correct, magnitude, n_atoms, w, g_s, g_V, g_R);
     SPK_LAUNCH_CHECK();
     return SPK_OK;
 }
@@ -597,8 +643,65 @@ extern "C" int spk_head_scalar_bwd(const float* q, const float* R, const int64_t
     if (n_atoms < 0 || H <= 0) return SPK_ERR_ARG;
     if (n_atoms == 0) return SPK_OK;
     if (!q || !R || !idx_m || !saved || !g_out || !w1 || !g_hid || !g_R) return SPK_ERR_ARG;
-    spk_launch(k_head_scalar_bwd, GRID1D(n_atoms * H, 256), q, R, idx_m, saved, g_out, correct, magnitude, w1, n_atoms,
-               H, g_hid, g_R);
+    spk_launch(k_head_scalar_bwd, GRID1D(n_atoms * H, 256), q, R, idx_m, saved, g_out, (const float*)nullptr, correct,
+               magnitude, w1, n_atoms, H, g_hid, g_R);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" size_t spk_head_charges_bwd_workspace_bytes(int64_t n_atoms, int64_t n_sys) {
+    const int64_t nb = n_atoms > 0 ? spk_cdiv(n_atoms, HC_T) : 0;
+    const int64_t B = n_sys > 0 ? n_sys : 0;
+    return sizeof(double) * (size_t)(2 * B + nb + 1);
+}
+
+extern "C" int spk_head_charges_bwd(const float* g_charges, const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms,
+                                    int64_t n_sys, int correct, float* g_q, void* workspace, size_t workspace_bytes,
+                                    spk_stream_t stream) {
+    if (n_atoms < 0 || n_sys < 0 || n_atoms >= (1ll << 31) - 1) return SPK_ERR_ARG;
+    if (n_atoms == 0) return SPK_OK;
+    if (!g_charges || !idx_m || !g_q) return SPK_ERR_ARG;
+    const cudaStream_t st = spk_st(stream);
+    double* mean = nullptr;
+    if (correct && n_sys > 0) {
+        if (!sys_ptr || !workspace || workspace_bytes < spk_head_charges_bwd_workspace_bytes(n_atoms, n_sys))
+            return SPK_ERR_ARG;
+        mean = reinterpret_cast<double*>(workspace);
+        double* sys_part = mean + n_sys;
+        double* head = sys_part + n_sys;
+        spk_launch(k_charges_bwd_partials, (unsigned)spk_cdiv(n_atoms, HC_T), HC_T, 0, st, g_charges, idx_m, sys_ptr,
+                   n_atoms, sys_part, head);
+        spk_launch(k_charges_bwd_mean, (unsigned)n_sys, SEG_FIN_T, 0, st, sys_ptr, (const double*)sys_part,
+                   (const double*)head, mean);
+    }
+    spk_launch(k_charges_bwd_apply, GRID1D(n_atoms, 256), g_charges, idx_m, (const double*)mean, n_atoms, g_q);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_head_bwd_q(int kind, const spk_head_tail_t* tail, const float* s, const float* V, const float* R,
+                              const int64_t* idx_m, const double* saved, const float* g_out, const float* g_q,
+                              int64_t n_atoms, int correct, int magnitude, float* g_s, float* g_V, float* g_R,
+                              spk_stream_t stream) {
+    if (n_atoms < 0 || kind != SPK_HEAD_DIPOLE) return SPK_ERR_ARG;
+    if (n_atoms == 0) return SPK_OK;
+    const int rc = check_tail(tail);
+    if (rc != SPK_OK) return rc;
+    if (!s || !V || !R || !idx_m || !saved || !g_out || !g_q || !g_s || !g_V || !g_R) return SPK_ERR_ARG;
+    spk_launch(k_head_tail_bwd<HEAD_DIPOLE>, (unsigned)spk_cdiv(n_atoms, HT_AB), HT_THREADS, 0, spk_st(stream), s, V, R,
+               idx_m, saved, g_out, g_q, correct, magnitude, n_atoms, tail_of(tail), g_s, g_V, g_R);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_head_scalar_bwd_q(const float* q, const float* R, const int64_t* idx_m, const double* saved,
+                                     const float* g_out, const float* g_q, int correct, int magnitude, const float* w1,
+                                     int64_t n_atoms, int H, float* g_hid, float* g_R, spk_stream_t stream) {
+    if (n_atoms < 0 || H <= 0) return SPK_ERR_ARG;
+    if (n_atoms == 0) return SPK_OK;
+    if (!q || !R || !idx_m || !saved || !g_out || !g_q || !w1 || !g_hid || !g_R) return SPK_ERR_ARG;
+    spk_launch(k_head_scalar_bwd, GRID1D(n_atoms * H, 256), q, R, idx_m, saved, g_out, g_q, correct, magnitude, w1,
+               n_atoms, H, g_hid, g_R);
     SPK_LAUNCH_CHECK();
     return SPK_OK;
 }

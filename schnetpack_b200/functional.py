@@ -639,9 +639,24 @@ class HeadPack(ParamPack):
             self.tail = None
 
 
+def _charges_grad(h, g_charges):
+    """dE/dq of the tail's charges from dE/dcharges (the correction's reverse), or None when no charge gradient arrives."""
+    if g_charges is None or not h.get("diff_charges") or g_charges.numel() == 0:
+        return None
+    return ops.head_charges_bwd(g_charges.contiguous(), h["idx_m"], h["sys_ptr"], h["n_sys"], h["correct"])
+
+
+def _dipole_grad_out(h, g_out, like):
+    if g_out is not None:
+        return g_out.contiguous()
+    shape = (h["n_sys"],) if h["magnitude"] else (h["n_sys"], 3)
+    return torch.zeros(shape, dtype=torch.float32, device=like.device)
+
+
 class GatedHeadFunction(torch.autograd.Function):
-    """(s [N,Fi], V [N,3,Fi], R [N,3]) -> (dipole [B,3] / |dipole| [B] / polarizability [B,3,3], charges [N]).  The
-    charges output is not differentiable; the head output is, with respect to s, V and R."""
+    """(s [N,Fi], V [N,3,Fi], R [N,3]) -> (dipole [B,3] / |dipole| [B] / polarizability [B,3,3], charges [N]).  The head
+    output is differentiable with respect to s, V and R, the charges too when ``holder["diff_charges"]`` is set; a charge
+    gradient takes the ``spk_head_bwd_q`` reverse, without one the reverse is exactly ``spk_head_bwd``."""
 
     @staticmethod
     def forward(ctx, s, V, R, holder):
@@ -663,20 +678,26 @@ class GatedHeadFunction(torch.autograd.Function):
                                               holder["magnitude"], holder["want_charges"])
             charges = ops.head_charges(q_atom, holder["idx_m"], saved) if q_atom is not None else s.new_zeros((0,))
         ctx.holder = dict(holder, tape=tape, s=s, V=V, R=Rd, saved=saved)
-        ctx.mark_non_differentiable(charges)
+        if not holder.get("diff_charges"):
+            ctx.mark_non_differentiable(charges)
         ctx.set_materialize_grads(False)
         return out, charges
 
     @staticmethod
     @torch.autograd.function.once_differentiable
-    def backward(ctx, g_out, _g_charges):
+    def backward(ctx, g_out, g_charges):
         h = ctx.holder
-        if g_out is None:
+        g_q = _charges_grad(h, g_charges)
+        if g_out is None and g_q is None:
             return None, None, None, None
         pk = h["pack"]
-        with ops.device_of(g_out):
-            g_s, g_V, g_R = ops.head_bwd(h["kind"], pk.tail, h["s"], h["V"], h["R"], h["idx_m"], h["saved"],
-                                         g_out.contiguous(), h["correct"], h["magnitude"])
+        with ops.device_of(h["s"]):
+            if g_q is None:
+                g_s, g_V, g_R = ops.head_bwd(h["kind"], pk.tail, h["s"], h["V"], h["R"], h["idx_m"], h["saved"],
+                                             g_out.contiguous(), h["correct"], h["magnitude"])
+            else:
+                g_s, g_V, g_R = ops.head_bwd_q(pk.tail, h["s"], h["V"], h["R"], h["idx_m"], h["saved"],
+                                               _dipole_grad_out(h, g_out, g_q), g_q, h["correct"], h["magnitude"])
             N = g_s.shape[0]
             for b, (VW, d0, x) in zip(reversed(pk.blocks), reversed(h["tape"])):
                 Fi, Fo = b["Fi"], b["Fo"]
@@ -690,7 +711,7 @@ class GatedHeadFunction(torch.autograd.Function):
 
 class ScalarDipoleFunction(torch.autograd.Function):
     """(s [N,F], R [N,3]) -> (dipole [B,3] / |dipole| [B], charges [N]) for charges from a plain MLP (Lin layers, then
-    ``spk_atomwise_out`` without aggregation for the last Dense H -> 1)."""
+    ``spk_atomwise_out`` without aggregation for the last Dense H -> 1).  Differentiable as ``GatedHeadFunction``."""
 
     @staticmethod
     def forward(ctx, s, R, holder):
@@ -707,20 +728,57 @@ class ScalarDipoleFunction(torch.autograd.Function):
                                          holder["magnitude"], False)
             charges = ops.head_charges(q, holder["idx_m"], saved) if holder["want_charges"] else q.new_zeros((0,))
         ctx.holder = dict(holder, tape=tape, q=q, R=Rd, saved=saved)
-        ctx.mark_non_differentiable(charges)
+        if not holder.get("diff_charges"):
+            ctx.mark_non_differentiable(charges)
         ctx.set_materialize_grads(False)
         return out, charges
 
     @staticmethod
     @torch.autograd.function.once_differentiable
-    def backward(ctx, g_out, _g_charges):
+    def backward(ctx, g_out, g_charges):
         h = ctx.holder
-        if g_out is None:
+        g_q = _charges_grad(h, g_charges)
+        if g_out is None and g_q is None:
             return None, None, None
         pk = h["pack"]
-        with ops.device_of(g_out):
-            g_h, g_R = ops.head_scalar_bwd(h["q"], h["R"], h["idx_m"], h["saved"], g_out.contiguous(), h["correct"],
-                                           h["magnitude"], pk.w1)
+        with ops.device_of(h["q"]):
+            if g_q is None:
+                g_h, g_R = ops.head_scalar_bwd(h["q"], h["R"], h["idx_m"], h["saved"], g_out.contiguous(), h["correct"],
+                                               h["magnitude"], pk.w1)
+            else:
+                g_h, g_R = ops.head_scalar_bwd_q(h["q"], h["R"], h["idx_m"], h["saved"], _dipole_grad_out(h, g_out, g_q),
+                                                 g_q, h["correct"], h["magnitude"], pk.w1)
             for b, d in zip(reversed(pk.blocks), reversed(h["tape"])):
                 g_h = b["lin"].bwd(g_h, a_pre=d, a_act=ops.ACT_GIVEN)
         return g_h, g_R, None
+
+
+# =====================================================================================================================
+# Pair energies: ZBL repulsion (atomistic/nuclear_repulsion.py:70-108) and Coulomb (atomistic/electrostatic.py:109-152)
+# =====================================================================================================================
+class PairEnergyFunction(torch.autograd.Function):
+    """(r_ij [E,3], q [N] | None) -> energy [B] of one pair term on csrc/pair_energy.cu; backward gives dE/dr_ij and, for
+    Coulomb, dE/dq (which reaches the charge head through its differentiable charges output)."""
+
+    @staticmethod
+    def forward(ctx, r_ij, q, holder):
+        rd = r_ij.detach().contiguous()
+        qd = q.detach().contiguous() if q is not None else None
+        with ops.device_of(rd, qd):
+            e = ops.pair_energy_fwd(holder["params"], rd, holder["idx_i"], holder["idx_j"], holder.get("Z"), qd,
+                                    holder["idx_m"], holder["graph"], holder["sys_ptr"], holder["n_sys"])
+        ctx.h = (holder, rd, qd)
+        ctx.want_q = q is not None and ctx.needs_input_grad[1]
+        ctx.set_materialize_grads(False)
+        return e
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_E):
+        if g_E is None:
+            return None, None, None
+        h, rd, qd = ctx.h
+        with ops.device_of(rd):
+            g_rij, g_q = ops.pair_energy_bwd(h["params"], rd, h["idx_i"], h["idx_j"], h.get("Z"), qd, h["idx_m"],
+                                             g_E.contiguous(), h["graph"], ctx.want_q)
+        return g_rij, g_q, None

@@ -230,3 +230,57 @@ def polarizability(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
     alpha = alpha + mur + mur.transpose(-2, -1)
     inputs[mod.polarizability_key] = scatter_add(alpha, inputs[properties.idx_m], _n_sys(inputs))
     return inputs
+
+
+def _norm(r_ij: Tensor) -> Tensor:
+    return torch.norm(r_ij, dim=1)
+
+
+def zbl_repulsion(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
+    """atomistic/nuclear_repulsion.py:70-108."""
+    z = inputs[properties.Z]
+    d_ij = _norm(inputs[properties.Rij])
+    idx_i, idx_j, idx_m = inputs[properties.idx_i], inputs[properties.idx_j], inputs[properties.idx_m]
+    a = z ** F_.softplus(mod.a_pow)
+    a_ij = (a[idx_i] + a[idx_j]) * F_.softplus(mod.a_div)
+    exponents = a_ij[..., None] * F_.softplus(mod.exponents)[None, ...]
+    coefficients = F_.normalize(F_.softplus(mod.coefficients)[None, ...], p=1.0, dim=1)
+    screening = torch.sum(coefficients * torch.exp(-exponents * d_ij[:, None]), dim=1)
+    repulsion = (z[idx_i] * z[idx_j]) / d_ij
+    if mod.cutoff_fn is not None:
+        repulsion = repulsion * cutoff(mod.cutoff_fn, d_ij)
+    y = scatter_add(repulsion * screening, idx_i, z.shape[0])
+    y = scatter_add(y, idx_m, _n_sys(inputs))
+    inputs[mod.output_key] = 0.5 * mod.ke * y
+    return inputs
+
+
+def energy_coulomb(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
+    """atomistic/electrostatic.py:109-152."""
+    q = inputs[mod.charges_key].squeeze(-1)
+    if mod.use_neighbors_lr:
+        r_ij, idx_i, idx_j = inputs[properties.Rij_lr], inputs[properties.idx_i_lr], inputs[properties.idx_j_lr]
+    else:
+        r_ij, idx_i, idx_j = inputs[properties.Rij], inputs[properties.idx_i], inputs[properties.idx_j]
+    d_ij = _norm(r_ij)
+    potential = mod.coulomb_potential(d_ij)
+    if mod.cutoff is not None:
+        potential = potential + mod.shift ** 2 / potential - 2.0 * mod.shift
+        potential = torch.where(d_ij <= mod.cutoff, potential, torch.zeros_like(potential))
+    y = scatter_add(q[idx_i] * q[idx_j] * potential, idx_i, q.shape[0])
+    y = scatter_add(y, inputs[properties.idx_m], _n_sys(inputs))
+    inputs[mod.output_key] = 0.5 * mod.ke * torch.squeeze(y, -1)
+    return inputs
+
+
+def filter_short_range(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
+    """atomistic/distances.py:42-57 (exact compaction; a host sync and a data-dependent shape)."""
+    idx_i, idx_j, Rij = inputs[properties.idx_i], inputs[properties.idx_j], inputs[properties.Rij]
+    cidx = torch.nonzero(_norm(Rij) <= mod.short_range_cutoff).squeeze(-1)
+    inputs[properties.Rij_lr] = Rij
+    inputs[properties.idx_i_lr] = idx_i
+    inputs[properties.idx_j_lr] = idx_j
+    inputs[properties.Rij] = Rij[cidx]
+    inputs[properties.idx_i] = idx_i[cidx]
+    inputs[properties.idx_j] = idx_j[cidx]
+    return inputs

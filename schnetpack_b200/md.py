@@ -949,6 +949,9 @@ class DeviceMD(_CapturedEvaluation):
             raise ValueError("DeviceMD: the NHC barostats contain their own thermostat (temperature_control = True); "
                              "pass either a thermostat or a barostat")
         self._check_ring_polymer(ring_polymer, thermostat, barostat, compute_stress)
+        from .atomistic.pair_terms import check_padded_pair_terms
+
+        check_padded_pair_terms(model, float(cutoff), "DeviceMD")
         self.ring_polymer = ring_polymer
         self.model = model
         self.dt = float(time_step)

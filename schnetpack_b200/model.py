@@ -75,6 +75,8 @@ class NeuralNetworkPotential(AtomisticModel):
         self.representation = representation
         self.input_modules = nn.ModuleList(input_modules)
         self.output_modules = nn.ModuleList(output_modules)
+        atomistic.pair_terms.check_short_range_cutoff(representation, self.input_modules)
+        atomistic.pair_terms.link_charges(self.output_modules)
         self.collect_derivatives()
         self.collect_outputs()
 
@@ -182,14 +184,54 @@ def _convert_head(m):
     return new
 
 
+def _convert_cutoff_fn(cf):
+    if cf is None:
+        return None
+    if type(cf).__name__ != "CosineCutoff":
+        raise NotImplementedError(f"cutoff {type(cf).__name__} of a pair term has no CUDA kernel")
+    return snn.CosineCutoff(float(cf.cutoff))
+
+
+def _convert_pair_term(m):
+    """ZBLRepulsionEnergy / EnergyCoulomb (with its potential and switch) -> the kernel modules, state_dict copied."""
+    if type(m).__name__ == "ZBLRepulsionEnergy":
+        new = atomistic.ZBLRepulsionEnergy(1.0, 1.0, m.output_key, cutoff_fn=_convert_cutoff_fn(m.cutoff_fn))
+        for name in ("a_pow", "a_div", "coefficients", "exponents"):
+            getattr(new, name).requires_grad_(getattr(m, name).requires_grad)
+    else:
+        pot = m.coulomb_potential
+        pn = type(pot).__name__
+        if pn == "CoulombPotential":
+            new_pot = atomistic.CoulombPotential()
+        elif pn == "DampedCoulombPotential" and type(pot.switch_fn).__name__ == "SwitchFunction":
+            new_pot = atomistic.DampedCoulombPotential(snn.SwitchFunction(float(pot.switch_fn.switch_on),
+                                                                          float(pot.switch_fn.switch_off)))
+        else:
+            raise NotImplementedError(f"EnergyCoulomb potential {pn} has no CUDA kernel")
+        new = atomistic.EnergyCoulomb(1.0, 1.0, new_pot, m.output_key, charges_key=m.charges_key,
+                                      use_neighbors_lr=m.use_neighbors_lr,
+                                      cutoff=float(m.cutoff) if m.cutoff is not None else None)
+    new.load_state_dict(m.state_dict())
+    return new
+
+
 def convert_model(model: nn.Module) -> NeuralNetworkPotential:
     """Build a CUDA ``NeuralNetworkPotential`` from a loaded reference model (duck-typed on class names; weights are
     copied through ``state_dict`` whose keys are identical).  ``Atomwise`` (n_out=1, n_layers=2), ``Forces``,
-    ``DipoleMoment`` and ``Polarizability`` heads are swapped for the CUDA modules; modules outside the hot path
-    (postprocessors, custom embeddings, other output heads) are reused as they are."""
+    ``DipoleMoment`` and ``Polarizability`` heads, the pair terms ``ZBLRepulsionEnergy`` (cutoff_fn None or CosineCutoff)
+    and ``EnergyCoulomb`` (CoulombPotential or DampedCoulombPotential with a SwitchFunction), ``Aggregation`` and the
+    input modules ``PairwiseDistances`` / ``FilterShortRange`` are swapped for the CUDA modules.  Passed through as they
+    are: postprocessors, custom embeddings and every other module (``EnergyEwald``, other output heads); a passed-through
+    module that reads the number of systems from ``idx_m`` keeps its host read."""
     in_mods = []
     for m in model.input_modules:
-        in_mods.append(atomistic.PairwiseDistances() if type(m).__name__ == "PairwiseDistances" else m)
+        n = type(m).__name__
+        if n == "PairwiseDistances":
+            in_mods.append(atomistic.PairwiseDistances())
+        elif n == "FilterShortRange":
+            in_mods.append(atomistic.FilterShortRange(float(m.short_range_cutoff)))
+        else:
+            in_mods.append(m)
     out_mods = []
     for m in model.output_modules:
         n = type(m).__name__
@@ -204,6 +246,10 @@ def convert_model(model: nn.Module) -> NeuralNetworkPotential:
             out_mods.append(atomistic.Forces(m.calc_forces, m.calc_stress, m.energy_key, m.force_key, m.stress_key))
         elif n in ("DipoleMoment", "Polarizability"):
             out_mods.append(_convert_head(m))
+        elif n in ("ZBLRepulsionEnergy", "EnergyCoulomb"):
+            out_mods.append(_convert_pair_term(m))
+        elif n == "Aggregation":
+            out_mods.append(atomistic.Aggregation(list(m.keys), m.output_key))
         else:
             out_mods.append(m)
     new = NeuralNetworkPotential(_convert_representation(model.representation), in_mods, out_mods,

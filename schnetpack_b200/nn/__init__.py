@@ -19,7 +19,7 @@ from .. import ops
 
 __all__ = ["GaussianRBF", "BesselRBF", "CosineCutoff", "cosine_cutoff", "gaussian_rbf", "Dense", "shifted_softplus",
            "scatter_add", "build_mlp", "replicate_module", "activation_code", "use_training_path", "GatedEquivariantBlock",
-           "build_gated_equivariant_mlp"]
+           "build_gated_equivariant_mlp", "SwitchFunction"]
 
 
 def use_training_path(module: nn.Module) -> bool:
@@ -162,6 +162,30 @@ class CosineCutoff(nn.Module):
 
     def forward(self, input: torch.Tensor):
         return _CutoffFn.apply(input, self.value())
+
+
+def _switch_component(x: torch.Tensor, ones: torch.Tensor, zeros: torch.Tensor) -> torch.Tensor:
+    """nn/cutoff.py:107-122."""
+    x_ = torch.where(x <= 0, ones, x)
+    return torch.where(x <= 0, zeros, torch.exp(-ones / x_))
+
+
+class SwitchFunction(nn.Module):
+    """nn/cutoff.py:125-158 -- decays from 1 to 0 between ``switch_on`` and ``switch_off`` (buffers of shape [1]).  Plain
+    tensor algebra: the Coulomb kernels of csrc/pair_energy.cu evaluate it in-kernel from the two buffers."""
+
+    def __init__(self, switch_on: float, switch_off: float):
+        super().__init__()
+        self.register_buffer("switch_on", torch.Tensor([switch_on]))
+        self.register_buffer("switch_off", torch.Tensor([switch_off]))
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        x = (x - self.switch_on) / (self.switch_off - self.switch_on)
+        ones = torch.ones_like(x)
+        zeros = torch.zeros_like(x)
+        fp = _switch_component(x, ones, zeros)
+        fm = _switch_component(1 - x, ones, zeros)
+        return torch.where(x <= 0, ones, torch.where(x >= 1, zeros, fm / (fp + fm)))
 
 
 # ------------------------------------------------------------------------------------------------- dense / mlp

@@ -723,3 +723,92 @@ def head_scalar_bwd(q: Tensor, R: Tensor, idx_m: Tensor, saved: Tensor, g_out: T
     _lib.call("spk_head_scalar_bwd", _p(q), _p(R), _p(idx_m), _p(saved), _p(f32(g_out, "g_out")), int(correct),
               int(magnitude), _p(w1), N, H, _p(g_hid), _p(g_R), _stream())
     return g_hid, g_R
+
+
+def head_charges_bwd(g_charges: Tensor, idx_m: Tensor, sys_ptr: Tensor, n_sys: int, correct: bool) -> Tensor:
+    """Reverse of the charge correction: g_q = g_charges - per-system mean (fp64 sums) with ``correct``."""
+    N = g_charges.shape[0]
+    g_q = torch.empty_like(g_charges)
+    nbytes = int(_lib.lib().spk_head_charges_bwd_workspace_bytes(N, n_sys))
+    ws = torch.empty(max(nbytes, 8), dtype=torch.uint8, device=g_charges.device)
+    _lib.call("spk_head_charges_bwd", _p(f32(g_charges, "g_charges")), _p(idx_m), _p(sys_ptr), N, n_sys, int(correct),
+              _p(g_q), _p(ws), nbytes, _stream(), launches=3 if correct and n_sys > 0 else 1)
+    return g_q
+
+
+def head_bwd_q(tail, s: Tensor, V: Tensor, R: Tensor, idx_m: Tensor, saved: Tensor, g_out: Tensor, g_q: Tensor,
+               correct: bool, magnitude: bool):
+    """``head_bwd`` of the dipole with the charges' own gradient ``g_q`` [N] added."""
+    N, Fi = s.shape
+    dev = s.device
+    g_s = torch.empty((N, Fi), dtype=torch.float32, device=dev)
+    g_V = torch.empty((N, 3, Fi), dtype=torch.float32, device=dev)
+    g_R = torch.empty((N, 3), dtype=torch.float32, device=dev)
+    _lib.call("spk_head_bwd_q", HEAD_DIPOLE, tail, _p(s), _p(V), _p(R), _p(idx_m), _p(saved), _p(f32(g_out, "g_out")),
+              _p(f32(g_q, "g_q")), N, int(correct), int(magnitude), _p(g_s), _p(g_V), _p(g_R), _stream())
+    return g_s, g_V, g_R
+
+
+def head_scalar_bwd_q(q: Tensor, R: Tensor, idx_m: Tensor, saved: Tensor, g_out: Tensor, g_q: Tensor, correct: bool,
+                      magnitude: bool, w1: Tensor):
+    """``head_scalar_bwd`` with the charges' own gradient ``g_q`` [N] added."""
+    N, H = q.shape[0], w1.numel()
+    g_hid = torch.empty((N, H), dtype=torch.float32, device=q.device)
+    g_R = torch.empty((N, 3), dtype=torch.float32, device=q.device)
+    _lib.call("spk_head_scalar_bwd_q", _p(q), _p(R), _p(idx_m), _p(saved), _p(f32(g_out, "g_out")), _p(f32(g_q, "g_q")),
+              int(correct), int(magnitude), _p(w1), N, H, _p(g_hid), _p(g_R), _stream())
+    return g_hid, g_R
+
+
+# ------------------------------------------------------------------------------------------------------------ pair energies
+PAIR_ZBL, PAIR_COULOMB, PAIR_DAMPED_COULOMB = _lib.PAIR_ZBL, _lib.PAIR_COULOMB, _lib.PAIR_DAMPED_COULOMB
+
+
+def pair_params(kind: int, ke: float, cutoff: Optional[float] = None, shift: float = 0.0, switch_on: float = 0.0,
+                switch_off: float = 0.0, d_max: Optional[float] = None, zbl=None):
+    """``spk_pair_t`` for a pair term; ``zbl`` = (a_pow, a_div, coefficients, exponents) device tensors, read by the kernels
+    at every launch (a captured graph sees updated values).  Returns (struct, tensors kept alive)."""
+    st = _lib.PairParams()
+    st.kind = int(kind)
+    keep = []
+    if zbl is not None:
+        keep = [f32(t.detach(), name) for t, name in zip(zbl, ("a_pow", "a_div", "coefficients", "exponents"))]
+        if keep[2].numel() != keep[3].numel() or not 0 < keep[2].numel() <= _lib.PAIR_MAX_TERMS:
+            raise ValueError(f"ZBL: coefficients and exponents must have equal length <= {_lib.PAIR_MAX_TERMS}")
+        st.a_pow, st.a_div, st.coefficients, st.exponents = (t.data_ptr() for t in keep)
+        st.n_terms = int(keep[2].numel())
+    st.ke = float(ke)
+    st.cutoff = float(cutoff) if cutoff is not None else 0.0
+    st.shift = float(shift)
+    st.switch_on, st.switch_off = float(switch_on), float(switch_off)
+    st.d_max = float(d_max) if d_max is not None else 0.0
+    return st, keep
+
+
+def pair_energy_fwd(params, r_ij: Tensor, idx_i: Tensor, idx_j: Tensor, Z: Optional[Tensor], q: Optional[Tensor],
+                    idx_m: Tensor, graph: EdgeGraph, sys_ptr: Tensor, n_sys: int) -> Tensor:
+    """energy [n_sys] = 0.5 ke sum over the edges received by the atoms of each system (fp64, fixed order)."""
+    dev = r_ij.device
+    energy = torch.empty((n_sys,), dtype=torch.float32, device=dev)
+    E = graph.n_edges
+    nbytes = int(_lib.lib().spk_pair_energy_workspace_bytes(E, n_sys))
+    ws = torch.empty(max(nbytes, 8), dtype=torch.uint8, device=dev)
+    _lib.call("spk_pair_energy_fwd", params, _p(f32(r_ij, "_Rij")), _p(i64(idx_i)), _p(i64(idx_j)),
+              _p(i64(Z, "_atomic_numbers")) if Z is not None else None, _p(f32(q, "charges")) if q is not None else None,
+              _p(i64(idx_m, "_idx_m")), _p(graph.rowptr), _p(graph.slot_eid), _p(sys_ptr), E, n_sys, _p(energy), _p(ws),
+              nbytes, _stream(), launches=2 if E > 0 else 1)
+    return energy
+
+
+def pair_energy_bwd(params, r_ij: Tensor, idx_i: Tensor, idx_j: Tensor, Z: Optional[Tensor], q: Optional[Tensor],
+                    idx_m: Tensor, g_E: Tensor, graph: EdgeGraph, want_q: bool):
+    """-> (g_rij [E,3] in edge order, g_q [N] or None)"""
+    dev = r_ij.device
+    E, N = graph.n_edges, graph.n_atoms
+    g_rij = torch.empty((E, 3), dtype=torch.float32, device=dev)
+    g_q = torch.empty((N,), dtype=torch.float32, device=dev) if want_q else None
+    _lib.call("spk_pair_energy_bwd", params, _p(r_ij), _p(idx_i), _p(idx_j), _p(Z), _p(q), _p(idx_m),
+              _p(f32(g_E, "g_E")), _p(graph.rowptr), _p(graph.slot_j), _p(graph.slot_eid), _p(graph.sptr),
+              _p(graph.pos_slot), _p(graph.pos_i), N, E, _p(g_rij), _p(g_q), _stream(),
+              launches=int(E > 0) + int(want_q and N > 0))
+    return g_rij, g_q
