@@ -595,10 +595,13 @@ int spk_head_scalar_bwd_q(const float* q, const float* R, const int64_t* idx_m, 
  *            e = Z_i Z_j / d sum_k c_k exp(-a_ij softplus(exponents_k) d), times the cosine cutoff if cutoff > 0
  *   Coulomb: e = q_i q_j V(d), V = 1/d or (damped) f_sw / sqrt(d^2 + 1) + (1 - f_sw) / d with the switch function of
  *            (switch_on, switch_off); with cutoff > 0, V + shift^2 / V - 2 shift for d <= cutoff and 0 beyond
+ *   Ewald real space (electrostatic.py:266-308): e = q_i q_j erfc(sqrt(alpha) d) / d, times 1 - f_sw(d) when
+ *            switch_off != switch_on (the SwitchFunction screen); no cutoff, so padded lists need d_max
  * The ZBL parameters are read raw from device memory (softplus and normalisation on the device). */
 #define SPK_PAIR_ZBL 0
 #define SPK_PAIR_COULOMB 1
 #define SPK_PAIR_DAMPED_COULOMB 2
+#define SPK_PAIR_EWALD_REAL 3
 #define SPK_PAIR_MAX_TERMS 16
 typedef struct {
     int32_t kind;
@@ -612,6 +615,7 @@ typedef struct {
     double shift;              /* Coulomb with cutoff: V(cutoff) */
     double switch_on, switch_off;
     double d_max;              /* distance mask d <= d_max; <= 0: none */
+    double alpha;              /* Ewald real space: the splitting parameter alpha (the square of the usual one) */
 } spk_pair_t;
 size_t spk_pair_energy_workspace_bytes(int64_t n_edges, int64_t n_sys);
 /* energy [B] = 0.5 ke sum_{e in m} e_ij over the receiver slots [rowptr[sys_ptr[m]], rowptr[sys_ptr[m+1]]), summed in fp64
@@ -628,6 +632,40 @@ int spk_pair_energy_bwd(const spk_pair_t* p, const float* r_ij, const int64_t* i
                         const int32_t* slot_j, const int32_t* slot_eid, const int32_t* sptr, const int32_t* pos_slot,
                         const int32_t* pos_i, int64_t n_atoms, int64_t n_edges, float* g_rij, float* g_q,
                         spk_stream_t stream);
+
+/* ---- Ewald reciprocal and self terms (csrc/ewald.cu; atomistic/electrostatic.py:310-375) ---------------------------
+ * Per system m with cell h [3,3] (rows = lattice vectors; fp32 in, fp64 inside), H = h^-1, V = |det h|, the integer
+ * triples n [K,3] (fp32, the reference's kvecs buffer) and k = 2 pi n H^T:
+ *   E_rec[m]  = ke (2 pi / V) sum_k f_k |S_k|^2,  f_k = exp(-k^2 / (4 alpha)) / k^2,  S_k = sum_{i in m} q_i e^{i k.r_i}
+ *   E_self[m] = ke sqrt(alpha / pi) sum_{i in m} q_i^2
+ *   energy[m] = addend[m] + E_rec[m] - E_self[m]      (addend: the real-space energy, or NULL)
+ * The phases are 2 pi n.s_i with the fractional coordinates s_i = r_i H reduced mod 1 in fp64 (exact for integer n, so
+ * unwrapped positions lose nothing).  Every sum runs in fp64 in a fixed order, without atomics: bitwise reproducible.
+ * A system of zero volume gets NaN; an empty system gets addend[m].  Systems are the atom ranges [sys_ptr[m],
+ * sys_ptr[m+1]) of spk_segment_ptr (idx_m sorted), n_sys <= 65535.  The launch shapes depend on n_atoms, n_sys and K
+ * only.
+ * workspace: spk_ewald_workspace_bytes(n_atoms, n_sys, K) bytes, 8-byte aligned; the forward leaves there what the
+ * reverse reads, so the reverse takes the same workspace, untouched in between, with the same inputs. */
+size_t spk_ewald_workspace_bytes(int64_t n_atoms, int64_t n_sys, int64_t n_k);
+int spk_ewald_fwd(const float* R, const float* q, const float* cell, const float* kvecs, const int64_t* idx_m,
+                  const int32_t* sys_ptr, int64_t n_atoms, int64_t n_sys, int64_t n_k, double ke, double alpha,
+                  const float* addend, float* energy, void* workspace, size_t workspace_bytes, spk_stream_t stream);
+/* Reverse for g_E [n_sys] (each output optional, NULL skips it):
+ *   g_R [N,3]      = ke (2 pi / V) g_E sum_k 2 f_k q_i k (Im S_k cos t_ik - Re S_k sin t_ik),  t_ik = k.r_i
+ *   g_q [N]       (+)= ke g_E [(2 pi / V) sum_k 2 f_k (Re S_k cos t_ik + Im S_k sin t_ik) - 2 sqrt(alpha / pi) q_i]
+ *                   (accumulate_q: added to what g_q holds, e.g. the real-space charge gradient)
+ *   g_cell [B,3,3] = -H^T [sum_i r_i (x) g_R_i - 2 g_E T + g_E E_rec I],  T = sum_k E_k (1/k^2 + 1/(4 alpha)) k (x) k
+ *   virial [B,3,3] (+)= -g_E (E_rec I - 2 T), fp64, the strain derivative in the convention of spk_pairwise_virial
+ *                   (accumulate_virial: added to what it holds) */
+int spk_ewald_bwd(const float* R, const float* q, const float* cell, const float* kvecs, const int64_t* idx_m,
+                  const int32_t* sys_ptr, int64_t n_atoms, int64_t n_sys, int64_t n_k, double ke, double alpha,
+                  const float* g_E, float* g_R, float* g_q, int accumulate_q, float* g_cell, double* virial,
+                  int accumulate_virial, void* workspace, size_t workspace_bytes, spk_stream_t stream);
+/* spk_pairwise_virial that adds W to what virial holds instead of overwriting it (the reciprocal Ewald virial is
+ * deposited there first) */
+int spk_pairwise_virial_add(const float* g_rij, const float* r_ij, const int32_t* rowptr, const int32_t* slot_eid,
+                            const int32_t* sys_ptr, int64_t n_edges, int64_t n_sys, double* virial, void* workspace,
+                            size_t workspace_bytes, spk_stream_t stream);
 
 /* ---- batchwise L-BFGS relaxation (csrc/relax.cu; interfaces/batchwise_optimization.py:613-917) ----------------------
  * One optimizer per system (atoms [sys_ptr[m], sys_ptr[m+1])), state fp64 on the device, positions in optimizer units

@@ -56,10 +56,11 @@ class PairParams(Structure):
     """spk_pair_t of include/spk_b200.h."""
     _fields_ = [("kind", c_int32), ("n_terms", c_int32), ("a_pow", c_void_p), ("a_div", c_void_p),
                 ("coefficients", c_void_p), ("exponents", c_void_p), ("ke", c_double), ("cutoff", c_double),
-                ("shift", c_double), ("switch_on", c_double), ("switch_off", c_double), ("d_max", c_double)]
+                ("shift", c_double), ("switch_on", c_double), ("switch_off", c_double), ("d_max", c_double),
+                ("alpha", c_double)]
 
 
-PAIR_ZBL, PAIR_COULOMB, PAIR_DAMPED_COULOMB = 0, 1, 2     # SPK_PAIR_*
+PAIR_ZBL, PAIR_COULOMB, PAIR_DAMPED_COULOMB, PAIR_EWALD_REAL = 0, 1, 2, 3     # SPK_PAIR_*
 PAIR_MAX_TERMS = 16                                       # SPK_PAIR_MAX_TERMS
 
 RELAX_WARP_ATOMS = 256      # SPK_RELAX_WARP_ATOMS
@@ -166,6 +167,11 @@ SIGNATURES = {
     "spk_pair_energy_workspace_bytes": [c_int64, c_int64],
     "spk_pair_energy_fwd": [POINTER(PairParams), P, P, P, P, P, P, P, P, P, c_int64, c_int64, P, P, c_size_t, P],
     "spk_pair_energy_bwd": [POINTER(PairParams), P, P, P, P, P, P, P, P, P, P, P, P, P, c_int64, c_int64, P, P, P],
+    "spk_ewald_workspace_bytes": [c_int64, c_int64, c_int64],
+    "spk_ewald_fwd": [P, P, P, P, P, P, c_int64, c_int64, c_int64, c_double, c_double, P, P, P, c_size_t, P],
+    "spk_ewald_bwd": [P, P, P, P, P, P, c_int64, c_int64, c_int64, c_double, c_double, P, P, P, c_int, P, P, c_int, P,
+                      c_size_t, P],
+    "spk_pairwise_virial_add": [P, P, P, P, P, c_int64, c_int64, P, P, c_size_t, P],
     "spk_relax_step": [POINTER(LBFGSState), P, P],
     "spk_relax_converged": [POINTER(LBFGSState), P, P],
 }
@@ -175,7 +181,8 @@ _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_siz
             "spk_painn_filter_packed_floats": c_size_t, "spk_neighbor_list_workspace_bytes": c_size_t,
             "spk_md_thermostat_workspace_bytes": c_size_t, "spk_rpmd_workspace_bytes": c_size_t,
             "spk_rpmd_barostat_workspace_bytes": c_size_t, "spk_head_workspace_bytes": c_size_t,
-            "spk_head_charges_bwd_workspace_bytes": c_size_t, "spk_pair_energy_workspace_bytes": c_size_t}
+            "spk_head_charges_bwd_workspace_bytes": c_size_t, "spk_pair_energy_workspace_bytes": c_size_t,
+            "spk_ewald_workspace_bytes": c_size_t}
 
 _lib = None
 
@@ -219,7 +226,8 @@ LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out
             "spk_md_kinetic_energy_tensor": 3, "spk_md_barostat_thermostat": 4, "spk_md_barostat_kick": 3,
             "spk_md_barostat_half_step": 2, "spk_md_barostat_main_step": 2, "spk_rpmd_barostat_half_step": 2,
             "spk_rpmd_barostat_main_step": 2, "spk_head_fwd": 2,
-            "spk_relax_converged": 2, "spk_pair_energy_fwd": 2, "spk_head_charges_bwd": 3}   # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global
+            "spk_relax_converged": 2, "spk_pair_energy_fwd": 2, "spk_head_charges_bwd": 3,
+            "spk_pairwise_virial_add": 2}   # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global
 launch_count = 0
 
 

@@ -17,7 +17,8 @@ from .. import ops
 from .. import properties
 
 __all__ = ["PairwiseDistances", "Atomwise", "Forces", "Strain", "DipoleMoment", "Polarizability", "ZBLRepulsionEnergy",
-           "CoulombPotential", "DampedCoulombPotential", "EnergyCoulomb", "Aggregation", "FilterShortRange"]
+           "CoulombPotential", "DampedCoulombPotential", "EnergyCoulomb", "EnergyEwald", "EnergyEwaldError", "Aggregation",
+           "FilterShortRange"]
 
 
 class PairwiseDistances(nn.Module):
@@ -28,7 +29,9 @@ class PairwiseDistances(nn.Module):
     writes W[m] = sum_{e in m} dE/dr_e (x) r_e into it (fp64 sums in a fixed order), so that stress = W / V without a strain
     leaf.  This costs one ``spk_segment_ptr`` launch in the forward and the two launches of ``spk_pairwise_virial`` (plus
     its small workspace) in the backward; the buffer is only written when a backward runs, so the evaluation needs grad
-    mode and positions that require grad.  Without the key nothing changes."""
+    mode and positions that require grad.  Without the key nothing changes.  An ``EnergyEwald`` deposits its reciprocal
+    virial, which does not go through r_ij, in the buffer first (its backward always runs before this one, which reads
+    r_ij's gradient from it); the pairwise pass then adds to the buffer instead of overwriting it."""
 
     @ops.on_tensor_device
     def forward(self, inputs: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
@@ -60,6 +63,7 @@ class PairwiseDistances(nn.Module):
                                  f"tensor on {R.device}")
             idx_m = idx_m if idx_m.dtype == torch.int64 else idx_m.long()
             holder.update(virial=virial, sys_ptr=ops.segment_ptr(idx_m.contiguous(), virial.shape[0]))
+            inputs[properties.virial_sink] = holder
         inputs[properties.Rij] = K.PairwiseDistancesFunction.apply(R, offsets, holder)
         return inputs
 
@@ -327,4 +331,4 @@ class Polarizability(_GatedHead):
 
 
 from .pair_terms import (Aggregation, CoulombPotential, DampedCoulombPotential, EnergyCoulomb,  # noqa: E402
-                         FilterShortRange, ZBLRepulsionEnergy)
+                         EnergyEwald, EnergyEwaldError, FilterShortRange, ZBLRepulsionEnergy)

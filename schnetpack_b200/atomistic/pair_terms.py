@@ -1,6 +1,7 @@
-"""Physics add-ons of PhysNet-style potentials on the kernels of csrc/pair_energy.cu: ZBL repulsion
+"""Physics add-ons of PhysNet-style potentials on the kernels of csrc/pair_energy.cu and csrc/ewald.cu: ZBL repulsion
 (atomistic/nuclear_repulsion.py:13-108), the Coulomb energy of point charges with its potentials
-(atomistic/electrostatic.py:14-152), ``Aggregation`` (atomistic/aggregation.py) and a capture-safe ``FilterShortRange``
+(atomistic/electrostatic.py:14-152), the Ewald sum of periodic systems (atomistic/electrostatic.py:155-375),
+``Aggregation`` (atomistic/aggregation.py) and a capture-safe ``FilterShortRange``
 (atomistic/distances.py:29-57).  Constructor signatures, parameters, buffers and ``state_dict`` keys are the
 reference's.
 
@@ -10,6 +11,7 @@ reaches the charge head through the differentiable ``charges`` output of ``Dipol
 parameters under grad mode: the ATen formulas of ``functional_torch``."""
 from __future__ import annotations
 
+import contextlib
 from typing import Callable, Dict, List, Optional, Union
 
 import torch
@@ -21,8 +23,9 @@ from .. import ops
 from .. import properties
 from ..units import convert_units
 
-__all__ = ["ZBLRepulsionEnergy", "CoulombPotential", "DampedCoulombPotential", "EnergyCoulomb", "Aggregation",
-           "FilterShortRange", "check_padded_pair_terms", "check_short_range_cutoff", "link_charges"]
+__all__ = ["ZBLRepulsionEnergy", "CoulombPotential", "DampedCoulombPotential", "EnergyCoulomb", "EnergyEwald",
+           "EnergyEwaldError", "Aggregation", "FilterShortRange", "check_padded_pair_terms", "check_ewald_cells", "padded_list_cutoff",
+           "check_short_range_cutoff", "link_charges"]
 
 
 def _softplus_inverse(x: torch.Tensor) -> torch.Tensor:
@@ -206,6 +209,98 @@ class EnergyCoulomb(nn.Module):
         return inputs
 
 
+class EnergyEwaldError(Exception):
+    """electrostatic.py:155-156: raised for a system whose cell has zero volume."""
+
+
+class EnergyEwald(nn.Module):
+    """electrostatic.py:159-375: Coulomb energy of the charges under ``charges_key`` in a periodic box by Ewald summation,
+    E = E_real + E_rec - E_self.  The real-space term runs over every pair of the long-range (``use_neighbors_lr``) or the
+    standard list, screened by ``1 - screening_fn(d)`` when a ``SwitchFunction`` is given; the reciprocal term over the
+    integer triples n of the ``kvecs`` buffer (the full sphere |n|^2 <= k_max^2 + 2, n != 0) with k = 2 pi n h^-T.
+    ``alpha`` is the square of the usual splitting parameter.  The cell is inverted, so triclinic cells work.
+
+    ``eval()``: one ``EwaldFunction`` (a pair-energy launch pair for the real space, four launches for the reciprocal and
+    self terms, no host read: the number of systems comes from ``_n_atoms``), differentiable with respect to r_ij, the
+    positions, the charges and the cell.  A system of zero volume gets a NaN energy there (the check would be a host read);
+    ``DeviceMD`` and ``DeviceLBFGS`` check the cells at construction and raise ``EnergyEwaldError`` as the reference does.
+    Inside ``padded_list_cutoff(model, cutoff)`` (``DeviceMD`` and ``DeviceLBFGS`` evaluate in it) the real-space term masks
+    d > the list cutoff, which drops the padding pairs of a fixed-capacity list and nothing else.  ``train()`` under grad mode: the ATen formulas of
+    ``functional_torch``."""
+
+    # the cutoff of the padded neighbour list being evaluated (set by ``padded_list_cutoff``), else None
+    list_cutoff: Optional[float] = None
+
+    def __init__(self, alpha: float, k_max: int, energy_unit: Union[str, float], position_unit: Union[str, float],
+                 output_key: str, charges_key: str = properties.partial_charges, use_neighbors_lr: bool = True,
+                 screening_fn: Optional[nn.Module] = None):
+        super().__init__()
+        ke = convert_units("Ha", energy_unit) * convert_units("Bohr", position_unit)
+        self.register_buffer("ke", torch.Tensor([ke]))
+        self.charges_key = charges_key
+        self.output_key = output_key
+        self.model_outputs = [output_key]
+        self.use_neighbors_lr = use_neighbors_lr
+        self.screening_fn = screening_fn
+        self.register_buffer("alpha", torch.Tensor([alpha]))
+        self.k_max = k_max
+        self.register_buffer("kvecs", self._generate_kvecs())
+        self._host = _HostScalars()
+
+    def _generate_kvecs(self) -> torch.Tensor:
+        """electrostatic.py:209-224."""
+        krange = torch.arange(0, self.k_max + 1, dtype=self.alpha.dtype)
+        krange = torch.cat([krange, -krange[1:]])
+        kvecs = torch.cartesian_prod(krange, krange, krange)
+        norm = torch.sum(kvecs ** 2, dim=1)
+        kvecs = kvecs[norm <= self.k_max ** 2 + 2, :]
+        norm = norm[norm <= self.k_max ** 2 + 2]
+        return kvecs[norm != 0, :]
+
+    def _screen(self):
+        sw = self.screening_fn
+        if sw is None:
+            return None
+        if type(sw).__name__ != "SwitchFunction":
+            raise NotImplementedError(f"EnergyEwald: screening_fn {type(sw).__name__} has no CUDA kernel "
+                                      "(SwitchFunction or None)")
+        return sw
+
+    @ops.on_tensor_device
+    def forward(self, inputs: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        if self.training and torch.is_grad_enabled():      # no parameters: the charges carry the training graph
+            from .. import functional_torch as T
+
+            return T.energy_ewald(self, inputs)
+        sw = self._screen()
+        ke, alpha, s_on, s_off = self._host.get(self.ke, self.alpha, sw.switch_on if sw is not None else None,
+                                                sw.switch_off if sw is not None else None)
+        q = inputs[self.charges_key].reshape(-1)
+        if q.dtype != torch.float32:
+            raise TypeError("EnergyEwald: the charges must be float32 on the kernel path")
+        idx_m, n_sys, sys_ptr = _systems(inputs, "EnergyEwald")
+        if self.use_neighbors_lr:
+            r_ij, idx_i, idx_j, graph = _edges(inputs, properties.Rij_lr, properties.idx_i_lr, properties.idx_j_lr,
+                                               q.shape[0])
+            d_max = None
+        else:
+            r_ij, idx_i, idx_j, graph = _edges(inputs, properties.Rij, properties.idx_i, properties.idx_j, q.shape[0])
+            d_max = _short_range_d_max(inputs)
+        if self.list_cutoff is not None:
+            d_max = self.list_cutoff if d_max is None else min(d_max, self.list_cutoff)
+        params, keep = ops.pair_params(ops.PAIR_EWALD_REAL, ke, switch_on=s_on or 0.0, switch_off=s_off or 0.0,
+                                       d_max=d_max, alpha=alpha)
+        kvecs = self.kvecs if self.kvecs.dtype == torch.float32 else self.kvecs.float()
+        holder = dict(params=params, keep=keep, idx_i=idx_i, idx_j=idx_j, idx_m=idx_m, graph=graph, sys_ptr=sys_ptr,
+                      n_sys=n_sys, kvecs=kvecs.contiguous(), ke=ke, alpha=alpha,
+                      sink=inputs.get(properties.virial_sink))
+        cell = inputs[properties.cell]
+        if cell.dtype != torch.float32 or cell.numel() != 9 * n_sys:
+            raise TypeError(f"EnergyEwald: the cell must be float32 [{n_sys}, 3, 3] on the kernel path")
+        inputs[self.output_key] = K.EwaldFunction.apply(r_ij, inputs[properties.R], q, cell, holder)
+        return inputs
+
+
 class Aggregation(nn.Module):
     """aggregation.py: the sum of several per-system outputs."""
 
@@ -266,7 +361,10 @@ def check_short_range_cutoff(representation: nn.Module, input_modules) -> None:
 
 def check_padded_pair_terms(model: nn.Module, list_cutoff: float, who: str) -> None:
     """The padded fixed-capacity neighbour list of the device drivers puts inert self pairs at distance 2 list_cutoff.
-    They are inert only for terms that vanish beyond a cutoff no larger than the list's."""
+    They are inert only for terms that vanish beyond a cutoff no larger than the list's.  ``EnergyEwald`` has no cutoff
+    (its real-space term is q_i^2 erfc(sqrt(alpha) d) / d on a padding pair); the drivers evaluate it inside
+    ``padded_list_cutoff``, where it masks d > list_cutoff, which is exact because an unpadded list at that cutoff holds
+    the same pairs."""
     for m in model.modules():
         name = type(m).__name__
         if name == "ZBLRepulsionEnergy":
@@ -285,10 +383,41 @@ def check_padded_pair_terms(model: nn.Module, list_cutoff: float, who: str) -> N
                 raise ValueError(f"{who}: EnergyCoulomb cutoff {rc} exceeds the neighbour-list cutoff {list_cutoff}")
 
 
+@contextlib.contextmanager
+def padded_list_cutoff(model: nn.Module, list_cutoff: float):
+    """Evaluate ``model`` on a padded fixed-capacity neighbour list of cutoff ``list_cutoff``: every ``EnergyEwald`` of it
+    masks real-space pairs with d > list_cutoff for the duration (the padding self pairs sit at 2 list_cutoff).  A plain
+    module attribute, read when the forward is traced, so nothing enters the batch and a captured graph keeps it.  Models
+    without an ``EnergyEwald`` are untouched."""
+    mods = [m for m in model.modules() if isinstance(m, EnergyEwald)]
+    old = [m.list_cutoff for m in mods]
+    for m in mods:
+        m.list_cutoff = float(list_cutoff)
+    try:
+        yield
+    finally:
+        for m, v in zip(mods, old):
+            m.list_cutoff = v
+
+
+def check_ewald_cells(model: nn.Module, batch: Dict[str, torch.Tensor], who: str) -> None:
+    """electrostatic.py:333-336 at the construction of a device driver: raise ``EnergyEwaldError`` when the model has an
+    ``EnergyEwald`` and a system's cell has (close to) zero volume.  One host read, outside the captured step."""
+    if not any(type(m).__name__ == "EnergyEwald" for m in model.modules()):
+        return
+    cell = batch.get(properties.cell)
+    if cell is None:
+        raise ValueError(f"{who}: EnergyEwald needs a periodic batch with a '{properties.cell}'")
+    v_box = torch.abs(torch.linalg.det(cell.detach().reshape(-1, 3, 3).double()))
+    if bool(torch.any(torch.isclose(v_box, torch.zeros_like(v_box)))):
+        raise EnergyEwaldError("Simulation box has no volume.")
+
+
 def link_charges(output_modules) -> None:
-    """Make the charges of a ``DipoleMoment`` differentiable when an ``EnergyCoulomb`` of the same model reads them (the
-    kernel head returns plain charges otherwise, so models that only output charges are unchanged)."""
-    keys = {m.charges_key for m in output_modules if type(m).__name__ == "EnergyCoulomb"}
+    """Make the charges of a ``DipoleMoment`` differentiable when an ``EnergyCoulomb`` or ``EnergyEwald`` of the same
+    model reads them (the kernel head returns plain charges otherwise, so models that only output charges are
+    unchanged)."""
+    keys = {m.charges_key for m in output_modules if type(m).__name__ in ("EnergyCoulomb", "EnergyEwald")}
     for m in output_modules:
         if hasattr(m, "differentiable_charges") and m.return_charges and m.charges_key in keys:
             m.differentiable_charges = True

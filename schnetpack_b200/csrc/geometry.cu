@@ -403,6 +403,38 @@ extern "C" int spk_pairwise_virial(const float* g_rij, const float* r_ij, const 
     return SPK_OK;
 }
 
+namespace {
+// the per-system pass of k_seg_finish<VIR_T, 9> that adds the totals to virial (after the reciprocal Ewald virial)
+__global__ void __launch_bounds__(SEG_FIN_T) k_virial_finish_add(const int32_t* __restrict__ rowptr,
+                                                                 const int32_t* __restrict__ sys_ptr,
+                                                                 const double* __restrict__ sys_part,
+                                                                 const double* __restrict__ head, double* __restrict__ out) {
+    __shared__ double red[9][SEG_FIN_T];
+    SPK_PDL_ENTER();
+    const int64_t s = blockIdx.x;
+    seg_finish_block<VIR_T, 9>(rowptr, sys_ptr, sys_part, head, s, red);
+    if (threadIdx.x < 9) out[s * 9 + threadIdx.x] += red[threadIdx.x][0];
+}
+}  // namespace
+
+extern "C" int spk_pairwise_virial_add(const float* g_rij, const float* r_ij, const int32_t* rowptr,
+                                       const int32_t* slot_eid, const int32_t* sys_ptr, int64_t n_edges, int64_t n_sys,
+                                       double* virial, void* workspace, size_t workspace_bytes, spk_stream_t stream) {
+    if (n_edges < 0 || n_sys <= 0 || n_edges >= (1ll << 31) - 1) return SPK_ERR_ARG;
+    if (!rowptr || !sys_ptr || !virial || !workspace) return SPK_ERR_ARG;
+    if (workspace_bytes < spk_pairwise_virial_workspace_bytes(n_edges, n_sys)) return SPK_ERR_ARG;
+    if (n_edges > 0 && (!g_rij || !r_ij || !slot_eid)) return SPK_ERR_ARG;
+    double* sys_part = reinterpret_cast<double*>(workspace);
+    double* head = sys_part + 9 * n_sys;
+    if (n_edges > 0)
+        spk_launch(k_virial_partials, (unsigned)spk_cdiv(n_edges, VIR_T), VIR_T, 0, spk_st(stream), g_rij, r_ij, rowptr,
+                   slot_eid, sys_ptr, n_sys, sys_part, head);
+    spk_launch(k_virial_finish_add, (unsigned)n_sys, SEG_FIN_T, 0, spk_st(stream), rowptr, sys_ptr, sys_part, head,
+               virial);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
 extern "C" int spk_md_property(const float* src, int64_t n, float conversion, float* dst, spk_stream_t stream) {
     if (n < 0) return SPK_ERR_ARG;
     if (n == 0) return SPK_OK;

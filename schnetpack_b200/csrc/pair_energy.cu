@@ -1,5 +1,7 @@
-// Pair energies of the physics add-ons: ZBL nuclear repulsion (atomistic/nuclear_repulsion.py:81-104) and the Coulomb
-// energy of point charges, plain or damped and optionally shifted to zero at a cutoff (atomistic/electrostatic.py:14-152).
+// Pair energies of the physics add-ons: ZBL nuclear repulsion (atomistic/nuclear_repulsion.py:81-104), the Coulomb
+// energy of point charges, plain or damped and optionally shifted to zero at a cutoff (atomistic/electrostatic.py:14-152),
+// and the real-space term of the Ewald sum (atomistic/electrostatic.py:266-308; the reciprocal and self terms are in
+// ewald.cu).
 //
 // Per edge e = (i, j) with d = |r_ij| the term e_ij is evaluated in fp64 from the fp32 inputs; per system the energy is
 // 0.5 ke sum_{e in m} e_ij.  The edges of system m are the receiver slots [rowptr[sys_ptr[m]], rowptr[sys_ptr[m+1]]), the
@@ -59,6 +61,41 @@ __device__ __forceinline__ void switch_component(double y, double& f, double& df
     }
 }
 
+// SwitchFunction of (switch_on, switch_off) (nn/cutoff.py:125-158): 1 below switch_on, 0 above switch_off, and its
+// derivative
+__device__ __forceinline__ void switch_function(const spk_pair_t& p, double d, double& sw, double& dsw) {
+    const double w = p.switch_off - p.switch_on;
+    const double x = (d - p.switch_on) / w;
+    sw = 1.0, dsw = 0.0;
+    if (x >= 1.0) {
+        sw = 0.0;
+    } else if (x > 0.0) {
+        double fp, dfp, fm, dfm;
+        switch_component(x, fp, dfp);
+        switch_component(1.0 - x, fm, dfm);
+        dfm = -dfm;
+        const double den = fp + fm;
+        sw = fm / den;
+        dsw = (dfm * fp - fm * dfp) / (den * den) / w;
+    }
+}
+
+// Ewald real-space potential (electrostatic.py:292-300) V = erfc(sqrt(alpha) d) / d, times 1 - screen(d) when a
+// SwitchFunction screen is given (switch_off != switch_on), and dV/dd.  No cutoff: every pair of the list counts.
+__device__ __forceinline__ void ewald_real_potential(const spk_pair_t& p, double d, double& V, double& dV) {
+    const double a = sqrt(p.alpha);
+    const double inv = 1.0 / d;
+    const double ec = erfc(a * d);
+    V = ec * inv;
+    dV = -(1.1283791670955126 * a * exp(-a * a * d * d) + V) * inv;    // 2 / sqrt(pi)
+    if (p.switch_off != p.switch_on) {
+        double sw, dsw;
+        switch_function(p, d, sw, dsw);
+        dV = dV * (1.0 - sw) - V * dsw;
+        V = V * (1.0 - sw);
+    }
+}
+
 // Coulomb potential V(d) and dV/dd: 1/d or the damped form of electrostatic.py:43-57 with SwitchFunction
 // (nn/cutoff.py:125-158), shifted to zero at the cutoff (electrostatic.py:141-145).
 __device__ __forceinline__ void coulomb_potential(const spk_pair_t& p, double d, double& V, double& dV) {
@@ -66,20 +103,8 @@ __device__ __forceinline__ void coulomb_potential(const spk_pair_t& p, double d,
     V = inv;
     dV = -inv * inv;
     if (p.kind == SPK_PAIR_DAMPED_COULOMB) {
-        const double w = p.switch_off - p.switch_on;
-        const double x = (d - p.switch_on) / w;
-        double sw = 1.0, dsw = 0.0;
-        if (x >= 1.0) {
-            sw = 0.0;
-        } else if (x > 0.0) {
-            double fp, dfp, fm, dfm;
-            switch_component(x, fp, dfp);
-            switch_component(1.0 - x, fm, dfm);
-            dfm = -dfm;
-            const double den = fp + fm;
-            sw = fm / den;
-            dsw = (dfm * fp - fm * dfp) / (den * den) / w;
-        }
+        double sw, dsw;
+        switch_function(p, d, sw, dsw);
         const double r2 = d * d + 1.0;
         const double damped = 1.0 / sqrt(r2);
         V = sw * damped + (1.0 - sw) * inv;
@@ -94,6 +119,12 @@ __device__ __forceinline__ void coulomb_potential(const spk_pair_t& p, double d,
             V = 0.0, dV = 0.0;
         }
     }
+}
+
+// the potential of a charge-pair kind: Coulomb, damped Coulomb or the Ewald real-space term
+__device__ __forceinline__ void charge_potential(const spk_pair_t& p, double d, double& V, double& dV) {
+    if (p.kind == SPK_PAIR_EWALD_REAL) ewald_real_potential(p, d, V, dV);
+    else coulomb_potential(p, d, V, dV);
 }
 
 __device__ __forceinline__ bool masked(const spk_pair_t& p, double d) { return p.d_max > 0.0 && !(d <= p.d_max); }
@@ -113,7 +144,7 @@ __device__ __forceinline__ void pair_term(const spk_pair_t& p, double d, const i
         zbl_term(p, d, (double)Z[i], (double)Z[j], e, de);
     } else {
         double dV;
-        coulomb_potential(p, d, V, dV);
+        charge_potential(p, d, V, dV);
         const double qq = (double)q[i] * (double)q[j];
         e = qq * V;
         de = qq * dV;
@@ -190,14 +221,14 @@ __global__ void k_pair_grad_q(spk_pair_t p, const float* __restrict__ r_ij, cons
         const int64_t e = slot_eid[s];
         const double d = edge_distance(r_ij + 3 * e);
         if (masked(p, d) || !(d > 0.0)) continue;
-        coulomb_potential(p, d, V, de);
+        charge_potential(p, d, V, de);
         acc += (double)q[slot_j[s]] * V;
     }
     for (int64_t k = sptr[a]; k < sptr[a + 1]; ++k) {
         const int64_t e = slot_eid[pos_slot[k]];
         const double d = edge_distance(r_ij + 3 * e);
         if (masked(p, d) || !(d > 0.0)) continue;
-        coulomb_potential(p, d, V, de);
+        charge_potential(p, d, V, de);
         acc += (double)q[pos_i[k]] * V;
     }
     g_q[a] = (float)(scale * (double)g_E[idx_m[a]] * acc);
@@ -205,12 +236,15 @@ __global__ void k_pair_grad_q(spk_pair_t p, const float* __restrict__ r_ij, cons
 
 int check_pair(const spk_pair_t* p) {
     if (!p) return SPK_ERR_ARG;
-    if (p->kind != SPK_PAIR_ZBL && p->kind != SPK_PAIR_COULOMB && p->kind != SPK_PAIR_DAMPED_COULOMB) return SPK_ERR_ARG;
+    if (p->kind != SPK_PAIR_ZBL && p->kind != SPK_PAIR_COULOMB && p->kind != SPK_PAIR_DAMPED_COULOMB &&
+        p->kind != SPK_PAIR_EWALD_REAL)
+        return SPK_ERR_ARG;
     if (p->kind == SPK_PAIR_ZBL) {
         if (p->n_terms <= 0 || p->n_terms > SPK_PAIR_MAX_TERMS) return SPK_ERR_ARG;
         if (!p->a_pow || !p->a_div || !p->coefficients || !p->exponents) return SPK_ERR_ARG;
     }
     if (p->kind == SPK_PAIR_DAMPED_COULOMB && !(p->switch_off != p->switch_on)) return SPK_ERR_ARG;
+    if (p->kind == SPK_PAIR_EWALD_REAL && !(p->alpha > 0.0)) return SPK_ERR_ARG;
     return SPK_OK;
 }
 

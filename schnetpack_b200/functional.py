@@ -604,7 +604,8 @@ class PairwiseDistancesFunction(torch.autograd.Function):
             g_R = ops.pairwise_bwd(g_rij, graph, 1.0)
             if h.get("virial") is not None:
                 (r_ij,) = ctx.saved_tensors
-                ops.pairwise_virial(g_rij, r_ij, graph, h["sys_ptr"], h["virial"])
+                ops.pairwise_virial(g_rij, r_ij, graph, h["sys_ptr"], h["virial"],
+                                    accumulate=h.pop("virial_deposited", False))
         return g_R, (g_rij if ctx.off_grad else None), None
 
 
@@ -782,3 +783,48 @@ class PairEnergyFunction(torch.autograd.Function):
             g_rij, g_q = ops.pair_energy_bwd(h["params"], rd, h["idx_i"], h["idx_j"], h.get("Z"), qd, h["idx_m"],
                                              g_E.contiguous(), h["graph"], ctx.want_q)
         return g_rij, g_q, None
+
+
+# =====================================================================================================================
+# Ewald summation (atomistic/electrostatic.py:155-375): real space on csrc/pair_energy.cu, reciprocal and self terms on
+# csrc/ewald.cu
+# =====================================================================================================================
+class EwaldFunction(torch.autograd.Function):
+    """(r_ij [E,3], R [N,3], q [N], cell [B,3,3]) -> energy [B] = E_real + E_rec - E_self.  Backward: dE/dr_ij (real
+    space), dE/dR (reciprocal), dE/dq (all three terms) and dE/dcell (reciprocal, for the Strain path).  With a virial
+    requested from PairwiseDistances (``holder["sink"]``) it also deposits the reciprocal virial there; this backward
+    always runs before PairwiseDistances' (which needs dE/dr_ij from it), so the pairwise pass then adds to it."""
+
+    @staticmethod
+    def forward(ctx, r_ij, R, q, cell, holder):
+        rd, Rd, qd = r_ij.detach().contiguous(), R.detach().contiguous(), q.detach().contiguous()
+        cd = cell.detach().reshape(-1, 3, 3).contiguous()
+        with ops.device_of(rd, Rd, qd, cd):
+            e_real = ops.pair_energy_fwd(holder["params"], rd, holder["idx_i"], holder["idx_j"], None, qd, holder["idx_m"],
+                                         holder["graph"], holder["sys_ptr"], holder["n_sys"])
+            energy, ws = ops.ewald_fwd(Rd, qd, cd, holder["kvecs"], holder["idx_m"], holder["sys_ptr"], holder["n_sys"],
+                                       holder["ke"], holder["alpha"], addend=e_real)
+        ctx.h = (holder, rd, Rd, qd, cd, ws)
+        ctx.cell_shape = cell.shape
+        ctx.set_materialize_grads(False)
+        return energy
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_E):
+        if g_E is None:
+            return None, None, None, None, None
+        h, rd, Rd, qd, cd, ws = ctx.h
+        _, want_R, want_q, want_cell, _ = ctx.needs_input_grad
+        sink = h.get("sink")
+        virial, acc = None, False
+        if sink is not None:
+            virial, acc = sink["virial"], sink.get("virial_deposited", False)
+            sink["virial_deposited"] = True
+        with ops.device_of(rd):
+            g_E = g_E.contiguous()
+            g_rij, g_q = ops.pair_energy_bwd(h["params"], rd, h["idx_i"], h["idx_j"], None, qd, h["idx_m"], g_E, h["graph"],
+                                             want_q)
+            g_R, g_cell = ops.ewald_bwd(Rd, qd, cd, h["kvecs"], h["idx_m"], h["sys_ptr"], h["n_sys"], h["ke"], h["alpha"],
+                                        g_E, ws, want_R, g_q, want_cell, virial, acc)
+        return g_rij, g_R, g_q, (g_cell.view(ctx.cell_shape) if g_cell is not None else None), None

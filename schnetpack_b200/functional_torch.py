@@ -273,6 +273,40 @@ def energy_coulomb(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
     return inputs
 
 
+def energy_ewald(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
+    """atomistic/electrostatic.py:226-375 with the number of systems from ``_n_atoms``."""
+    q = inputs[mod.charges_key].squeeze(-1)
+    idx_m = inputs[properties.idx_m]
+    if mod.use_neighbors_lr:
+        r_ij, idx_i, idx_j = inputs[properties.Rij_lr], inputs[properties.idx_i_lr], inputs[properties.idx_j_lr]
+    else:
+        r_ij, idx_i, idx_j = inputs[properties.Rij], inputs[properties.idx_i], inputs[properties.idx_j]
+    d_ij = _norm(r_ij)
+    R, cell = inputs[properties.R], inputs[properties.cell]
+    n_sys = _n_sys(inputs)
+    f_r = torch.erfc(torch.sqrt(mod.alpha) * d_ij) / d_ij
+    if mod.screening_fn is not None:
+        f_r = f_r * (1.0 - mod.screening_fn(d_ij))
+    y = scatter_add(q[idx_i] * q[idx_j] * f_r, idx_i, q.shape[0])
+    y_real = 0.5 * mod.ke * scatter_add(y, idx_m, n_sys).squeeze(-1)
+    recip_box = 2.0 * math.pi * torch.linalg.inv(cell).transpose(1, 2)
+    v_box = torch.abs(torch.linalg.det(cell))
+    if torch.any(torch.isclose(v_box, torch.zeros_like(v_box))):
+        from .atomistic.pair_terms import EnergyEwaldError
+
+        raise EnergyEwaldError("Simulation box has no volume.")
+    kvecs = torch.matmul(mod.kvecs[None, :, :], recip_box)
+    k_squared = torch.sum(kvecs ** 2, dim=2)
+    q_gauss = torch.exp(-0.25 * k_squared / mod.alpha)
+    kvec_dot_pos = torch.sum(kvecs[idx_m] * R[:, None, :], dim=2)
+    q_real = scatter_add(q[:, None] * torch.cos(kvec_dot_pos), idx_m, n_sys)
+    q_imag = scatter_add(q[:, None] * torch.sin(kvec_dot_pos), idx_m, n_sys)
+    y_ewald = 2.0 * math.pi / v_box * torch.sum((q_real ** 2 + q_imag ** 2) * q_gauss / k_squared, dim=1)
+    self_interaction = torch.sqrt(mod.alpha / math.pi) * scatter_add(q ** 2, idx_m, n_sys)
+    inputs[mod.output_key] = y_real + mod.ke * (y_ewald - self_interaction)
+    return inputs
+
+
 def filter_short_range(mod, inputs: Dict[str, Tensor]) -> Dict[str, Tensor]:
     """atomistic/distances.py:42-57 (exact compaction; a host sync and a data-dependent shape)."""
     idx_i, idx_j, Rij = inputs[properties.idx_i], inputs[properties.idx_j], inputs[properties.Rij]

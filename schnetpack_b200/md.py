@@ -60,6 +60,7 @@ import torch
 
 from . import _lib, ops
 from . import properties as P
+from .atomistic.pair_terms import padded_list_cutoff
 from .neighbors import CellListNeighborList
 
 __all__ = ["DeviceMD", "BerendsenThermostat", "LangevinThermostat", "NHCThermostat", "NHCBarostatIsotropic",
@@ -872,7 +873,8 @@ class _CapturedEvaluation:
         if self.virial is not None:
             x[P.virial] = self.virial
         x = self.nl(x)
-        out = self.model(x)
+        with padded_list_cutoff(self.model, self.nl._cutoff):     # the padding pairs of the fixed-capacity list
+            out = self.model(x)
         e, f = out[self.energy_key].detach(), out[self.force_key].detach()
         if self.energy is None:
             self.energy, self.forces, self.n_pairs = e.clone(), f.clone(), x["_n_pairs"].clone()
@@ -949,9 +951,10 @@ class DeviceMD(_CapturedEvaluation):
             raise ValueError("DeviceMD: the NHC barostats contain their own thermostat (temperature_control = True); "
                              "pass either a thermostat or a barostat")
         self._check_ring_polymer(ring_polymer, thermostat, barostat, compute_stress)
-        from .atomistic.pair_terms import check_padded_pair_terms
+        from .atomistic.pair_terms import check_ewald_cells, check_padded_pair_terms
 
         check_padded_pair_terms(model, float(cutoff), "DeviceMD")
+        check_ewald_cells(model, batch, "DeviceMD")
         self.ring_polymer = ring_polymer
         self.model = model
         self.dt = float(time_step)

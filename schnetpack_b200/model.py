@@ -215,14 +215,27 @@ def _convert_pair_term(m):
     return new
 
 
+def _convert_ewald(m):
+    """EnergyEwald (screening_fn None or SwitchFunction) -> the kernel module, state_dict (ke, alpha, kvecs) copied."""
+    sw = m.screening_fn
+    if sw is not None and type(sw).__name__ != "SwitchFunction":
+        raise NotImplementedError(f"EnergyEwald screening_fn {type(sw).__name__} has no CUDA kernel")
+    new_sw = snn.SwitchFunction(float(sw.switch_on), float(sw.switch_off)) if sw is not None else None
+    new = atomistic.EnergyEwald(float(m.alpha), int(m.k_max), 1.0, 1.0, m.output_key, charges_key=m.charges_key,
+                                use_neighbors_lr=m.use_neighbors_lr, screening_fn=new_sw)
+    new.load_state_dict(m.state_dict())
+    return new
+
+
 def convert_model(model: nn.Module) -> NeuralNetworkPotential:
     """Build a CUDA ``NeuralNetworkPotential`` from a loaded reference model (duck-typed on class names; weights are
     copied through ``state_dict`` whose keys are identical).  ``Atomwise`` (n_out=1, n_layers=2), ``Forces``,
     ``DipoleMoment`` and ``Polarizability`` heads, the pair terms ``ZBLRepulsionEnergy`` (cutoff_fn None or CosineCutoff)
-    and ``EnergyCoulomb`` (CoulombPotential or DampedCoulombPotential with a SwitchFunction), ``Aggregation`` and the
-    input modules ``PairwiseDistances`` / ``FilterShortRange`` are swapped for the CUDA modules.  Passed through as they
-    are: postprocessors, custom embeddings and every other module (``EnergyEwald``, other output heads); a passed-through
-    module that reads the number of systems from ``idx_m`` keeps its host read."""
+    and ``EnergyCoulomb`` (CoulombPotential or DampedCoulombPotential with a SwitchFunction), ``EnergyEwald``
+    (screening_fn None or SwitchFunction), ``Aggregation`` and the input modules ``PairwiseDistances`` /
+    ``FilterShortRange`` are swapped for the CUDA modules.  Passed through as they are: postprocessors, custom embeddings
+    and every other module (other output heads); a passed-through module that reads the number of systems from ``idx_m``
+    keeps its host read."""
     in_mods = []
     for m in model.input_modules:
         n = type(m).__name__
@@ -248,6 +261,8 @@ def convert_model(model: nn.Module) -> NeuralNetworkPotential:
             out_mods.append(_convert_head(m))
         elif n in ("ZBLRepulsionEnergy", "EnergyCoulomb"):
             out_mods.append(_convert_pair_term(m))
+        elif n == "EnergyEwald":
+            out_mods.append(_convert_ewald(m))
         elif n == "Aggregation":
             out_mods.append(atomistic.Aggregation(list(m.keys), m.output_key))
         else:

@@ -200,15 +200,17 @@ def pairwise_bwd(g_rij: Tensor, graph: EdgeGraph, sign: float = 1.0) -> Tensor:
     return out
 
 
-def pairwise_virial(g_rij: Tensor, r_ij: Tensor, graph: EdgeGraph, sys_ptr: Tensor, virial: Tensor):
-    """virial[m] = sum over the edges received by the atoms of system m of g_rij (x) r_ij, fp64, in place."""
+def pairwise_virial(g_rij: Tensor, r_ij: Tensor, graph: EdgeGraph, sys_ptr: Tensor, virial: Tensor,
+                    accumulate: bool = False):
+    """virial[m] = sum over the edges received by the atoms of system m of g_rij (x) r_ij, fp64, in place (``accumulate``:
+    added to what virial holds)."""
     f32(g_rij, "g_rij")
     f32(r_ij, "_Rij")
     n_sys = virial.shape[0]
     nbytes = int(_lib.lib().spk_pairwise_virial_workspace_bytes(graph.n_edges, n_sys))
     ws = torch.empty(nbytes, dtype=torch.uint8, device=g_rij.device)
-    _lib.call("spk_pairwise_virial", _p(g_rij), _p(r_ij), _p(graph.rowptr), _p(graph.slot_eid), _p(sys_ptr), graph.n_edges,
-              n_sys, _p(virial), _p(ws), nbytes, _stream())
+    _lib.call("spk_pairwise_virial_add" if accumulate else "spk_pairwise_virial", _p(g_rij), _p(r_ij), _p(graph.rowptr),
+              _p(graph.slot_eid), _p(sys_ptr), graph.n_edges, n_sys, _p(virial), _p(ws), nbytes, _stream())
 
 
 def edge_geometry(r_ij: Tensor, graph: Optional[EdgeGraph], rbf_kind: int, n_rbf: int, p0: Tensor, p1: Optional[Tensor],
@@ -762,10 +764,11 @@ def head_scalar_bwd_q(q: Tensor, R: Tensor, idx_m: Tensor, saved: Tensor, g_out:
 
 # ------------------------------------------------------------------------------------------------------------ pair energies
 PAIR_ZBL, PAIR_COULOMB, PAIR_DAMPED_COULOMB = _lib.PAIR_ZBL, _lib.PAIR_COULOMB, _lib.PAIR_DAMPED_COULOMB
+PAIR_EWALD_REAL = _lib.PAIR_EWALD_REAL
 
 
 def pair_params(kind: int, ke: float, cutoff: Optional[float] = None, shift: float = 0.0, switch_on: float = 0.0,
-                switch_off: float = 0.0, d_max: Optional[float] = None, zbl=None):
+                switch_off: float = 0.0, d_max: Optional[float] = None, zbl=None, alpha: float = 0.0):
     """``spk_pair_t`` for a pair term; ``zbl`` = (a_pow, a_div, coefficients, exponents) device tensors, read by the kernels
     at every launch (a captured graph sees updated values).  Returns (struct, tensors kept alive)."""
     st = _lib.PairParams()
@@ -782,6 +785,7 @@ def pair_params(kind: int, ke: float, cutoff: Optional[float] = None, shift: flo
     st.shift = float(shift)
     st.switch_on, st.switch_off = float(switch_on), float(switch_off)
     st.d_max = float(d_max) if d_max is not None else 0.0
+    st.alpha = float(alpha)
     return st, keep
 
 
@@ -812,3 +816,36 @@ def pair_energy_bwd(params, r_ij: Tensor, idx_i: Tensor, idx_j: Tensor, Z: Optio
               _p(graph.pos_slot), _p(graph.pos_i), N, E, _p(g_rij), _p(g_q), _stream(),
               launches=int(E > 0) + int(want_q and N > 0))
     return g_rij, g_q
+
+
+# ------------------------------------------------------------------------------------------------------------ Ewald
+def ewald_fwd(R: Tensor, q: Tensor, cell: Tensor, kvecs: Tensor, idx_m: Tensor, sys_ptr: Tensor, n_sys: int, ke: float,
+              alpha: float, addend: Optional[Tensor] = None):
+    """-> (energy [n_sys] = addend + E_rec - E_self, workspace the reverse reads)"""
+    dev = R.device
+    N, K = R.shape[0], kvecs.shape[0]
+    energy = torch.empty((n_sys,), dtype=torch.float32, device=dev)
+    nbytes = int(_lib.lib().spk_ewald_workspace_bytes(N, n_sys, K))
+    ws = torch.empty(max(nbytes, 8), dtype=torch.uint8, device=dev)
+    _lib.call("spk_ewald_fwd", _p(f32(R, "_positions")), _p(f32(q, "charges")), _p(f32(cell, "_cell")),
+              _p(f32(kvecs, "kvecs")), _p(i64(idx_m, "_idx_m")), _p(sys_ptr), N, n_sys, K, float(ke), float(alpha),
+              _p(f32(addend, "energy")) if addend is not None else None, _p(energy), _p(ws), nbytes, _stream(),
+              launches=(2 if N > 0 else 1) + (1 if K > 0 else 0) + 1)
+    return energy, ws
+
+
+def ewald_bwd(R: Tensor, q: Tensor, cell: Tensor, kvecs: Tensor, idx_m: Tensor, sys_ptr: Tensor, n_sys: int, ke: float,
+              alpha: float, g_E: Tensor, ws: Tensor, want_R: bool, g_q: Optional[Tensor], want_cell: bool,
+              virial: Optional[Tensor] = None, accumulate_virial: bool = False):
+    """-> (g_R [N,3] or None, g_cell [n_sys,3,3] or None); ``g_q`` [N] (the real-space charge gradient) gets the reciprocal
+    and self terms added in place; ``virial`` [n_sys,3,3] fp64 gets the reciprocal virial (added with
+    ``accumulate_virial``)."""
+    dev = R.device
+    N, K = R.shape[0], kvecs.shape[0]
+    g_R = torch.empty((N, 3), dtype=torch.float32, device=dev) if want_R else None
+    g_cell = torch.empty((n_sys, 3, 3), dtype=torch.float32, device=dev) if want_cell else None
+    _lib.call("spk_ewald_bwd", _p(R), _p(q), _p(cell), _p(kvecs), _p(idx_m), _p(sys_ptr), N, n_sys, K, float(ke),
+              float(alpha), _p(f32(g_E, "g_E")), _p(g_R), _p(g_q), 1, _p(g_cell), _p(virial), int(accumulate_virial),
+              _p(ws), ws.numel(), _stream(),
+              launches=(int(K > 0) + 1 if N > 0 else 0) + int(want_cell or virial is not None))
+    return g_R, g_cell

@@ -37,3 +37,6 @@ virial = "_virial"
 # set by FilterShortRange (not a reference key): the short-range keys keep the full list, and pair terms that read it
 # mask d > short_range_cutoff (a CPU scalar tensor, so reading it is no device sync)
 short_range_cutoff = "_short_range_cutoff"
+# set by PairwiseDistances when a virial is requested (not a reference key): the state its backward shares with terms
+# that deposit a virial of their own first (the reciprocal Ewald term)
+virial_sink = "_virial_sink"

@@ -162,9 +162,10 @@ class DeviceLBFGS(_CapturedEvaluation):
         if outputs is not None and (force_key not in outputs or energy_key not in outputs):
             raise ValueError(f"DeviceLBFGS: the model must output '{energy_key}' and '{force_key}' (it outputs "
                              f"{sorted(outputs)})")
-        from .atomistic.pair_terms import check_padded_pair_terms
+        from .atomistic.pair_terms import check_ewald_cells, check_padded_pair_terms
 
         check_padded_pair_terms(model, float(cutoff), "DeviceLBFGS")
+        check_ewald_cells(model, batch, "DeviceLBFGS")
         self.model = model
         self.energy_key, self.force_key = energy_key, force_key
         self.p_conv = float(position_conversion)

@@ -381,7 +381,8 @@ def to_scriptable(model: NeuralNetworkPotential) -> ScriptedPotential:
             outs.append(ScriptAtomwise(m))
         elif n == "Forces":
             outs.append(ScriptForces(m))
-        elif n in ("DipoleMoment", "Polarizability", "ZBLRepulsionEnergy", "EnergyCoulomb", "Aggregation"):
+        elif n in ("DipoleMoment", "Polarizability", "ZBLRepulsionEnergy", "EnergyCoulomb", "EnergyEwald",
+                   "Aggregation"):
             raise NotImplementedError(f"to_scriptable: {n} has no TorchScript twin (its kernels run through "
                                       "torch.autograd.Function); evaluate the model in Python")
         else:
