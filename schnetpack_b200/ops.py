@@ -372,13 +372,20 @@ class Lin:
             self.wt_pk = tc_pack_weight(self.wt)
 
     @staticmethod
-    def _tc_ok(A: Tensor, n_out: int, kw) -> bool:
-        """shapes the tensor-core kernel's vector fast path covers (otherwise the fp32 kernel runs)"""
+    def _tc_ok(A: Tensor, n_out: int, act: int, bias: Optional[Tensor], kw) -> bool:
+        """calls the tensor-core kernel's vector fast path covers; spk_dense_tc refuses every other one, and the fp32
+        kernel runs it: K, N, lda and ldy multiples of 4, 16 B-aligned base pointers, and not both a backward prologue
+        (a_act) and a forward activation"""
         k = kw.get("k")
         K = A.shape[1] if k is None else int(k)
         out = kw.get("out")
         ldy = n_out if out is None else out.shape[1]
-        return K % 4 == 0 and n_out % 4 == 0 and A.shape[1] % 4 == 0 and ldy % 4 == 0
+        if K % 4 or n_out % 4 or A.shape[1] % 4 or ldy % 4:
+            return False
+        a_pre = kw.get("a_pre")
+        if a_pre is not None and kw.get("a_act", ACT_NONE) != ACT_NONE and (act & ~SAVE_DERIV) != ACT_NONE:
+            return False
+        return all(t.data_ptr() % 16 == 0 for t in (A, a_pre, bias, kw.get("addend"), out) if t is not None)
 
     def fwd(self, A: Tensor, act: int = ACT_NONE, save_deriv: bool = False, **kw):
         """act(A W^T + b) [+ addend].  ``save_deriv=True`` returns (Y, act'(pre)): the tensor the input-gradient layer
@@ -386,13 +393,13 @@ class Lin:
         if save_deriv:
             kw["save_pre"] = True
             act = act | SAVE_DERIV
-        if self.w_pk is not None and self._tc_ok(A, self.w.shape[0], kw):
+        if self.w_pk is not None and self._tc_ok(A, self.w.shape[0], act, self.b, kw):
             return dense_tc(A, self.w_pk, self.w.shape[0], self.b, act, **kw)
         return dense(A, self.wt, self.b, act, **kw)
 
     def bwd(self, G: Tensor, **kw):
         """(G .* act'(a_pre)) W [+ addend]  -- input gradient of the layer"""
-        if self.wt_pk is not None and self._tc_ok(G, self.wt.shape[0], kw):
+        if self.wt_pk is not None and self._tc_ok(G, self.wt.shape[0], ACT_NONE, None, kw):
             return dense_tc(G, self.wt_pk, self.wt.shape[0], None, ACT_NONE, **kw)
         return dense(G, self.w, None, ACT_NONE, **kw)
 
