@@ -710,6 +710,35 @@ typedef struct {
 int spk_relax_step(const spk_lbfgs_t* state, const float* forces, spk_stream_t stream);
 int spk_relax_converged(const spk_lbfgs_t* state, const float* forces, spk_stream_t stream);
 
+/* ---- model ensembles (csrc/ensemble.cu; md/calculators/ensemble_calculator.py:38-59,
+ * interfaces/batchwise_optimization.py:36-72, interfaces/ase_interface.py:340-432) ------------------------------------
+ * The K members' outputs are stacked fp32 slots [K, ...] (slot k = member k).  Every statistic runs in fp64 over k in
+ * ascending order, in two passes (the mean, then the sum of squared deviations ss from it), without atomics: bitwise
+ * reproducible.
+ *
+ * spk_ensemble_moments, element-wise over x [K, n]: mean = sum_k x / K, var = ss / (K - ddof) (ddof 0 or 1, K > ddof);
+ *   mean_out = mean * mean_scale, var_out = var * spread_scale, std_out = sqrt(var) * spread_scale (each optional).
+ * spk_ensemble_forces, one thread per atom of forces [K, N, 3] (K >= 2): mean [N, 3] = mean * mean_scale, var [N, 3] =
+ *   the unbiased variance * spread_scale (each optional) and, with sys_terms, per system s (atoms [sys_ptr[s],
+ *   sys_ptr[s+1]), idx_m sorted) sys_terms[s] = (sum_i ||sd_i||, sum_i ||sd_i|| / (||mu_i|| + 1e-8)) with sd_i the
+ *   ddof-0 standard deviation and mu_i the mean of F_i * spread_scale; 0 for an empty system.  workspace:
+ *   spk_ensemble_workspace_bytes(N, n_sys) bytes, 8-byte aligned (only with sys_terms).
+ * spk_ensemble_uncertainty, one thread per system: out [n_sys] fp64 = w_e u_E + w_f u_F + w_s u_S, each term only if
+ *   its weight is > 0.  u_E = std_0(E * energy_scale) of energy [K, n_sys] (relative: over |mean| + 1e-8); u_F =
+ *   sys_terms[s][relative] / n_atoms(s), 0 for a system without atoms (the reference would take the mean of nothing);
+ *   u_S = the mean over the 3 rows of ||std_0 of the row|| of stress [K, n_sys, 3, 3] * stress_scale (relative: each
+ *   row over ||mean row|| + 1e-8).  out_f32 [n_sys] (optional, as out) receives the same values rounded to fp32. */
+size_t spk_ensemble_workspace_bytes(int64_t n_atoms, int64_t n_sys);
+int spk_ensemble_moments(const float* x, int64_t K, int64_t n, int ddof, double mean_scale, double spread_scale,
+                         float* mean, float* var, float* std, spk_stream_t stream);
+int spk_ensemble_forces(const float* forces, int64_t K, const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms,
+                        int64_t n_sys, double mean_scale, double spread_scale, float* mean, float* var,
+                        double* sys_terms, void* workspace, size_t workspace_bytes, spk_stream_t stream);
+int spk_ensemble_uncertainty(const float* energy, double energy_scale, const double* force_sums, const int32_t* sys_ptr,
+                             const float* stress, double stress_scale, int64_t K, int64_t n_sys, int relative,
+                             double energy_weight, double force_weight, double stress_weight, double* out,
+                             float* out_f32, spk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -174,6 +174,11 @@ SIGNATURES = {
     "spk_pairwise_virial_add": [P, P, P, P, P, c_int64, c_int64, P, P, c_size_t, P],
     "spk_relax_step": [POINTER(LBFGSState), P, P],
     "spk_relax_converged": [POINTER(LBFGSState), P, P],
+    "spk_ensemble_workspace_bytes": [c_int64, c_int64],
+    "spk_ensemble_moments": [P, c_int64, c_int64, c_int, c_double, c_double, P, P, P, P],
+    "spk_ensemble_forces": [P, c_int64, P, P, c_int64, c_int64, c_double, c_double, P, P, P, P, c_size_t, P],
+    "spk_ensemble_uncertainty": [P, c_double, P, P, P, c_double, c_int64, c_int64, c_int, c_double, c_double, c_double, P,
+                                 P, P],
 }
 _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_size_t,
             "spk_pairwise_virial_workspace_bytes": c_size_t, "spk_md_barostat_workspace_bytes": c_size_t,
@@ -182,7 +187,7 @@ _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_siz
             "spk_md_thermostat_workspace_bytes": c_size_t, "spk_rpmd_workspace_bytes": c_size_t,
             "spk_rpmd_barostat_workspace_bytes": c_size_t, "spk_head_workspace_bytes": c_size_t,
             "spk_head_charges_bwd_workspace_bytes": c_size_t, "spk_pair_energy_workspace_bytes": c_size_t,
-            "spk_ewald_workspace_bytes": c_size_t}
+            "spk_ewald_workspace_bytes": c_size_t, "spk_ensemble_workspace_bytes": c_size_t}
 
 _lib = None
 

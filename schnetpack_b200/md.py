@@ -865,6 +865,9 @@ class _CapturedEvaluation:
     force_key = P.forces
     virial: Optional[Tensor] = None
     required_properties: List[str] = []
+    # members of an ensemble run (None: one model); their outputs are stacked into ``self.stacks[key]`` [K, ...]
+    ensemble: Optional[List[torch.nn.Module]] = None
+    stacks: Dict[str, Tensor] = {}
 
     # ---- one force evaluation on the current positions (calculator.calculate) ---------------------------------------------
     def _calculate(self):
@@ -873,6 +876,8 @@ class _CapturedEvaluation:
         if self.virial is not None:
             x[P.virial] = self.virial
         x = self.nl(x)
+        if self.ensemble is not None:
+            return self._calculate_ensemble(x)
         with padded_list_cutoff(self.model, self.nl._cutoff):     # the padding pairs of the fixed-capacity list
             out = self.model(x)
         e, f = out[self.energy_key].detach(), out[self.force_key].detach()
@@ -885,6 +890,61 @@ class _CapturedEvaluation:
         torch.maximum(self.nl_watch, x["_n_pairs"], out=self.nl_watch)
         if self.required_properties:
             self._refresh_properties(out)
+
+    def _calculate_ensemble(self, x: Dict[str, Tensor]):
+        """EnsembleCalculator.calculate (ensemble_calculator.py:20-35): every member on the same neighbour list (and so on
+        the same EdgeGraph of ops._GRAPH_CACHE), each output copied into its slot before the next member reuses its
+        buffers, then the statistics over the slots (``_ensemble_statistics``)."""
+        keys = [self.energy_key, self.force_key] + [p for p in self.required_properties
+                                                     if p not in (self.energy_key, self.force_key)]
+        K = len(self.ensemble)
+        first = not self.stacks
+        for k, member in enumerate(self.ensemble):
+            with padded_list_cutoff(member, self.nl._cutoff):
+                out = member(dict(x))
+            for p in keys:
+                v = out[p].detach()
+                if first and k == 0:
+                    if v.dtype != torch.float32 or not v.is_contiguous():
+                        raise TypeError(f"{type(self).__name__}: output '{p}' must be a contiguous float32 tensor")
+                    self.stacks[p] = torch.empty((K,) + tuple(v.shape), dtype=torch.float32, device=v.device)
+                elif tuple(v.shape) != tuple(self.stacks[p].shape[1:]):
+                    raise ValueError(f"{type(self).__name__}: ensemble member {k} predicts '{p}' of shape "
+                                     f"{tuple(v.shape)}, member 0 {tuple(self.stacks[p].shape[1:])}")
+                self.stacks[p][k].copy_(v)
+        if self.energy is None:
+            e, f = self.stacks[self.energy_key], self.stacks[self.force_key]
+            self.energy = torch.empty(e.shape[1:], dtype=torch.float32, device=e.device)
+            self.forces = torch.empty(f.shape[1:], dtype=torch.float32, device=f.device)
+            self.n_pairs = x["_n_pairs"].clone()
+        else:
+            self.n_pairs.copy_(x["_n_pairs"])
+        torch.maximum(self.nl_watch, x["_n_pairs"], out=self.nl_watch)
+        self._ensemble_statistics()
+
+    def _ensemble_statistics(self):
+        """the mean energies and forces that drive the step (BatchwiseEnsembleCalculator.calculate)"""
+        from .ensemble import ensemble_forces, ensemble_moments
+
+        ensemble_moments(self.stacks[self.energy_key], var=False, out_mean=self.energy)
+        ensemble_forces(self.stacks[self.force_key], var=False, out_mean=self.forces)
+
+    def _set_ensemble(self, model, who: str) -> torch.nn.Module:
+        """``model`` as the module the driver keeps: an ``nn.ModuleList`` of the members of an ensemble (``self.ensemble``)
+        or the single model"""
+        from .ensemble import members_of
+
+        members = members_of(model)
+        if members is None:
+            return model
+        self.ensemble = members
+        self.stacks = {}
+        for m in members:
+            outputs = getattr(m, "model_outputs", None)
+            if outputs is not None and (self.energy_key not in outputs or self.force_key not in outputs):
+                raise ValueError(f"{who}: every ensemble member must output '{self.energy_key}' and '{self.force_key}' "
+                                 f"(one outputs {sorted(outputs)})")
+        return torch.nn.ModuleList(members)
 
     def _capture_step(self, state: List[Tensor]) -> "torch.cuda.CUDAGraph":
         """Capture ``self._step()`` into a CUDA graph.  Capture works on copies of ``state`` (every tensor the step writes)
@@ -923,7 +983,7 @@ class DeviceMD(_CapturedEvaluation):
                  compute_stress: bool = False, ring_polymer: Optional[RingPolymer] = None,
                  required_properties: Optional[List[str]] = None,
                  property_conversion: Optional[Dict[str, float]] = None, record_every: int = 1,
-                 record_capacity: int = 0):
+                 record_capacity: int = 0, uncertainty_fn: Optional[object] = None):
         """``batch[_positions]`` (and ``_cell``) are in MODEL units as everywhere in this package; ``self.positions`` is the
         MD-unit state (= model positions / position_conversion).  ``thermostat`` (None = NVE) is bound to the systems of
         the batch and applied around every step.  ``barostat`` (an NHC barostat, which thermostats the particles itself)
@@ -943,10 +1003,23 @@ class DeviceMD(_CapturedEvaluation):
         ASE's unit tables.  With ``record_capacity`` > 0 the step also appends them to a device-side time series every
         ``record_every`` steps (steps s with s % record_every == 0, counted from the start), written inside the captured
         step; ``recorded(name)`` returns the series, ``drain()`` empties it, and ``run`` refuses a call that would store
-        more than ``record_capacity`` records since the last drain."""
+        more than ``record_capacity`` records since the last drain.
+
+        ``model`` may be a list (or ``nn.ModuleList``) of at least two members: an ensemble run
+        (md/calculators/ensemble_calculator.py).  Every member runs on the step's one neighbour list, the mean energies and
+        forces drive the dynamics, and ``self.properties`` holds ``energy``, ``forces`` and every required property as
+        the member mean times ``property_conversion[p]`` (default 1.0, for the energy and forces too, as the reference's
+        calculator), plus ``{p}_var``: the unbiased variance over the members times the same linear factor
+        (ensemble_calculator.py:70-81).  ``uncertainty_fn`` (an ``ensemble.AbsoluteUncertainty`` /
+        ``RelativeUncertainty`` on the run's energy and force keys, without a stress weight) adds
+        ``properties["uncertainty"]`` [n_replicas, B] of the energies and forces as ``properties`` holds them.  Stress
+        and barostats are refused with an ensemble, as in the reference."""
         dev = batch[P.R].device
         if dev.type != "cuda":
             raise ValueError("DeviceMD needs a CUDA batch (no CPU fallback)")
+        model = self._set_ensemble(model, "DeviceMD")
+        self._check_ensemble(barostat, compute_stress, uncertainty_fn)
+        self.uncertainty_fn = uncertainty_fn
         if barostat is not None and thermostat is not None and getattr(barostat, "temperature_control", True):
             raise ValueError("DeviceMD: the NHC barostats contain their own thermostat (temperature_control = True); "
                              "pass either a thermostat or a barostat")
@@ -1043,6 +1116,29 @@ class DeviceMD(_CapturedEvaluation):
         n_sys = static[P.n_atoms].shape[0] if P.n_atoms in static else 1
         return _Systems(masses, idx_m.to(torch.int64).contiguous(), n_sys)
 
+    def _check_ensemble(self, barostat, compute_stress: bool, uncertainty_fn):
+        if self.ensemble is None:
+            if uncertainty_fn is not None:
+                raise ValueError("DeviceMD: uncertainty_fn needs an ensemble (model=[m1, m2, ...])")
+            return
+        if compute_stress or barostat is not None:
+            raise NotImplementedError("DeviceMD: stress and constant pressure are not available for ensembles (the "
+                                      "reference's EnsembleCalculator._activate_stress raises, "
+                                      "md/calculators/ensemble_calculator.py:62-68)")
+        if uncertainty_fn is None:
+            return
+        from .ensemble import Uncertainty
+
+        if not isinstance(uncertainty_fn, Uncertainty):
+            raise TypeError(f"DeviceMD: uncertainty_fn must be an AbsoluteUncertainty or RelativeUncertainty, got "
+                            f"{type(uncertainty_fn).__name__}")
+        if uncertainty_fn.stress_weight > 0:
+            raise NotImplementedError("DeviceMD: an ensemble run has no stress, so uncertainty_fn takes no stress_weight")
+        keys = (uncertainty_fn.energy_key, uncertainty_fn.force_key)
+        if keys != (self.energy_key, self.force_key):
+            raise ValueError(f"DeviceMD: uncertainty_fn reads {keys}, the run predicts ('{self.energy_key}', "
+                             f"'{self.force_key}')")
+
     # ---- ring-polymer set-up ------------------------------------------------------------------------------------------------
     @staticmethod
     def _check_ring_polymer(ring_polymer, thermostat, barostat, compute_stress):
@@ -1102,22 +1198,27 @@ class DeviceMD(_CapturedEvaluation):
     def _setup_properties(self, required, conversion, every, capacity):
         self.required_properties = list(dict.fromkeys(required or []))
         conversion = dict(conversion or {})
-        unknown = sorted(set(conversion) - set(self.required_properties))
+        known = list(self.required_properties)
+        if self.ensemble is not None:                # energy and forces are always required (base_calculator.py:65-69)
+            known += [p for p in (self.energy_key, self.force_key) if p not in known]
+        unknown = sorted(set(conversion) - set(known))
         if unknown:
             raise ValueError(f"DeviceMD: property_conversion names properties that are not required: {unknown}")
         for k, v in conversion.items():
             if isinstance(v, str):
                 raise NotImplementedError(f"DeviceMD: property_conversion['{k}'] = {v!r}: give the conversion factor as a "
                                           "number (unit strings need ASE's unit tables)")
-        self.property_conversion = {p: float(conversion.get(p, 1.0)) for p in self.required_properties}
-        outputs = getattr(self.model, "model_outputs", None)
-        if outputs is not None:
-            missing = [p for p in self.required_properties if p not in outputs]
-            if missing:
-                raise ValueError(f"DeviceMD: required properties {missing} are not model outputs ({sorted(outputs)})")
+        self.property_conversion = {p: float(conversion.get(p, 1.0)) for p in known}
+        for model in self.ensemble or [self.model]:
+            outputs = getattr(model, "model_outputs", None)
+            if outputs is not None:
+                missing = [p for p in self.required_properties if p not in outputs]
+                if missing:
+                    raise ValueError(f"DeviceMD: required properties {missing} are not model outputs "
+                                     f"({sorted(outputs)})")
         if int(every) < 1 or int(capacity) < 0:
             raise ValueError("DeviceMD: record_every must be >= 1 and record_capacity >= 0")
-        if int(capacity) > 0 and not self.required_properties:
+        if int(capacity) > 0 and not self.required_properties and self.ensemble is None:
             raise ValueError("DeviceMD: record_capacity needs required_properties")
         self.record_every, self.record_capacity = int(every), int(capacity)
         self.properties: Dict[str, Tensor] = {}
@@ -1144,13 +1245,59 @@ class DeviceMD(_CapturedEvaluation):
                                                    device=v.device)
             _lib.call("spk_md_property", ops._p(v), v.numel(), self.property_conversion[p], ops._p(buf), ops._stream())
 
+    def _property_buffer(self, name: str, shape, dtype=torch.float32) -> Tensor:
+        """properties[name] of ``shape`` (and its record series), allocated on first use"""
+        buf = self.properties.get(name)
+        if buf is None:
+            buf = torch.empty(shape, dtype=dtype, device=self.positions.device)
+            self.properties[name] = buf
+            if self.record_capacity:
+                self._records[name] = torch.zeros((self.record_capacity,) + tuple(buf.shape), dtype=dtype,
+                                                  device=buf.device)
+        return buf
+
+    def _ensemble_statistics(self):
+        """EnsembleCalculator._accumulate_results (ensemble_calculator.py:38-59) and _update_system (base_calculator.py:
+        120-141) with the conversions of _update_required_properties (ensemble_calculator.py:70-81): the mean energies
+        and forces drive the step in model units; properties[p] = mean x property_conversion[p] and properties[p_var] =
+        unbiased variance x the same factor, for the energy and forces too (default 1.0); with ``uncertainty_fn`` the
+        per-system uncertainty of the energies and forces as properties holds them."""
+        from .ensemble import ensemble_forces, ensemble_moments, ensemble_workspace
+
+        ek, fk, st, n_rep = self.energy_key, self.force_key, self.stacks, self._n_replicas()
+        conv = self.property_conversion
+        prop = {}
+        for p in conv:
+            view = (n_rep, int(st[p].shape[1]) // n_rep) + tuple(st[p].shape[2:])      # [n_replicas, B, ...]
+            prop[p] = self._property_buffer(p, view)
+            prop[p + "_var"] = self._property_buffer(p + "_var", view)
+        s, unc = self.systems, self.uncertainty_fn
+        need_terms = unc is not None and unc.force_weight > 0
+        if need_terms and not hasattr(self, "_ens_terms"):
+            self._ens_terms = torch.empty(s.n_sys, 2, dtype=torch.float64, device=self.positions.device)
+            self._ens_ws = ensemble_workspace(s.n_atoms, s.n_sys, self.positions.device)
+        ensemble_moments(st[ek], ddof=1, spread_scale=conv[ek], out_mean=self.energy, out_var=prop[ek + "_var"])
+        _lib.call("spk_md_property", ops._p(self.energy), self.energy.numel(), conv[ek], ops._p(prop[ek]), ops._stream())
+        ensemble_forces(st[fk], s.idx_m, s.sys_ptr, s.n_sys, spread_scale=conv[fk], out_mean=self.forces,
+                        out_var=prop[fk + "_var"], terms=need_terms, out_terms=self._ens_terms if need_terms else None,
+                        workspace=self._ens_ws if need_terms else None)
+        _lib.call("spk_md_property", ops._p(self.forces), self.forces.numel(), conv[fk], ops._p(prop[fk]), ops._stream())
+        for p in conv:
+            if p not in (ek, fk):
+                ensemble_moments(st[p], ddof=1, mean_scale=conv[p], spread_scale=conv[p], out_mean=prop[p],
+                                 out_var=prop[p + "_var"])
+        if unc is not None:
+            out = self._property_buffer("uncertainty", (n_rep, s.n_sys // n_rep))
+            unc.combine(st[ek] if unc.energy_weight > 0 else None, self._ens_terms if need_terms else None, s.sys_ptr,
+                        None, None, energy_scale=conv[ek], out_f32=out)
+
     def _record(self):
         if not self.record_capacity:
             return
-        for p in self.required_properties:
+        for p, rec in self._records.items():
             buf = self.properties[p]
             _lib.call("spk_md_record", ops._p(buf), buf.numel(), ops._p(self._rec_counter), self.record_every,
-                      self.record_capacity, ops._p(self._records[p]), ops._stream())
+                      self.record_capacity, ops._p(rec), ops._stream())
         _lib.call("spk_md_record_advance", ops._p(self._rec_counter), self.record_every, self.record_capacity,
                   ops._stream())
 
@@ -1258,6 +1405,7 @@ class DeviceMD(_CapturedEvaluation):
         if self.barostat is not None:
             state.extend(self.barostat._state().values())
         state.extend(self.properties.values())
+        state.extend(self.stacks.values())
         if self.record_capacity:
             state.extend([self._rec_counter] + list(self._records.values()))
         self._graph = self._capture_step(state)
@@ -1372,7 +1520,7 @@ class DeviceMD(_CapturedEvaluation):
             sd.update(cell=self.cell.clone(), model_cell=self.model_cell.clone(), virial=self.virial.clone())
         if self.barostat is not None:
             sd["barostat"] = self.barostat.state_dict()
-        if self.required_properties:
+        if self.properties:
             sd["properties"] = {p: v.clone() for p, v in self.properties.items()}
         if self.record_capacity:
             sd["recorder"] = {"counter": self._rec_counter.clone(), "n_records": self._n_records,

@@ -382,7 +382,10 @@ class GraphedPotential:
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
             out = run()
-        static_out = {k: v.detach() for k, v in out.items()}
+        if isinstance(out, tuple):                   # NNEnsemble: (means, stds)
+            static_out = tuple({k: v.detach() for k, v in o.items()} for o in out)
+        else:
+            static_out = {k: v.detach() for k, v in out.items()}
         return graph, static_in, static_out
 
     def __call__(self, inputs: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:

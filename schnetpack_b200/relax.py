@@ -146,7 +146,11 @@ class DeviceLBFGS(_CapturedEvaluation):
 
     One step is the optimizer kernels, the neighbour list, the model and the convergence test, captured once as a CUDA
     graph (``use_graph``).  ``run`` replays it in chunks of ``check_every`` steps and reads the count of unconverged
-    systems once per chunk; steps replayed after every system has converged leave the positions bitwise unchanged."""
+    systems once per chunk; steps replayed after every system has converged leave the positions bitwise unchanged.
+
+    ``model`` may be a list (or ``nn.ModuleList``) of at least two members, as the reference's
+    BatchwiseEnsembleCalculator (interfaces/batchwise_optimization.py:229-347): the mean forces drive the optimizer
+    and its ``fmax`` test, and ``get_uncertainty`` gives the unbiased std over the members."""
 
     def __init__(self, model: torch.nn.Module, batch: Dict[str, Tensor], cutoff: float, capacity: int,
                  maxstep: float = 0.2, memory: int = 100, damping: float = 1.0, alpha: float = 70.0,
@@ -164,10 +168,12 @@ class DeviceLBFGS(_CapturedEvaluation):
                              f"{sorted(outputs)})")
         from .atomistic.pair_terms import check_ewald_cells, check_padded_pair_terms
 
+        self.energy_key, self.force_key = energy_key, force_key
+        model = self._set_ensemble(model, "DeviceLBFGS")
+
         check_padded_pair_terms(model, float(cutoff), "DeviceLBFGS")
         check_ewald_cells(model, batch, "DeviceLBFGS")
         self.model = model
-        self.energy_key, self.force_key = energy_key, force_key
         self.p_conv = float(position_conversion)
         self.e_conv = float(energy_conversion)
         self.f_conv = self.e_conv / self.p_conv
@@ -202,7 +208,8 @@ class DeviceLBFGS(_CapturedEvaluation):
         self.opt.check(self.forces)
 
     def _state_tensors(self):
-        return list(self.opt.tensors().values()) + [self.energy, self.forces, self.n_pairs, self.nl_watch]
+        return (list(self.opt.tensors().values()) + [self.energy, self.forces, self.n_pairs, self.nl_watch]
+                + list(self.stacks.values()))
 
     def run(self, fmax: float = 0.05, steps: Optional[int] = None, check_every: int = 10) -> bool:
         """Relax until every system's largest force is below ``fmax`` or ``steps`` steps (default: unlimited) were taken
@@ -252,6 +259,17 @@ class DeviceLBFGS(_CapturedEvaluation):
         if self.opt.fixed is not None:
             f = f * (1 - self.opt.fixed.double())[:, None]
         return f
+
+    def get_uncertainty(self) -> Dict[str, Tensor]:
+        """Ensemble runs: the unbiased std over the members of the energies [n_sys] and forces [N, 3] at the current
+        positions, in optimizer units (BatchwiseEnsembleCalculator.calculate, :329-335)"""
+        if self.ensemble is None:
+            raise RuntimeError("DeviceLBFGS: get_uncertainty needs an ensemble (model=[m1, m2, ...])")
+        from .ensemble import ensemble_moments
+
+        e = ensemble_moments(self.stacks[self.energy_key], ddof=1, spread_scale=self.e_conv, var=False, std=True)[2]
+        f = ensemble_moments(self.stacks[self.force_key], ddof=1, spread_scale=self.f_conv, var=False, std=True)[2]
+        return {"energy_uncertainty": e, "forces_uncertainty": f}
 
     @property
     def fmax(self) -> Tensor:
