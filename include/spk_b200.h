@@ -739,6 +739,51 @@ int spk_ensemble_uncertainty(const float* energy, double energy_scale, const dou
                              double energy_weight, double force_weight, double stress_weight, double* out,
                              float* out_f32, spk_stream_t stream);
 
+/* ---- vibrational analysis (csrc/vibrations.cu; ASE's Vibrations / Infrared, atomistic/response.py:95-431,
+ * nn/utils.py:21-126) --------------------------------------------------------------------------------------------------
+ * Finite-difference Hessians of a B-system batch (N atoms, system m = atoms [sys_ptr[m], sys_ptr[m+1]), n_m atoms,
+ * coordinates d = 3 a + k) from C = n_cols * nfree replica-major copies: copy c = d_local * nfree + s holds atoms
+ * [c N, (c+1) N) and systems [c B, (c+1) B) and displaces coordinate d = chunk * n_cols + d_local of every system by
+ * (float)(o_s * delta), o = (-1, +1) for nfree 2 and (-2, -1, +1, +2) for nfree 4; systems with d >= 3 n_m stay
+ * undisplaced in that copy (idle).  counter (int64[2]) = (chunk the next displacement reads, chunk the last displacement
+ * wrote + 1); zero it before the first chunk.
+ *
+ * spk_vib_displace: positions [C N, 3] = base with the displacement rounded to fp32 (__fadd_rn); steps [C, B] fp64 =
+ *   (double)displaced - (double)base of the displaced coordinate (0 for idle copies); counter[1] = counter[0] + 1.
+ * spk_vib_assemble, after the model wrote forces [C N, 3] (and dipole [C B, 3] / polar [C B, 3, 3]): for chunk =
+ *   counter[1] - 1 and every non-idle (system, d): with w_s the weights of the derivative at 0 of the polynomial through
+ *   (steps[c_s, m], y_s), h_raw[hess_ptr[m] + d 3 n_m + r] = -sum_s w_s forces_r (column d, stored transposed),
+ *   dipole_deriv [N, 3, 3] element [i, comp, dir] and polar_deriv [N, 3, 3, 3] element [i, a, b, dir] (each optional)
+ *   = sum_s w_s y_s with atom i = sys_ptr[m] + d / 3, dir = d % 3; counter[0] = counter[1].
+ * spk_vib_finish, once after the last chunk: H = (h_raw + h_raw^T) / 2 per system; hessian [sum n_m^2, 3, 3] fp64 in
+ *   the Response layout (row i n_m + j, block [a, b] = H[3 i + a, 3 j + b]) at hess_ptr[m] (= 9 sum_{m' < m} n_m'^2) and
+ *   hessian_mw [3 n_m, 3 n_m] at the same offset = H * mw_scale / sqrt(masses[i] masses[j]).  max_atoms = max_m n_m.
+ * No atomics; every value is written once: bitwise reproducible. */
+typedef struct {
+    const float* base;         /* [N, 3] undisplaced model positions */
+    float* positions;          /* [C N, 3] replica positions */
+    double* steps;             /* [C, B] realised steps */
+    int64_t* counter;          /* [2] */
+    const float* forces;       /* [C N, 3] */
+    const float* dipole;       /* [C B, 3] or NULL */
+    const float* polar;        /* [C B, 3, 3] or NULL */
+    const int64_t* idx_m;      /* [N] */
+    const int32_t* sys_ptr;    /* [B + 1] */
+    const int64_t* hess_ptr;   /* [B + 1] */
+    const double* masses;      /* [N] */
+    double* h_raw;             /* [sum 9 n_m^2] */
+    double* hessian;           /* [sum n_m^2, 3, 3] */
+    double* hessian_mw;        /* [sum 9 n_m^2] */
+    double* dipole_deriv;      /* [N, 3, 3] or NULL */
+    double* polar_deriv;       /* [N, 3, 3, 3] or NULL */
+    int64_t n_atoms, n_sys, n_cols, nfree, max_atoms;
+    double delta;              /* step in model length units */
+    double mw_scale;           /* energy_conversion / position_conversion^2 */
+} spk_vib_t;
+int spk_vib_displace(const spk_vib_t* params, spk_stream_t stream);
+int spk_vib_assemble(const spk_vib_t* params, spk_stream_t stream);
+int spk_vib_finish(const spk_vib_t* params, spk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -63,6 +63,16 @@ class PairParams(Structure):
 PAIR_ZBL, PAIR_COULOMB, PAIR_DAMPED_COULOMB, PAIR_EWALD_REAL = 0, 1, 2, 3     # SPK_PAIR_*
 PAIR_MAX_TERMS = 16                                       # SPK_PAIR_MAX_TERMS
 
+class VibParams(Structure):
+    """spk_vib_t of include/spk_b200.h (device pointers of the replica batch and the vibrational-analysis buffers)."""
+    _fields_ = [("base", c_void_p), ("positions", c_void_p), ("steps", c_void_p), ("counter", c_void_p),
+                ("forces", c_void_p), ("dipole", c_void_p), ("polar", c_void_p), ("idx_m", c_void_p),
+                ("sys_ptr", c_void_p), ("hess_ptr", c_void_p), ("masses", c_void_p), ("h_raw", c_void_p),
+                ("hessian", c_void_p), ("hessian_mw", c_void_p), ("dipole_deriv", c_void_p), ("polar_deriv", c_void_p),
+                ("n_atoms", c_int64), ("n_sys", c_int64), ("n_cols", c_int64), ("nfree", c_int64),
+                ("max_atoms", c_int64), ("delta", c_double), ("mw_scale", c_double)]
+
+
 RELAX_WARP_ATOMS = 256      # SPK_RELAX_WARP_ATOMS
 RELAX_MAX_MEMORY = 4096     # SPK_RELAX_MAX_MEMORY
 
@@ -179,6 +189,9 @@ SIGNATURES = {
     "spk_ensemble_forces": [P, c_int64, P, P, c_int64, c_int64, c_double, c_double, P, P, P, P, c_size_t, P],
     "spk_ensemble_uncertainty": [P, c_double, P, P, P, c_double, c_int64, c_int64, c_int, c_double, c_double, c_double, P,
                                  P, P],
+    "spk_vib_displace": [POINTER(VibParams), P],
+    "spk_vib_assemble": [POINTER(VibParams), P],
+    "spk_vib_finish": [POINTER(VibParams), P],
 }
 _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_size_t,
             "spk_pairwise_virial_workspace_bytes": c_size_t, "spk_md_barostat_workspace_bytes": c_size_t,

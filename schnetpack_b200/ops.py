@@ -5,6 +5,7 @@ torch arithmetic on the hot path and no CPU fallback (non-CUDA tensors raise).
 """
 from __future__ import annotations
 
+import ctypes
 import os
 import weakref
 from ctypes import c_void_p
@@ -856,3 +857,19 @@ def ewald_bwd(R: Tensor, q: Tensor, cell: Tensor, kvecs: Tensor, idx_m: Tensor, 
               _p(ws), ws.numel(), _stream(),
               launches=(int(K > 0) + 1 if N > 0 else 0) + int(want_cell or virial is not None))
     return g_R, g_cell
+
+
+# ------------------------------------------------------------------------------------------------------- vibrations
+def vib_displace(params: "_lib.VibParams"):
+    """replica positions and realised steps of the chunk the counter names (csrc/vibrations.cu)"""
+    _lib.call("spk_vib_displace", ctypes.byref(params), _stream())
+
+
+def vib_assemble(params: "_lib.VibParams"):
+    """the chunk's Hessian columns and dipole / polarizability derivatives from the replica outputs"""
+    _lib.call("spk_vib_assemble", ctypes.byref(params), _stream())
+
+
+def vib_finish(params: "_lib.VibParams"):
+    """symmetrised Hessian in the Response layout and its mass-weighted blocks, once after the last chunk"""
+    _lib.call("spk_vib_finish", ctypes.byref(params), _stream())
