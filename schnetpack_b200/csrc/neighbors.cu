@@ -4,6 +4,7 @@
 // vesin front ends :213-286 return the same set):
 //   pair (i, j, S) listed  <=>  | R[j] - R[i] + S @ cell | < cutoff,  S integer, S_a = 0 on non-periodic axes,
 //   (i == j, S == 0) excluded, self images (i == j, S != 0) listed;  offsets = S @ cell;  sorted by idx_i.
+// Positions may lie any number of cells away from the cell, and the rows of non-periodic axes may be zero.
 // Everything is enqueue-only on the caller's stream (no host synchronisation: the pair count stays on the device and the
 // tail of the fixed-capacity output can be padded with edges that lie outside the cutoff), deterministic (no atomics: the
 // atoms are ordered by cell with a stable radix sort, rows are written in traversal order), and works in fp32 with the
@@ -38,6 +39,38 @@ __device__ __forceinline__ int find_system(const int32_t* __restrict__ sys_ptr, 
     return lo;
 }
 
+// unit vector along x cross y
+__device__ void cross_unit(const double* x, const double* y, double* out) {
+    const double z[3] = {x[1] * y[2] - x[2] * y[1], x[2] * y[0] - x[0] * y[2], x[0] * y[1] - x[1] * y[0]};
+    const double il = 1.0 / sqrt(z[0] * z[0] + z[1] * z[1] + z[2] * z[2]);
+    for (int k = 0; k < 3; ++k) out[k] = z[k] * il;
+}
+
+// The cell with the rows of the non-periodic axes replaced by an orthonormal completion of the periodic rows: the unit
+// normal of two periodic rows, or two orthogonal unit vectors normal to one.  Fractional coordinates, heights and wraps
+// along the periodic axes then depend on the periodic rows only, and a sheet or a wire whose non-periodic rows are zero
+// (ase.build.graphene(vacuum=None), nanotubes) gets an invertible cell; offsets still use the caller's rows, whose
+// images are 0 on those axes.  A degenerate PERIODIC row is invalid input and is not detected here.
+__device__ void complete_cell(const float* c, const int* pbc, double* m) {
+    int per[3], non[3], n_per = 0, n_non = 0;
+    for (int a = 0; a < 3; ++a) {
+        for (int k = 0; k < 3; ++k) m[3 * a + k] = c[3 * a + k];
+        if (pbc[a]) per[n_per++] = a; else non[n_non++] = a;
+    }
+    if (n_per == 2) {
+        cross_unit(m + 3 * per[0], m + 3 * per[1], m + 3 * non[0]);
+    } else if (n_per == 1) {
+        const double* p = m + 3 * per[0];
+        int least = 0;                                               // the coordinate axis least aligned with p
+        for (int k = 1; k < 3; ++k)
+            if (fabs(p[k]) < fabs(p[least])) least = k;
+        double e[3] = {0.0, 0.0, 0.0};
+        e[least] = 1.0;
+        cross_unit(p, e, m + 3 * non[0]);
+        cross_unit(p, m + 3 * non[0], m + 3 * non[1]);
+    }
+}
+
 __global__ void __launch_bounds__(1024) k_nl_setup(const float* __restrict__ cell, const uint8_t* __restrict__ pbc,
                                                    const int32_t* __restrict__ sys_ptr, int n_sys, float cutoff,
                                                    SysGrid* __restrict__ grid, int* __restrict__ total_cells) {
@@ -58,9 +91,10 @@ __global__ void __launch_bounds__(1024) k_nl_setup(const float* __restrict__ cel
         }
         for (int k = 0; k < 9; ++k) g.inv[k] = 0.f;
         if (any) {
-            // inverse by cofactors in double (3x3)
-            const double a0 = g.c[0], a1 = g.c[1], a2 = g.c[2], b0 = g.c[3], b1 = g.c[4], b2 = g.c[5], c0 = g.c[6], c1 = g.c[7],
-                         c2 = g.c[8];
+            // inverse of the completed cell by cofactors in double (3x3)
+            double m[9];
+            complete_cell(g.c, g.pbc, m);
+            const double a0 = m[0], a1 = m[1], a2 = m[2], b0 = m[3], b1 = m[4], b2 = m[5], c0 = m[6], c1 = m[7], c2 = m[8];
             const double det = a0 * (b1 * c2 - b2 * c1) - a1 * (b0 * c2 - b2 * c0) + a2 * (b0 * c1 - b1 * c0);
             const double id = 1.0 / det;
             double inv[9];

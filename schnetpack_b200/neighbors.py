@@ -35,7 +35,10 @@ def neighbor_list(positions: Tensor, cell: Optional[Tensor], pbc: Optional[Tenso
     * ``capacity=None`` (default): exact size -- a counting pass, one host read of the pair count, then the fill pass;
     * ``capacity=E_max``: no host synchronisation; with ``pad=True`` the result always has ``E_max`` entries, the unused
       capacity being spread over the rows as self pairs at distance 2*cutoff (zero contribution to any cutoff-weighted
-      model; ``idx_i`` stays sorted, no row grows long) -- the form to use under CUDA-graph capture; the returned ``n_pairs`` tensor (device, int64 [2]) holds the true count and an overflow flag.
+      model; ``idx_i`` stays sorted, no row grows long) -- the form to use under CUDA-graph capture; the returned ``n_pairs`` tensor (device, int64 [2]) holds the true count and an overflow flag;
+    * ``capacity=0``: count only, ``n_pairs`` = (pairs, 1 if there are any).
+
+    Positions may lie any number of cells away from the cell, and the rows of non-periodic axes may be zero.
     """
     if not positions.is_cuda:
         raise ValueError("schnetpack_b200.neighbors: positions must be a CUDA tensor (no CPU fallback)")
@@ -65,7 +68,8 @@ def neighbor_list(positions: Tensor, cell: Optional[Tensor], pbc: Optional[Tenso
         _lib.call("spk_neighbor_list", p(R), p(cell), p(pbc), p(sys_ptr), N, B, float(cutoff), cap, 1 if do_pad else 0,
                   p(idx_i), p(idx_j), p(off), p(sh), p(n_pairs), p(ws), ws.numel(), ops._stream())
 
-    if capacity is None:
+    exact = capacity is None
+    if exact:
         run(0, None, None, None, None, False)            # count only
         capacity = int(n_pairs[0].item())                # the one host read of the exact-size mode
         pad = False
@@ -73,7 +77,7 @@ def neighbor_list(positions: Tensor, cell: Optional[Tensor], pbc: Optional[Tenso
     idx_j = torch.empty(capacity, dtype=torch.int64, device=dev)
     off = torch.empty((capacity, 3), dtype=torch.float32, device=dev)
     sh = torch.empty((capacity, 3), dtype=torch.int32, device=dev) if return_shifts else None
-    if capacity > 0 or pad:
+    if capacity > 0 or not exact:                        # capacity=0 counts: n_pairs = (total, total > 0)
         run(capacity, idx_i, idx_j, off, sh, pad)
     out = (idx_i, idx_j, off) + ((sh,) if return_shifts else ())
     return out + (n_pairs,)

@@ -35,6 +35,12 @@ def cases():
     slab = np.diag([11.0, 12.5, 30.0])
     out["slab"] = dict(R=rng.uniform(0, 1, size=(80, 3)) @ np.diag([11.0, 12.5, 9.0]), cell=slab,
                        pbc=[True, True, False], cutoff=5.0)
+    # primitive fcc cell: one atom, 60 degree angles, every height a / sqrt(3) far below the cutoff
+    fcc = 4.05 / 2 * np.array([[0.0, 1.0, 1.0], [1.0, 0.0, 1.0], [1.0, 1.0, 0.0]])
+    out["fcc_primitive"] = dict(R=np.array([[0.3, -0.2, 0.1]]), cell=fcc, pbc=[True] * 3, cutoff=5.0)
+    # strongly skewed triclinic cell: edges of 8-10 A, one height of 2.4 A below the cutoff
+    skew = np.array([[8.0, 0.0, 0.0], [7.0, 3.5, 0.0], [6.0, 1.5, 2.4]])
+    out["skewed"] = dict(R=rng.uniform(0, 1, size=(30, 3)) @ skew, cell=skew, pbc=[True] * 3, cutoff=4.0)
     return out
 
 

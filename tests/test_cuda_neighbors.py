@@ -40,7 +40,7 @@ def _same_set(out, ref, n=None):
     return n
 
 
-@pytest.mark.parametrize("name", ["molecule", "cubic", "small_box", "triclinic", "slab"])
+@pytest.mark.parametrize("name", ["molecule", "cubic", "small_box", "triclinic", "slab", "fcc_primitive", "skewed"])
 def test_neighbor_list_matches_reference_fixture(name):
     d = np.load(os.path.join(GOLD, f"nl_{name}.npz"))
     R = d["positions"].astype(np.float32)
