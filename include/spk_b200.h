@@ -521,6 +521,10 @@ int spk_md_property(const float* src, int64_t n, float conversion, float* dst, s
 int spk_md_record(const float* src, int64_t n, const int64_t* counter, int64_t every, int64_t capacity, float* buf,
                   spk_stream_t stream);
 int spk_md_record_advance(int64_t* counter, int64_t every, int64_t capacity, spk_stream_t stream);
+/* velocity record (the FileLogger's MoleculeStream with store_velocities): on a recorded step (as spk_md_record)
+ * buf[counter[1] * 3 n_atoms + 3 a + k] = momenta[a, k] / masses[a]; call it before spk_md_record_advance. */
+int spk_md_record_velocities(const float* momenta, const float* masses, int64_t n_atoms, const int64_t* counter,
+                             int64_t every, int64_t capacity, float* buf, spk_stream_t stream);
 
 /* ---- gated equivariant output heads (csrc/equivariant.cu) -------------------------------------------------------------
  * nn/equivariant.py:57-71 (GatedEquivariantBlock), atomistic/atomwise.py:172-213 (DipoleMoment), :267-293
@@ -783,6 +787,31 @@ typedef struct {
 int spk_vib_displace(const spk_vib_t* params, spk_stream_t stream);
 int spk_vib_assemble(const spk_vib_t* params, spk_stream_t stream);
 int spk_vib_finish(const spk_vib_t* params, spk_stream_t stream);
+
+/* ---- vibrational spectra from recorded MD series (csrc/spectra.cu; md/data/spectra.py) ------------------------------
+ * spk_spectrum_series: records [T, P, stride] fp32 (P replicas).  Output field f (of F) is
+ *   x_f[t] = sum_{j<3, index[f, j] >= 0} coef[f, j] d(index[f, j], t),  d(i, t) = c(i, t) (derivative == 0, n = T) or
+ *   (c(i, t + 2) - c(i, t)) / (2 dt_fs) (derivative != 0, n = T - 2),  c(i, t) = (sum_r records[t, r, i]) / P,
+ *   all in fp64; then mean[f] = sum_t x_f / n, std[f] = sqrt(sum_t (x_f - mean)^2 / n) and z [F, n] = (x - mean) / std.
+ *   index [F, 3] int64, coef [F, 3] fp64, mean / std [F] fp64 (device).  Fixed-order sums, no atomics.
+ * spk_spectrum_autocorrelation: channel c holds the fields [ch_ptr[c], ch_ptr[c+1]) of z [F, n] with weights w [F]:
+ *   acf [C, L] = (1/n) sum_f w_f sum_{t < n-k} z_f[t] z_f[t+k] for k < L (L <= n - 1), computed as the band of the Gram
+ *   matrix on the fp64 tensor cores over fixed time chunks of SPK_SPECTRUM_CHUNK rows; the per-chunk partials (in the
+ *   workspace) are summed in a fixed order, so a channel's result does not depend on the other channels of the launch.
+ * spk_spectrum_transform: out [C, 4L] = 2 dt_fs |sum_{i<L} acf[c, i] window[i] cos(pi m (2i+1) / (8L))| (window NULL:
+ *   none), the DCT-II form of |dt FFT| of the zero-padded, mirrored series; m (2i+1) is reduced modulo 16 L before the
+ *   cosine, which comes from a quarter-wave table of cospi values.
+ * Both take spk_spectrum_workspace_bytes(C, n, L) bytes of workspace, 8-byte aligned. */
+#define SPK_SPECTRUM_CHUNK 2048
+size_t spk_spectrum_workspace_bytes(int64_t n_channels, int64_t n, int64_t n_lags);
+int spk_spectrum_series(const float* records, int64_t T, int64_t P, int64_t stride, const int64_t* index,
+                        const double* coef, int64_t F, int derivative, double dt_fs, double* z, double* mean, double* std,
+                        spk_stream_t stream);
+int spk_spectrum_autocorrelation(const double* z, int64_t n, const int64_t* ch_ptr, const double* weight,
+                                 int64_t n_channels, int64_t n_lags, double* acf, void* workspace,
+                                 size_t workspace_bytes, spk_stream_t stream);
+int spk_spectrum_transform(const double* acf, int64_t n_channels, int64_t n_lags, const double* window, double dt_fs,
+                           double* out, void* workspace, size_t workspace_bytes, spk_stream_t stream);
 
 #ifdef __cplusplus
 }

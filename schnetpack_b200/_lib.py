@@ -192,6 +192,11 @@ SIGNATURES = {
     "spk_vib_displace": [POINTER(VibParams), P],
     "spk_vib_assemble": [POINTER(VibParams), P],
     "spk_vib_finish": [POINTER(VibParams), P],
+    "spk_md_record_velocities": [P, P, c_int64, P, c_int64, c_int64, P, P],
+    "spk_spectrum_workspace_bytes": [c_int64, c_int64, c_int64],
+    "spk_spectrum_series": [P, c_int64, c_int64, c_int64, P, P, c_int64, c_int, c_double, P, P, P, P],
+    "spk_spectrum_autocorrelation": [P, c_int64, P, P, c_int64, c_int64, P, P, c_size_t, P],
+    "spk_spectrum_transform": [P, c_int64, c_int64, P, c_double, P, P, c_size_t, P],
 }
 _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_size_t,
             "spk_pairwise_virial_workspace_bytes": c_size_t, "spk_md_barostat_workspace_bytes": c_size_t,
@@ -200,7 +205,8 @@ _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_siz
             "spk_md_thermostat_workspace_bytes": c_size_t, "spk_rpmd_workspace_bytes": c_size_t,
             "spk_rpmd_barostat_workspace_bytes": c_size_t, "spk_head_workspace_bytes": c_size_t,
             "spk_head_charges_bwd_workspace_bytes": c_size_t, "spk_pair_energy_workspace_bytes": c_size_t,
-            "spk_ewald_workspace_bytes": c_size_t, "spk_ensemble_workspace_bytes": c_size_t}
+            "spk_ewald_workspace_bytes": c_size_t, "spk_ensemble_workspace_bytes": c_size_t,
+            "spk_spectrum_workspace_bytes": c_size_t}
 
 _lib = None
 
@@ -245,7 +251,7 @@ LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out
             "spk_md_barostat_half_step": 2, "spk_md_barostat_main_step": 2, "spk_rpmd_barostat_half_step": 2,
             "spk_rpmd_barostat_main_step": 2, "spk_head_fwd": 2,
             "spk_relax_converged": 2, "spk_pair_energy_fwd": 2, "spk_head_charges_bwd": 3,
-            "spk_pairwise_virial_add": 2}   # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global
+            "spk_pairwise_virial_add": 2, "spk_spectrum_autocorrelation": 2, "spk_spectrum_transform": 2}   # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global
 launch_count = 0
 
 

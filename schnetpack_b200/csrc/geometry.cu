@@ -261,6 +261,16 @@ __global__ void k_md_record(const float* __restrict__ src, int64_t n, const int6
     buf[slot * n + i] = src[i];
 }
 
+__global__ void k_md_record_velocities(const float* __restrict__ momenta, const float* __restrict__ masses, int64_t n,
+                                       const int64_t* __restrict__ counter, int64_t every, int64_t capacity,
+                                       float* __restrict__ buf) {
+    SPK_PDL_ENTER();
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const int64_t step = counter[0] + 1, slot = counter[1];
+    if (i >= 3 * n || step % every != 0 || slot >= capacity) return;
+    buf[slot * 3 * n + i] = momenta[i] / masses[i / 3];
+}
+
 __global__ void k_md_record_advance(int64_t* __restrict__ counter, int64_t every, int64_t capacity) {
     SPK_PDL_ENTER();
     if (threadIdx.x != 0) return;
@@ -457,6 +467,17 @@ extern "C" int spk_md_record(const float* src, int64_t n, const int64_t* counter
 extern "C" int spk_md_record_advance(int64_t* counter, int64_t every, int64_t capacity, spk_stream_t stream) {
     if (!counter || every <= 0 || capacity <= 0) return SPK_ERR_ARG;
     spk_launch(k_md_record_advance, 1, 32, 0, spk_st(stream), counter, every, capacity);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_md_record_velocities(const float* momenta, const float* masses, int64_t n_atoms,
+                                        const int64_t* counter, int64_t every, int64_t capacity, float* buf,
+                                        spk_stream_t stream) {
+    if (n_atoms < 0 || every <= 0 || capacity <= 0) return SPK_ERR_ARG;
+    if (n_atoms == 0) return SPK_OK;
+    if (!momenta || !masses || !counter || !buf) return SPK_ERR_ARG;
+    spk_launch(k_md_record_velocities, GRID1D(3 * n_atoms, 256), momenta, masses, n_atoms, counter, every, capacity, buf);
     SPK_LAUNCH_CHECK();
     return SPK_OK;
 }

@@ -983,7 +983,7 @@ class DeviceMD(_CapturedEvaluation):
                  compute_stress: bool = False, ring_polymer: Optional[RingPolymer] = None,
                  required_properties: Optional[List[str]] = None,
                  property_conversion: Optional[Dict[str, float]] = None, record_every: int = 1,
-                 record_capacity: int = 0, uncertainty_fn: Optional[object] = None):
+                 record_capacity: int = 0, uncertainty_fn: Optional[object] = None, record_velocities: bool = False):
         """``batch[_positions]`` (and ``_cell``) are in MODEL units as everywhere in this package; ``self.positions`` is the
         MD-unit state (= model positions / position_conversion).  ``thermostat`` (None = NVE) is bound to the systems of
         the batch and applied around every step.  ``barostat`` (an NHC barostat, which thermostats the particles itself)
@@ -1003,7 +1003,10 @@ class DeviceMD(_CapturedEvaluation):
         ASE's unit tables.  With ``record_capacity`` > 0 the step also appends them to a device-side time series every
         ``record_every`` steps (steps s with s % record_every == 0, counted from the start), written inside the captured
         step; ``recorded(name)`` returns the series, ``drain()`` empties it, and ``run`` refuses a call that would store
-        more than ``record_capacity`` records since the last drain.
+        more than ``record_capacity`` records since the last drain.  ``record_velocities`` adds the series
+        ``"velocities"`` [record_capacity, n_replicas, N, 3] = momenta / masses in MD units (the FileLogger's
+        MoleculeStream with store_velocities), which power spectra need; it needs ``record_capacity`` > 0 and no
+        required property of that name.  ``series()`` hands the records since the last drain to ``spectra``.
 
         ``model`` may be a list (or ``nn.ModuleList``) of at least two members: an ensemble run
         (md/calculators/ensemble_calculator.py).  Every member runs on the step's one neighbour list, the mean energies and
@@ -1099,7 +1102,8 @@ class DeviceMD(_CapturedEvaluation):
                 barostat.bind(self._rp_base, self.dt, ring_polymer)               # on_simulation_start
             else:
                 barostat.bind(self.systems, self.dt)
-        self._setup_properties(required_properties, property_conversion, record_every, record_capacity)
+        self._setup_properties(required_properties, property_conversion, record_every, record_capacity,
+                               record_velocities)
         self._calculate()                       # forces at t = 0 (simulator.py:118)
 
     @property
@@ -1195,8 +1199,11 @@ class DeviceMD(_CapturedEvaluation):
         return out
 
     # ---- per-step model properties and their device-side time series ------------------------------------------------------
-    def _setup_properties(self, required, conversion, every, capacity):
+    def _setup_properties(self, required, conversion, every, capacity, velocities=False):
         self.required_properties = list(dict.fromkeys(required or []))
+        if velocities and "velocities" in self.required_properties:
+            raise ValueError("DeviceMD: record_velocities records the series 'velocities'; a required property of that "
+                             "name would share it")
         conversion = dict(conversion or {})
         known = list(self.required_properties)
         if self.ensemble is not None:                # energy and forces are always required (base_calculator.py:65-69)
@@ -1218,11 +1225,17 @@ class DeviceMD(_CapturedEvaluation):
                                      f"({sorted(outputs)})")
         if int(every) < 1 or int(capacity) < 0:
             raise ValueError("DeviceMD: record_every must be >= 1 and record_capacity >= 0")
-        if int(capacity) > 0 and not self.required_properties and self.ensemble is None:
-            raise ValueError("DeviceMD: record_capacity needs required_properties")
+        if int(capacity) > 0 and not self.required_properties and self.ensemble is None and not velocities:
+            raise ValueError("DeviceMD: record_capacity needs required_properties or record_velocities")
+        if velocities and int(capacity) < 1:
+            raise ValueError("DeviceMD: record_velocities needs record_capacity > 0")
         self.record_every, self.record_capacity = int(every), int(capacity)
         self.properties: Dict[str, Tensor] = {}
         self._records: Dict[str, Tensor] = {}
+        if velocities:
+            n_rep = self._n_replicas()
+            self._records["velocities"] = torch.zeros(self.record_capacity, n_rep, self.positions.shape[0] // n_rep, 3,
+                                                      dtype=torch.float32, device=self.positions.device)
         self._n_records = 0                      # host mirror of the device count: the record count is deterministic
         self._rec_counter = torch.zeros(2, dtype=torch.int64, device=self.positions.device)
 
@@ -1295,6 +1308,11 @@ class DeviceMD(_CapturedEvaluation):
         if not self.record_capacity:
             return
         for p, rec in self._records.items():
+            if p == "velocities":
+                _lib.call("spk_md_record_velocities", ops._p(self.momenta), ops._p(self.masses), self.momenta.shape[0],
+                          ops._p(self._rec_counter), self.record_every, self.record_capacity, ops._p(rec),
+                          ops._stream())
+                continue
             buf = self.properties[p]
             _lib.call("spk_md_record", ops._p(buf), buf.numel(), ops._p(self._rec_counter), self.record_every,
                       self.record_capacity, ops._p(rec), ops._stream())
@@ -1312,6 +1330,20 @@ class DeviceMD(_CapturedEvaluation):
             raise KeyError(f"DeviceMD: '{name}' is not recorded (required_properties={self.required_properties}, "
                            f"record_capacity={self.record_capacity})")
         return self._records[name][:self._n_records].cpu()
+
+    def series(self):
+        """The records since the last ``drain`` as a ``spectra.RecordedSeries``: device views (no copy) with the record
+        time step ``record_every * time_step`` in fs and the systems of one replica."""
+        from .spectra import RecordedSeries
+
+        if not self.record_capacity:
+            raise RuntimeError("DeviceMD: series() needs a recorder (record_capacity > 0)")
+        n = self._n_records
+        base = self._rp_base if self.ring_polymer is not None else self.systems
+        vel = self._records.get("velocities")
+        return RecordedSeries(self.record_every * self.dt / FS_MD, base.sys_ptr, self._n_replicas(),
+                              velocities=None if vel is None else vel[:n],
+                              properties={p: v[:n] for p, v in self._records.items() if p != "velocities"})
 
     def drain(self) -> Dict[str, Tensor]:
         """Return every recorded series (as ``recorded``) and empty the recorder."""

@@ -1,0 +1,299 @@
+"""Vibrational spectra from the series ``DeviceMD`` records (md/data/spectra.py: PowerSpectrum, IRSpectrum,
+RamanSpectrum; DESIGN.md section 17).
+
+The reference reads an HDF5 file, takes the centroid over the replicas, differentiates dipoles and polarizabilities by
+central differences, normalises every field, autocorrelates it through a zero-padded FFT, combines the fields into
+channels, windows the first ``resolution`` lags and takes |dt FFT| of the zero-padded, mirrored result.  Here the same
+numbers come from three fp64 kernels on the device records (csrc/spectra.cu): the series preparation, the lag-window
+autocorrelation (direct, on the fp64 tensor cores) and the spectral transform (its DCT-II form).  Results are fp64
+device tensors.  ``molecule_idx=None`` computes every system of the batch in the same launches, with a leading B axis on
+the intensities; each row is bitwise equal to the call for that index.
+
+Raman intensities use the reference's cross-section exactly as written, with ``hbar2icm`` and ``kB`` in the MD unit
+system (units.py:79-88); DESIGN.md section 17 notes what that factor evaluates to.
+"""
+from __future__ import annotations
+
+from typing import Callable, Dict, List, Optional, Tuple, Union
+
+import numpy as np
+import torch
+
+from . import _lib, ops
+from . import properties as P
+from .md import HBAR_MD, KB_MD
+from .units import _UNITS
+
+__all__ = ["RecordedSeries", "PowerSpectrum", "IRSpectrum", "RamanSpectrum", "cosine_sq_window", "HBAR2ICM"]
+
+Tensor = torch.Tensor
+
+_C = _UNITS["_c"]                                           # ase.units._c, m/s
+HBAR2ICM = HBAR_MD * 100.0 * _C * _UNITS["_aut"]            # units.py:88, in MD units
+RAMAN_FACTOR = 4.160440e-18                                 # md/data/spectra.py:478
+
+
+def cosine_sq_window(n_points: int) -> np.ndarray:
+    """cos(pi i / (n - 1) / 2)^2 for i < n (md/data/spectra.py:24-35)"""
+    points = np.arange(n_points)
+    return np.cos(np.pi * points / (n_points - 1) / 2) ** 2
+
+
+class RecordedSeries:
+    """Records of a ``DeviceMD`` run in the layout its recorder writes: ``velocities`` [T, n_replicas, N, 3] and
+    ``properties[name]`` [T, n_replicas, B, ...] (fp32), with the record time step ``dt_fs`` in fs and ``sys_ptr``
+    [B + 1], the first atom of every system of one replica.  ``DeviceMD.series()`` builds one from device views; build
+    one from tensors to feed drained or stored records back (they are moved to ``device``, default: where they are)."""
+
+    def __init__(self, dt_fs: float, sys_ptr, n_replicas: int, velocities: Optional[Tensor] = None,
+                 properties: Optional[Dict[str, Tensor]] = None, device=None):
+        self.dt_fs = float(dt_fs)
+        self.n_replicas = int(n_replicas)
+        ptr = torch.as_tensor(sys_ptr).reshape(-1)
+        self.sys_ptr = [int(v) for v in ptr.tolist()]
+        if not (self.dt_fs > 0.0) or self.n_replicas < 1 or len(self.sys_ptr) < 2:
+            raise ValueError("RecordedSeries: needs dt_fs > 0, n_replicas >= 1 and sys_ptr with at least two entries")
+        if any(b < a for a, b in zip(self.sys_ptr, self.sys_ptr[1:])) or self.sys_ptr[0] != 0:
+            raise ValueError("RecordedSeries: sys_ptr must start at 0 and be non-decreasing")
+
+        def _take(v):
+            v = torch.as_tensor(v)
+            return (v if device is None else v.to(device)).to(torch.float32).contiguous()
+
+        self.velocities = None if velocities is None else _take(velocities)
+        if self.velocities is not None and tuple(self.velocities.shape[1:]) != (self.n_replicas, self.sys_ptr[-1], 3):
+            raise ValueError(f"RecordedSeries: velocities must be [T, {self.n_replicas}, {self.sys_ptr[-1]}, 3], got "
+                             f"{tuple(self.velocities.shape)}")
+        self.properties = {k: _take(v) for k, v in (properties or {}).items()}
+
+    @property
+    def n_systems(self) -> int:
+        return len(self.sys_ptr) - 1
+
+
+Window = Optional[Callable[[int], np.ndarray]]
+
+
+class VibrationalSpectrum:
+    """Base of the spectra (md/data/spectra.py:58-230): ``compute_spectrum(molecule_idx)`` then ``get_spectrum()``."""
+
+    derivative = True
+
+    def __init__(self, data, resolution: int = 4096, window: Window = cosine_sq_window):
+        if not hasattr(data, "series") and not isinstance(data, RecordedSeries):
+            raise TypeError(f"{type(self).__name__}: data must be a DeviceMD or a RecordedSeries")
+        if int(resolution) < 1:
+            raise ValueError(f"{type(self).__name__}: resolution must be positive, got {resolution}")
+        self.data = data
+        self.resolution = int(resolution)
+        self.window = window
+        self.timestep = self._series().dt_fs
+        self.res = 0.5 / self.timestep / (_C / 1e13) / (4 * self.resolution)      # spectral resolution, cm^-1
+        self.frequencies: List[Tensor] = []
+        self.intensities: List[Tensor] = []
+
+    def _series(self) -> RecordedSeries:
+        return self.data if isinstance(self.data, RecordedSeries) else self.data.series()
+
+    # ---- what the subclasses define -------------------------------------------------------------------------------------
+    def _records(self, s: RecordedSeries) -> Tensor:
+        raise NotImplementedError
+
+    def _fields(self, s: RecordedSeries, m: int):
+        """(index rows [F_m, 3], coefficient rows [F_m, 3], channels [(first field, weights)]) of molecule m"""
+        raise NotImplementedError
+
+    def _process_spectrum(self, intensities: List[Tensor], frequencies: Tensor) -> List[Tensor]:
+        return intensities
+
+    # ---- the computation -------------------------------------------------------------------------------------------------
+    def compute_spectrum(self, molecule_idx: Optional[int] = 0):
+        """Spectra of system ``molecule_idx`` of the batch, or of every system (``None``, leading B axis)."""
+        s = self._series()
+        B = s.n_systems
+        if molecule_idx is None:
+            mols = list(range(B))
+        else:
+            if isinstance(molecule_idx, bool) or not isinstance(molecule_idx, (int, np.integer)):
+                raise TypeError(f"{type(self).__name__}: molecule_idx must be an int or None")
+            m = int(molecule_idx)
+            if not -B <= m < B:
+                raise IndexError(f"{type(self).__name__}: molecule_idx {m} out of range for {B} systems")
+            mols = [m % B]
+        rec = self._records(s)
+        if rec.device.type != "cuda":
+            raise ValueError(f"{type(self).__name__}: the records must be on a CUDA device (no CPU fallback)")
+        T = int(rec.shape[0])
+        n = T - 2 if self.derivative else T
+        if n < 3:
+            raise ValueError(f"{type(self).__name__}: {T} records give {n} points, fewer than the 3 that 2 lags need "
+                             f"(need at least {5 if self.derivative else 3} records)")
+        L = min(self.resolution, n - 1)
+        index, coef, ch_ptr, weight = [], [], [0], []
+        n_out = None
+        for m in mols:
+            idx_m, coef_m, channels = self._fields(s, m)
+            base = len(index)
+            index += idx_m
+            coef += coef_m
+            for first, w in channels:
+                ch_ptr.append(base + first + len(w))
+                weight += list(w)
+            n_out = len(channels)
+        dev = rec.device
+        F, C = len(index), len(ch_ptr) - 1
+        assert len(weight) == F and ch_ptr[-1] == F
+        index_t = torch.tensor(index, dtype=torch.int64).to(dev)
+        coef_t = torch.tensor(coef, dtype=torch.float64).to(dev)
+        ch_t = torch.tensor(ch_ptr, dtype=torch.int64).to(dev)
+        w_t = torch.tensor(weight, dtype=torch.float64).to(dev)
+        z = torch.empty(F, n, dtype=torch.float64, device=dev)
+        mean = torch.empty(F, dtype=torch.float64, device=dev)
+        std = torch.empty(F, dtype=torch.float64, device=dev)
+        stride = rec[0, 0].numel()
+        with torch.cuda.device(dev):
+            _lib.call("spk_spectrum_series", ops._p(rec), T, s.n_replicas, stride, ops._p(index_t), ops._p(coef_t), F,
+                      1 if self.derivative else 0, self.timestep, ops._p(z), ops._p(mean), ops._p(std), ops._stream())
+            acf = autocorrelation(z, ch_t, w_t, L)
+            win = None
+            if self.window is not None:
+                win = torch.as_tensor(np.asarray(self.window(L), dtype=np.float64)).reshape(-1).to(dev)
+                if win.numel() != L:
+                    raise ValueError(f"{type(self).__name__}: the window gave {win.numel()} points for {L} lags")
+            spec = transform(acf, win, self.timestep)
+        self.autocorrelation = acf.reshape(len(mols), n_out, L)
+        spec = spec.reshape(len(mols), n_out, 4 * L)
+        frequencies = np.arange(8 * L // 2) / (8 * L * self.timestep)       # numpy divides as the reference does
+        frequencies = torch.as_tensor(frequencies / (_C / 1e13)).to(dev)
+        intensities = [spec[:, j] for j in range(n_out)]
+        intensities = self._process_spectrum(intensities, frequencies)
+        if molecule_idx is not None:
+            intensities = [v[0] for v in intensities]
+        self.frequencies = [frequencies] * len(intensities)
+        self.intensities = intensities
+
+    def get_spectrum(self) -> Union[Tuple[Tensor, Tensor], List[Tuple[Tensor, Tensor]]]:
+        """(frequencies in cm^-1, intensities) of every computed spectrum; the tuple itself when there is one"""
+        spectrum = list(zip(self.frequencies, self.intensities))
+        return spectrum[0] if len(spectrum) == 1 else spectrum
+
+
+class PowerSpectrum(VibrationalSpectrum):
+    """Vibrational density of states from the recorded velocities (``DeviceMD(..., record_velocities=True)``):
+    the autocorrelations of every velocity component, summed over xyz and averaged over the atoms."""
+
+    derivative = False
+
+    def __init__(self, data, resolution: int = 4096, window: Window = cosine_sq_window):
+        super().__init__(data, resolution=resolution, window=window)
+
+    def _records(self, s):
+        if s.velocities is None:
+            raise KeyError("PowerSpectrum: velocities are not recorded (create DeviceMD with record_velocities=True)")
+        return s.velocities
+
+    def _fields(self, s, m):
+        a0, a1 = s.sys_ptr[m], s.sys_ptr[m + 1]
+        if a1 == a0:
+            raise ValueError(f"PowerSpectrum: system {m} has no atoms")
+        idx = [[3 * a + k, -1, -1] for a in range(a0, a1) for k in range(3)]
+        coef = [[1.0, 0.0, 0.0]] * len(idx)
+        return idx, coef, [(0, [1.0 / (a1 - a0)] * len(idx))]
+
+
+class IRSpectrum(VibrationalSpectrum):
+    """Infrared spectrum from the recorded dipole moments: autocorrelations of the central-difference derivative,
+    summed over xyz."""
+
+    def __init__(self, data, resolution: int = 4096, dipole_moment_handle: str = P.dipole_moment,
+                 window: Window = cosine_sq_window):
+        self.dipole_moment_handle = dipole_moment_handle
+        super().__init__(data, resolution=resolution, window=window)
+
+    def _records(self, s):
+        return _property(s, self.dipole_moment_handle, (3,), "IRSpectrum")
+
+    def _fields(self, s, m):
+        return [[3 * m + k, -1, -1] for k in range(3)], [[1.0, 0.0, 0.0]] * 3, [(0, [1.0, 1.0, 1.0])]
+
+
+class RamanSpectrum(VibrationalSpectrum):
+    """Raman spectrum from the recorded polarizabilities: isotropic and anisotropic channels of the central-difference
+    derivative (xx and xy; rotationally averaged with ``averaged=True``), times the reference's cross-section.  With
+    ``averaged`` the spectra are the parallel and orthogonal polarisations."""
+
+    def __init__(self, data, incident_frequency: float, temperature: float,
+                 polarizability_handle: str = P.polarizability, resolution: int = 4096, averaged: bool = False,
+                 window: Window = cosine_sq_window):
+        if not float(temperature) > 0.0:
+            raise ValueError(f"RamanSpectrum: temperature must be positive, got {temperature}")
+        self.incident_frequency = float(incident_frequency)
+        self.temperature = float(temperature)
+        self.averaged = bool(averaged)
+        self.polarizability_handle = polarizability_handle
+        super().__init__(data, resolution=resolution, window=window)
+
+    def _records(self, s):
+        return _property(s, self.polarizability_handle, (3, 3), "RamanSpectrum")
+
+    def _fields(self, s, m):
+        o = 9 * m
+        xx, xy, xz, yy, yz, zz = o, o + 1, o + 2, o + 4, o + 5, o + 8
+        if not self.averaged:
+            return [[xx, -1, -1], [xy, -1, -1]], [[1.0, 0.0, 0.0]] * 2, [(0, [1.0]), (1, [1.0])]
+        third = 1.0 / 3.0
+        idx = [[xx, yy, zz], [xx, yy, -1], [yy, zz, -1], [zz, xx, -1], [xy, -1, -1], [xz, -1, -1], [yz, -1, -1]]
+        coef = [[third] * 3, [1.0, -1.0, 0.0], [1.0, -1.0, 0.0], [1.0, -1.0, 0.0]] + [[1.0, 0.0, 0.0]] * 3
+        return idx, coef, [(0, [1.0]), (1, [0.5, 0.5, 0.5, 3.0, 3.0, 3.0])]
+
+    def _process_spectrum(self, intensities, frequencies):
+        """md/data/spectra.py:462-485, as the reference writes it"""
+        cross_section = ((self.incident_frequency - frequencies) ** 4 / frequencies
+                         / (1 - torch.exp(-(HBAR2ICM * frequencies) / (KB_MD * self.temperature))))
+        cross_section[0] = 0
+        out = []
+        for v in intensities:
+            v = v * cross_section * RAMAN_FACTOR
+            v[..., 0] = 0.0
+            out.append(v)
+        if self.averaged:
+            iso, aniso = out
+            out = [iso + 4 / 45 * aniso, aniso / 15]
+        return out
+
+
+def _property(s: RecordedSeries, name: str, shape, who: str) -> Tensor:
+    v = s.properties.get(name)
+    if v is None:
+        raise KeyError(f"{who}: '{name}' is not recorded (recorded: {sorted(s.properties)}); add it to "
+                       "required_properties with record_capacity > 0")
+    want = (s.n_replicas, s.n_systems) + tuple(shape)
+    if tuple(v.shape[1:]) != want:
+        raise ValueError(f"{who}: '{name}' records must be [T, {', '.join(map(str, want))}], got {tuple(v.shape)}")
+    return v
+
+
+def _workspace(n_channels: int, n: int, L: int, dev) -> Tensor:
+    nbytes = int(_lib.lib().spk_spectrum_workspace_bytes(n_channels, n, L))
+    return torch.empty(max(nbytes, 8), dtype=torch.uint8, device=dev)
+
+
+def autocorrelation(z: Tensor, ch_ptr: Tensor, weight: Tensor, n_lags: int) -> Tensor:
+    """acf [C, n_lags] = (1/n) sum_{f in channel c} w_f sum_t z_f[t] z_f[t + k] of normalised series z [F, n] fp64"""
+    F, n = z.shape
+    C = int(ch_ptr.numel()) - 1
+    out = torch.empty(C, n_lags, dtype=torch.float64, device=z.device)
+    ws = _workspace(C, n, n_lags, z.device)
+    _lib.call("spk_spectrum_autocorrelation", ops._p(z), n, ops._p(ch_ptr), ops._p(weight), C, n_lags, ops._p(out),
+              ops._p(ws), ws.numel(), ops._stream())
+    return out
+
+
+def transform(acf: Tensor, window: Optional[Tensor], dt_fs: float) -> Tensor:
+    """intensities [C, 4L] = |dt FFT| of the windowed, zero-padded, mirrored acf [C, L] (its DCT-II form)"""
+    C, L = acf.shape
+    out = torch.empty(C, 4 * L, dtype=torch.float64, device=acf.device)
+    ws = _workspace(0, 1, L, acf.device)
+    _lib.call("spk_spectrum_transform", ops._p(acf), C, L, ops._p(window), float(dt_fs), ops._p(out), ops._p(ws),
+              ws.numel(), ops._stream())
+    return out
