@@ -60,8 +60,9 @@ import torch
 
 from . import _lib, ops
 from . import properties as P
-from .atomistic.pair_terms import padded_list_cutoff
+from .atomistic.pair_terms import check_ewald_cells, check_padded_pair_terms, padded_list_cutoff
 from .neighbors import CellListNeighborList
+from .units import _amu, _e, _hbar, _k, _Nav
 
 __all__ = ["DeviceMD", "BerendsenThermostat", "LangevinThermostat", "NHCThermostat", "NHCBarostatIsotropic",
            "NHCBarostatAnisotropic", "RingPolymer", "PILELocalThermostat", "PILEGlobalThermostat", "TRPMDThermostat",
@@ -71,30 +72,28 @@ __all__ = ["DeviceMD", "BerendsenThermostat", "LangevinThermostat", "NHCThermost
 Tensor = torch.Tensor
 
 # ---- MD units of the reference (units.py:10-40): energy kJ/mol, length nm, mass Da; time = nm sqrt(Da / (kJ/mol)).
-# Restated from the CODATA-2014 constants that ASE's units module is built on (Boltzmann constant, elementary charge,
-# Avogadro constant, atomic mass unit), in ASE's frame (eV, Angstrom, amu): kJ/mol = 1e3 / (e N_A) eV, nm = 10 Angstrom,
+# From the CODATA-2014 constants of ``units`` (Boltzmann constant, elementary charge, Avogadro constant, atomic mass
+# unit, reduced Planck constant), in ASE's frame (eV, Angstrom, amu): kJ/mol = 1e3 / (e N_A) eV, nm = 10 Angstrom,
 # fs = 1e-15 s with s = 1e10 sqrt(e / amu).
-_CODATA_K, _CODATA_E, _CODATA_NA, _CODATA_AMU = 1.38064852e-23, 1.6021766208e-19, 6.022140857e23, 1.660539040e-27
-_MD_ENERGY = 1e3 / _CODATA_E / _CODATA_NA                      # kJ/mol in eV
+_MD_ENERGY = 1e3 / _e / _Nav                                    # kJ/mol in eV
 _MD_TIME = 10.0 * math.sqrt(1.0 / _MD_ENERGY)                 # units.py:37, in ASE time units
-KB_MD = (_CODATA_K / _CODATA_E) / _MD_ENERGY                   # units.py:79: ~0.0083144598 kJ/mol/K
-FS_MD = 1e-15 * 1e10 * math.sqrt(_CODATA_E / _CODATA_AMU) / _MD_TIME   # units.py:59: ~1.0e-3
+KB_MD = (_k / _e) / _MD_ENERGY                                 # units.py:79: ~0.0083144598 kJ/mol/K
+FS_MD = 1e-15 * 1e10 * math.sqrt(_e / _amu) / _MD_TIME         # units.py:59: ~1.0e-3
 # units.py:37-40,64-65: 1 bar = 1e5 Pa = 1e5 J/m^3 = 1e5 N_A / 1e30 kJ/mol/nm^3 (~0.0602214)
-BAR_MD = 1e5 * _CODATA_NA / 1e30
-# units.py:80-82: hbar = h / 2 pi in J s, times ASE's J * s = (1 / e) eV * 1e10 sqrt(e / amu), over energy * time (~0.0635)
-_CODATA_H = 6.626070040e-34
-HBAR_MD = (_CODATA_H / (2.0 * math.pi)) / _CODATA_E * 1e10 * math.sqrt(_CODATA_E / _CODATA_AMU) / (_MD_ENERGY * _MD_TIME)
+BAR_MD = 1e5 * _Nav / 1e30
+# units.py:80-82: hbar in J s, times ASE's J * s = (1 / e) eV * 1e10 sqrt(e / amu), over energy * time (~0.0635)
+HBAR_MD = _hbar / _e * 1e10 * math.sqrt(_e / _amu) / (_MD_ENERGY * _MD_TIME)
 # units of gle4md matrix files (thermostat_utils.py:78-86), CODATA 2014: Hartree energy in J, atomic unit of time in s;
 # energies go through kelvin (x kB) and times through femtoseconds (x fs), so custom MD units need no further constant
 _CODATA_HARTREE, _CODATA_AUT = 4.359744650e-18, 2.418884326509e-17
-_EV_K = _CODATA_E / _CODATA_K                                   # 1 eV in K (~11604.5)
-_HARTREE_K = _CODATA_HARTREE / _CODATA_K                        # 1 Hartree in K (~315775)
+_EV_K = _e / _k                                                 # 1 eV in K (~11604.5)
+_HARTREE_K = _CODATA_HARTREE / _k                               # 1 Hartree in K (~315775)
 _AUT_FS = _CODATA_AUT * 1e15                                    # 1 atomic time unit in fs (~0.0241888)
 
 
 class _Systems:
     """The systems of a collated batch as the thermostat kernels address them: per-atom masses and system index, the
-    first atom of every system and the fp64 workspace of the per-system sums (allocated once, outside any capture)."""
+    first atom of every system and the fp64 workspaces of the per-system sums."""
 
     def __init__(self, masses: Tensor, idx_m: Tensor, n_sys: int):
         self.masses = masses
@@ -103,12 +102,21 @@ class _Systems:
         self.n_atoms = int(masses.shape[0])
         self.sys_ptr = ops.segment_ptr(idx_m, self.n_sys)
         self.n_atoms_sys = (self.sys_ptr[1:] - self.sys_ptr[:-1]).to(torch.float64)
-        nbytes = int(_lib.lib().spk_md_thermostat_workspace_bytes(self.n_atoms, self.n_sys))
-        self.ws = torch.empty(nbytes, dtype=torch.uint8, device=masses.device)
+        self._workspaces: Dict[str, Tensor] = {}
+
+    def workspace(self, size_fn: str) -> Tensor:
+        """The workspace of the kernels sized by the library's ``size_fn(n_atoms, n_sys)``, allocated on first use (the
+        eager warm-up before a capture, so never inside one)."""
+        ws = self._workspaces.get(size_fn)
+        if ws is None:
+            nbytes = int(getattr(_lib.lib(), size_fn)(self.n_atoms, self.n_sys))
+            ws = self._workspaces[size_fn] = torch.empty(nbytes, dtype=torch.uint8, device=self.masses.device)
+        return ws
 
     def call(self, name: str, momenta: Tensor, *args):
+        ws = self.workspace("spk_md_thermostat_workspace_bytes")
         _lib.call(name, ops._p(momenta), ops._p(self.masses), ops._p(self.idx_m), ops._p(self.sys_ptr), self.n_atoms,
-                  self.n_sys, *args, ops._p(self.ws), self.ws.numel(), ops._stream())
+                  self.n_sys, *args, ops._p(ws), ws.numel(), ops._stream())
 
     def kinetic_energy_and_temperature(self, momenta: Tensor, kB: float):
         dev = momenta.device
@@ -117,24 +125,115 @@ class _Systems:
         self.call("spk_md_kinetic_energy", momenta, float(kB), ops._p(ke), ops._p(temp))
         return ke, temp
 
-    @property
-    def baro_ws(self) -> Tensor:
-        """fp64 workspace of the barostat kernels (allocated on first use, outside any capture)"""
-        if getattr(self, "_baro_ws", None) is None:
-            nbytes = int(_lib.lib().spk_md_barostat_workspace_bytes(self.n_atoms, self.n_sys))
-            self._baro_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.masses.device)
-        return self._baro_ws
-
     def kinetic_energy_tensor(self, momenta: Tensor) -> Tensor:
         """1/2 sum_a p_a p_a^T / m_a per system, [n_sys, 3, 3] fp64 (system.py:389-404)"""
         out = torch.empty(self.n_sys, 3, 3, dtype=torch.float64, device=momenta.device)
-        ws = self.baro_ws
+        ws = self.workspace("spk_md_barostat_workspace_bytes")
         _lib.call("spk_md_kinetic_energy_tensor", ops._p(momenta), ops._p(self.masses), ops._p(self.idx_m),
                   ops._p(self.sys_ptr), self.n_atoms, self.n_sys, ops._p(out), ops._p(ws), ws.numel(), ops._stream())
         return out
 
 
-class _Thermostat:
+def _batch_layout(static: Dict[str, Tensor]):
+    """(idx_m int64, n_sys) of a collated batch: one system when it has no ``_idx_m`` / ``_n_atoms``"""
+    idx_m = static.get(P.idx_m)
+    if idx_m is None:
+        idx_m = torch.zeros(static[P.R].shape[0], dtype=torch.int64, device=static[P.R].device)
+    n_sys = static[P.n_atoms].shape[0] if P.n_atoms in static else 1
+    return idx_m.to(torch.int64).contiguous(), n_sys
+
+
+def replicate_batch(static: Dict[str, Tensor], n_copies: int, n_sys: int) -> Dict[str, Tensor]:
+    """``n_copies`` replicas of the batch, replica-major as the reference's calculator collates ring-polymer beads
+    (md/calculators/base_calculator.py:154-221): ``_idx_m`` + r B, every other tensor repeated along its first axis.
+    A ``_cell`` / ``_pbc`` shared by all B systems ([3, 3] or [1, 3, 3] / [3] or [1, 3], which the neighbour list
+    broadcasts) is first expanded to one row per system, so the replica batch has one per replica system."""
+    out = {}
+    for k, v in static.items():
+        if k == P.idx_m:
+            out[k] = torch.cat([v + r * n_sys for r in range(n_copies)])
+            continue
+        if k in (P.cell, P.pbc):
+            width = 9 if k == P.cell else 3
+            rows = v.reshape(-1, width)
+            if rows.shape[0] == 1:
+                rows = rows.expand(n_sys, width)
+            if rows.shape[0] != n_sys:
+                raise ValueError(f"'{k}' of shape {tuple(v.shape)} is neither shared nor one per system for {n_sys} "
+                                 "systems")
+            v = rows.reshape(n_sys, 3, 3) if k == P.cell else rows.reshape(-1) if v.dim() == 1 else rows
+        out[k] = torch.cat([v] * n_copies).contiguous()
+    return out
+
+
+def _flatten(state: Dict[str, object]) -> List[Tensor]:
+    return [t for v in state.values() for t in (_flatten(v) if isinstance(v, dict) else [v])]
+
+
+def _clone_state(state: Dict[str, object]) -> Dict[str, object]:
+    return {k: _clone_state(v) if isinstance(v, dict) else v.clone() for k, v in state.items()}
+
+
+def _load_state(dst: Dict[str, object], src: Dict[str, object]):
+    """copy the (nested) dict ``src`` into the tensors of ``dst``, key by key"""
+    for k, v in dst.items():
+        if isinstance(v, dict):
+            _load_state(v, src[k])
+        else:
+            v.copy_(src[k])
+
+
+class _TensorState:
+    """``state_dict`` / ``load_state_dict`` over the device tensors ``_state()`` names (the state a step writes)."""
+
+    def _state(self) -> Dict[str, Tensor]:
+        return {}
+
+    def state_dict(self) -> Dict[str, Tensor]:
+        return _clone_state(self._state())
+
+    def load_state_dict(self, state: Dict[str, Tensor]):
+        _load_state(self._state(), state)
+
+
+def _noise(seed: int, device) -> tuple:
+    """(seed, counter) of a Philox noise hook: the seed taken to 64 bits and a fresh device counter laid out as
+    advance_counter (md_common.cuh) reads it, [0] = application index, [1] = the kernel's internal ticket (zero between
+    calls)"""
+    return int(seed) & 0xFFFFFFFFFFFFFFFF, torch.zeros(2, dtype=torch.int64, device=device)
+
+
+# ---- Nose-Hoover chains -------------------------------------------------------------------------------------------------
+_YS_WEIGHTS = {                                                          # md/utils/thermostat_utils.py:18-44
+    3: (1.35120719195966, -1.70241438391932, 1.35120719195966),
+    5: (0.41449077179438, 0.41449077179438, -0.65796308717750, 0.41449077179438, 0.41449077179438),
+    7: (0.78451361047756, 0.23557321335936, -1.17767998417887, 1.31518632068390, -1.17767998417887,
+        0.23557321335936, 0.78451361047756),
+}
+
+
+def _check_nhc(chain_length: int, multi_step: int, integration_order: int):
+    if integration_order not in _YS_WEIGHTS:
+        raise ValueError(f"Order {integration_order:d} not supported for YS integration weights")
+    if int(chain_length) < 1 or int(multi_step) < 1:
+        raise ValueError("chain_length and multi_step must be >= 1")
+
+
+def _ys_steps(time_step: float, multi_step: int, integration_order: int):
+    """the Yoshida-Suzuki sub-steps dt w_k / multi_step as the kernels' 7-entry array (thermostats.py:339-341)"""
+    w = _YS_WEIGHTS[integration_order]
+    return (ctypes.c_double * 7)(*([time_step * wk / multi_step for wk in w] + [0.0] * (7 - len(w))))
+
+
+def _chain_masses(n_chains: int, dof, chain_length: int, kbt: float, frequency: float, device) -> Tensor:
+    """[n_chains, chain_length] fp64 chain masses kB T / omega^2, the first link times the degrees of freedom ``dof`` of
+    its chain (a number or an [n_chains] tensor) (thermostats.py:387-396)"""
+    masses = torch.full((n_chains, chain_length), kbt / frequency ** 2, dtype=torch.float64, device=device)
+    masses[:, 0] = dof * kbt / frequency ** 2
+    return masses
+
+
+class _Thermostat(_TensorState):
     """Common part of the device thermostats (ThermostatHook, thermostats.py:41-146): bath temperature in K, time constant
     in fs.  ``kB`` (MD energy per kelvin) and ``fs`` (one femtosecond in MD time) define the caller's MD units; the
     defaults are the reference's (kJ/mol, nm, Da).  ``bind`` sizes the state for a batch, ``apply`` updates the momenta in
@@ -158,16 +257,6 @@ class _Thermostat:
     def apply(self, momenta: Tensor):
         raise NotImplementedError
 
-    def _state(self) -> Dict[str, Tensor]:
-        return {}
-
-    def state_dict(self) -> Dict[str, Tensor]:
-        return {k: v.clone() for k, v in self._state().items()}
-
-    def load_state_dict(self, state: Dict[str, Tensor]):
-        for k, v in self._state().items():
-            v.copy_(state[k])
-
 
 class BerendsenThermostat(_Thermostat):
     """Berendsen rescaling (thermostats.py:149-189): p *= sqrt(1 + dt / tau (T_bath / T - 1)) per system.  A system whose
@@ -186,15 +275,13 @@ class LangevinThermostat(_Thermostat):
     def __init__(self, temperature_bath: float, time_constant: float, seed: int = 0, kB: float = KB_MD,
                  fs: float = FS_MD):
         super().__init__(temperature_bath, time_constant, kB=kB, fs=fs)
-        self.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-        self.counter: Optional[Tensor] = None
+        self.seed = seed
 
     def _init_state(self):
         gamma = 1.0 / self.time_constant                                 # :227-230
         self.c1 = math.exp(-0.5 * self.time_step * gamma)                 # :233
         self.c2 = math.sqrt(1.0 - self.c1 ** 2)                           # :234
-        # [0] = application index, [1] = the kernel's internal ticket (zero between calls)
-        self.counter = torch.zeros(2, dtype=torch.int64, device=self.systems.masses.device)
+        self.seed, self.counter = _noise(self.seed, self.systems.masses.device)
 
     def apply(self, momenta: Tensor):
         s = self.systems
@@ -210,20 +297,10 @@ class NHCThermostat(_Thermostat):
     system, or per degree of freedom with ``massive``; ``multi_step`` sub-steps of a Yoshida-Suzuki scheme of order
     ``integration_order`` (3, 5 or 7).  The chain state is fp64 on the device."""
 
-    YS_WEIGHTS = {                                                       # md/utils/thermostat_utils.py:18-44
-        3: (1.35120719195966, -1.70241438391932, 1.35120719195966),
-        5: (0.41449077179438, 0.41449077179438, -0.65796308717750, 0.41449077179438, 0.41449077179438),
-        7: (0.78451361047756, 0.23557321335936, -1.17767998417887, 1.31518632068390, -1.17767998417887,
-            0.23557321335936, 0.78451361047756),
-    }
-
     def __init__(self, temperature_bath: float, time_constant: float, chain_length: int = 3, massive: bool = False,
                  multi_step: int = 2, integration_order: int = 3, kB: float = KB_MD, fs: float = FS_MD):
         super().__init__(temperature_bath, time_constant, kB=kB, fs=fs)
-        if integration_order not in self.YS_WEIGHTS:
-            raise ValueError(f"Order {integration_order:d} not supported for YS integration weights")
-        if int(chain_length) < 1 or int(multi_step) < 1:
-            raise ValueError("chain_length and multi_step must be >= 1")
+        _check_nhc(chain_length, multi_step, integration_order)
         self.chain_length = int(chain_length)
         self.massive = bool(massive)
         self.multi_step = int(multi_step)
@@ -234,20 +311,15 @@ class NHCThermostat(_Thermostat):
         s = self.systems
         dev = s.masses.device
         kbt = self.temperature_bath * self.kB                             # :308
-        freq2 = (1.0 / self.time_constant) ** 2                          # :304
         if self.massive:                                                  # :348-359
             dof = torch.ones(3 * s.n_atoms, dtype=torch.float64, device=dev)
         else:
             dof = 3.0 * s.n_atoms_sys
-        L = self.chain_length
-        self.masses = torch.full((dof.shape[0], L), kbt / freq2, dtype=torch.float64, device=dev)     # :387-396
-        self.masses[:, 0] = dof * kbt / freq2
+        self.masses = _chain_masses(dof.shape[0], dof, self.chain_length, kbt, 1.0 / self.time_constant, dev)  # :304
         self.velocities = torch.zeros_like(self.masses)
         self.forces = torch.zeros_like(self.masses)
-        w = self.YS_WEIGHTS[self.integration_order]
-        steps = [self.time_step * wk / self.multi_step for wk in w] + [0.0] * (7 - len(w))   # :339-341
-        self.params = _lib.NHCParams(L, self.multi_step, self.integration_order, int(self.massive), kbt,
-                                     (ctypes.c_double * 7)(*steps))
+        self.params = _lib.NHCParams(self.chain_length, self.multi_step, self.integration_order, int(self.massive), kbt,
+                                     _ys_steps(self.time_step, self.multi_step, self.integration_order))
 
     def apply(self, momenta: Tensor):
         self.systems.call("spk_md_nhc", momenta, ctypes.byref(self.params), ops._p(self.velocities),
@@ -257,7 +329,7 @@ class NHCThermostat(_Thermostat):
         return {"velocities": self.velocities, "forces": self.forces}
 
 
-class _NHCBarostat:
+class _NHCBarostat(_TensorState):
     """Nose-Hoover-chain barostat (barostats.py:162-705) with the reference's keywords and defaults: target pressure in bar,
     bath temperature in K, time constants in fs; ``kB``, ``fs`` and ``bar`` define the caller's MD units (defaults: the
     reference's kJ/mol, nm, Da).  Two chains as in the reference: one on the particles (per system, or per degree of freedom
@@ -267,16 +339,12 @@ class _NHCBarostat:
     anisotropic = False
     ring_polymer = False
     temperature_control = True
-    YS_WEIGHTS = NHCThermostat.YS_WEIGHTS
 
     def __init__(self, target_pressure: float, temperature_bath: float, time_constant: float,
                  time_constant_cell: Optional[float] = None, time_constant_barostat: Optional[float] = None,
                  chain_length: int = 4, multi_step: int = 4, integration_order: int = 7, massive: bool = False,
                  kB: float = KB_MD, fs: float = FS_MD, bar: float = BAR_MD):
-        if integration_order not in self.YS_WEIGHTS:
-            raise ValueError(f"Order {integration_order:d} not supported for YS integration weights")
-        if int(chain_length) < 1 or int(multi_step) < 1:
-            raise ValueError("chain_length and multi_step must be >= 1")
+        _check_nhc(chain_length, multi_step, integration_order)
         self.target_pressure = float(target_pressure) * float(bar)               # :51-53
         self.temperature_bath = float(temperature_bath)
         self.time_constant = float(time_constant) * float(fs)
@@ -308,27 +376,22 @@ class _NHCBarostat:
             self.b_velocities = torch.zeros(s.n_sys, **f64)
         self.b_forces = torch.zeros_like(self.b_velocities)
         dof_p = torch.ones(3 * s.n_atoms, **f64) if self.massive else dof       # :293-302
-        self.t_masses = torch.full((dof_p.shape[0], L), kbt / self.frequency ** 2, **f64)       # :343-371
-        self.t_masses[:, 0] = dof_p * kbt / self.frequency ** 2
+        self.t_masses = _chain_masses(dof_p.shape[0], dof_p, L, kbt, self.frequency, dev)       # :343-371
         dof_cell = 6.0 if self.anisotropic else 1.0                              # :328-330, :794-796
-        self.t_masses_cell = torch.full((s.n_sys, L), kbt / self.cell_frequency ** 2, **f64)
-        self.t_masses_cell[:, 0] = dof_cell * kbt / self.cell_frequency ** 2
+        self.t_masses_cell = _chain_masses(s.n_sys, dof_cell, L, kbt, self.cell_frequency, dev)
         self.t_velocities = torch.zeros_like(self.t_masses)
         self.t_forces = torch.zeros_like(self.t_masses)
         self.t_velocities_cell = torch.zeros_like(self.t_masses_cell)
         self.t_forces_cell = torch.zeros_like(self.t_masses_cell)
-        w = self.YS_WEIGHTS[self.integration_order]
-        steps = [self.time_step * wk / self.multi_step for wk in w] + [0.0] * (7 - len(w))   # :273-281
         p = ops._p
         self.params = _lib.NHCBarostat(
             int(self.anisotropic), int(self.massive), L, self.multi_step, self.integration_order, 0, kbt, self.time_step,
-            self.target_pressure, (ctypes.c_double * 7)(*steps), p(self.t_velocities), p(self.t_forces), p(self.t_masses),
-            p(self.t_velocities_cell), p(self.t_forces_cell), p(self.t_masses_cell), p(self.b_velocities),
-            p(self.b_forces), p(self.b_masses))
+            self.target_pressure, _ys_steps(self.time_step, self.multi_step, self.integration_order),   # :273-281
+            p(self.t_velocities), p(self.t_forces), p(self.t_masses), p(self.t_velocities_cell), p(self.t_forces_cell),
+            p(self.t_masses_cell), p(self.b_velocities), p(self.b_forces), p(self.b_masses))
 
     def _call(self, name: str, *args, launches: Optional[int] = None):
-        s = self.systems
-        ws = s.baro_ws
+        ws = self.systems.workspace("spk_md_barostat_workspace_bytes")
         _lib.call(name, ctypes.byref(self.params), *args, ops._p(ws), ws.numel(), ops._stream(), launches=launches)
 
     def apply_thermostat(self, momenta: Tensor):
@@ -361,13 +424,6 @@ class _NHCBarostat:
         return {"t_velocities": self.t_velocities, "t_forces": self.t_forces,
                 "t_velocities_cell": self.t_velocities_cell, "t_forces_cell": self.t_forces_cell,
                 "b_velocities": self.b_velocities, "b_forces": self.b_forces}
-
-    def state_dict(self) -> Dict[str, Tensor]:
-        return {k: v.clone() for k, v in self._state().items()}
-
-    def load_state_dict(self, state: Dict[str, Tensor]):
-        for k, v in self._state().items():
-            v.copy_(state[k])
 
 
 class NHCBarostatIsotropic(_NHCBarostat):
@@ -468,13 +524,6 @@ class _RingPolymerThermostat(_Thermostat):
         self.rp = ring_polymer
         super().bind(systems, time_step)
 
-    def _ws(self) -> Tensor:
-        if getattr(self, "_rp_ws", None) is None:
-            s = self.systems
-            nbytes = int(_lib.lib().spk_rpmd_workspace_bytes(s.n_atoms, s.n_sys))
-            self._rp_ws = torch.empty(nbytes, dtype=torch.uint8, device=s.masses.device)
-        return self._rp_ws
-
 
 class PILELocalThermostat(_RingPolymerThermostat):
     """Local path-integral Langevin thermostat (thermostats_rpmd.py:33-119): in normal-mode space p~_k = c1_k p~_k +
@@ -489,8 +538,7 @@ class PILELocalThermostat(_RingPolymerThermostat):
         super().__init__(temperature_bath, time_constant, kB=kB, fs=fs)
         self.thermostat_centroid = bool(thermostat_centroid)
         self.damping_factor = float(damping_factor)
-        self.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-        self.counter: Optional[Tensor] = None
+        self.seed = seed
 
     def _init_state(self):
         dev = self.systems.masses.device
@@ -501,13 +549,14 @@ class PILELocalThermostat(_RingPolymerThermostat):
         c1 = torch.exp(-0.5 * self.time_step * gamma)                         # :85
         self.c1, self.c2 = c1.to(dev), torch.sqrt(1.0 - c1 ** 2).to(dev)      # :86
         self.kbt_p = self.kB * self.rp.n_beads * self.temperature_bath        # :92-97
-        self.counter = torch.zeros(2, dtype=torch.int64, device=dev)
+        self.seed, self.counter = _noise(self.seed, dev)
 
     def apply(self, momenta: Tensor):
         s = self.systems
+        ws = s.workspace("spk_rpmd_workspace_bytes")
         _lib.call("spk_rpmd_pile", ops._p(momenta), ops._p(s.masses), ops._p(s.idx_m), ops._p(s.sys_ptr), s.n_atoms,
                   s.n_sys, self.rp.n_beads, ops._p(self.rp.c_transform), ops._p(self.c1), ops._p(self.c2), self.kbt_p,
-                  self._global, self.seed, ops._p(self.counter), ops._p(self._ws()), self._ws().numel(), ops._stream(),
+                  self._global, self.seed, ops._p(self.counter), ops._p(ws), ws.numel(), ops._stream(),
                   launches=3 if self._global else 1)
 
     def _state(self):
@@ -551,15 +600,10 @@ class NHCRingPolymerThermostat(_RingPolymerThermostat):
     sum |p~_0|^2 / m, with 3 N_s degrees of freedom and its first link 3 N_s times heavier.  The chain state is fp64 on the
     device, [P 3 N, chain_length]."""
 
-    YS_WEIGHTS = NHCThermostat.YS_WEIGHTS
-
     def __init__(self, temperature_bath: float, time_constant: float, local: bool = True, chain_length: int = 3,
                  multi_step: int = 2, integration_order: int = 3, kB: float = KB_MD, fs: float = FS_MD):
         super().__init__(temperature_bath, time_constant, kB=kB, fs=fs)
-        if integration_order not in self.YS_WEIGHTS:
-            raise ValueError(f"Order {integration_order:d} not supported for YS integration weights")
-        if int(chain_length) < 1 or int(multi_step) < 1:
-            raise ValueError("chain_length and multi_step must be >= 1")
+        _check_nhc(chain_length, multi_step, integration_order)
         self.local = bool(local)
         self.chain_length = int(chain_length)
         self.multi_step = int(multi_step)
@@ -580,17 +624,17 @@ class NHCRingPolymerThermostat(_RingPolymerThermostat):
         self.masses = masses.reshape(P * n_dof, L).to(dev)
         self.velocities = torch.zeros_like(self.masses)
         self.forces = torch.zeros_like(self.masses)
-        w = self.YS_WEIGHTS[self.integration_order]
-        steps = [self.time_step * wk / self.multi_step for wk in w] + [0.0] * (7 - len(w))
-        self.params = _lib.NHCParams(L, self.multi_step, self.integration_order, 1, kbt, (ctypes.c_double * 7)(*steps))
+        self.params = _lib.NHCParams(L, self.multi_step, self.integration_order, 1, kbt,
+                                     _ys_steps(self.time_step, self.multi_step, self.integration_order))
 
     def apply(self, momenta: Tensor):
         s = self.systems
+        ws = s.workspace("spk_rpmd_workspace_bytes")
         g = 0 if self.local else 1
         _lib.call("spk_rpmd_nhc", ops._p(momenta), ops._p(s.masses), ops._p(s.idx_m), ops._p(s.sys_ptr), s.n_atoms,
                   s.n_sys, self.rp.n_beads, ops._p(self.rp.c_transform), ctypes.byref(self.params), g,
-                  ops._p(self.velocities), ops._p(self.forces), ops._p(self.masses), ops._p(self._ws()),
-                  self._ws().numel(), ops._stream(), launches=3 if g else 1)
+                  ops._p(self.velocities), ops._p(self.forces), ops._p(self.masses), ops._p(ws), ws.numel(),
+                  ops._stream(), launches=3 if g else 1)
 
     def _state(self):
         return {"velocities": self.velocities, "forces": self.forces}
@@ -703,13 +747,12 @@ class _GLE:
         super().__init__(temperature_bath, 0.0, kB=kB, fs=fs)          # thermostats.py:557-559
         self.gle_file = str(gle_file)
         self.free_particle_limit = bool(free_particle_limit)
-        self.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self.seed = seed
         self.A, self.C = load_gle_matrices(self.gle_file, kB=kB, fs=fs)
         if not self._per_mode and self.A.shape[0] > 1:                    # thermostats.py:603-606
             raise ValueError(f"{type(self).__name__}: more than one A matrix found in {self.gle_file}. Could be PIGLET "
                              "input (PIGLETThermostat).")
         self.state: Optional[Tensor] = None
-        self.counter: Optional[Tensor] = None
 
     def _n_beads(self) -> int:
         return self.rp.n_beads if self.ring_polymer else 1
@@ -731,8 +774,7 @@ class _GLE:
         self.c_transform = self.rp.c_transform if self.ring_polymer else torch.ones(1, 1, dtype=torch.float64,
                                                                                     device=dev)
         self.state = torch.zeros(P * 3 * s.n_atoms, D, dtype=torch.float64, device=dev)
-        # [0] = application index, [1] = the kernel's internal ticket (zero between calls)
-        self.counter = torch.zeros(2, dtype=torch.int64, device=dev)
+        self.seed, self.counter = _noise(self.seed, dev)
         if self.free_particle_limit:
             self._call(None, 1)
 
@@ -775,7 +817,7 @@ class PIGLETThermostat(RPMDGLEThermostat):
         super().__init__(temperature_bath, gle_file, free_particle_limit=True, seed=seed, kB=kB, fs=fs)
 
 
-class PILEBarostat:
+class PILEBarostat(_TensorState):
     """Isotropic barostat of ring-polymer NPT (barostats_rpmd.py:21-208, after i-PI 2.0, Kapil et al. 2019) with the
     reference's keywords: target pressure in bar, bath temperature of the cell in K, time constant in fs; ``kB``, ``fs``
     and ``bar`` define the caller's MD units.  It acts on the centroid mode and the cell only and thermostats the cell
@@ -797,9 +839,8 @@ class PILEBarostat:
         self.frequency = 1.0 / self.time_constant                               # barostats_rpmd.py:53
         self.kB = float(kB)
         self.kb_temperature = self.temperature_bath * self.kB                   # :56
-        self.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self.seed = seed
         self.cell_momenta: Optional[Tensor] = None
-        self.counter: Optional[Tensor] = None
 
     def bind(self, systems: _Systems, time_step: float, ring_polymer: Optional[RingPolymer] = None):
         """_init_barostat (:66-99) for the base batch ``systems`` (one copy of every molecule)."""
@@ -814,10 +855,7 @@ class PILEBarostat:
         self.cell_mass = 3.0 * s.n_atoms_sys * kbt / self.frequency ** 2                # :83-85
         self.c1 = math.exp(-0.5 * self.frequency * self.time_step)                      # :88-93
         self.c2 = torch.sqrt(ring_polymer.n_beads * self.cell_mass * kbt * (1.0 - self.c1 ** 2))   # :94-99
-        # [0] = application index, [1] = the kernel's internal ticket (zero between calls)
-        self.counter = torch.zeros(2, dtype=torch.int64, device=dev)
-        nbytes = int(_lib.lib().spk_rpmd_barostat_workspace_bytes(s.n_atoms, s.n_sys))
-        self.ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        self.seed, self.counter = _noise(self.seed, dev)
 
     def apply_thermostat(self):
         """_update_barostat (:101-110) at on_step_begin and on_step_end"""
@@ -829,37 +867,33 @@ class PILEBarostat:
         """propagate_half_step (:164-205) up to the particle kick, which DeviceMD enqueues next: p_c from the momenta
         before the kick, the forces * force_conversion, and the bead systems' cells and virials"""
         s, rp = self.systems, self.rp
+        ws = s.workspace("spk_rpmd_barostat_workspace_bytes")
         _lib.call("spk_rpmd_barostat_half_step", ops._p(momenta), ops._p(forces), float(force_conversion),
                   ops._p(s.masses), ops._p(s.idx_m), ops._p(s.sys_ptr), s.n_atoms, s.n_sys, rp.n_beads,
                   ops._p(rp.c_transform), ops._p(cell), ops._p(virial), float(virial_scale), self.target_pressure,
                   self.kb_temperature, self.time_step, ops._p(self.cell_mass), ops._p(self.cell_momenta),
-                  ops._p(self.ws), self.ws.numel(), ops._stream())
+                  ops._p(ws), ws.numel(), ops._stream())
 
     def main_step(self, positions: Tensor, momenta: Tensor, model_positions: Optional[Tensor], cell: Tensor,
                   model_cell: Optional[Tensor], position_conversion: float):
         """propagate_main_step (:113-162): centroid mode and cell scaled by the cell momentum, modes k >= 1 free"""
         s, rp = self.systems, self.rp
+        ws = s.workspace("spk_rpmd_barostat_workspace_bytes")
         _lib.call("spk_rpmd_barostat_main_step", ops._p(positions), ops._p(momenta), ops._p(model_positions),
                   ops._p(s.masses), ops._p(s.idx_m), s.n_atoms, s.n_sys, rp.n_beads, ops._p(rp.c_transform),
                   ops._p(rp.u), self.time_step, ops._p(self.cell_momenta), ops._p(self.cell_mass), ops._p(cell),
-                  ops._p(model_cell), float(position_conversion), ops._p(self.ws), self.ws.numel(), ops._stream())
+                  ops._p(model_cell), float(position_conversion), ops._p(ws), ws.numel(), ops._stream())
 
     def _state(self) -> Dict[str, Tensor]:
         return {"cell_momenta": self.cell_momenta, "counter": self.counter}
-
-    def state_dict(self) -> Dict[str, Tensor]:
-        return {k: v.clone() for k, v in self._state().items()}
-
-    def load_state_dict(self, state: Dict[str, Tensor]):
-        for k, v in self._state().items():
-            v.copy_(state[k])
 
 
 class _CapturedEvaluation:
     """The force evaluation of a device-resident loop (calculator.calculate) and the capture of one whole step with it:
     neighbour list on the fixed-capacity ``self.nl``, ``self.model`` on ``self.static`` and copies of the outputs into
-    ``self.energy`` / ``self.forces``, with the sticky overflow watch ``self.nl_watch``.  ``DeviceMD`` and
-    ``relax.DeviceLBFGS`` build their steps around it."""
+    ``self.energy`` / ``self.forces``, with the sticky overflow watch ``self.nl_watch``.  ``DeviceMD``,
+    ``relax.DeviceLBFGS`` and ``vibrations.DeviceVibrations`` build their steps around it: each defines ``_step()`` and
+    ``_step_state()``, the (nested) dict of every tensor the step writes."""
 
     energy_key = P.energy
     force_key = P.forces
@@ -868,6 +902,29 @@ class _CapturedEvaluation:
     # members of an ensemble run (None: one model); their outputs are stacked into ``self.stacks[key]`` [K, ...]
     ensemble: Optional[List[torch.nn.Module]] = None
     stacks: Dict[str, Tensor] = {}
+
+    def _setup(self, model, batch: Dict[str, Tensor], cutoff: float, capacity: int, use_graph: bool):
+        """The set-up every driver shares: checks of the batch and the model, ``self.model`` (``_set_ensemble``),
+        ``self.static`` (the batch without its neighbour list), the padded neighbour list of ``capacity`` pairs and the
+        empty evaluation buffers.  Returns the batch layout (idx_m, n_sys)."""
+        name = type(self).__name__
+        if batch[P.R].device.type != "cuda":
+            raise ValueError(f"{name} needs a CUDA batch (no CPU fallback)")
+        model = self._set_ensemble(model, name)
+        check_padded_pair_terms(model, float(cutoff), name)
+        check_ewald_cells(model, batch, name)
+        self.model = model
+        self.use_graph = use_graph
+        self.static = {k: v.detach().clone() for k, v in batch.items() if k not in (P.idx_i, P.idx_j, P.offsets)}
+        self.nl = CellListNeighborList(cutoff, capacity=int(capacity), pad=True)
+        self.energy: Optional[Tensor] = None
+        self.forces: Optional[Tensor] = None
+        self.n_pairs: Optional[Tensor] = None
+        # sticky bookkeeping of the fixed-capacity neighbour list, updated INSIDE the captured step: [0] = largest pair
+        # count seen so far, [1] = 1 if any step overflowed ``capacity`` (its list was then truncated)
+        self.nl_watch = torch.zeros(2, dtype=torch.int64, device=batch[P.R].device)
+        self._graph = None
+        return _batch_layout(self.static)
 
     # ---- one force evaluation on the current positions (calculator.calculate) ---------------------------------------------
     def _calculate(self):
@@ -946,10 +1003,24 @@ class _CapturedEvaluation:
                                  f"(one outputs {sorted(outputs)})")
         return torch.nn.ModuleList(members)
 
-    def _capture_step(self, state: List[Tensor]) -> "torch.cuda.CUDAGraph":
-        """Capture ``self._step()`` into a CUDA graph.  Capture works on copies of ``state`` (every tensor the step writes)
-        so that the warm-up iteration does not advance the run."""
+    def _evaluation_state(self) -> Dict[str, Tensor]:
+        return {"energy": self.energy, "forces": self.forces, "n_pairs": self.n_pairs, "nl_watch": self.nl_watch}
+
+    def _run_steps(self, n: int):
+        """``n`` steps: replays of the step, captured on first use, or eager ``_step()`` calls without ``use_graph``."""
+        if n > 0 and self.use_graph and self._graph is None:
+            self._graph = self._capture_step()
+        for _ in range(n):
+            if self.use_graph:
+                self._graph.replay()
+            else:
+                self._step()
+
+    def _capture_step(self) -> "torch.cuda.CUDAGraph":
+        """Capture ``self._step()`` into a CUDA graph.  The tensors of ``_step_state()`` are restored after the warm-up
+        iteration, so that capturing does not advance the run."""
         dev = self.static[P.R].device
+        state = _flatten(self._step_state())
         saved = [t.clone() for t in state]
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
@@ -1017,39 +1088,35 @@ class DeviceMD(_CapturedEvaluation):
         ``RelativeUncertainty`` on the run's energy and force keys, without a stress weight) adds
         ``properties["uncertainty"]`` [n_replicas, B] of the energies and forces as ``properties`` holds them.  Stress
         and barostats are refused with an ensemble, as in the reference."""
-        dev = batch[P.R].device
-        if dev.type != "cuda":
-            raise ValueError("DeviceMD needs a CUDA batch (no CPU fallback)")
-        model = self._set_ensemble(model, "DeviceMD")
+        idx_m, n_sys = self._setup(model, batch, cutoff, capacity, use_graph)
         self._check_ensemble(barostat, compute_stress, uncertainty_fn)
         self.uncertainty_fn = uncertainty_fn
         if barostat is not None and thermostat is not None and getattr(barostat, "temperature_control", True):
             raise ValueError("DeviceMD: the NHC barostats contain their own thermostat (temperature_control = True); "
                              "pass either a thermostat or a barostat")
         self._check_ring_polymer(ring_polymer, thermostat, barostat, compute_stress)
-        from .atomistic.pair_terms import check_ewald_cells, check_padded_pair_terms
-
-        check_padded_pair_terms(model, float(cutoff), "DeviceMD")
-        check_ewald_cells(model, batch, "DeviceMD")
+        dev = batch[P.R].device
         self.ring_polymer = ring_polymer
-        self.model = model
         self.dt = float(time_step)
         self.p_conv = float(position_conversion)
         self.e_conv = float(energy_conversion)
         self.f_conv = self.e_conv / self.p_conv                                   # base_calculator.py:96
-        self.static = {k: v.detach().clone() for k, v in batch.items() if k not in (P.idx_i, P.idx_j, P.offsets)}
         masses = masses.to(dev, torch.float32).reshape(-1).contiguous().clone()
         self._rp_base: Optional[_Systems] = None
         if ring_polymer is not None:
-            self._rp_base = self._base_systems(masses)
-            b = self._rp_base
-            self.static.setdefault(P.idx_m, b.idx_m)
+            n = self.static[P.R].shape[0]
+            if masses.shape[0] != n:
+                raise ValueError(f"DeviceMD: {masses.shape[0]} masses for {n} atoms")
+            self._rp_base = b = _Systems(masses, idx_m, n_sys)
+            self.static.setdefault(P.idx_m, idx_m)
             self.static.setdefault(P.n_atoms, (b.sys_ptr[1:] - b.sys_ptr[:-1]).to(torch.int64))
-            self.static = self._bead_batch(self.static, ring_polymer.n_beads, self._rp_base.n_sys)
+            self.static = replicate_batch(self.static, ring_polymer.n_beads, n_sys)
             masses = masses.repeat(ring_polymer.n_beads)
-            ring_polymer.bind(self._rp_base, self.dt)
+            ring_polymer.bind(b, self.dt)
         self.model_positions = self.static[P.R]                                   # what the model reads
         self.positions = self.model_positions if self.p_conv == 1.0 else self.model_positions / self.p_conv
+        # the model-unit copy the position kernels update next to the MD positions (None when the units agree)
+        self._mp = self.model_positions if self.model_positions is not self.positions else None
         self.masses = masses
         if momenta is None:
             self.momenta = torch.zeros_like(self.positions)
@@ -1063,15 +1130,6 @@ class DeviceMD(_CapturedEvaluation):
                 raise ValueError(f"DeviceMD: ring-polymer momenta must be [N, 3] or [P, N, 3], got "
                                  f"{momenta.shape[0]} rows for N = {self._rp_base.n_atoms}, P = {ring_polymer.n_beads}")
             self.momenta = momenta.contiguous().clone()
-        self.nl = CellListNeighborList(cutoff, capacity=int(capacity), pad=True)
-        self.use_graph = use_graph
-        self.energy: Optional[Tensor] = None
-        self.forces: Optional[Tensor] = None
-        self.n_pairs: Optional[Tensor] = None
-        # sticky bookkeeping of the fixed-capacity neighbour list, updated INSIDE the captured step: [0] = largest pair
-        # count seen so far, [1] = 1 if any step overflowed ``capacity`` (its list was then truncated)
-        self.nl_watch = torch.zeros(2, dtype=torch.int64, device=dev)
-        self._graph = None
         self.steps_done = 0
         self._systems: Optional[_Systems] = None
         self.thermostat = thermostat
@@ -1109,16 +1167,8 @@ class DeviceMD(_CapturedEvaluation):
     @property
     def systems(self) -> _Systems:
         if self._systems is None:
-            self._systems = self._batch_systems(self.static, self.masses)
+            self._systems = _Systems(self.masses, *_batch_layout(self.static))
         return self._systems
-
-    @staticmethod
-    def _batch_systems(static: Dict[str, Tensor], masses: Tensor) -> _Systems:
-        idx_m = static.get(P.idx_m)
-        if idx_m is None:
-            idx_m = torch.zeros(masses.shape[0], dtype=torch.int64, device=masses.device)
-        n_sys = static[P.n_atoms].shape[0] if P.n_atoms in static else 1
-        return _Systems(masses, idx_m.to(torch.int64).contiguous(), n_sys)
 
     def _check_ensemble(self, barostat, compute_stress: bool, uncertainty_fn):
         if self.ensemble is None:
@@ -1168,35 +1218,6 @@ class DeviceMD(_CapturedEvaluation):
                              "ring-polymer NPT takes PILEBarostat")
         if compute_stress:
             raise ValueError("DeviceMD: compute_stress is not supported for ring-polymer MD")
-
-    def _base_systems(self, masses: Tensor) -> _Systems:
-        n = self.static[P.R].shape[0]
-        if masses.shape[0] != n:
-            raise ValueError(f"DeviceMD: {masses.shape[0]} masses for {n} atoms")
-        return self._batch_systems(self.static, masses)
-
-    @staticmethod
-    def _bead_batch(static: Dict[str, Tensor], n_beads: int, n_sys: int) -> Dict[str, Tensor]:
-        """P replicas of the batch, replica-major as the reference's calculator collates them
-        (md/calculators/base_calculator.py:154-221): ``_idx_m`` + r B, every other tensor repeated along its first axis.
-        A ``_cell`` / ``_pbc`` shared by all B systems ([3, 3] or [1, 3, 3] / [3] or [1, 3], which the neighbour list
-        broadcasts) is first expanded to one row per system, so the bead batch has one per bead system."""
-        out = {}
-        for k, v in static.items():
-            if k == P.idx_m:
-                out[k] = torch.cat([v + r * n_sys for r in range(n_beads)])
-                continue
-            if k in (P.cell, P.pbc):
-                width = 9 if k == P.cell else 3
-                rows = v.reshape(-1, width)
-                if rows.shape[0] == 1:
-                    rows = rows.expand(n_sys, width)
-                if rows.shape[0] != n_sys:
-                    raise ValueError(f"DeviceMD: '{k}' of shape {tuple(v.shape)} is neither shared nor one per system "
-                                     f"for {n_sys} systems")
-                v = rows.reshape(n_sys, 3, 3) if k == P.cell else rows.reshape(-1) if v.dim() == 1 else rows
-            out[k] = torch.cat([v] * n_beads).contiguous()
-        return out
 
     # ---- per-step model properties and their device-side time series ------------------------------------------------------
     def _setup_properties(self, required, conversion, every, capacity, velocities=False):
@@ -1354,8 +1375,8 @@ class DeviceMD(_CapturedEvaluation):
 
     def _verlet(self, drift: bool):
         n = self.positions.shape[0]
-        mp = self.model_positions if self.model_positions is not self.positions else None
-        _lib.call("spk_md_velocity_verlet", ops._p(self.momenta), ops._p(self.positions), ops._p(mp), ops._p(self.forces),
+        _lib.call("spk_md_velocity_verlet", ops._p(self.momenta), ops._p(self.positions), ops._p(self._mp),
+                  ops._p(self.forces),
                   ops._p(self.masses), n, self.dt, self.f_conv, self.p_conv, 1 if drift else 0, ops._stream())
 
     def _virial_scale(self) -> float:
@@ -1364,11 +1385,10 @@ class DeviceMD(_CapturedEvaluation):
 
     def _npt_step(self):
         b = self.barostat
-        mp = self.model_positions if self.model_positions is not self.positions else None
         b.apply_thermostat(self.momenta)                                           # simulator.py:127-128 on_step_begin
         b.kick(self.momenta, self.cell, self.virial, self._virial_scale())
         b.half_step(self.momenta, self.forces, self.f_conv)                        # integrators.py:249-257
-        b.main_step(self.positions, self.momenta, self.cell, mp, self.model_cell, self.p_conv)   # :259-263
+        b.main_step(self.positions, self.momenta, self.cell, self._mp, self.model_cell, self.p_conv)   # :259-263
         self._calculate()                                                          # neighbour list on the new cell
         b.half_step(self.momenta, self.forces, self.f_conv)
         b.kick(self.momenta, self.cell, self.virial, self._virial_scale())        # simulator.py:149-150 on_step_end
@@ -1378,11 +1398,10 @@ class DeviceMD(_CapturedEvaluation):
         """md/simulator.py:124-150 with the RingPolymer integrator (integrators.py:59-70,204-229): thermostat, half kick on
         every bead, ring-polymer main step, neighbour list + energy + forces on all P B bead systems, half kick,
         thermostat"""
-        mp = self.model_positions if self.model_positions is not self.positions else None
         if self.thermostat is not None:
             self.thermostat.apply(self.momenta)
         self._verlet(False)
-        self.ring_polymer.main_step(self.positions, self.momenta, mp, self.p_conv)
+        self.ring_polymer.main_step(self.positions, self.momenta, self._mp, self.p_conv)
         self._calculate()
         self._verlet(False)
         if self.thermostat is not None:
@@ -1393,13 +1412,12 @@ class DeviceMD(_CapturedEvaluation):
         thermostat, cell PILE, barostat half step + kick, centroid / cell / free-mode propagation, neighbour list on the new
         cells + energy + forces + virial on all P B bead systems, half step + kick, cell PILE, thermostat"""
         b = self.barostat
-        mp = self.model_positions if self.model_positions is not self.positions else None
         if self.thermostat is not None:
             self.thermostat.apply(self.momenta)
         b.apply_thermostat()
         b.half_step(self.momenta, self.forces, self.f_conv, self.cell, self.virial, self._virial_scale())
         self._verlet(False)                                                        # barostats_rpmd.py:207-208
-        b.main_step(self.positions, self.momenta, mp, self.cell, self.model_cell, self.p_conv)
+        b.main_step(self.positions, self.momenta, self._mp, self.cell, self.model_cell, self.p_conv)
         self._calculate()
         b.half_step(self.momenta, self.forces, self.f_conv, self.cell, self.virial, self._virial_scale())
         self._verlet(False)
@@ -1426,21 +1444,23 @@ class DeviceMD(_CapturedEvaluation):
         if self.thermostat is not None:
             self.thermostat.apply(self.momenta)   # simulator.py:149-150 on_step_end
 
-    def _capture(self):
-        state = [self.positions, self.momenta, self.forces, self.energy]
-        if self.model_positions is not self.positions:
-            state.append(self.model_positions)
+    def _step_state(self) -> Dict[str, object]:
+        """the MD state, the neighbour-list bookkeeping, the hooks' state, the properties and the records held"""
+        state = dict(positions=self.positions, momenta=self.momenta, **self._evaluation_state())
+        if self._mp is not None:
+            state["model_positions"] = self._mp
         if self.thermostat is not None:
-            state.extend(self.thermostat._state().values())
+            state["thermostat"] = self.thermostat._state()
         if self.virial is not None:
-            state.extend([self.virial, self.cell, self.model_cell])
+            state.update(cell=self.cell, model_cell=self.model_cell, virial=self.virial)
         if self.barostat is not None:
-            state.extend(self.barostat._state().values())
-        state.extend(self.properties.values())
-        state.extend(self.stacks.values())
+            state["barostat"] = self.barostat._state()
+        if self.properties:
+            state["properties"] = self.properties
         if self.record_capacity:
-            state.extend([self._rec_counter] + list(self._records.values()))
-        self._graph = self._capture_step(state)
+            state["recorder"] = {"counter": self._rec_counter,
+                                 "records": {p: v[:self._n_records] for p, v in self._records.items()}}
+        return state
 
     def run(self, n_steps: int):
         """Advance ``n_steps`` velocity-Verlet steps; returns (energy, forces) buffers of the last step (device).  With a
@@ -1452,13 +1472,7 @@ class DeviceMD(_CapturedEvaluation):
                 raise RuntimeError(f"DeviceMD: run({int(n_steps)}) would store {new} records on top of the "
                                    f"{self._n_records} held, more than record_capacity = {self.record_capacity}; "
                                    "call drain() first")
-        if self.use_graph and self._graph is None:
-            self._capture()
-        for _ in range(int(n_steps)):
-            if self.use_graph:
-                self._graph.replay()
-            else:
-                self._step()
+        self._run_steps(int(n_steps))
         if self.record_capacity:
             self._n_records += self._records_in(int(n_steps))
         self.steps_done += int(n_steps)
@@ -1524,66 +1538,27 @@ class DeviceMD(_CapturedEvaluation):
         if self.virial is None:
             raise RuntimeError("DeviceMD: the centroid pressure needs a ring-polymer NPT run (barostat=PILEBarostat(...))")
         P_ = rp.n_beads
-        vol = self.volume().reshape(P_, -1).mean(0)
-        p = -self.stress.reshape(P_, -1, 3, 3).mean(0)
-        if tensor:
-            if kinetic_component:
-                pc = self.centroid_momenta().contiguous()
-                p = p + 2.0 * self._rp_base.kinetic_energy_tensor(pc) / vol[:, None, None]
-            return p
-        p = torch.diagonal(p, dim1=1, dim2=2).sum(-1) / 3.0
-        if kinetic_component:
-            pc = self.centroid_momenta().contiguous()
-            ke = self._rp_base.kinetic_energy_and_temperature(pc, KB_MD)[0]
-            p = p + 2.0 * ke / vol / 3.0
-        return p
+        return self._pressure(-self.stress.reshape(P_, -1, 3, 3).mean(0), self.volume().reshape(P_, -1).mean(0),
+                              self._rp_base, self.centroid_momenta().contiguous(), tensor, kinetic_component)
 
     def state_dict(self) -> Dict[str, object]:
         """Everything a restarted run needs to continue bitwise: the MD state, the neighbour-list bookkeeping and the
         thermostat state (chain velocities / forces, Langevin application counter)."""
-        sd = {"positions": self.positions.clone(), "momenta": self.momenta.clone(), "forces": self.forces.clone(),
-              "energy": self.energy.clone(), "n_pairs": self.n_pairs.clone(), "nl_watch": self.nl_watch.clone(),
-              "steps_done": self.steps_done}
-        if self.model_positions is not self.positions:
-            sd["model_positions"] = self.model_positions.clone()
-        if self.thermostat is not None:
-            sd["thermostat"] = self.thermostat.state_dict()
-        if self.virial is not None:
-            sd.update(cell=self.cell.clone(), model_cell=self.model_cell.clone(), virial=self.virial.clone())
-        if self.barostat is not None:
-            sd["barostat"] = self.barostat.state_dict()
-        if self.properties:
-            sd["properties"] = {p: v.clone() for p, v in self.properties.items()}
+        sd = _clone_state(self._step_state())
+        sd["steps_done"] = self.steps_done
         if self.record_capacity:
-            sd["recorder"] = {"counter": self._rec_counter.clone(), "n_records": self._n_records,
-                              "records": {p: v[:self._n_records].clone() for p, v in self._records.items()}}
+            sd["recorder"]["n_records"] = self._n_records
         return sd
 
     def load_state_dict(self, state: Dict[str, object]):
         """Copy a ``state_dict`` into the existing buffers (a captured graph stays valid)."""
-        for k in ("positions", "momenta", "forces", "energy", "n_pairs", "nl_watch"):
-            getattr(self, k).copy_(state[k])
-        if self.model_positions is not self.positions:
-            self.model_positions.copy_(state["model_positions"])
-        if self.thermostat is not None:
-            self.thermostat.load_state_dict(state["thermostat"])
-        if self.virial is not None:
-            for k in ("cell", "model_cell", "virial"):
-                getattr(self, k).copy_(state[k])
-        if self.barostat is not None:
-            self.barostat.load_state_dict(state["barostat"])
-        for p, v in state.get("properties", {}).items():
-            self.properties[p].copy_(v)
         if self.record_capacity:
-            rec = state["recorder"]
-            n = int(rec["n_records"])
+            n = int(state["recorder"]["n_records"])
             if n > self.record_capacity:
                 raise ValueError(f"DeviceMD: the state holds {n} records, more than record_capacity = "
                                  f"{self.record_capacity}")
-            self._rec_counter.copy_(rec["counter"])
-            for p, v in rec["records"].items():
-                self._records[p][:n].copy_(v)
             self._n_records = n
+        _load_state(self._step_state(), state)
         self.steps_done = int(state["steps_done"])
 
     # ---- cell, stress and pressure (system.py:567-614), MD units, per system, fp64 on the device ----------------------------
@@ -1606,14 +1581,19 @@ class DeviceMD(_CapturedEvaluation):
 
     def pressure(self, tensor: bool = False, kinetic_component: bool = False) -> Tensor:
         """system.py:583-614: -stress ([n_sys, 3, 3]) or its trace / 3 ([n_sys]), optionally with the kinetic part."""
-        vol = self.volume()
-        p = -self.stress
+        return self._pressure(-self.stress, self.volume(), self.systems, self.momenta, tensor, kinetic_component)
+
+    @staticmethod
+    def _pressure(p: Tensor, vol: Tensor, systems: _Systems, momenta: Tensor, tensor: bool,
+                  kinetic_component: bool) -> Tensor:
+        """the pressure tensor ``p`` (-stress) or its trace / 3, optionally plus the kinetic part 2 K / V of ``momenta``
+        in ``systems`` (2 K / (3 V) for the trace)"""
         if tensor:
             if kinetic_component:
-                p = p + 2.0 * self.systems.kinetic_energy_tensor(self.momenta) / vol[:, None, None]
+                p = p + 2.0 * systems.kinetic_energy_tensor(momenta) / vol[:, None, None]
             return p
         p = torch.diagonal(p, dim1=1, dim2=2).sum(-1) / 3.0
         if kinetic_component:
-            ke = self.systems.kinetic_energy_and_temperature(self.momenta, KB_MD)[0]
+            ke = systems.kinetic_energy_and_temperature(momenta, KB_MD)[0]
             p = p + 2.0 * ke / vol / 3.0
         return p

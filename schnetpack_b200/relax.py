@@ -20,8 +20,7 @@ import torch
 
 from . import _lib, ops
 from . import properties as P
-from .md import _CapturedEvaluation
-from .neighbors import CellListNeighborList
+from .md import _CapturedEvaluation, _clone_state, _load_state, _TensorState
 
 __all__ = ["DeviceLBFGS", "LBFGSState"]
 
@@ -48,7 +47,7 @@ def _fixed_mask(fixed_atoms_mask, n_atoms: int, dev) -> Optional[Tensor]:
     return out.to(torch.uint8).to(dev)
 
 
-class LBFGSState:
+class LBFGSState(_TensorState):
     """Optimizer state of a batch and the launches of its kernels (the step and the convergence test), given a forces
     tensor.  ``positions`` [N, 3] are the starting positions in optimizer units (model positions x
     ``position_conversion``); forces are model forces, multiplied by ``force_conversion`` in the kernels.  Systems are
@@ -128,12 +127,8 @@ class LBFGSState:
                 "converged": self.converged, "steps_to_converge": self.steps_to_converge,
                 "n_unconverged": self.n_unconverged, "model_positions": self.model_positions}
 
-    def state_dict(self) -> Dict[str, Tensor]:
-        return {k: v.clone() for k, v in self.tensors().items()}
-
-    def load_state_dict(self, state: Dict[str, Tensor]):
-        for k, v in self.tensors().items():
-            v.copy_(state[k])
+    def _state(self) -> Dict[str, Tensor]:
+        return self.tensors()
 
 
 class DeviceLBFGS(_CapturedEvaluation):
@@ -156,9 +151,6 @@ class DeviceLBFGS(_CapturedEvaluation):
                  maxstep: float = 0.2, memory: int = 100, damping: float = 1.0, alpha: float = 70.0,
                  fixed_atoms_mask=None, position_conversion: float = 1.0, energy_conversion: float = 1.0,
                  energy_key: str = P.energy, force_key: str = P.forces, use_graph: bool = True):
-        dev = batch[P.R].device
-        if dev.type != "cuda":
-            raise ValueError("DeviceLBFGS needs a CUDA batch (no CPU fallback)")
         if float(maxstep) > 1.0:                                                 # batchwise_optimization.py:711-715
             raise ValueError("You are using a much too large value for the maximum step size: %.1f Angstrom"
                              % float(maxstep))
@@ -166,34 +158,14 @@ class DeviceLBFGS(_CapturedEvaluation):
         if outputs is not None and (force_key not in outputs or energy_key not in outputs):
             raise ValueError(f"DeviceLBFGS: the model must output '{energy_key}' and '{force_key}' (it outputs "
                              f"{sorted(outputs)})")
-        from .atomistic.pair_terms import check_ewald_cells, check_padded_pair_terms
-
         self.energy_key, self.force_key = energy_key, force_key
-        model = self._set_ensemble(model, "DeviceLBFGS")
-
-        check_padded_pair_terms(model, float(cutoff), "DeviceLBFGS")
-        check_ewald_cells(model, batch, "DeviceLBFGS")
-        self.model = model
+        idx_m, n_sys = self._setup(model, batch, cutoff, capacity, use_graph)
         self.p_conv = float(position_conversion)
         self.e_conv = float(energy_conversion)
         self.f_conv = self.e_conv / self.p_conv
-        self.static = {k: v.detach().clone() for k, v in batch.items() if k not in (P.idx_i, P.idx_j, P.offsets)}
         mp = self.static[P.R]
         if mp.dtype != torch.float32 or not mp.is_contiguous():
             raise ValueError("DeviceLBFGS: '_positions' must be a contiguous float32 tensor")
-        n = mp.shape[0]
-        idx_m = self.static.get(P.idx_m)
-        if idx_m is None:
-            idx_m = torch.zeros(n, dtype=torch.int64, device=dev)
-        n_sys = self.static[P.n_atoms].shape[0] if P.n_atoms in self.static else 1
-        self.nl = CellListNeighborList(cutoff, capacity=int(capacity), pad=True)
-        self.use_graph = use_graph
-        self.energy: Optional[Tensor] = None
-        self.forces: Optional[Tensor] = None
-        self.n_pairs: Optional[Tensor] = None
-        # [0] = largest pair count seen, [1] = 1 if any evaluation overflowed ``capacity``
-        self.nl_watch = torch.zeros(2, dtype=torch.int64, device=dev)
-        self._graph = None
         self.opt = LBFGSState(mp.double() * self.p_conv, idx_m, n_sys, memory=memory, maxstep=maxstep,
                               damping=damping, alpha=alpha, fixed_atoms_mask=fixed_atoms_mask,
                               position_conversion=self.p_conv, force_conversion=self.f_conv, model_positions=mp)
@@ -207,9 +179,8 @@ class DeviceLBFGS(_CapturedEvaluation):
         self._calculate()
         self.opt.check(self.forces)
 
-    def _state_tensors(self):
-        return (list(self.opt.tensors().values()) + [self.energy, self.forces, self.n_pairs, self.nl_watch]
-                + list(self.stacks.values()))
+    def _step_state(self) -> Dict[str, object]:
+        return dict(opt=self.opt.tensors(), **self._evaluation_state())
 
     def run(self, fmax: float = 0.05, steps: Optional[int] = None, check_every: int = 10) -> bool:
         """Relax until every system's largest force is below ``fmax`` or ``steps`` steps (default: unlimited) were taken
@@ -220,17 +191,11 @@ class DeviceLBFGS(_CapturedEvaluation):
         budget = DEFAULT_MAX_STEPS if not steps else int(steps)
         self.opt.set_fmax(fmax)
         self.opt.check(self.forces)              # the convergence test under this fmax
-        if self.use_graph and self._graph is None:
-            self._graph = self._capture_step(self._state_tensors())
         done = 0
         left = int(self.opt.n_unconverged.item())
         while left and done < budget:
             k = min(int(check_every), budget - done)
-            for _ in range(k):
-                if self.use_graph:
-                    self._graph.replay()
-                else:
-                    self._step()
+            self._run_steps(k)
             done += k
             self.iterations += k
             left = int(self.opt.n_unconverged.item())
@@ -287,14 +252,10 @@ class DeviceLBFGS(_CapturedEvaluation):
 
     def state_dict(self) -> Dict[str, object]:
         """Everything a restart needs to continue bitwise (it replaces the reference's pickle restart file)."""
-        return {"opt": self.opt.state_dict(), "energy": self.energy.clone(), "forces": self.forces.clone(),
-                "n_pairs": self.n_pairs.clone(), "nl_watch": self.nl_watch.clone(), "iterations": self.iterations,
-                "nsteps": self.nsteps}
+        return dict(_clone_state(self._step_state()), iterations=self.iterations, nsteps=self.nsteps)
 
     def load_state_dict(self, state: Dict[str, object]):
         """Copy a ``state_dict`` into the existing buffers (a captured graph stays valid)."""
-        self.opt.load_state_dict(state["opt"])
-        for k in ("energy", "forces", "n_pairs", "nl_watch"):
-            getattr(self, k).copy_(state[k])
+        _load_state(self._step_state(), state)
         self.iterations = int(state["iterations"])
         self.nsteps = int(state["nsteps"])

@@ -1,8 +1,8 @@
 """Unit conversion of the reference (units.py:132-189) without ``ase``: ``convert_units(src, tgt)`` parses unit strings
 such as ``"kcal / mol"`` or ``"Bohr"`` into ASE's frame (eV, Angstrom, amu) and returns the factor src / tgt.
 
-The unit names and values are those of ASE's units module for CODATA 2014 (the constants ``md.py`` restates), so that a
-conversion here gives the number the reference computes."""
+The unit names and values are those of ASE's units module for CODATA 2014 (the constants ``md.py`` builds its MD units
+from), so that a conversion here gives the number the reference computes."""
 from __future__ import annotations
 
 import math

@@ -22,8 +22,7 @@ import torch
 
 from . import _lib, ops
 from . import properties as P
-from .md import DeviceMD, _CapturedEvaluation
-from .neighbors import CellListNeighborList
+from .md import _CapturedEvaluation, replicate_batch
 from .units import _amu, _e, _hbar, _UNITS
 
 __all__ = ["DeviceVibrations"]
@@ -58,9 +57,6 @@ class DeviceVibrations(_CapturedEvaluation):
     def __init__(self, model: torch.nn.Module, batch: Dict[str, Tensor], masses: Tensor, cutoff: float, capacity: int,
                  delta: float = 0.01, nfree: int = 2, position_conversion: float = 1.0, energy_conversion: float = 1.0,
                  properties: Sequence[str] = (), max_replica_atoms: Optional[int] = None, use_graph: bool = True):
-        dev = batch[P.R].device
-        if dev.type != "cuda":
-            raise ValueError("DeviceVibrations needs a CUDA batch (no CPU fallback)")
         if int(nfree) not in (2, 4):
             raise ValueError(f"DeviceVibrations: nfree must be 2 or 4 (ase/vibrations/vibrations.py), got {nfree}")
         if not float(delta) > 0.0:
@@ -82,26 +78,16 @@ class DeviceVibrations(_CapturedEvaluation):
             missing = [p for p in [self.energy_key, self.force_key] + properties if p not in outputs]
             if missing:
                 raise ValueError(f"DeviceVibrations: the model does not output {missing} (it outputs {sorted(outputs)})")
-        from .atomistic.pair_terms import check_ewald_cells, check_padded_pair_terms
-
-        check_padded_pair_terms(model, float(cutoff), "DeviceVibrations")
-        check_ewald_cells(model, batch, "DeviceVibrations")
-        self.model = model
+        idx_m, n_sys = self._setup(model, batch, cutoff, capacity, use_graph)
         self.required_properties = properties
-        self.use_graph = use_graph
         self.nfree, self.p_conv, self.e_conv = int(nfree), float(position_conversion), float(energy_conversion)
         self.delta = float(delta)
 
-        base = {k: v.detach().clone() for k, v in batch.items() if k not in (P.idx_i, P.idx_j, P.offsets)}
+        base, dev = self.static, batch[P.R].device
         pos = base[P.R]
         if pos.dtype != torch.float32 or not pos.is_contiguous():
             raise ValueError("DeviceVibrations: '_positions' must be a contiguous float32 tensor")
         n = pos.shape[0]
-        n_sys = base[P.n_atoms].shape[0] if P.n_atoms in base else 1
-        idx_m = base.get(P.idx_m)
-        if idx_m is None:
-            idx_m = torch.zeros(n, dtype=torch.int64, device=dev)
-        idx_m = idx_m.to(torch.int64).contiguous()
         masses = torch.as_tensor(masses).reshape(-1)
         if masses.shape[0] != n:
             raise ValueError(f"DeviceVibrations: {masses.shape[0]} masses for {n} atoms")
@@ -125,8 +111,8 @@ class DeviceVibrations(_CapturedEvaluation):
         base.setdefault(P.idx_m, idx_m)
         base.setdefault(P.n_atoms, sizes.to(dev))
         self.base_positions = pos
-        self.static = DeviceMD._bead_batch(base, self.n_copies, n_sys)
-        self.nl = CellListNeighborList(cutoff, capacity=int(capacity) * self.n_copies, pad=True)
+        self.static = replicate_batch(base, self.n_copies, n_sys)
+        self.nl.capacity *= self.n_copies                # ``capacity`` is that of ``batch``, once per copy
         f64 = dict(dtype=torch.float64, device=dev)
         self.steps = torch.zeros(self.n_copies, n_sys, **f64)
         self.counter = torch.zeros(2, dtype=torch.int64, device=dev)
@@ -137,11 +123,6 @@ class DeviceVibrations(_CapturedEvaluation):
         self.polarizability_derivatives = (torch.zeros(n, 3, 3, 3, **f64) if P.polarizability in properties
                                            else None)
         self.outputs: Dict[str, Tensor] = {}       # the replica batch's dipoles / polarizabilities, copied per step
-        self.energy: Optional[Tensor] = None
-        self.forces: Optional[Tensor] = None
-        self.n_pairs: Optional[Tensor] = None
-        self.nl_watch = torch.zeros(2, dtype=torch.int64, device=dev)
-        self._graph = None
         self._eig: Optional[List[tuple]] = None
         self._calculate()                          # shapes of the outputs, buffers of the captured step
         p = ops._p
@@ -174,22 +155,17 @@ class DeviceVibrations(_CapturedEvaluation):
         self._calculate()
         ops.vib_assemble(self._params)
 
-    def _state_tensors(self):
-        return ([self.static[P.R], self.steps, self.counter, self.energy, self.forces, self.n_pairs, self.nl_watch,
-                 self.h_raw] + list(self.outputs.values())
-                + [t for t in (self.dipole_derivatives, self.polarizability_derivatives) if t is not None])
+    def _step_state(self) -> Dict[str, object]:
+        state = dict(positions=self.static[P.R], steps=self.steps, counter=self.counter, h_raw=self.h_raw,
+                     outputs=self.outputs, dipole_derivatives=self.dipole_derivatives,
+                     polarizability_derivatives=self.polarizability_derivatives, **self._evaluation_state())
+        return {k: v for k, v in state.items() if v is not None}
 
     def run(self):
         """Evaluate every displaced copy (``n_chunks`` replays of the captured step) and finish the Hessian and the
         derivatives."""
         self.counter.zero_()
-        if self.use_graph and self._graph is None and self.n_chunks:
-            self._graph = self._capture_step(self._state_tensors())
-        for _ in range(self.n_chunks):
-            if self.use_graph:
-                self._graph.replay()
-            else:
-                self._step()
+        self._run_steps(self.n_chunks)
         ops.vib_finish(self._params)
         self.check_neighbor_list()
         self._eig = None

@@ -183,13 +183,13 @@ def test_shared_cell_and_pbc_are_expanded_per_bead_system():
     cell = torch.eye(3)[None] * 7.0
     static = {"_positions": torch.zeros(5, 3), "_idx_m": torch.tensor([0, 0, 1, 2, 2]), "_n_atoms": torch.tensor([2, 1, 2]),
               "_cell": cell, "_pbc": torch.tensor([True, False, True])}
-    out = md.DeviceMD._bead_batch(static, P, B)
+    out = md.replicate_batch(static, P, B)
     assert out["_cell"].shape == (P * B, 3, 3) and torch.equal(out["_cell"], cell.expand(P * B, 3, 3))
     assert out["_pbc"].shape == (3 * P * B,) and torch.equal(out["_pbc"].reshape(-1, 3), static["_pbc"].expand(P * B, 3))
     assert torch.equal(out["_idx_m"][5:10], static["_idx_m"] + B) and out["_positions"].shape == (P * 5, 3)
     per_system = dict(static, _cell=cell.expand(B, 3, 3).clone(), _pbc=static["_pbc"].repeat(B))
-    out2 = md.DeviceMD._bead_batch(per_system, P, B)
+    out2 = md.replicate_batch(per_system, P, B)
     for k in out:
         assert torch.equal(out[k], out2[k]), k
     with pytest.raises(ValueError, match="neither shared nor one per system"):
-        md.DeviceMD._bead_batch(dict(static, _cell=torch.eye(3).repeat(2, 1, 1)), P, B)
+        md.replicate_batch(dict(static, _cell=torch.eye(3).repeat(2, 1, 1)), P, B)
