@@ -714,6 +714,68 @@ typedef struct {
 int spk_relax_step(const spk_lbfgs_t* state, const float* forces, spk_stream_t stream);
 int spk_relax_converged(const spk_lbfgs_t* state, const float* forces, spk_stream_t stream);
 
+/* ---- batchwise FIRE relaxation with an optional unit-cell filter (csrc/fire.cu; ASE's FIRE without downhill_check and
+ * ASE's UnitCellFilter) ---------------------------------------------------------------------------------------------
+ * One optimizer per system (atoms [sys_ptr[m], sys_ptr[m+1]), idx_m sorted), state fp64 on the device, in optimizer
+ * units (model positions / cells x position_conversion, model energies x energy_conversion).  The generalized
+ * coordinates of system m are the rows s [N, 3] of its atoms and, with filter = 1, the 9 values h[m] = cell_factor[m] F
+ * (row-major), F the deformation gradient with cell = cell0 F^T (rows = lattice vectors); without a filter F = I and
+ * s are the positions.  counter (int64[2]) = (steps taken as the next step reads it, steps taken as the last step wrote
+ * it).  spk_fire_forces must run between two steps, on the forces (and virial) of the current positions.
+ *
+ * spk_fire_forces, with f = forces x force_conversion (0 on fixed atoms) and F = h / cell_factor:
+ *   g [N, 3] = f_i F; with the filter hg [n_sys, 9] = P(Vir F^-T) / cell_factor, Vir = -(energy_conversion sym(W) +
+ *   scalar_pressure V I), W = virial [n_sys, 3, 3] (fp64, model units, the strain derivative of spk_pairwise_virial),
+ *   V = |det cell|, P the projections in ASE's order: hydrostatic_strain (tr / 3 I), the element-wise mask [9],
+ *   constant_volume (tr / 3 off the diagonal);
+ *   sums [n_sys, 3] = (v.g, v.v, g.g) over all generalized coordinates (fixed-order CTA partials, no atomics);
+ *   fmax_sys[m] = sqrt(max_row |g_row|^2), converged[m] = fmax_sys^2 < fmax[0]^2, steps[m] = the counter[1] at which
+ *   the system became converged (kept while it stays converged, -1 otherwise), n_unconverged[0], counter[0] = counter[1].
+ * spk_fire_step, per unconverged system (a converged one keeps all its state): if started, ASE's mixing when v.g > 0
+ *   (v = (1 - a) v + a g / |g| |v|; dt = min(dt finc, dtmax) and a *= fa if nsteps > nmin; nsteps += 1), else the
+ *   reset (v = 0, a = astart, dt *= fdec, nsteps = 0); then v += dt g, dr = dt v, dr *= maxstep / |dr| if |dr| >
+ *   maxstep (|dr| over all the system's coordinates, from the three sums); s += dr, h += dr, r = s F^T,
+ *   model_positions = float(r / position_conversion), model_cell = float(cell0 F^T / position_conversion);
+ *   counter[1] = counter[0] + 1.
+ * workspace: spk_fire_workspace_bytes(n_atoms, n_sys) bytes, 8-byte aligned, untouched between the two calls. */
+typedef struct {
+    double* s;                 /* [N, 3] generalized atom coordinates */
+    double* r;                 /* [N, 3] positions (may alias s without a filter) */
+    double* v;                 /* [N, 3] */
+    double* g;                 /* [N, 3] */
+    double* h;                 /* [n_sys, 9] cell_factor F (filter only) */
+    double* hv;                /* [n_sys, 9] (filter only) */
+    double* hg;                /* [n_sys, 9] (filter only) */
+    const double* cell0;       /* [n_sys, 9] the starting cell (filter only) */
+    const double* cell_factor; /* [n_sys] (filter only) */
+    double* dt;                /* [n_sys] */
+    double* a;                 /* [n_sys] */
+    int64_t* nsteps;           /* [n_sys] */
+    int32_t* started;          /* [n_sys] 0 until the system's first step */
+    double* sums;              /* [n_sys, 3] */
+    double* coef;              /* [n_sys, 7] step coefficients, written and read by spk_fire_step */
+    double* workspace;
+    int64_t* counter;          /* [2] */
+    const double* fmax;        /* [1] convergence threshold */
+    double* fmax_sys;          /* [n_sys] */
+    int32_t* converged;        /* [n_sys] */
+    int64_t* steps;            /* [n_sys] */
+    int32_t* n_unconverged;    /* [1] */
+    const uint8_t* fixed;      /* [N] or NULL */
+    float* model_positions;    /* [N, 3] */
+    float* model_cell;         /* [n_sys, 3, 3] (filter only) */
+    const int64_t* idx_m;      /* [N] */
+    const int32_t* sys_ptr;    /* [n_sys + 1] */
+    double mask[9];            /* element-wise mask of the cell forces (ones: no mask) */
+    int64_t n_atoms, n_sys, nmin;
+    int32_t filter, hydrostatic_strain, constant_volume, reserved;
+    double force_conversion, energy_conversion, position_conversion, scalar_pressure;
+    double maxstep, dtmax, finc, fdec, astart, fa;
+} spk_fire_t;
+size_t spk_fire_workspace_bytes(int64_t n_atoms, int64_t n_sys);
+int spk_fire_forces(const spk_fire_t* state, const float* forces, const double* virial, spk_stream_t stream);
+int spk_fire_step(const spk_fire_t* state, spk_stream_t stream);
+
 /* ---- model ensembles (csrc/ensemble.cu; md/calculators/ensemble_calculator.py:38-59,
  * interfaces/batchwise_optimization.py:36-72, interfaces/ase_interface.py:340-432) ------------------------------------
  * The K members' outputs are stacked fp32 slots [K, ...] (slot k = member k).  Every statistic runs in fp64 over k in

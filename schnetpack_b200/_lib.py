@@ -73,6 +73,22 @@ class VibParams(Structure):
                 ("max_atoms", c_int64), ("delta", c_double), ("mw_scale", c_double)]
 
 
+class FIREState(Structure):
+    """spk_fire_t of include/spk_b200.h (device pointers of the FIRE state, the filter settings and the parameters)."""
+    _fields_ = [("s", c_void_p), ("r", c_void_p), ("v", c_void_p), ("g", c_void_p), ("h", c_void_p), ("hv", c_void_p),
+                ("hg", c_void_p), ("cell0", c_void_p), ("cell_factor", c_void_p), ("dt", c_void_p), ("a", c_void_p),
+                ("nsteps", c_void_p), ("started", c_void_p), ("sums", c_void_p), ("coef", c_void_p),
+                ("workspace", c_void_p), ("counter", c_void_p), ("fmax", c_void_p), ("fmax_sys", c_void_p),
+                ("converged", c_void_p), ("steps", c_void_p), ("n_unconverged", c_void_p), ("fixed", c_void_p),
+                ("model_positions", c_void_p), ("model_cell", c_void_p), ("idx_m", c_void_p), ("sys_ptr", c_void_p),
+                ("mask", c_double * 9), ("n_atoms", c_int64), ("n_sys", c_int64), ("nmin", c_int64),
+                ("filter", c_int32), ("hydrostatic_strain", c_int32), ("constant_volume", c_int32),
+                ("reserved", c_int32), ("force_conversion", c_double), ("energy_conversion", c_double),
+                ("position_conversion", c_double), ("scalar_pressure", c_double), ("maxstep", c_double),
+                ("dtmax", c_double), ("finc", c_double), ("fdec", c_double), ("astart", c_double), ("fa", c_double)]
+
+
+FIRE_COEF = 7               # step coefficients per system (spk_fire_t.coef)
 RELAX_WARP_ATOMS = 256      # SPK_RELAX_WARP_ATOMS
 RELAX_MAX_MEMORY = 4096     # SPK_RELAX_MAX_MEMORY
 
@@ -197,6 +213,9 @@ SIGNATURES = {
     "spk_spectrum_series": [P, c_int64, c_int64, c_int64, P, P, c_int64, c_int, c_double, P, P, P, P],
     "spk_spectrum_autocorrelation": [P, c_int64, P, P, c_int64, c_int64, P, P, c_size_t, P],
     "spk_spectrum_transform": [P, c_int64, c_int64, P, c_double, P, P, c_size_t, P],
+    "spk_fire_workspace_bytes": [c_int64, c_int64],
+    "spk_fire_forces": [POINTER(FIREState), P, P, P],
+    "spk_fire_step": [POINTER(FIREState), P],
 }
 _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_size_t,
             "spk_pairwise_virial_workspace_bytes": c_size_t, "spk_md_barostat_workspace_bytes": c_size_t,
@@ -206,7 +225,7 @@ _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_siz
             "spk_rpmd_barostat_workspace_bytes": c_size_t, "spk_head_workspace_bytes": c_size_t,
             "spk_head_charges_bwd_workspace_bytes": c_size_t, "spk_pair_energy_workspace_bytes": c_size_t,
             "spk_ewald_workspace_bytes": c_size_t, "spk_ensemble_workspace_bytes": c_size_t,
-            "spk_spectrum_workspace_bytes": c_size_t}
+            "spk_spectrum_workspace_bytes": c_size_t, "spk_fire_workspace_bytes": c_size_t}
 
 _lib = None
 
@@ -251,7 +270,8 @@ LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out
             "spk_md_barostat_half_step": 2, "spk_md_barostat_main_step": 2, "spk_rpmd_barostat_half_step": 2,
             "spk_rpmd_barostat_main_step": 2, "spk_head_fwd": 2,
             "spk_relax_converged": 2, "spk_pair_energy_fwd": 2, "spk_head_charges_bwd": 3,
-            "spk_pairwise_virial_add": 2, "spk_spectrum_autocorrelation": 2, "spk_spectrum_transform": 2}   # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global
+            "spk_pairwise_virial_add": 2, "spk_spectrum_autocorrelation": 2, "spk_spectrum_transform": 2,
+            "spk_fire_forces": 3, "spk_fire_step": 2}   # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global
 launch_count = 0
 
 

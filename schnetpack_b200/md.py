@@ -1006,6 +1006,27 @@ class _CapturedEvaluation:
     def _evaluation_state(self) -> Dict[str, Tensor]:
         return {"energy": self.energy, "forces": self.forces, "n_pairs": self.n_pairs, "nl_watch": self.nl_watch}
 
+    def _setup_virial(self, n_sys: int, what: str) -> Tensor:
+        """The model cell ``static[_cell]`` (checked to be a contiguous fp32 [n_sys, 3, 3] tensor, returned as it is) and
+        ``self.virial``, the fp64 [n_sys, 3, 3] model-unit virial that every evaluation then writes."""
+        name = type(self).__name__
+        if P.cell not in self.static:
+            raise ValueError(f"{name}: {what} need a periodic batch with a '_cell'")
+        model_cell = self.static[P.cell]
+        if model_cell.dtype != torch.float32 or not model_cell.is_contiguous() or model_cell.numel() != 9 * n_sys:
+            raise ValueError(f"{name}: '_cell' must be a contiguous float32 [n_sys, 3, 3] tensor")
+        self.virial = torch.zeros(n_sys, 3, 3, dtype=torch.float64, device=model_cell.device)
+        return model_cell
+
+    def _check_periodic(self, n_sys: int, volume: Tensor, what: str):
+        """refuse a batch in which a system is not periodic on all three axes or has zero ``volume`` [n_sys]"""
+        name = type(self).__name__
+        pbc = self.static.get(P.pbc)
+        if pbc is None or not bool(pbc.reshape(-1, 3).all()) or pbc.reshape(-1, 3).shape[0] not in (1, n_sys):
+            raise ValueError(f"{name}: {what} needs every system periodic on all three axes (system.py:599-602)")
+        if bool((volume == 0.0).any()):
+            raise ValueError(f"{name}: {what} needs a non-zero cell volume for every system (system.py:599-602)")
+
     def _run_steps(self, n: int):
         """``n`` steps: replays of the step, captured on first use, or eager ``_step()`` calls without ``use_graph``."""
         if n > 0 and self.use_graph and self._graph is None:
@@ -1142,20 +1163,10 @@ class DeviceMD(_CapturedEvaluation):
         self.virial: Optional[Tensor] = None        # model-unit virial [n_sys, 3, 3] fp64, written by every evaluation
         if barostat is not None or compute_stress:
             n_sys = self.systems.n_sys
-            if P.cell not in self.static:
-                raise ValueError("DeviceMD: stress and NPT need a periodic batch with a '_cell'")
-            self.model_cell = self.static[P.cell]
-            if (self.model_cell.dtype != torch.float32 or not self.model_cell.is_contiguous()
-                    or self.model_cell.numel() != 9 * n_sys):
-                raise ValueError("DeviceMD: '_cell' must be a contiguous float32 [n_sys, 3, 3] tensor")
+            self.model_cell = self._setup_virial(n_sys, "stress and NPT")
             self.cell = self.model_cell.reshape(n_sys, 3, 3).double() / self.p_conv
-            self.virial = torch.zeros(n_sys, 3, 3, dtype=torch.float64, device=dev)
         if barostat is not None:
-            pbc = self.static.get(P.pbc)
-            if pbc is None or not bool(pbc.reshape(-1, 3).all()) or pbc.reshape(-1, 3).shape[0] not in (1, n_sys):
-                raise ValueError("DeviceMD: NPT needs every system periodic on all three axes (system.py:599-602)")
-            if bool((self.volume() == 0.0).any()):
-                raise ValueError("DeviceMD: NPT needs a non-zero cell volume for every system (system.py:599-602)")
+            self._check_periodic(n_sys, self.volume(), "NPT")
             if ring_polymer is not None:
                 barostat.bind(self._rp_base, self.dt, ring_polymer)               # on_simulation_start
             else:

@@ -10,10 +10,15 @@ unconverged systems), and ``DeviceLBFGS.run`` reads that count once per ``check_
 
 Systems may differ in size (the reference needs equal atom counts).  The fp64 recursion departs on purpose from the
 reference, whose float32 forces keep ``q`` and ``z`` in float32 through numpy's in-place updates.
+
+``DeviceFIRE`` (DESIGN.md section 18) relaxes with ASE's FIRE instead, optionally on the generalized coordinates of ASE's
+``UnitCellFilter``, so that periodic systems relax their cells too, under an external pressure.  Its kernels are those of
+``csrc/fire.cu``: ``spk_fire_forces`` after every evaluation and ``spk_fire_step``.
 """
 from __future__ import annotations
 
 import ctypes
+import math
 from typing import Dict, Optional
 
 import torch
@@ -22,7 +27,7 @@ from . import _lib, ops
 from . import properties as P
 from .md import _CapturedEvaluation, _clone_state, _load_state, _TensorState
 
-__all__ = ["DeviceLBFGS", "LBFGSState"]
+__all__ = ["DeviceLBFGS", "LBFGSState", "DeviceFIRE", "FIREState", "UnitCellFilter"]
 
 Tensor = torch.Tensor
 DEFAULT_MAX_STEPS = 100_000_000          # ASE's Dynamics default, which the reference's run loop inherits
@@ -45,6 +50,18 @@ def _fixed_mask(fixed_atoms_mask, n_atoms: int, dev) -> Optional[Tensor]:
         out = torch.zeros(n_atoms, dtype=torch.bool)
         out[idx] = True
     return out.to(torch.uint8).to(dev)
+
+
+def _ensemble_uncertainty(driver) -> Dict[str, Tensor]:
+    """the unbiased std over the ensemble members of the energies [n_sys] and forces [N, 3] at the current positions,
+    in optimizer units (BatchwiseEnsembleCalculator.calculate, :329-335)"""
+    if driver.ensemble is None:
+        raise RuntimeError(f"{type(driver).__name__}: get_uncertainty needs an ensemble (model=[m1, m2, ...])")
+    from .ensemble import ensemble_moments
+
+    e = ensemble_moments(driver.stacks[driver.energy_key], ddof=1, spread_scale=driver.e_conv, var=False, std=True)[2]
+    f = ensemble_moments(driver.stacks[driver.force_key], ddof=1, spread_scale=driver.f_conv, var=False, std=True)[2]
+    return {"energy_uncertainty": e, "forces_uncertainty": f}
 
 
 class LBFGSState(_TensorState):
@@ -228,13 +245,7 @@ class DeviceLBFGS(_CapturedEvaluation):
     def get_uncertainty(self) -> Dict[str, Tensor]:
         """Ensemble runs: the unbiased std over the members of the energies [n_sys] and forces [N, 3] at the current
         positions, in optimizer units (BatchwiseEnsembleCalculator.calculate, :329-335)"""
-        if self.ensemble is None:
-            raise RuntimeError("DeviceLBFGS: get_uncertainty needs an ensemble (model=[m1, m2, ...])")
-        from .ensemble import ensemble_moments
-
-        e = ensemble_moments(self.stacks[self.energy_key], ddof=1, spread_scale=self.e_conv, var=False, std=True)[2]
-        f = ensemble_moments(self.stacks[self.force_key], ddof=1, spread_scale=self.f_conv, var=False, std=True)[2]
-        return {"energy_uncertainty": e, "forces_uncertainty": f}
+        return _ensemble_uncertainty(self)
 
     @property
     def fmax(self) -> Tensor:
@@ -252,6 +263,345 @@ class DeviceLBFGS(_CapturedEvaluation):
 
     def state_dict(self) -> Dict[str, object]:
         """Everything a restart needs to continue bitwise (it replaces the reference's pickle restart file)."""
+        return dict(_clone_state(self._step_state()), iterations=self.iterations, nsteps=self.nsteps)
+
+    def load_state_dict(self, state: Dict[str, object]):
+        """Copy a ``state_dict`` into the existing buffers (a captured graph stays valid)."""
+        _load_state(self._step_state(), state)
+        self.iterations = int(state["iterations"])
+        self.nsteps = int(state["nsteps"])
+
+
+# ---- FIRE and the unit-cell filter -------------------------------------------------------------------------------------
+class UnitCellFilter:
+    """The settings of ASE's ``UnitCellFilter`` for ``DeviceFIRE``: the cell of every system relaxes with its atoms.
+    ``mask``: 6 Voigt components (xx, yy, zz, yz, xz, xy) or a 3 x 3 array multiplied into the cell forces;
+    ``cell_factor`` scales the cell coordinates (default: each system's atom count); ``hydrostatic_strain`` keeps the
+    cell shape; ``constant_volume`` removes the trace of the cell forces; ``scalar_pressure`` is the external pressure in
+    optimizer energy / length^3 (eV / Angstrom^3 in ASE's units; ``units.convert_units("GPa", "eV / Ang / Ang / Ang")``
+    gives the factor from GPa)."""
+
+    def __init__(self, mask=None, cell_factor: Optional[float] = None, hydrostatic_strain: bool = False,
+                 constant_volume: bool = False, scalar_pressure: float = 0.0):
+        if mask is None:
+            full = torch.ones(3, 3, dtype=torch.float64)
+        else:
+            m = torch.as_tensor(mask, dtype=torch.float64).cpu()
+            if m.shape == (6,):
+                xx, yy, zz, yz, xz, xy = m.tolist()              # ASE's voigt_6_to_full_3x3_stress
+                full = torch.tensor([[xx, xy, xz], [xy, yy, yz], [xz, yz, zz]], dtype=torch.float64)
+            elif m.shape == (3, 3):
+                full = m.clone()
+            else:
+                raise ValueError(f"UnitCellFilter: mask must have 6 Voigt components or be 3 x 3, got shape "
+                                 f"{tuple(m.shape)}")
+        if cell_factor is not None and not float(cell_factor) > 0.0:
+            raise ValueError(f"UnitCellFilter: cell_factor must be > 0, got {cell_factor}")
+        if not math.isfinite(float(scalar_pressure)):
+            raise ValueError("UnitCellFilter: scalar_pressure must be finite")
+        self.mask = full
+        self.cell_factor = None if cell_factor is None else float(cell_factor)
+        self.hydrostatic_strain = bool(hydrostatic_strain)
+        self.constant_volume = bool(constant_volume)
+        self.scalar_pressure = float(scalar_pressure)
+
+
+FIRE_DEFAULTS = dict(dt=0.1, maxstep=0.2, dtmax=1.0, Nmin=5, finc=1.1, fdec=0.5, astart=0.1, fa=0.99, a=0.1)
+
+
+def _check_fire_keywords(kw: Dict[str, float]):
+    for k in ("dt", "maxstep", "dtmax", "finc", "fdec", "fa"):
+        if not float(kw[k]) > 0.0:
+            raise ValueError(f"FIRE: {k} must be > 0, got {kw[k]}")
+    for k in ("astart", "a"):
+        if not 0.0 <= float(kw[k]) <= 1.0:
+            raise ValueError(f"FIRE: {k} must be in [0, 1], got {kw[k]}")
+    if int(kw["Nmin"]) != kw["Nmin"] or int(kw["Nmin"]) < 0:
+        raise ValueError(f"FIRE: Nmin must be a non-negative integer, got {kw['Nmin']}")
+
+
+class FIREState(_TensorState):
+    """FIRE state of a batch and the launches of its kernels, given a forces tensor (and, with ``cell_filter``, the fp64
+    model virial [n_sys, 3, 3]).  ``positions`` [N, 3] are the starting positions in optimizer units (model positions x
+    ``position_conversion``), ``cell`` [n_sys, 3, 3] the starting cells in the same units (needed with the filter);
+    forces are model forces, multiplied by ``force_conversion``, and the virial is multiplied by ``energy_conversion``.
+    ``check(forces, virial)`` must run on the forces of the current positions before every ``step``.
+    ``model_positions`` (fp32 [N, 3]) and ``model_cell`` (fp32 [n_sys, 3, 3]), allocated if not given, receive the new
+    positions and cells / position_conversion at every step.  Keywords are those of ASE's FIRE."""
+
+    def __init__(self, positions: Tensor, idx_m: Tensor, n_sys: int, dt: float = 0.1, maxstep: float = 0.2,
+                 dtmax: float = 1.0, Nmin: int = 5, finc: float = 1.1, fdec: float = 0.5, astart: float = 0.1,
+                 fa: float = 0.99, a: float = 0.1, fixed_atoms_mask=None, cell: Optional[Tensor] = None,
+                 cell_filter: Optional[UnitCellFilter] = None, position_conversion: float = 1.0,
+                 force_conversion: float = 1.0, energy_conversion: float = 1.0,
+                 model_positions: Optional[Tensor] = None, model_cell: Optional[Tensor] = None, fmax: float = 0.05):
+        dev = positions.device
+        if dev.type != "cuda":
+            raise ValueError("FIREState needs CUDA tensors (no CPU fallback)")
+        kw = dict(dt=dt, maxstep=maxstep, dtmax=dtmax, Nmin=Nmin, finc=finc, fdec=fdec, astart=astart, fa=fa, a=a)
+        _check_fire_keywords(kw)
+        if cell_filter is not None and not isinstance(cell_filter, UnitCellFilter):
+            raise TypeError("FIREState: cell_filter must be a UnitCellFilter")
+        n, n_sys = int(positions.shape[0]), int(n_sys)
+        if n_sys < 1:
+            raise ValueError("FIREState: the batch has no system")
+        f64 = dict(dtype=torch.float64, device=dev)
+        self.n_atoms, self.n_sys, self.filter = n, n_sys, cell_filter
+        self.idx_m = idx_m.to(dev, torch.int64).contiguous()
+        self.sys_ptr = ops.segment_ptr(self.idx_m, n_sys)
+        p_conv = float(position_conversion)
+        self.s = positions.detach().to(**f64).reshape(n, 3).contiguous().clone()
+        self.r = torch.zeros_like(self.s) if cell_filter is not None else self.s
+        self.v = torch.zeros_like(self.s)
+        self.g = torch.zeros_like(self.s)
+        self.dt = torch.full((n_sys,), float(dt), **f64)
+        self.a = torch.full((n_sys,), float(a), **f64)
+        self.nsteps = torch.zeros(n_sys, dtype=torch.int64, device=dev)
+        self.started = torch.zeros(n_sys, dtype=torch.int32, device=dev)
+        self.sums = torch.zeros(n_sys, 3, **f64)
+        self.coef = torch.zeros(n_sys, _lib.FIRE_COEF, **f64)
+        nbytes = int(_lib.lib().spk_fire_workspace_bytes(n, n_sys))
+        self.workspace = torch.zeros(max(nbytes // 8, 1), **f64)
+        self.counter = torch.zeros(2, dtype=torch.int64, device=dev)
+        self.fmax_target = torch.full((1,), float(fmax), **f64)
+        self.fmax = torch.zeros(n_sys, **f64)
+        self.converged = torch.zeros(n_sys, dtype=torch.int32, device=dev)
+        self.steps_to_converge = torch.full((n_sys,), -1, dtype=torch.int64, device=dev)
+        self.n_unconverged = torch.full((1,), n_sys, dtype=torch.int32, device=dev)
+        self.fixed = _fixed_mask(fixed_atoms_mask, n, dev)
+        if model_positions is None:
+            model_positions = (self.s / p_conv).float()
+        self.model_positions = ops.f32(model_positions, "model_positions")
+        self.h = self.hv = self.hg = self.cell0 = self.cell_factor = self.model_cell = None
+        mask = [1.0] * 9
+        if cell_filter is not None:
+            if cell is None:
+                raise ValueError("FIREState: a cell filter needs the starting cells")
+            self.cell0 = cell.detach().to(**f64).reshape(n_sys, 9).contiguous().clone()
+            sizes = (self.sys_ptr[1:] - self.sys_ptr[:-1]).to(torch.float64)
+            cf = sizes if cell_filter.cell_factor is None else torch.full_like(sizes, cell_filter.cell_factor)
+            if bool((cf <= 0).any()):
+                raise ValueError("FIREState: the default cell_factor (the atom count) needs atoms in every system")
+            self.cell_factor = cf.contiguous()
+            self.h = (torch.eye(3, **f64).reshape(1, 9) * cf[:, None]).contiguous()    # cell_factor F with F = I
+            self.hv = torch.zeros_like(self.h)
+            self.hg = torch.zeros_like(self.h)
+            self.r.copy_(self.s)
+            if model_cell is None:
+                model_cell = (self.cell0 / p_conv).float()
+            self.model_cell = ops.f32(model_cell, "model_cell")
+            if self.model_cell.numel() != 9 * n_sys:
+                raise ValueError(f"FIREState: model_cell of {self.model_cell.numel()} values for {n_sys} systems")
+            mask = cell_filter.mask.reshape(-1).tolist()
+        p = ops._p
+        self._params = _lib.FIREState(
+            p(self.s), p(self.r), p(self.v), p(self.g), p(self.h), p(self.hv), p(self.hg), p(self.cell0),
+            p(self.cell_factor), p(self.dt), p(self.a), p(self.nsteps), p(self.started), p(self.sums), p(self.coef),
+            p(self.workspace), p(self.counter), p(self.fmax_target), p(self.fmax), p(self.converged),
+            p(self.steps_to_converge), p(self.n_unconverged), p(self.fixed), p(self.model_positions),
+            p(self.model_cell), p(self.idx_m), p(self.sys_ptr), (ctypes.c_double * 9)(*mask), n, n_sys, int(Nmin),
+            int(cell_filter is not None), int(bool(cell_filter and cell_filter.hydrostatic_strain)),
+            int(bool(cell_filter and cell_filter.constant_volume)), 0, float(force_conversion),
+            float(energy_conversion), p_conv, float(cell_filter.scalar_pressure) if cell_filter else 0.0,
+            float(maxstep), float(dtmax), float(finc), float(fdec), float(astart), float(fa))
+
+    def check(self, forces: Tensor, virial: Optional[Tensor] = None):
+        """the generalized forces at the current positions and the convergence test (fmax, converged,
+        steps_to_converge and the unconverged count, on the device)"""
+        f = ops.f32(forces, "forces")
+        if f.numel() != 3 * self.n_atoms:
+            raise ValueError(f"FIREState: forces of {f.numel()} values for {self.n_atoms} atoms")
+        w = None
+        if self.filter is not None:
+            if (virial is None or virial.dtype != torch.float64 or not virial.is_contiguous()
+                    or virial.numel() != 9 * self.n_sys or virial.device != f.device):
+                raise ValueError("FIREState: a cell filter needs the fp64 contiguous [n_sys, 3, 3] model virial")
+            w = virial
+        _lib.call("spk_fire_forces", ctypes.byref(self._params), ops._p(f), ops._p(w), ops._stream(),
+                  launches=2 + int(self.n_atoms > 0))
+
+    def step(self):
+        """one FIRE step with the generalized forces of the last ``check``"""
+        _lib.call("spk_fire_step", ctypes.byref(self._params), ops._stream(), launches=1 + int(self.n_atoms > 0))
+
+    def set_fmax(self, fmax: float):
+        self.fmax_target.fill_(float(fmax))
+
+    def deformation_gradient(self) -> Optional[Tensor]:
+        """F [n_sys, 3, 3] fp64 (cell = cell0 F^T), None without a filter"""
+        if self.filter is None:
+            return None
+        return (self.h / self.cell_factor[:, None]).reshape(-1, 3, 3)
+
+    def cell(self) -> Optional[Tensor]:
+        """the current cells [n_sys, 3, 3] fp64 in optimizer units, None without a filter"""
+        if self.filter is None:
+            return None
+        return torch.matmul(self.cell0.reshape(-1, 3, 3), self.deformation_gradient().transpose(1, 2))
+
+    def tensors(self) -> Dict[str, Tensor]:
+        """every buffer the step and the force side write and a later step reads"""
+        out = {"s": self.s, "v": self.v, "g": self.g, "dt": self.dt, "a": self.a, "nsteps": self.nsteps,
+               "started": self.started, "sums": self.sums, "counter": self.counter, "fmax_target": self.fmax_target,
+               "fmax": self.fmax, "converged": self.converged, "steps_to_converge": self.steps_to_converge,
+               "n_unconverged": self.n_unconverged, "model_positions": self.model_positions}
+        if self.filter is not None:
+            out.update(r=self.r, h=self.h, hv=self.hv, hg=self.hg, model_cell=self.model_cell)
+        return out
+
+    def _state(self) -> Dict[str, Tensor]:
+        return self.tensors()
+
+
+class DeviceFIRE(_CapturedEvaluation):
+    """Relax every system of ``batch`` with ASE's FIRE (its keywords and defaults; no ``downhill_check``), one optimizer
+    per system, with the batch semantics of ``DeviceLBFGS``: a system whose largest (generalized) force is below
+    ``fmax`` takes no step and keeps its optimizer state, and systems may differ in size.  ``batch[_positions]`` (and
+    ``_cell``) are in model units; ``position_conversion`` and ``energy_conversion`` turn model lengths and energies into
+    the optimizer's units, in which ``dt``, ``maxstep``, ``fmax`` and the filter's ``scalar_pressure`` are given.
+    ``fixed_atoms_mask`` (boolean mask or atom indices) zeroes the forces of atoms that must not move; under a filter
+    they keep their scaled coordinates and so move with the cell.
+
+    ``cell_filter`` (a ``UnitCellFilter``) relaxes the cells too: every system must be periodic on all three axes, the
+    model's virial is evaluated at every step, and the neighbour list is rebuilt on the new cell.  It is refused for
+    an ensemble, which has no stress.
+
+    One step is the optimizer kernels, the neighbour list, the model and the convergence test, captured once as a CUDA
+    graph (``use_graph``).  ``model`` may be a list of at least two members: their mean forces drive a fixed-cell
+    relaxation and ``get_uncertainty`` gives the unbiased std over the members, as in ``DeviceLBFGS``."""
+
+    def __init__(self, model: torch.nn.Module, batch: Dict[str, Tensor], cutoff: float, capacity: int,
+                 dt: float = 0.1, maxstep: float = 0.2, dtmax: float = 1.0, Nmin: int = 5, finc: float = 1.1,
+                 fdec: float = 0.5, astart: float = 0.1, fa: float = 0.99, a: float = 0.1, fixed_atoms_mask=None,
+                 cell_filter: Optional[UnitCellFilter] = None, position_conversion: float = 1.0,
+                 energy_conversion: float = 1.0, energy_key: str = P.energy, force_key: str = P.forces,
+                 use_graph: bool = True):
+        _check_fire_keywords(dict(dt=dt, maxstep=maxstep, dtmax=dtmax, Nmin=Nmin, finc=finc, fdec=fdec,
+                                  astart=astart, fa=fa, a=a))
+        if cell_filter is not None and not isinstance(cell_filter, UnitCellFilter):
+            raise TypeError("DeviceFIRE: cell_filter must be a UnitCellFilter")
+        outputs = getattr(model, "model_outputs", None)
+        if outputs is not None and (force_key not in outputs or energy_key not in outputs):
+            raise ValueError(f"DeviceFIRE: the model must output '{energy_key}' and '{force_key}' (it outputs "
+                             f"{sorted(outputs)})")
+        self.energy_key, self.force_key = energy_key, force_key
+        idx_m, n_sys = self._setup(model, batch, cutoff, capacity, use_graph)
+        if cell_filter is not None and self.ensemble is not None:
+            raise NotImplementedError("DeviceFIRE: a cell filter needs the stress, which an ensemble does not have (the "
+                                      "reference's EnsembleCalculator._activate_stress raises)")
+        self.p_conv = float(position_conversion)
+        self.e_conv = float(energy_conversion)
+        self.f_conv = self.e_conv / self.p_conv
+        mp = self.static[P.R]
+        if mp.dtype != torch.float32 or not mp.is_contiguous():
+            raise ValueError("DeviceFIRE: '_positions' must be a contiguous float32 tensor")
+        cell = model_cell = None
+        if cell_filter is not None:
+            model_cell = self._setup_virial(n_sys, "a cell filter")
+            cell = model_cell.reshape(n_sys, 3, 3).double() * self.p_conv
+            self._check_periodic(n_sys, torch.linalg.det(cell), "a cell filter")
+        self.opt = FIREState(mp.double() * self.p_conv, idx_m, n_sys, dt=dt, maxstep=maxstep, dtmax=dtmax, Nmin=Nmin,
+                             finc=finc, fdec=fdec, astart=astart, fa=fa, a=a, fixed_atoms_mask=fixed_atoms_mask,
+                             cell=cell, cell_filter=cell_filter, position_conversion=self.p_conv,
+                             force_conversion=self.f_conv, energy_conversion=self.e_conv, model_positions=mp,
+                             model_cell=model_cell)
+        self.iterations = 0
+        self.nsteps = 0
+        self._calculate()
+        self.opt.check(self.forces, self.virial)
+
+    def _step(self):
+        self.opt.step()
+        self._calculate()
+        self.opt.check(self.forces, self.virial)
+
+    def _step_state(self) -> Dict[str, object]:
+        state = dict(opt=self.opt.tensors(), **self._evaluation_state())
+        if self.virial is not None:
+            state["virial"] = self.virial
+        return state
+
+    def run(self, fmax: float = 0.05, steps: Optional[int] = None, check_every: int = 10) -> bool:
+        """Relax until every system's largest generalized force is below ``fmax`` or ``steps`` steps (default:
+        unlimited) were taken in this call; returns whether every system converged."""
+        if int(check_every) < 1:
+            raise ValueError("DeviceFIRE: check_every must be >= 1")
+        budget = DEFAULT_MAX_STEPS if not steps else int(steps)
+        self.opt.set_fmax(fmax)
+        self.opt.check(self.forces, self.virial)
+        done = 0
+        left = int(self.opt.n_unconverged.item())
+        while left and done < budget:
+            k = min(int(check_every), budget - done)
+            self._run_steps(k)
+            done += k
+            self.iterations += k
+            left = int(self.opt.n_unconverged.item())
+        self.check_neighbor_list()
+        self.nsteps = int(self.opt.steps_to_converge.max().item()) if left == 0 else self.iterations
+        return left == 0
+
+    # ---- results, in optimizer units ----------------------------------------------------------------------------------
+    @property
+    def positions(self) -> Tensor:
+        """[N, 3] fp64 positions"""
+        return self.opt.r
+
+    @property
+    def model_positions(self) -> Tensor:
+        """[N, 3] fp32 positions the model reads (positions / position_conversion)"""
+        return self.static[P.R]
+
+    @property
+    def cell(self) -> Optional[Tensor]:
+        """[n_sys, 3, 3] fp64 cells (rows = lattice vectors) under a cell filter, else None"""
+        return self.opt.cell()
+
+    def get_energy(self) -> Tensor:
+        """energies of the current positions [n_sys]"""
+        return self.energy * self.e_conv
+
+    def get_forces(self) -> Tensor:
+        """Cartesian forces of the current positions [N, 3] fp64, zero on fixed atoms"""
+        f = self.forces.double() * self.f_conv
+        if self.opt.fixed is not None:
+            f = f * (1 - self.opt.fixed.double())[:, None]
+        return f
+
+    def get_stress(self) -> Tensor:
+        """stress of the current cells [n_sys, 3, 3] fp64: the symmetric part of W / V (cell filter only)"""
+        if self.virial is None:
+            raise RuntimeError("DeviceFIRE: the stress is evaluated under a cell filter only")
+        w = 0.5 * (self.virial + self.virial.transpose(1, 2)) * self.e_conv
+        return w / torch.linalg.det(self.cell).abs()[:, None, None]
+
+    def get_enthalpy(self) -> Tensor:
+        """E + p V per system [n_sys] fp64 (the energy without a cell filter)"""
+        e = self.get_energy().double()
+        if self.opt.filter is None:
+            return e
+        return e + self.opt.filter.scalar_pressure * torch.linalg.det(self.cell).abs()
+
+    def get_uncertainty(self) -> Dict[str, Tensor]:
+        """Ensemble runs: the unbiased std over the members of the energies [n_sys] and forces [N, 3]"""
+        return _ensemble_uncertainty(self)
+
+    @property
+    def fmax(self) -> Tensor:
+        """largest generalized force per system [n_sys] fp64 (the quantity the convergence test compares with fmax)"""
+        return self.opt.fmax
+
+    @property
+    def converged(self) -> Tensor:
+        return self.opt.converged.bool()
+
+    @property
+    def steps_to_converge(self) -> Tensor:
+        """[n_sys] the step count at which each system met the criterion (-1 while it has not)"""
+        return self.opt.steps_to_converge
+
+    def state_dict(self) -> Dict[str, object]:
+        """Everything a restart needs to continue bitwise."""
         return dict(_clone_state(self._step_state()), iterations=self.iterations, nsteps=self.nsteps)
 
     def load_state_dict(self, state: Dict[str, object]):
