@@ -875,6 +875,47 @@ int spk_spectrum_autocorrelation(const double* z, int64_t n, const int64_t* ch_p
 int spk_spectrum_transform(const double* acf, int64_t n_channels, int64_t n_lags, const double* window, double dt_fs,
                            double* out, void* workspace, size_t workspace_bytes, spk_stream_t stream);
 
+/* ---- set-up and steadying of the device MD state (csrc/system_motion.cu; md/system.py:258-315,652-684,
+ * md/initial_conditions.py:50-188, md/simulation_hooks/basic_hooks.py:55-78) --------------------------------------------
+ * Systems as for the thermostats: idx_m [n_atoms] int64 sorted, sys_ptr [n_sys+1] int32; positions / momenta [n_atoms,3]
+ * fp32 in place, model_positions (nullable) = positions * position_conversion.  step (nullable) is a device int64 step
+ * counter: with it, a call does nothing unless step[0] % every == 0 (hooks inside a captured step); it is not advanced.
+ * spk_md_remove_motion: in the order of the flags' bits, per system, with all sums in fp64 and a fixed order (no atomics):
+ *   SPK_MOTION_CENTER_OF_MASS  x -= sum m x / sum m;
+ *   SPK_MOTION_TRANSLATION     p -= sum p / n_s (unweighted mean, system.py:278-283);
+ *   SPK_MOTION_ROTATION        about the origin: I = sum m (|x|^2 1 - x x^T), L = sum x x p, w = I^+ L, p -= m (w x x),
+ *                              with I^+ the pseudo-inverse that drops eigenvalues <= SPK_MOTION_PINV_RTOL x the largest
+ *                              (single atoms, linear molecules, empty systems); I^-1 where I is regular.
+ * spk_md_wrap_positions: positions [n_beads, n_atoms, 3] (n_beads = 1: classical); the centroid of the beads of atom a has
+ *   fractional coordinates f = x_c C^-1 in the fp64 cell C = cell + idx_m[a] * cell_stride (rows = lattice vectors,
+ *   cell_stride 0 = one cell for all systems, or 9); on the axes j with pbc[idx_m[a] * pbc_stride + j] != 0 (pbc_stride 0
+ *   or 3) every bead moves by -floor(f_j + eps) C_j, so the centroid's f_j ends in [-eps, 1 - eps).  Every cell must have a
+ *   non-zero volume.
+ * spk_md_initial_momenta: p = w xi with w = m (uniform != 0) or sqrt(m kB temperature[idx_m]) (Maxwell-Boltzmann),
+ *   xi ~ N(0,1) from Philox4x32-10 with key = seed and counter = (atom index, SPK_MOTION_DRAW_APPLICATION), normals 0..2
+ *   for x, y, z as in spk_md_langevin, whose application counter never reaches that index.  uniform != 0 then rescales
+ *   every system to its temperature exactly (the fixed-order sum of spk_md_kinetic_energy); a system at T = 0 keeps its p.
+ *   temperature [n_sys] fp64 on the device.
+ * spk_md_step_advance: step[0] += 1, once per step after the hooks.
+ * Both per-system entry points take spk_md_motion_workspace_bytes(n_atoms, n_sys) bytes of workspace, 8-byte aligned. */
+#define SPK_MOTION_CENTER_OF_MASS 1
+#define SPK_MOTION_TRANSLATION 2
+#define SPK_MOTION_ROTATION 4
+#define SPK_MOTION_PINV_RTOL 1e-10
+#define SPK_MOTION_DRAW_APPLICATION 0xFFFFFFFFFFFFFFFFull
+size_t spk_md_motion_workspace_bytes(int64_t n_atoms, int64_t n_sys);
+int spk_md_remove_motion(float* positions, float* model_positions, float* momenta, const float* masses,
+                         const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms, int64_t n_sys, int flags,
+                         float position_conversion, const int64_t* step, int64_t every, void* workspace,
+                         size_t workspace_bytes, spk_stream_t stream);
+int spk_md_wrap_positions(float* positions, float* model_positions, const int64_t* idx_m, int64_t n_atoms,
+                          int32_t n_beads, const double* cell, int64_t cell_stride, const uint8_t* pbc, int64_t pbc_stride,
+                          double eps, float position_conversion, const int64_t* step, int64_t every, spk_stream_t stream);
+int spk_md_initial_momenta(float* momenta, const float* masses, const int64_t* idx_m, const int32_t* sys_ptr,
+                           int64_t n_atoms, int64_t n_sys, int uniform, double kB, const double* temperature, uint64_t seed,
+                           void* workspace, size_t workspace_bytes, spk_stream_t stream);
+int spk_md_step_advance(int64_t* step, spk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -49,6 +49,13 @@ freedom) in fp64 on the device.  One kernel (``spk_rpmd_gle``) transforms to nor
 c2 xi and transforms back; the classical thermostat is the same kernel at P = 1.  It uses the propagator of the GLE
 papers, where the reference multiplies by the transpose of c1, which samples a wrong distribution for a non-normal drift
 matrix.  RPMD-GLE and PIGLET also run next to ``PILEBarostat``.
+
+Initial conditions and basic hooks (DESIGN.md section 19): ``DeviceMD(..., initializer=MaxwellBoltzmannInit(...) or
+UniformInit(...))`` sets the starting state as the reference's system.initializer (md/initial_conditions.py) -- centre of
+mass, wrapping, momenta from Philox, translation and rotation removal -- and ``hooks=[RemoveCOMMotion(...),
+WrapPositions(...)]`` run the reference's basic simulation hooks (md/simulation_hooks/basic_hooks.py) inside the captured
+step, gated by a device step counter.  A singular inertia tensor gets its pseudo-inverse, and ring polymers wrap by their
+centroids.
 """
 from __future__ import annotations
 
@@ -67,7 +74,8 @@ from .units import _amu, _e, _hbar, _k, _Nav
 __all__ = ["DeviceMD", "BerendsenThermostat", "LangevinThermostat", "NHCThermostat", "NHCBarostatIsotropic",
            "NHCBarostatAnisotropic", "RingPolymer", "PILELocalThermostat", "PILEGlobalThermostat", "TRPMDThermostat",
            "NHCRingPolymerThermostat", "PILEBarostat", "GLEThermostat", "RPMDGLEThermostat", "PIGLETThermostat",
-           "load_gle_matrices", "KB_MD", "FS_MD", "BAR_MD", "HBAR_MD"]
+           "load_gle_matrices", "MaxwellBoltzmannInit", "UniformInit", "RemoveCOMMotion", "WrapPositions", "KB_MD",
+           "FS_MD", "BAR_MD", "HBAR_MD"]
 
 Tensor = torch.Tensor
 
@@ -888,6 +896,118 @@ class PILEBarostat(_TensorState):
         return {"cell_momenta": self.cell_momenta, "counter": self.counter}
 
 
+# ---- initial conditions and basic simulation hooks --------------------------------------------------------------------------
+WRAP_EPS = 1e-6          # system.py:652, the buffer of wrap_positions
+
+
+class _Initializer:
+    """Common part of the initializers (md/initial_conditions.py:17-116) with the reference's keywords and defaults plus
+    ``seed`` and ``kB`` (MD energy per kelvin).  ``DeviceMD(..., initializer=...)`` applies it once, after ring-polymer
+    replication and the binding of the hooks and before the forces at t = 0, in the reference's order: centre of mass,
+    wrapping, momenta, translation, rotation.  ``temperature`` in K is one number or one per system of the batch; every
+    bead of a ring polymer draws its own momenta.
+
+    Deliberate differences from the reference: the normals come from Philox4x32-10 keyed by ``seed`` with the counter
+    (atom, 2^64 - 1), an application index that no thermostat reaches (the reference uses torch.randn); the rotation of a
+    single atom or a linear molecule uses the pseudo-inverse of its inertia tensor (``RemoveCOMMotion``); ring polymers
+    wrap by their centroids (``WrapPositions``)."""
+
+    uniform = 0
+
+    def __init__(self, temperature, remove_center_of_mass: bool = True, remove_translation: bool = True,
+                 remove_rotation: bool = False, wrap_positions: bool = False, seed: int = 0, kB: float = KB_MD):
+        name = type(self).__name__
+        temps = temperature.tolist() if isinstance(temperature, torch.Tensor) else temperature
+        temps = [float(t) for t in (temps if isinstance(temps, (list, tuple)) else [temps])]
+        if not temps or not all(t >= 0.0 for t in temps):
+            raise ValueError(f"{name}: temperature must be one or more values >= 0 K, got {temperature}")
+        self.temperature = temps
+        self.remove_center_of_mass = bool(remove_center_of_mass)
+        self.remove_translation = bool(remove_translation)
+        self.remove_rotation = bool(remove_rotation)
+        self.wrap_positions = bool(wrap_positions)
+        self.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self.kB = float(kB)
+
+    def system_temperatures(self, n_sys: int, n_copies: int, device) -> Tensor:
+        """[n_copies n_sys] fp64 target temperature of every (bead) system (initial_conditions.py:57-61)"""
+        t = self.temperature
+        if len(t) not in (1, n_sys):
+            raise ValueError(f"{type(self).__name__}: {len(t)} temperatures for {n_sys} systems; give one temperature or "
+                             "one per system")
+        t = torch.tensor(t * (n_sys if len(t) == 1 else 1), dtype=torch.float64)
+        return t.repeat(n_copies).to(device)
+
+    def initialize(self, md: "DeviceMD"):
+        """initialize_system (initial_conditions.py:50-75) on the state of ``md``, in place"""
+        s = md.systems
+        base = md._rp_base if md._rp_base is not None else s
+        temps = self.system_temperatures(base.n_sys, md._n_replicas(), md.positions.device)
+        if self.remove_center_of_mass:
+            md._remove_motion(_lib.MOTION_CENTER_OF_MASS)
+        if self.wrap_positions:
+            md._wrap_positions()
+        ws = s.workspace("spk_md_motion_workspace_bytes")
+        _lib.call("spk_md_initial_momenta", ops._p(md.momenta), ops._p(s.masses), ops._p(s.idx_m), ops._p(s.sys_ptr),
+                  s.n_atoms, s.n_sys, self.uniform, self.kB, ops._p(temps), self.seed, ops._p(ws), ws.numel(),
+                  ops._stream(), launches=4 if self.uniform else 1)
+        flags = (_lib.MOTION_TRANSLATION if self.remove_translation else 0) | \
+                (_lib.MOTION_ROTATION if self.remove_rotation else 0)
+        if flags:
+            md._remove_motion(flags)
+
+
+class MaxwellBoltzmannInit(_Initializer):
+    """Momenta from the Maxwell-Boltzmann distribution (initial_conditions.py:138-188): p = sqrt(m kB T_s) xi per atom,
+    with T_s the temperature of the atom's system.  (With one temperature per system the reference fails in
+    ``expand_atoms``; here each system gets its own width.)"""
+
+
+class UniformInit(_Initializer):
+    """Momenta p = m xi, then every (bead) system rescaled to exactly its temperature (initial_conditions.py:91-135; the
+    weight is the mass, not its square root, as in the reference).  A system whose draw has zero kinetic energy (no
+    atoms) is left unchanged."""
+
+    uniform = 1
+
+
+def _check_every(every_n_steps, who: str) -> int:
+    if int(every_n_steps) != every_n_steps or int(every_n_steps) < 1:
+        raise ValueError(f"{who}: every_n_steps must be an integer >= 1, got {every_n_steps}")
+    return int(every_n_steps)
+
+
+class RemoveCOMMotion:
+    """md/simulation_hooks/basic_hooks.py:41-61: on steps s % every_n_steps == 0 (s = 0, 1, ... counted on the device, so
+    the first step runs it) move every (bead) system to its centre of mass, remove its mean momentum and, with
+    ``remove_rotation``, its rotation about the origin.  Runs after the thermostat and barostat of the step and before the
+    recorder, inside the captured step.  The rotation uses the pseudo-inverse of the inertia tensor: eigenvalues at or
+    below 1e-10 x the largest give no angular velocity (a single atom, a linear molecule), where the reference's
+    torch.inverse fails; where the tensor is regular this is I^-1 L."""
+
+    def __init__(self, every_n_steps: int, remove_rotation: bool):
+        self.every_n_steps = _check_every(every_n_steps, "RemoveCOMMotion")
+        self.remove_rotation = bool(remove_rotation)
+
+    def apply(self, md: "DeviceMD"):
+        flags = _lib.MOTION_CENTER_OF_MASS | _lib.MOTION_TRANSLATION
+        md._remove_motion(flags | (_lib.MOTION_ROTATION if self.remove_rotation else 0), self.every_n_steps)
+
+
+class WrapPositions:
+    """md/simulation_hooks/basic_hooks.py:64-78: on steps s % every_n_steps == 0 wrap the atoms back into the cell on its
+    periodic axes (system.py:652-684, eps = 1e-6).  The cell is the run's MD cell when it keeps one (barostat or
+    ``compute_stress``), else the batch's ``_cell`` / position_conversion.  All beads of a ring-polymer atom move by the
+    lattice translation that wraps their centroid (the reference wraps every bead on its own, which tears a ring polymer
+    that straddles a face and changes its spring energy)."""
+
+    def __init__(self, every_n_steps: int):
+        self.every_n_steps = _check_every(every_n_steps, "WrapPositions")
+
+    def apply(self, md: "DeviceMD"):
+        md._wrap_positions(self.every_n_steps)
+
+
 class _CapturedEvaluation:
     """The force evaluation of a device-resident loop (calculator.calculate) and the capture of one whole step with it:
     neighbour list on the fixed-capacity ``self.nl``, ``self.model`` on ``self.static`` and copies of the outputs into
@@ -1075,7 +1195,8 @@ class DeviceMD(_CapturedEvaluation):
                  compute_stress: bool = False, ring_polymer: Optional[RingPolymer] = None,
                  required_properties: Optional[List[str]] = None,
                  property_conversion: Optional[Dict[str, float]] = None, record_every: int = 1,
-                 record_capacity: int = 0, uncertainty_fn: Optional[object] = None, record_velocities: bool = False):
+                 record_capacity: int = 0, uncertainty_fn: Optional[object] = None, record_velocities: bool = False,
+                 initializer: Optional[_Initializer] = None, hooks: Optional[List[object]] = None):
         """``batch[_positions]`` (and ``_cell``) are in MODEL units as everywhere in this package; ``self.positions`` is the
         MD-unit state (= model positions / position_conversion).  ``thermostat`` (None = NVE) is bound to the systems of
         the batch and applied around every step.  ``barostat`` (an NHC barostat, which thermostats the particles itself)
@@ -1108,8 +1229,16 @@ class DeviceMD(_CapturedEvaluation):
         (ensemble_calculator.py:70-81).  ``uncertainty_fn`` (an ``ensemble.AbsoluteUncertainty`` /
         ``RelativeUncertainty`` on the run's energy and force keys, without a stress weight) adds
         ``properties["uncertainty"]`` [n_replicas, B] of the energies and forces as ``properties`` holds them.  Stress
-        and barostats are refused with an ensemble, as in the reference."""
+        and barostats are refused with an ensemble, as in the reference.
+
+        ``initializer`` (a ``MaxwellBoltzmannInit`` or ``UniformInit``) sets the starting state as the reference's
+        system.initializer does (md/cli.py:154-157): after ring-polymer replication and the binding of the thermostat and
+        barostat, before the forces at t = 0; it replaces ``momenta``, which it refuses next to it.  ``hooks`` (a list of
+        ``RemoveCOMMotion`` / ``WrapPositions``) run in the listed order after the step's thermostat or barostat and
+        before the recorder, as the reference's simulation hooks at on_step_finalize; they are gated by a device step
+        counter, which ``state_dict`` carries, so a restarted run keeps their phase."""
         idx_m, n_sys = self._setup(model, batch, cutoff, capacity, use_graph)
+        self.hooks = self._check_hooks(hooks, initializer, momenta)
         self._check_ensemble(barostat, compute_stress, uncertainty_fn)
         self.uncertainty_fn = uncertainty_fn
         if barostat is not None and thermostat is not None and getattr(barostat, "temperature_control", True):
@@ -1173,7 +1302,68 @@ class DeviceMD(_CapturedEvaluation):
                 barostat.bind(self.systems, self.dt)
         self._setup_properties(required_properties, property_conversion, record_every, record_capacity,
                                record_velocities)
+        self._wrap_cell = None
+        if any(isinstance(h, WrapPositions) for h in self.hooks) or getattr(initializer, "wrap_positions", False):
+            self._setup_wrap()
+        if initializer is not None:
+            initializer.initialize(self)        # md/cli.py:154-157
         self._calculate()                       # forces at t = 0 (simulator.py:118)
+
+    @staticmethod
+    def _check_hooks(hooks, initializer, momenta) -> list:
+        if initializer is not None:
+            if not isinstance(initializer, _Initializer):
+                raise TypeError(f"DeviceMD: initializer must be a MaxwellBoltzmannInit or UniformInit, got "
+                                f"{type(initializer).__name__}")
+            if momenta is not None:
+                raise ValueError("DeviceMD: pass either momenta or an initializer, which draws them")
+        hooks = list(hooks or [])
+        for h in hooks:
+            if not isinstance(h, (RemoveCOMMotion, WrapPositions)):
+                raise TypeError(f"DeviceMD: hooks take RemoveCOMMotion and WrapPositions, got {type(h).__name__}")
+        return hooks
+
+    # ---- motion removal and wrapping (system.py:258-315,652-684) -------------------------------------------------------
+    def _remove_motion(self, flags: int, every: Optional[int] = None):
+        """spk_md_remove_motion on every (bead) system; with ``every`` gated by the device step counter"""
+        s = self.systems
+        ws = s.workspace("spk_md_motion_workspace_bytes")
+        _lib.call("spk_md_remove_motion", ops._p(self.positions), ops._p(self._mp), ops._p(self.momenta),
+                  ops._p(s.masses), ops._p(s.idx_m), ops._p(s.sys_ptr), s.n_atoms, s.n_sys, int(flags), self.p_conv,
+                  ops._p(self._rec_counter if every else None), int(every or 1), ops._p(ws), ws.numel(), ops._stream())
+
+    def _setup_wrap(self):
+        """The cell and pbc rows the wrap reads: the MD cell when the run keeps one (it follows the barostat), else the
+        batch's ``_cell`` / position_conversion, shared or one per system as the neighbour list takes them."""
+        n_sys = self.systems.n_sys
+        pbc = self.static.get(P.pbc)
+        if self.cell is not None:
+            cell = self.cell
+        else:
+            if P.cell not in self.static:
+                raise ValueError("DeviceMD: wrapping positions needs a periodic batch with a '_cell'")
+            cell = self.static[P.cell].reshape(-1, 3, 3).to(torch.float64) / self.p_conv
+            if cell.shape[0] not in (1, n_sys):
+                raise ValueError(f"DeviceMD: '_cell' has {cell.shape[0]} cells for {n_sys} systems")
+            cell = cell.contiguous()
+        if bool((torch.linalg.det(cell) == 0.0).any()):
+            raise ValueError("DeviceMD: wrapping positions needs a non-zero cell volume for every system "
+                             "(system.py:662-663)")
+        if pbc is None:
+            pbc = torch.zeros(1, 3, dtype=torch.uint8, device=cell.device)
+        pbc = pbc.reshape(-1, 3).to(torch.uint8).contiguous()
+        if pbc.shape[0] not in (1, n_sys):
+            raise ValueError(f"DeviceMD: '_pbc' has {pbc.shape[0]} rows for {n_sys} systems")
+        self._wrap_cell, self._wrap_pbc = cell, pbc
+
+    def _wrap_positions(self, every: Optional[int] = None):
+        """spk_md_wrap_positions on the (bead) positions; ring polymers move by their centroids' translations"""
+        base = self._rp_base if self._rp_base is not None else self.systems
+        cell, pbc = self._wrap_cell, self._wrap_pbc
+        _lib.call("spk_md_wrap_positions", ops._p(self.positions), ops._p(self._mp), ops._p(base.idx_m), base.n_atoms,
+                  self._n_replicas(), ops._p(cell), 9 if cell.shape[0] > 1 else 0, ops._p(pbc),
+                  3 if pbc.shape[0] > 1 else 0, WRAP_EPS, self.p_conv, ops._p(self._rec_counter if every else None),
+                  int(every or 1), ops._stream())
 
     @property
     def systems(self) -> _Systems:
@@ -1338,6 +1528,8 @@ class DeviceMD(_CapturedEvaluation):
 
     def _record(self):
         if not self.record_capacity:
+            if self.hooks:                       # the hooks' step counter: the recorder's, which advances it otherwise
+                _lib.call("spk_md_step_advance", ops._p(self._rec_counter), ops._stream())
             return
         for p, rec in self._records.items():
             if p == "velocities":
@@ -1438,6 +1630,8 @@ class DeviceMD(_CapturedEvaluation):
 
     def _step(self):
         self._dynamics()
+        for hook in self.hooks:                  # simulation hooks at on_step_finalize (md/cli.py:231-314)
+            hook.apply(self)
         self._record()
 
     def _dynamics(self):
@@ -1471,6 +1665,8 @@ class DeviceMD(_CapturedEvaluation):
         if self.record_capacity:
             state["recorder"] = {"counter": self._rec_counter,
                                  "records": {p: v[:self._n_records] for p, v in self._records.items()}}
+        elif self.hooks:
+            state["step_counter"] = self._rec_counter
         return state
 
     def run(self, n_steps: int):
