@@ -875,6 +875,36 @@ int spk_spectrum_autocorrelation(const double* z, int64_t n, const int64_t* ch_p
 int spk_spectrum_transform(const double* acf, int64_t n_channels, int64_t n_lags, const double* window, double dt_fs,
                            double* out, void* workspace, size_t workspace_bytes, spk_stream_t stream);
 
+/* ---- streaming autocorrelation of the live MD state (csrc/spectra.cu) -----------------------------------------------
+ * A stream of F fields and L lags keeps, per field, y[t] = x[t] - x[0] and S[k] = sum_{t < n-k} y[t] y[t+k] (k < L),
+ * Y = sum_t y[t], the first L values and a ring of the last L + SPK_SPECTRUM_STREAM_BLOCK values, all fp64, in one
+ * zero-initialised buffer of spk_spectrum_stream_state_bytes(F, L) = 8 F (3 L + SPK_SPECTRUM_STREAM_BLOCK + 8) bytes
+ * (2.43 GB, 0.81 GB per array, for the 24 576 velocity components of 8192 atoms at L = 4096; 76 MB for the 768 IR
+ * fields of 256 molecules).
+ * spk_spectrum_stream_push: on the steps with (counter[0] + 1) % every == 0 (the recorder's), frame
+ *   r = counter[0] / every of field f is x_f as spk_spectrum_series forms it from a record, here read from the live
+ *   state: component i of replica p is source[p stride + i] (fp32), divided by masses[(p stride + i) / 3] when masses
+ *   is not NULL (velocities from momenta [P N, 3], stride = 3 N, as spk_md_record_velocities); derivative fields lag
+ *   two frames.  After every SPK_SPECTRUM_STREAM_BLOCK samples the block's band products are added to S in a fixed order:
+ *   the accumulators do not depend on how the steps are grouped into calls.  Two launches, no atomics,
+ *   graph-capturable; counter is not advanced.
+ * spk_spectrum_stream_finalise: after n samples (n - 1 >= n_out, n_out <= L), channel c of the fields
+ *   fields[ch_ptr[c] .. ch_ptr[c+1]) with weights w: acf [C, n_out] = sum_i w_i C_i[k] with the normalised
+ *   autocorrelation of field i, n var C[k] = S[k] - m (2 Y - H[k] - tail[k]) + (n - k) m^2, m = Y / n,
+ *   var = S[0] / n - m^2, H[k] / tail[k] the sums of the first / last k values (the partial block is added to S on the
+ *   fly; the state is not changed).  Workspace: spk_spectrum_stream_finalise_workspace_bytes(n_sel, n_out) =
+ *   8 n_sel n_out bytes.  Two launches. */
+#define SPK_SPECTRUM_STREAM_BLOCK 64
+size_t spk_spectrum_stream_state_bytes(int64_t n_fields, int64_t n_lags);
+size_t spk_spectrum_stream_finalise_workspace_bytes(int64_t n_fields, int64_t n_lags);
+int spk_spectrum_stream_push(const float* source, const float* masses, int64_t P, int64_t stride, const int64_t* index,
+                             const double* coef, int64_t F, int derivative, double dt_fs, const int64_t* counter,
+                             int64_t every, int64_t n_lags, double* state, spk_stream_t stream);
+int spk_spectrum_stream_finalise(const double* state, int64_t F, int64_t n_lags, int64_t n, const int64_t* fields,
+                                 int64_t n_sel, const int64_t* ch_ptr, const double* weight, int64_t n_channels,
+                                 int64_t n_out, double* acf, void* workspace, size_t workspace_bytes,
+                                 spk_stream_t stream);
+
 /* ---- set-up and steadying of the device MD state (csrc/system_motion.cu; md/system.py:258-315,652-684,
  * md/initial_conditions.py:50-188, md/simulation_hooks/basic_hooks.py:55-78) --------------------------------------------
  * Systems as for the thermostats: idx_m [n_atoms] int64 sorted, sys_ptr [n_sys+1] int32; positions / momenta [n_atoms,3]

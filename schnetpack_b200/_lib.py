@@ -213,6 +213,11 @@ SIGNATURES = {
     "spk_spectrum_series": [P, c_int64, c_int64, c_int64, P, P, c_int64, c_int, c_double, P, P, P, P],
     "spk_spectrum_autocorrelation": [P, c_int64, P, P, c_int64, c_int64, P, P, c_size_t, P],
     "spk_spectrum_transform": [P, c_int64, c_int64, P, c_double, P, P, c_size_t, P],
+    "spk_spectrum_stream_state_bytes": [c_int64, c_int64],
+    "spk_spectrum_stream_finalise_workspace_bytes": [c_int64, c_int64],
+    "spk_spectrum_stream_push": [P, P, c_int64, c_int64, P, P, c_int64, c_int, c_double, P, c_int64, c_int64, P, P],
+    "spk_spectrum_stream_finalise": [P, c_int64, c_int64, c_int64, P, c_int64, P, P, c_int64, c_int64, P, P, c_size_t,
+                                     P],
     "spk_fire_workspace_bytes": [c_int64, c_int64],
     "spk_fire_forces": [POINTER(FIREState), P, P, P],
     "spk_fire_step": [POINTER(FIREState), P],
@@ -231,7 +236,8 @@ _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_siz
             "spk_head_charges_bwd_workspace_bytes": c_size_t, "spk_pair_energy_workspace_bytes": c_size_t,
             "spk_ewald_workspace_bytes": c_size_t, "spk_ensemble_workspace_bytes": c_size_t,
             "spk_spectrum_workspace_bytes": c_size_t, "spk_fire_workspace_bytes": c_size_t,
-            "spk_md_motion_workspace_bytes": c_size_t}
+            "spk_md_motion_workspace_bytes": c_size_t, "spk_spectrum_stream_state_bytes": c_size_t,
+            "spk_spectrum_stream_finalise_workspace_bytes": c_size_t}
 
 _lib = None
 
@@ -277,7 +283,8 @@ LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out
             "spk_rpmd_barostat_main_step": 2, "spk_head_fwd": 2,
             "spk_relax_converged": 2, "spk_pair_energy_fwd": 2, "spk_head_charges_bwd": 3,
             "spk_pairwise_virial_add": 2, "spk_spectrum_autocorrelation": 2, "spk_spectrum_transform": 2,
-            "spk_fire_forces": 3, "spk_fire_step": 2, "spk_md_remove_motion": 3}
+            "spk_fire_forces": 3, "spk_fire_step": 2, "spk_md_remove_motion": 3, "spk_spectrum_stream_push": 2,
+            "spk_spectrum_stream_finalise": 2}
 # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global; spk_md_initial_momenta: 4 if uniform
 MOTION_CENTER_OF_MASS, MOTION_TRANSLATION, MOTION_ROTATION = 1, 2, 4       # SPK_MOTION_*
 launch_count = 0

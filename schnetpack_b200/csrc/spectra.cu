@@ -19,6 +19,8 @@
 // Transform: I[m] = 2 dt |sum_i a_i cos(pi m (2i+1) / (8L))| for m < 4L, the DCT-II form of the reference's |dt FFT| of
 // the zero-padded, mirrored series.  m (2i+1) is reduced modulo 16L in integers and the cosine read from a quarter-wave
 // table of cospi values (in shared memory when it fits), so no cosine of a large argument is ever taken.
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace {
@@ -293,6 +295,258 @@ extern "C" int spk_spectrum_transform(const double* acf, int64_t n_channels, int
     spk_launch(k_spectrum_transform, dim3((unsigned)spk_cdiv(4 * n_lags, TR_T), (unsigned)ygrid), TR_T,
                stage ? smem : 0, spk_st(stream), acf, n_channels, n_lags, window, dt_fs, (const double*)tab, stage,
                out);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+// ---- streaming autocorrelation inside the captured MD step ----------------------------------------------------------
+// A stream keeps, per field f of its F fields, the shifted values y = x - x[0] and
+//   S[k] = sum_{t < n - k} y[t] y[t + k] (k < L),  Y = sum_t y[t],  head[t] = y[t] (t < L),  ring[t % R] = y[t],
+// with R = L + SPK_SPECTRUM_STREAM_BLOCK.  The push (one thread per field) forms the field from the live state exactly
+// as spk_md_record_velocities / spk_md_record and spk_spectrum_series would (fp32 values, fp64 centroid, central
+// difference from a two-frame history per field), and the block update adds the band products of every complete block
+// of SPK_SPECTRUM_STREAM_BLOCK samples: S[k] += sum_{j < BLOCK} y[b0 + j] y[b0 + j - k].  Samples are counted from the
+// recorder's device step counter (frame r = counter[0] / every on the steps with (counter[0] + 1) % every == 0), so the
+// host launches both kernels every step and no counter of the stream's own is needed.  A block update CTA of T threads
+// owns one field and a tile of KT = T Q lags (Q lags per thread in registers; the tile is sized from L, up to 1024
+// lags, so a short lag window computes no lags it throws away beyond rounding T up to a warp): it stages the block and
+// the KT + BLOCK - 1 ring values it needs in shared memory and reads and writes S once per block.  Sums run in sample
+// order and in fixed blocks, so the accumulators do not depend on how the run is chunked.
+namespace {
+
+constexpr int SB = SPK_SPECTRUM_STREAM_BLOCK;   // samples per block update
+constexpr int SP_T = 256;                       // fields per CTA of the push
+constexpr int SU_T = 256;                       // largest CTA of the block update
+constexpr int SU_KT = 4 * SU_T;                 // largest lag tile of the block update (Q = 4)
+constexpr int SF_T = 256;                       // threads per field of the finalisation
+constexpr int SC_T = 256;                       // lags per CTA of the channel sums
+constexpr int SCAL = 8;                         // per-field scalars: Y, shift, two frames of three components
+
+struct StreamView {
+    double *S, *head, *ring, *scal;
+    int64_t R;
+};
+
+__host__ __device__ __forceinline__ StreamView stream_view(double* st, int64_t F, int64_t L) {
+    StreamView v;
+    v.R = L + SB;
+    v.S = st;
+    v.head = st + F * L;
+    v.ring = st + 2 * F * L;
+    v.scal = st + F * (2 * L + v.R);
+    return v;
+}
+
+// the centroid of component i of the live state: fp32 src (divided by the fp32 masses when given, as the velocity
+// recorder does), replicas summed in order in fp64 and divided by P, as spk_spectrum_series does on the records
+__device__ __forceinline__ double live_centroid(const float* __restrict__ src, const float* __restrict__ masses,
+                                                int64_t P, int64_t stride, int64_t i) {
+    double s = 0.0;
+    for (int64_t r = 0; r < P; ++r) {
+        const int64_t j = r * stride + i;
+        const float v = masses ? src[j] / masses[j / 3] : src[j];
+        s += (double)v;
+    }
+    return s / (double)P;
+}
+
+__global__ void __launch_bounds__(SP_T) k_stream_push(const float* __restrict__ src, const float* __restrict__ masses,
+                                                      int64_t P, int64_t stride, const int64_t* __restrict__ index,
+                                                      const double* __restrict__ coef, int64_t F, int derivative,
+                                                      double dt_fs, const int64_t* __restrict__ counter, int64_t every,
+                                                      int64_t L, double* __restrict__ state) {
+    SPK_PDL_ENTER();
+    const int64_t f = blockIdx.x * (int64_t)SP_T + threadIdx.x;
+    const int64_t c0 = counter[0];
+    if (f >= F || (c0 + 1) % every != 0) return;
+    const int64_t r = c0 / every;
+    const int64_t u = derivative ? r - 2 : r;
+    const StreamView v = stream_view(state, F, L);
+    double* sc = v.scal + SCAL * f;
+    double x = 0.0;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        const int64_t i = index[3 * f + j];
+        if (i < 0) continue;
+        double d = live_centroid(src, masses, P, stride, i);
+        if (derivative) {
+            double* h = sc + 2 + 3 * (r & 1) + j;       // c(r - 2), then c(r) for frame r + 2
+            const double c = d;
+            d = (c - *h) / (2.0 * dt_fs);
+            *h = c;
+        }
+        x += coef[3 * f + j] * d;
+    }
+    if (u < 0) return;
+    if (u == 0) sc[1] = x;
+    const double y = x - sc[1];
+    v.ring[f * v.R + u % v.R] = y;
+    if (u < L) v.head[f * L + u] = y;
+    sc[0] += y;
+}
+
+// T threads (SU_T when Q > 1, else blockDim.x), Q lags each: a tile of KT = T Q lags
+template <int Q>
+__global__ void __launch_bounds__(SU_T) k_stream_update(int64_t F, int derivative, const int64_t* __restrict__ counter,
+                                                        int64_t every, int64_t L, double* __restrict__ state) {
+    SPK_PDL_ENTER();
+    __shared__ double blk[SB];
+    __shared__ double seg[SU_KT + SB];
+    const int64_t c0 = counter[0];
+    if ((c0 + 1) % every != 0) return;
+    const int64_t u = c0 / every - (derivative ? 2 : 0);
+    if (u < 0 || (u + 1) % SB != 0) return;
+    const int64_t b0 = u + 1 - SB;
+    const StreamView v = stream_view(state, F, L);
+    const int T = Q > 1 ? SU_T : (int)blockDim.x, KT = T * Q, tid = (int)threadIdx.x;     // T is fixed when Q > 1
+    const int64_t n_tiles = (L + KT - 1) / KT, items = F * n_tiles;
+    for (int64_t it = blockIdx.x; it < items; it += gridDim.x) {
+        const int64_t f = it / n_tiles, k0 = (it % n_tiles) * KT;
+        const double* ring = v.ring + f * v.R;
+        const int64_t base = b0 - k0 - KT + 1;       // seg[i] = y[base + i]
+        __syncthreads();
+        for (int i = tid; i < KT + SB - 1; i += T) {
+            const int64_t t = base + i;
+            seg[i] = t >= 0 ? ring[t % v.R] : 0.0;
+        }
+        for (int i = tid; i < SB; i += T) blk[i] = ring[(b0 + i) % v.R];
+        __syncthreads();
+        double acc[Q];
+#pragma unroll
+        for (int q = 0; q < Q; ++q) acc[q] = 0.0;
+#pragma unroll 4
+        for (int j = 0; j < SB; ++j) {
+            const double a = blk[j];
+#pragma unroll
+            for (int q = 0; q < Q; ++q) acc[q] = fma(a, seg[j - tid - T * q + KT - 1], acc[q]);
+        }
+        double* S = v.S + f * L;
+#pragma unroll
+        for (int q = 0; q < Q; ++q) {
+            const int64_t k = k0 + tid + T * q;
+            if (k < L) S[k] += acc[q];
+        }
+    }
+}
+
+// C[i, k] for k < Lo of stream field fields[i] after n samples: the partial block is added to S, the head and tail
+// sums come from chunked prefix sums (thread t owns lags [t per, (t + 1) per)), then
+// C[k] = (S[k] - m (2 Y - H[k] - tail[k]) + (n - k) m^2) / (n var),  m = Y / n,  var = S[0] / n - m^2.
+__global__ void __launch_bounds__(SF_T) k_stream_finalise(const double* __restrict__ state, int64_t F, int64_t L,
+                                                          int64_t n, const int64_t* __restrict__ fields, int64_t Lo,
+                                                          double* __restrict__ out) {
+    SPK_PDL_ENTER();
+    __shared__ double part[2][SF_T + 1];
+    const int64_t i = blockIdx.x, f = fields[i];
+    const StreamView v = stream_view(const_cast<double*>(state), F, L);
+    const double* S = v.S + f * L;
+    const double* head = v.head + f * L;
+    const double* ring = v.ring + f * v.R;
+    const double Y = v.scal[SCAL * f];
+    const int64_t b0 = n - n % SB;
+    const int64_t per = (Lo + SF_T - 1) / SF_T;
+    const int64_t ka = min(Lo, threadIdx.x * per), kb = min(Lo, ka + per);
+    double* o = out + i * Lo;
+    double h = 0.0, tl = 0.0;
+    for (int64_t k = ka; k < kb; ++k) {
+        double s = S[k];
+        for (int64_t t = max(b0, k); t < n; ++t) s += ring[t % v.R] * ring[(t - k) % v.R];
+        o[k] = s;
+        h += head[k];
+        tl += ring[(n - 1 - k) % v.R];
+    }
+    part[0][threadIdx.x] = h;
+    part[1][threadIdx.x] = tl;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double a = 0.0, b = 0.0;
+        for (int t = 0; t < SF_T; ++t) {
+            const double pa = part[0][t], pb = part[1][t];
+            part[0][t] = a;
+            part[1][t] = b;
+            a += pa;
+            b += pb;
+        }
+        part[0][SF_T] = o[0];
+    }
+    __syncthreads();
+    const double dn = (double)n, m = Y / dn;
+    const double var = part[0][SF_T] / dn - m * m;
+    double H = part[0][threadIdx.x], T = part[1][threadIdx.x];
+    for (int64_t k = ka; k < kb; ++k) {
+        o[k] = (o[k] - m * (2.0 * Y - H - T) + (double)(n - k) * m * m) / (dn * var);
+        H += head[k];
+        T += ring[(n - 1 - k) % v.R];
+    }
+}
+
+// acf[c, k] = sum_{i in [ch_ptr[c], ch_ptr[c+1])} weight[i] C[i, k], fields in order
+__global__ void __launch_bounds__(SC_T) k_stream_channels(const double* __restrict__ C, int64_t Lo,
+                                                          const int64_t* __restrict__ ch_ptr,
+                                                          const double* __restrict__ weight, double* __restrict__ acf) {
+    SPK_PDL_ENTER();
+    const int64_t k = blockIdx.x * (int64_t)SC_T + threadIdx.x, c = blockIdx.y;
+    if (k >= Lo) return;
+    double s = 0.0;
+    for (int64_t i = ch_ptr[c]; i < ch_ptr[c + 1]; ++i) s += weight[i] * C[i * Lo + k];
+    acf[c * Lo + k] = s;
+}
+
+}  // namespace
+
+extern "C" size_t spk_spectrum_stream_state_bytes(int64_t n_fields, int64_t n_lags) {
+    if (n_fields < 0 || n_lags < 1) return 0;
+    return sizeof(double) * (size_t)n_fields * (size_t)(3 * n_lags + SB + SCAL);
+}
+
+extern "C" size_t spk_spectrum_stream_finalise_workspace_bytes(int64_t n_fields, int64_t n_lags) {
+    if (n_fields < 0 || n_lags < 1) return 0;
+    return sizeof(double) * (size_t)n_fields * (size_t)n_lags;
+}
+
+extern "C" int spk_spectrum_stream_push(const float* source, const float* masses, int64_t P, int64_t stride,
+                                        const int64_t* index, const double* coef, int64_t F, int derivative,
+                                        double dt_fs, const int64_t* counter, int64_t every, int64_t n_lags,
+                                        double* state, spk_stream_t stream) {
+    if (P < 1 || stride < 1 || F < 0 || every < 1 || n_lags < 1 || n_lags > MAX_LAGS) return SPK_ERR_ARG;
+    if (derivative && !(dt_fs > 0.0)) return SPK_ERR_ARG;
+    if (F == 0) return SPK_OK;
+    if (!source || !index || !coef || !counter || !state || (masses && stride % 3 != 0)) return SPK_ERR_ARG;
+    const cudaStream_t st = spk_st(stream);
+    spk_launch(k_stream_push, (unsigned)spk_cdiv(F, SP_T), SP_T, 0, st, source, masses, P, stride, index, coef, F,
+               derivative, dt_fs, counter, every, n_lags, state);
+    // the lag tile from L: 1024 lags (Q = 4) above 512, 512 (Q = 2) above 256, else one lag per thread of a CTA of
+    // L rounded up to a warp
+    const int Q = n_lags > 512 ? 4 : n_lags > 256 ? 2 : 1;
+    const int T = Q > 1 ? SU_T : (int)spk_cdiv(n_lags, 32) * 32;
+    const int64_t items = F * spk_cdiv(n_lags, (int64_t)T * Q);
+    const int64_t grid = std::min<int64_t>(items, 8 * (int64_t)spk_num_sms());
+    if (Q == 4)
+        spk_launch(k_stream_update<4>, (unsigned)grid, T, 0, st, F, derivative, counter, every, n_lags, state);
+    else if (Q == 2)
+        spk_launch(k_stream_update<2>, (unsigned)grid, T, 0, st, F, derivative, counter, every, n_lags, state);
+    else
+        spk_launch(k_stream_update<1>, (unsigned)grid, T, 0, st, F, derivative, counter, every, n_lags, state);
+    SPK_LAUNCH_CHECK();
+    return SPK_OK;
+}
+
+extern "C" int spk_spectrum_stream_finalise(const double* state, int64_t F, int64_t n_lags, int64_t n,
+                                            const int64_t* fields, int64_t n_sel, const int64_t* ch_ptr,
+                                            const double* weight, int64_t n_channels, int64_t n_out, double* acf,
+                                            void* workspace, size_t workspace_bytes, spk_stream_t stream) {
+    if (F < 0 || n_lags < 1 || n_sel < 0 || n_channels < 0 || n_out < 1 || n_out > n_lags || n_out > n - 1)
+        return SPK_ERR_ARG;
+    if (n_channels == 0) return SPK_OK;
+    if (!state || !fields || !ch_ptr || !weight || !acf || !workspace || n_sel > 0x7fffffff || n_channels > 65535)
+        return SPK_ERR_ARG;
+    if (workspace_bytes < spk_spectrum_stream_finalise_workspace_bytes(n_sel, n_out)) return SPK_ERR_ARG;
+    const cudaStream_t st = spk_st(stream);
+    double* C = reinterpret_cast<double*>(workspace);
+    if (n_sel > 0)
+        spk_launch(k_stream_finalise, (unsigned)n_sel, SF_T, 0, st, state, F, n_lags, n, fields, n_out, C);
+    spk_launch(k_stream_channels, dim3((unsigned)spk_cdiv(n_out, SC_T), (unsigned)n_channels), SC_T, 0, st,
+               (const double*)C, n_out, ch_ptr, weight, acf);
     SPK_LAUNCH_CHECK();
     return SPK_OK;
 }

@@ -1196,7 +1196,8 @@ class DeviceMD(_CapturedEvaluation):
                  required_properties: Optional[List[str]] = None,
                  property_conversion: Optional[Dict[str, float]] = None, record_every: int = 1,
                  record_capacity: int = 0, uncertainty_fn: Optional[object] = None, record_velocities: bool = False,
-                 initializer: Optional[_Initializer] = None, hooks: Optional[List[object]] = None):
+                 initializer: Optional[_Initializer] = None, hooks: Optional[List[object]] = None,
+                 stream: Optional[object] = None):
         """``batch[_positions]`` (and ``_cell``) are in MODEL units as everywhere in this package; ``self.positions`` is the
         MD-unit state (= model positions / position_conversion).  ``thermostat`` (None = NVE) is bound to the systems of
         the batch and applied around every step.  ``barostat`` (an NHC barostat, which thermostats the particles itself)
@@ -1236,7 +1237,11 @@ class DeviceMD(_CapturedEvaluation):
         barostat, before the forces at t = 0; it replaces ``momenta``, which it refuses next to it.  ``hooks`` (a list of
         ``RemoveCOMMotion`` / ``WrapPositions``) run in the listed order after the step's thermostat or barostat and
         before the recorder, as the reference's simulation hooks at on_step_finalize; they are gated by a device step
-        counter, which ``state_dict`` carries, so a restarted run keeps their phase."""
+        counter, which ``state_dict`` carries, so a restarted run keeps their phase.
+
+        ``stream`` (a ``spectra.SpectrumStream``) accumulates the autocorrelations the spectra need inside the step, on
+        the steps the recorder would record, before the step counter advances; it works without a recorder, reads the
+        properties it needs from ``required_properties``, is carried by ``state_dict`` and untouched by ``drain``."""
         idx_m, n_sys = self._setup(model, batch, cutoff, capacity, use_graph)
         self.hooks = self._check_hooks(hooks, initializer, momenta)
         self._check_ensemble(barostat, compute_stress, uncertainty_fn)
@@ -1302,12 +1307,31 @@ class DeviceMD(_CapturedEvaluation):
                 barostat.bind(self.systems, self.dt)
         self._setup_properties(required_properties, property_conversion, record_every, record_capacity,
                                record_velocities)
+        self.stream = self._check_stream(stream)
         self._wrap_cell = None
         if any(isinstance(h, WrapPositions) for h in self.hooks) or getattr(initializer, "wrap_positions", False):
             self._setup_wrap()
         if initializer is not None:
             initializer.initialize(self)        # md/cli.py:154-157
         self._calculate()                       # forces at t = 0 (simulator.py:118)
+        if stream is not None:
+            base = self._rp_base if self.ring_polymer is not None else self.systems
+            stream._bind(self, base.sys_ptr.tolist(), self._n_replicas())
+
+    def _check_stream(self, stream):
+        if stream is None:
+            return None
+        from .spectra import SpectrumStream
+
+        if not isinstance(stream, SpectrumStream):
+            raise TypeError(f"DeviceMD: stream must be a spectra.SpectrumStream, got {type(stream).__name__}")
+        if stream._md is not None:
+            raise ValueError("DeviceMD: this SpectrumStream already belongs to another DeviceMD")
+        missing = [p for p in stream.required_properties if p not in self.required_properties]
+        if missing:
+            raise ValueError(f"DeviceMD: the stream reads {missing}, which are not in required_properties "
+                             f"{self.required_properties}")
+        return stream
 
     @staticmethod
     def _check_hooks(hooks, initializer, momenta) -> list:
@@ -1527,8 +1551,10 @@ class DeviceMD(_CapturedEvaluation):
                         None, None, energy_scale=conv[ek], out_f32=out)
 
     def _record(self):
+        if self.stream is not None:              # reads the counter before this step's advance, as the recorder does
+            self.stream._push(self)
         if not self.record_capacity:
-            if self.hooks:                       # the hooks' step counter: the recorder's, which advances it otherwise
+            if self.hooks or self.stream is not None:    # the step counter: the recorder's, which advances it otherwise
                 _lib.call("spk_md_step_advance", ops._p(self._rec_counter), ops._stream())
             return
         for p, rec in self._records.items():
@@ -1665,8 +1691,10 @@ class DeviceMD(_CapturedEvaluation):
         if self.record_capacity:
             state["recorder"] = {"counter": self._rec_counter,
                                  "records": {p: v[:self._n_records] for p, v in self._records.items()}}
-        elif self.hooks:
+        elif self.hooks or self.stream is not None:
             state["step_counter"] = self._rec_counter
+        if self.stream is not None:
+            state["stream"] = self.stream._state()
         return state
 
     def run(self, n_steps: int):
