@@ -60,6 +60,7 @@ constexpr int PROD_BAR = 1 + NG;               // named barrier of the producer 
 constexpr int NR = 32;                         // operand rows per chunk = wgmma N
 constexpr int NBUF = 2;                        // filter tiles (and their metadata) in flight
 constexpr int KT = 16;                         // floats per operand K-tile (64 B rows, SWIZZLE_64B)
+constexpr int K_TC = 24;                       // K = n_rbf + 1 covered by the three k-steps of filter_third
 constexpr int A_TILE = F_TC * KT * 4;          // 8192 B
 constexpr int A_BYTES = 3 * 2 * 2 * A_TILE;    // [third][hi,lo][k-tile]
 constexpr int B_TILE = NR * KT * 4;            // 2048 B
@@ -804,7 +805,7 @@ extern "C" size_t spk_painn_filter_packed_floats(void) { return (size_t)A_BYTES 
 extern "C" int spk_painn_pack_filter(const float* wf, const float* bf, int F, int n_rbf, float* packed,
                                      spk_stream_t stream) {
     if (!wf || !bf || !packed) return SPK_ERR_ARG;
-    if (F != F_TC || n_rbf <= 0 || n_rbf > 31) return SPK_ERR_UNSUPPORTED;
+    if (F != F_TC || n_rbf <= 0 || n_rbf + 1 > K_TC) return SPK_ERR_UNSUPPORTED;
     spk_launch(k_pack_filter, (unsigned)spk_cdiv(3 * F_TC * 32, 256), 256, 0, spk_st(stream), wf, bf, n_rbf, packed);
     SPK_LAUNCH_CHECK();
     return SPK_OK;
@@ -815,7 +816,7 @@ extern "C" int spk_painn_edge_fwd_tc(const float* x, const float* mu, const floa
                                      int64_t n_atoms, int64_t n_edges, int F, int n_rbf, float* q_out, float* mu_out,
                                      spk_stream_t stream) {
     if (n_atoms < 0 || n_edges < 0 || F <= 0 || n_rbf <= 0) return SPK_ERR_ARG;
-    if (F != F_TC || n_rbf > 31 || n_edges == 0) return SPK_ERR_UNSUPPORTED;      // caller uses spk_painn_edge_fwd
+    if (F != F_TC || n_rbf + 1 > K_TC || n_edges == 0) return SPK_ERR_UNSUPPORTED;      // caller uses spk_painn_edge_fwd
     if (n_atoms == 0) return SPK_OK;
     if (!x || !q || !phi || !geo || !rowptr || !slot_j || !wf_packed || !q_out || !mu_out) return SPK_ERR_ARG;
     if (mu && mu == mu_out) return SPK_ERR_ARG;
@@ -845,7 +846,7 @@ extern "C" int spk_painn_edge_bwd_tc(const float* x, const float* mu, const floa
                                      const float* wf_packed, int64_t n_atoms, int64_t n_edges, int F, int n_rbf,
                                      float* g_x, float* g_mu_in, float* g_rij, int accumulate, spk_stream_t stream) {
     if (n_atoms < 0 || n_edges < 0 || F <= 0 || n_rbf <= 0) return SPK_ERR_ARG;
-    if (F != F_TC || n_rbf > 31 || n_edges == 0) return SPK_ERR_UNSUPPORTED;      // caller uses spk_painn_edge_bwd
+    if (F != F_TC || n_rbf + 1 > K_TC || n_edges == 0) return SPK_ERR_UNSUPPORTED;      // caller uses spk_painn_edge_bwd
     if (n_atoms == 0) return SPK_OK;
     if (!x || !g_q || !g_mu || !phi || !dphi || !geo || !sptr || !pos_slot || !pos_i || !slot_eid || !wf_packed || !g_x ||
         !g_rij)

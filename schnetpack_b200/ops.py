@@ -411,16 +411,16 @@ CHAIN_IMPL = False
 
 # ------------------------------------------------------------------------------------------------------------ PaiNN
 # edge kernels: "tc" (default) = persistent kernels with the continuous filter on the tensor cores (csrc/painn_tc.cu:
-# wgmma 3xTF32, channels on the M side) for F == 128, n_rbf <= 31 and >= EDGE_TC_MIN_EDGES edges; everything else, and
+# wgmma 3xTF32, channels on the M side) for F == 128, n_rbf <= 23 and >= EDGE_TC_MIN_EDGES edges; everything else, and
 # SPK_B200_EDGE=ldg, runs the streaming kernels with the filter on the CUDA cores (csrc/painn.cu).
 EDGE_IMPL = os.environ.get("SPK_B200_EDGE", "tc")
 EDGE_TC_MIN_EDGES = 4096
 
 
 def edge_tc_ok(F: int, n_rbf: int, n_edges: int) -> bool:
-    """The tensor-core filter path (csrc/painn_tc.cu) covers F == 128, n_rbf <= 31; tiny edge lists stay on the
-    streaming kernel (a persistent CTA per SM needs work for its 4 consumer groups)."""
-    return EDGE_IMPL == "tc" and F == 128 and n_rbf <= 31 and n_edges >= EDGE_TC_MIN_EDGES
+    """The tensor-core filter path (csrc/painn_tc.cu) covers F == 128, n_rbf <= 23 (its filter GEMM has K = n_rbf + 1 <=
+    24); tiny edge lists stay on the streaming kernel (a persistent CTA per SM needs work for its 4 consumer groups)."""
+    return EDGE_IMPL == "tc" and F == 128 and n_rbf <= 23 and n_edges >= EDGE_TC_MIN_EDGES
 
 
 def painn_pack_filter(wf: Tensor, bf: Tensor, F: int, n_rbf: int) -> Tensor:
@@ -531,6 +531,33 @@ CFCONV_TC_MIN_EDGES = 2048
 
 def cfconv_tc_ok(F: int, n_filters: int, n_rbf: int, n_edges: int) -> bool:
     return CFCONV_IMPL == "tc" and F == 128 and n_filters == 128 and n_rbf <= 31 and n_edges >= CFCONV_TC_MIN_EDGES
+
+
+# ------------------------------------------------------------------------------------------------------------ shapes
+# Widths the per-channel edge kernels are compiled for: one thread per channel, F / 32 warps in {1, 2, 4, 8}
+# (DISPATCH_F_NRB of csrc/painn.cu, k_cfconv_{fwd,bwd}<NW> of csrc/schnet.cu).  The radial-basis records of the PaiNN
+# edge kernels and of spk_radial_bwd hold at most 32 functions.
+EDGE_WIDTHS = (32, 64, 128, 256)
+MAX_N_RBF = 32
+
+
+def check_painn_shape(F: int, n_rbf: int):
+    """Raise NotImplementedError, before anything is launched, for a PaiNN the edge kernels cannot evaluate."""
+    if F not in EDGE_WIDTHS:
+        raise NotImplementedError(f"PaiNN: n_atom_basis = {F} has no edge kernel (supported: {EDGE_WIDTHS})")
+    if n_rbf > MAX_N_RBF:
+        raise NotImplementedError(f"PaiNN: n_rbf = {n_rbf} has no edge kernel (supported: n_rbf <= {MAX_N_RBF})")
+
+
+def check_schnet_shape(n_filters: int, n_rbf: int, need_grad: bool):
+    """Raise NotImplementedError, before anything is launched, for a SchNet evaluation the kernels cannot run: the
+    convolution needs one of EDGE_WIDTHS filters, and the radial reverse (forces) at most MAX_N_RBF basis functions.
+    Energy-only evaluations with more basis functions run on the materialised-filter path."""
+    if n_filters not in EDGE_WIDTHS:
+        raise NotImplementedError(f"SchNet: n_filters = {n_filters} has no convolution kernel (supported: {EDGE_WIDTHS})")
+    if need_grad and n_rbf > MAX_N_RBF:
+        raise NotImplementedError(f"SchNet: n_rbf = {n_rbf} has no radial reverse kernel for forces "
+                                  f"(supported: n_rbf <= {MAX_N_RBF}; energy-only evaluations take any n_rbf)")
 
 
 def schnet_pack_filter(w0: Tensor, b0: Tensor, w1: Tensor, n_rbf: int) -> Tensor:

@@ -172,6 +172,7 @@ class PaiNN(nn.Module):
         if not isinstance(self.radial_basis, (snn.GaussianRBF, snn.BesselRBF)) or not isinstance(
                 self.cutoff_fn, snn.CosineCutoff):
             raise NotImplementedError("fused PaiNN kernels support GaussianRBF/BesselRBF x CosineCutoff")
+        ops.check_painn_shape(self.n_atom_basis, self.radial_basis.n_rbf)
         graph = ops.get_graph(idx_i, idx_j, n_atoms)
 
         if isinstance(self.embedding, nn.Embedding) and len(self.electronic_embeddings) == 0:

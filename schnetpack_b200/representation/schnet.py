@@ -119,8 +119,10 @@ class SchNet(nn.Module):
         if not isinstance(self.radial_basis, (snn.GaussianRBF, snn.BesselRBF)) or not isinstance(
                 self.cutoff_fn, snn.CosineCutoff):
             raise NotImplementedError("fused SchNet kernels support GaussianRBF/BesselRBF x CosineCutoff")
+        need_grad = r_ij.requires_grad and torch.is_grad_enabled()
+        ops.check_schnet_shape(self.n_filters, self.radial_basis.n_rbf, need_grad)
         # inference on the fused forward kernels builds its own receiver view over the ACTIVE edges (d < cutoff) from r_ij
-        fused = (not (r_ij.requires_grad and torch.is_grad_enabled())
+        fused = (not need_grad
                  and ops.cfconv_tc_ok(self.n_atom_basis, self.n_filters, self.radial_basis.n_rbf, r_ij.shape[0]))
         graph = None if fused else ops.get_graph(idx_i, idx_j, n_atoms)
         if isinstance(self.embedding, nn.Embedding) and len(self.electronic_embeddings) == 0:
