@@ -776,6 +776,54 @@ size_t spk_fire_workspace_bytes(int64_t n_atoms, int64_t n_sys);
 int spk_fire_forces(const spk_fire_t* state, const float* forces, const double* virial, spk_stream_t stream);
 int spk_fire_step(const spk_fire_t* state, spk_stream_t stream);
 
+/* ---- climbing-image nudged elastic band forces (csrc/neb.cu; Henkelman & Jonsson, J. Chem. Phys. 113, 9978 (2000);
+ * Henkelman, Uberuaga & Jonsson, J. Chem. Phys. 113, 9901 (2000)) ---------------------------------------------------
+ * A band is images 0 .. n+1 of the same atoms in the same order; images 0 and n+1 are fixed endpoints, the n =
+ * n_images interior images move.  The batch holds the interior images of n_bands bands, band-major, image-major: band b
+ * owns atoms [band_ptr[b], band_ptr[b+1]) = n images of A_b = (band_ptr[b+1] - band_ptr[b]) / n atoms, interior image
+ * img = b n + i (i = 0 .. n-1 is image i+1 of the band) owns atoms [img_ptr[img], img_ptr[img+1]), idx_img [N] its
+ * image per atom.  Endpoint rows: atom k of band b is row band_ptr[b] / n + k of r_initial / r_final [sum_b A_b, 3].
+ * Everything is in optimizer units: positions (model x position_conversion), V = energies x energy_conversion,
+ * F = forces x force_conversion, 0 on fixed atoms; end_energies [n_bands, 2] = (V_0, V_n+1) already in those units.
+ *
+ * spk_neb_forces, per interior image with D+ = R_{i+1} - R_i, D- = R_i - R_{i-1} over its 3 A_b coordinates (plain
+ *   differences, never wrapped):
+ *   sums a = D+.D+, b = D-.D-, c = D+.D-, d = F.D+, e = F.D- (fixed-order CTA partials, no atomics);
+ *   tau = alpha D+ + beta D-: (1, 0) if V_{i+1} > V_i > V_{i-1}, (0, 1) if V_{i+1} < V_i < V_{i-1}, else with dV_max /
+ *   dV_min the larger / smaller of |V_{i+-1} - V_i|: (dV_max, dV_min) if V_{i+1} > V_{i-1}, else (dV_min, dV_max); if
+ *   that gives |tau| = 0 (a flat stretch), the bisector (1 / |D+|, 1 / |D-|) (a zero difference gives a zero weight);
+ *   |tau|^2 = alpha^2 a + 2 alpha beta c + beta^2 b, F.tau = alpha d + beta e;
+ *   the climbing image of a band, when climb[0] != 0: the interior image of the highest V, ties to the lowest index;
+ *   gamma = -2 F.tau / |tau|^2 for the climbing image, else -F.tau / |tau|^2 + k (|D+| - |D-|) / |tau|; 0 if |tau| = 0;
+ *   neb_forces [N, 3] fp32 = F + gamma tau, 0 on fixed atoms (F - (F.t) t + k (|D+| - |D-|) t with t = tau / |tau|,
+ *   or F - 2 (F.t) t for the climbing image);
+ *   coef [n_img, 3] = (alpha, beta, gamma); diag [n_img, 6] = (|tau|, F.t, the spring term k (|D+| - |D-|) (0 for the
+ *   climbing image), |D+|, |D-|, 1 for the climbing image else 0); climbing [n_bands] = the climbing image's interior
+ *   index i, -1 when climb[0] == 0.
+ * climb is read on the device, so a captured call follows it.  The NEB forces drive spk_fire_step with the band as the
+ * system (force_conversion = 1), whose |dr| cap and fmax test then run over every moving coordinate of the band.
+ * Three launches; workspace: spk_neb_workspace_bytes(n_atoms, n_img) bytes, 8-byte aligned. */
+typedef struct {
+    const double* r;            /* [N, 3] interior positions (FIRE's r) */
+    const double* r_initial;    /* [sum_b A_b, 3] image 0 of every band */
+    const double* r_final;      /* [sum_b A_b, 3] image n+1 of every band */
+    const double* end_energies; /* [n_bands, 2] */
+    const int32_t* climb;       /* [1] 0: plain NEB, else climbing image */
+    const uint8_t* fixed;       /* [N] or NULL */
+    const int64_t* idx_img;     /* [N] */
+    const int32_t* img_ptr;     /* [n_img + 1] */
+    const int32_t* band_ptr;    /* [n_bands + 1] */
+    double* coef;               /* [n_img, 3] */
+    double* diag;               /* [n_img, 6] */
+    int32_t* climbing;          /* [n_bands] */
+    float* neb_forces;          /* [N, 3] */
+    double* workspace;
+    int64_t n_atoms, n_images, n_bands;
+    double k, force_conversion, energy_conversion;
+} spk_neb_t;
+size_t spk_neb_workspace_bytes(int64_t n_atoms, int64_t n_images);
+int spk_neb_forces(const spk_neb_t* state, const float* forces, const float* energies, spk_stream_t stream);
+
 /* ---- model ensembles (csrc/ensemble.cu; md/calculators/ensemble_calculator.py:38-59,
  * interfaces/batchwise_optimization.py:36-72, interfaces/ase_interface.py:340-432) ------------------------------------
  * The K members' outputs are stacked fp32 slots [K, ...] (slot k = member k).  Every statistic runs in fp64 over k in

@@ -88,7 +88,18 @@ class FIREState(Structure):
                 ("dtmax", c_double), ("finc", c_double), ("fdec", c_double), ("astart", c_double), ("fa", c_double)]
 
 
+class NEBState(Structure):
+    """spk_neb_t of include/spk_b200.h (device pointers of the band layout and the NEB buffers, and the parameters)."""
+    _fields_ = [("r", c_void_p), ("r_initial", c_void_p), ("r_final", c_void_p), ("end_energies", c_void_p),
+                ("climb", c_void_p), ("fixed", c_void_p), ("idx_img", c_void_p), ("img_ptr", c_void_p),
+                ("band_ptr", c_void_p), ("coef", c_void_p), ("diag", c_void_p), ("climbing", c_void_p),
+                ("neb_forces", c_void_p), ("workspace", c_void_p), ("n_atoms", c_int64), ("n_images", c_int64),
+                ("n_bands", c_int64), ("k", c_double), ("force_conversion", c_double),
+                ("energy_conversion", c_double)]
+
+
 FIRE_COEF = 7               # step coefficients per system (spk_fire_t.coef)
+NEB_COEF, NEB_DIAG = 3, 6   # per interior image: spk_neb_t.coef and spk_neb_t.diag
 RELAX_WARP_ATOMS = 256      # SPK_RELAX_WARP_ATOMS
 RELAX_MAX_MEMORY = 4096     # SPK_RELAX_MAX_MEMORY
 
@@ -221,6 +232,8 @@ SIGNATURES = {
     "spk_fire_workspace_bytes": [c_int64, c_int64],
     "spk_fire_forces": [POINTER(FIREState), P, P, P],
     "spk_fire_step": [POINTER(FIREState), P],
+    "spk_neb_workspace_bytes": [c_int64, c_int64],
+    "spk_neb_forces": [POINTER(NEBState), P, P, P],
     "spk_md_motion_workspace_bytes": [c_int64, c_int64],
     "spk_md_remove_motion": [P, P, P, P, P, P, c_int64, c_int64, c_int, c_float, P, c_int64, P, c_size_t, P],
     "spk_md_wrap_positions": [P, P, P, c_int64, c_int32, P, c_int64, P, c_int64, c_double, c_float, P, c_int64, P],
@@ -237,7 +250,7 @@ _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_siz
             "spk_ewald_workspace_bytes": c_size_t, "spk_ensemble_workspace_bytes": c_size_t,
             "spk_spectrum_workspace_bytes": c_size_t, "spk_fire_workspace_bytes": c_size_t,
             "spk_md_motion_workspace_bytes": c_size_t, "spk_spectrum_stream_state_bytes": c_size_t,
-            "spk_spectrum_stream_finalise_workspace_bytes": c_size_t}
+            "spk_spectrum_stream_finalise_workspace_bytes": c_size_t, "spk_neb_workspace_bytes": c_size_t}
 
 _lib = None
 
@@ -284,7 +297,7 @@ LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out
             "spk_relax_converged": 2, "spk_pair_energy_fwd": 2, "spk_head_charges_bwd": 3,
             "spk_pairwise_virial_add": 2, "spk_spectrum_autocorrelation": 2, "spk_spectrum_transform": 2,
             "spk_fire_forces": 3, "spk_fire_step": 2, "spk_md_remove_motion": 3, "spk_spectrum_stream_push": 2,
-            "spk_spectrum_stream_finalise": 2}
+            "spk_spectrum_stream_finalise": 2, "spk_neb_forces": 3}
 # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global; spk_md_initial_momenta: 4 if uniform
 MOTION_CENTER_OF_MASS, MOTION_TRANSLATION, MOTION_ROTATION = 1, 2, 4       # SPK_MOTION_*
 launch_count = 0
