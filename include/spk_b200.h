@@ -665,6 +665,42 @@ int spk_ewald_bwd(const float* R, const float* q, const float* cell, const float
                   const int32_t* sys_ptr, int64_t n_atoms, int64_t n_sys, int64_t n_k, double ke, double alpha,
                   const float* g_E, float* g_R, float* g_q, int accumulate_q, float* g_cell, double* virial,
                   int accumulate_virial, void* workspace, size_t workspace_bytes, spk_stream_t stream);
+/* ---- Smooth particle-mesh Ewald, reciprocal and self terms (csrc/pme.cu; Essmann et al., J. Chem. Phys. 103, 8577) --
+ * Per system m with cell h [3,3] (fp32 in, fp64 inside), H = h^-1, V = |det h|, one mesh of n1 x n2 x n3 points for every
+ * system and cardinal B-splines M_p of order p in {4, 6, 8}, with p <= n_a on every axis (an atom's p support points
+ * along an axis are then distinct mesh points):
+ *   Q_m(x)    = sum_{i in m} q_i prod_a M_p(n_a s_ia - x_a mod n_a),  s_i = r_i H reduced mod 1 in fp64
+ *   E_rec[m]  = sum_{j != 0} theta_j |Q^_m(j)|^2,  theta_j = ke (2 pi / V) f_k |b(j)|^2,  f_k = exp(-k^2 / (4 alpha)) / k^2
+ *   energy[m] = addend[m] + E_rec[m] - ke sqrt(alpha / pi) sum_{i in m} q_i^2
+ * over the signed mesh frequencies j (a Nyquist index n_a / 2 of an even axis is left out), k = 2 pi H j and the Euler
+ * spline moduli |b|^2.  The FFTs are the caller's, between the calls: spectrum = rfftn(mesh) over the three mesh axes
+ * ([n_sys, n1, n2, n3 / 2 + 1] complex fp64, re/im interleaved) and potential = irfftn(conv) (fp64 [n_sys, n1, n2, n3]).
+ * Every sum runs in fp64 in a fixed order without floating-point atomics: bitwise reproducible.  A system of zero volume
+ * gets NaN; systems are the atom ranges of spk_segment_ptr, n_sys <= 65535, n_sys n1 n2 (n3 / 2 + 1) < 2^31.  The
+ * launch shapes depend on n_atoms, n_sys and the mesh only.
+ * workspace: spk_pme_workspace_bytes(...) bytes (0 for an invalid order or mesh), 8-byte aligned; spk_pme_spread leaves
+ * there what spk_pme_energy and spk_pme_bwd read, so all three take the same workspace, untouched in between. */
+size_t spk_pme_workspace_bytes(int64_t n_atoms, int64_t n_sys, int64_t n1, int64_t n2, int64_t n3, int order);
+/* mesh [n_sys, n1, n2, n3] (fp64) = Q_m: bins the atoms by mesh brick and spreads their charges, every mesh point written
+ * once */
+int spk_pme_spread(const float* R, const float* q, const float* cell, const int64_t* idx_m, const int32_t* sys_ptr,
+                   int64_t n_atoms, int64_t n_sys, int64_t n1, int64_t n2, int64_t n3, int order, double* mesh,
+                   void* workspace, size_t workspace_bytes, spk_stream_t stream);
+/* energy [n_sys] from spectrum = rfftn(mesh); conv (the spectrum's shape) = 2 n1 n2 n3 theta spectrum, whose irfftn is
+ * the potential mesh dE_rec/dQ the reverse reads */
+int spk_pme_energy(const float* q, const int32_t* sys_ptr, const double* spectrum, int64_t n_atoms, int64_t n_sys,
+                   int64_t n1, int64_t n2, int64_t n3, int order, double ke, double alpha, const float* addend,
+                   float* energy, double* conv, void* workspace, size_t workspace_bytes, spk_stream_t stream);
+/* Reverse for g_E [n_sys] from potential = irfftn(conv) (each output optional, NULL skips it), with phi_i and grad phi_i
+ * gathered over the p^3 support of atom i:
+ *   g_R [N,3]      = g_E q_i H grad_s phi_i
+ *   g_q [N]       (+)= g_E (phi_i - 2 ke sqrt(alpha / pi) q_i)          (accumulate_q as in spk_ewald_bwd)
+ *   g_cell [B,3,3] = -H^T [sum_i r_i (x) g_R_i - 2 g_E T + g_E E_rec I],  T = sum_j E_j (1/k^2 + 1/(4 alpha)) k (x) k
+ *   virial [B,3,3] (+)= -g_E (E_rec I - 2 T), fp64                        (accumulate_virial as in spk_ewald_bwd) */
+int spk_pme_bwd(const float* R, const float* q, const int64_t* idx_m, const int32_t* sys_ptr, const double* potential,
+                int64_t n_atoms, int64_t n_sys, int64_t n1, int64_t n2, int64_t n3, int order, double ke, double alpha,
+                const float* g_E, float* g_R, float* g_q, int accumulate_q, float* g_cell, double* virial,
+                int accumulate_virial, void* workspace, size_t workspace_bytes, spk_stream_t stream);
 /* spk_pairwise_virial that adds W to what virial holds instead of overwriting it (the reciprocal Ewald virial is
  * deposited there first) */
 int spk_pairwise_virial_add(const float* g_rij, const float* r_ij, const int32_t* rowptr, const int32_t* slot_eid,

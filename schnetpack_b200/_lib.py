@@ -239,6 +239,12 @@ SIGNATURES = {
     "spk_md_wrap_positions": [P, P, P, c_int64, c_int32, P, c_int64, P, c_int64, c_double, c_float, P, c_int64, P],
     "spk_md_initial_momenta": [P, P, P, P, c_int64, c_int64, c_int, c_double, P, c_uint64, P, c_size_t, P],
     "spk_md_step_advance": [P, P],
+    "spk_pme_workspace_bytes": [c_int64, c_int64, c_int64, c_int64, c_int64, c_int],
+    "spk_pme_spread": [P, P, P, P, P, c_int64, c_int64, c_int64, c_int64, c_int64, c_int, P, P, c_size_t, P],
+    "spk_pme_energy": [P, P, P, c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_double, c_double, P, P, P, P,
+                       c_size_t, P],
+    "spk_pme_bwd": [P, P, P, P, P, c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_double, c_double, P, P, P, c_int,
+                    P, P, c_int, P, c_size_t, P],
 }
 _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_size_t,
             "spk_pairwise_virial_workspace_bytes": c_size_t, "spk_md_barostat_workspace_bytes": c_size_t,
@@ -250,7 +256,8 @@ _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_siz
             "spk_ewald_workspace_bytes": c_size_t, "spk_ensemble_workspace_bytes": c_size_t,
             "spk_spectrum_workspace_bytes": c_size_t, "spk_fire_workspace_bytes": c_size_t,
             "spk_md_motion_workspace_bytes": c_size_t, "spk_spectrum_stream_state_bytes": c_size_t,
-            "spk_spectrum_stream_finalise_workspace_bytes": c_size_t, "spk_neb_workspace_bytes": c_size_t}
+            "spk_spectrum_stream_finalise_workspace_bytes": c_size_t, "spk_neb_workspace_bytes": c_size_t,
+            "spk_pme_workspace_bytes": c_size_t}
 
 _lib = None
 
@@ -297,7 +304,9 @@ LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out
             "spk_relax_converged": 2, "spk_pair_energy_fwd": 2, "spk_head_charges_bwd": 3,
             "spk_pairwise_virial_add": 2, "spk_spectrum_autocorrelation": 2, "spk_spectrum_transform": 2,
             "spk_fire_forces": 3, "spk_fire_step": 2, "spk_md_remove_motion": 3, "spk_spectrum_stream_push": 2,
-            "spk_spectrum_stream_finalise": 2, "spk_neb_forces": 3}
+            "spk_spectrum_stream_finalise": 2, "spk_neb_forces": 3, "spk_pme_spread": 8,
+            "spk_pme_energy": 2, "spk_pme_bwd": 2}
+# spk_pme_spread: 4 without atoms (cell, setup, scan, spread); spk_pme_bwd: 1 per part present (atoms, cell or virial);
 # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global; spk_md_initial_momenta: 4 if uniform
 MOTION_CENTER_OF_MASS, MOTION_TRANSLATION, MOTION_ROTATION = 1, 2, 4       # SPK_MOTION_*
 launch_count = 0

@@ -18,7 +18,7 @@ from .. import properties
 
 __all__ = ["PairwiseDistances", "Atomwise", "Forces", "Strain", "DipoleMoment", "Polarizability", "ZBLRepulsionEnergy",
            "CoulombPotential", "DampedCoulombPotential", "EnergyCoulomb", "EnergyEwald", "EnergyEwaldError", "Aggregation",
-           "FilterShortRange"]
+           "FilterShortRange", "EnergyPME", "pme_mesh", "use_pme"]
 
 
 class PairwiseDistances(nn.Module):
@@ -331,4 +331,5 @@ class Polarizability(_GatedHead):
 
 
 from .pair_terms import (Aggregation, CoulombPotential, DampedCoulombPotential, EnergyCoulomb,  # noqa: E402
-                         EnergyEwald, EnergyEwaldError, FilterShortRange, ZBLRepulsionEnergy)
+                         EnergyEwald, EnergyEwaldError, EnergyPME, FilterShortRange, ZBLRepulsionEnergy, pme_mesh,
+                         use_pme)

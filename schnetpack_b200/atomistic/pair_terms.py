@@ -12,6 +12,7 @@ parameters under grad mode: the ATen formulas of ``functional_torch``."""
 from __future__ import annotations
 
 import contextlib
+import math
 from typing import Callable, Dict, List, Optional, Union
 
 import torch
@@ -23,7 +24,8 @@ from .. import ops
 from .. import properties
 from ..units import convert_units
 
-__all__ = ["ZBLRepulsionEnergy", "CoulombPotential", "DampedCoulombPotential", "EnergyCoulomb", "EnergyEwald",
+__all__ = ["ZBLRepulsionEnergy", "CoulombPotential", "DampedCoulombPotential", "EnergyCoulomb", "EnergyEwald", "EnergyPME",
+           "pme_mesh", "use_pme",
            "EnergyEwaldError", "Aggregation", "FilterShortRange", "check_padded_pair_terms", "check_ewald_cells", "padded_list_cutoff",
            "check_short_range_cutoff", "link_charges"]
 
@@ -213,7 +215,65 @@ class EnergyEwaldError(Exception):
     """electrostatic.py:155-156: raised for a system whose cell has zero volume."""
 
 
-class EnergyEwald(nn.Module):
+class _EwaldSum(nn.Module):
+    """What ``EnergyEwald`` and ``EnergyPME`` share: the buffers ``ke`` and ``alpha``, the keys, the list choice and the
+    screen, and the kernel inputs of the real-space and self terms (``_kernel_inputs``)."""
+
+    # the cutoff of the padded neighbour list being evaluated (set by ``padded_list_cutoff``), else None
+    list_cutoff: Optional[float] = None
+
+    def __init__(self, alpha: float, energy_unit: Union[str, float], position_unit: Union[str, float], output_key: str,
+                 charges_key: str, use_neighbors_lr: bool, screening_fn: Optional[nn.Module]):
+        super().__init__()
+        ke = convert_units("Ha", energy_unit) * convert_units("Bohr", position_unit)
+        self.register_buffer("ke", torch.Tensor([ke]))
+        self.charges_key = charges_key
+        self.output_key = output_key
+        self.model_outputs = [output_key]
+        self.use_neighbors_lr = use_neighbors_lr
+        self.screening_fn = screening_fn
+        self.register_buffer("alpha", torch.Tensor([alpha]))
+        self._host = _HostScalars()
+
+    def _screen(self):
+        sw = self.screening_fn
+        if sw is None:
+            return None
+        if type(sw).__name__ != "SwitchFunction":
+            raise NotImplementedError(f"{type(self).__name__}: screening_fn {type(sw).__name__} has no CUDA kernel "
+                                      "(SwitchFunction or None)")
+        return sw
+
+    def _kernel_inputs(self, inputs: Dict[str, torch.Tensor]):
+        """-> (r_ij, q, cell, holder) of the real-space launch pair and the reciprocal and self terms"""
+        who = type(self).__name__
+        sw = self._screen()
+        ke, alpha, s_on, s_off = self._host.get(self.ke, self.alpha, sw.switch_on if sw is not None else None,
+                                                sw.switch_off if sw is not None else None)
+        q = inputs[self.charges_key].reshape(-1)
+        if q.dtype != torch.float32:
+            raise TypeError(f"{who}: the charges must be float32 on the kernel path")
+        idx_m, n_sys, sys_ptr = _systems(inputs, who)
+        if self.use_neighbors_lr:
+            r_ij, idx_i, idx_j, graph = _edges(inputs, properties.Rij_lr, properties.idx_i_lr, properties.idx_j_lr,
+                                               q.shape[0])
+            d_max = None
+        else:
+            r_ij, idx_i, idx_j, graph = _edges(inputs, properties.Rij, properties.idx_i, properties.idx_j, q.shape[0])
+            d_max = _short_range_d_max(inputs)
+        if self.list_cutoff is not None:
+            d_max = self.list_cutoff if d_max is None else min(d_max, self.list_cutoff)
+        params, keep = ops.pair_params(ops.PAIR_EWALD_REAL, ke, switch_on=s_on or 0.0, switch_off=s_off or 0.0,
+                                       d_max=d_max, alpha=alpha)
+        holder = dict(params=params, keep=keep, idx_i=idx_i, idx_j=idx_j, idx_m=idx_m, graph=graph, sys_ptr=sys_ptr,
+                      n_sys=n_sys, ke=ke, alpha=alpha, sink=inputs.get(properties.virial_sink))
+        cell = inputs[properties.cell]
+        if cell.dtype != torch.float32 or cell.numel() != 9 * n_sys:
+            raise TypeError(f"{who}: the cell must be float32 [{n_sys}, 3, 3] on the kernel path")
+        return r_ij, q, cell, holder
+
+
+class EnergyEwald(_EwaldSum):
     """electrostatic.py:159-375: Coulomb energy of the charges under ``charges_key`` in a periodic box by Ewald summation,
     E = E_real + E_rec - E_self.  The real-space term runs over every pair of the long-range (``use_neighbors_lr``) or the
     standard list, screened by ``1 - screening_fn(d)`` when a ``SwitchFunction`` is given; the reciprocal term over the
@@ -228,24 +288,12 @@ class EnergyEwald(nn.Module):
     d > the list cutoff, which drops the padding pairs of a fixed-capacity list and nothing else.  ``train()`` under grad mode: the ATen formulas of
     ``functional_torch``."""
 
-    # the cutoff of the padded neighbour list being evaluated (set by ``padded_list_cutoff``), else None
-    list_cutoff: Optional[float] = None
-
     def __init__(self, alpha: float, k_max: int, energy_unit: Union[str, float], position_unit: Union[str, float],
                  output_key: str, charges_key: str = properties.partial_charges, use_neighbors_lr: bool = True,
                  screening_fn: Optional[nn.Module] = None):
-        super().__init__()
-        ke = convert_units("Ha", energy_unit) * convert_units("Bohr", position_unit)
-        self.register_buffer("ke", torch.Tensor([ke]))
-        self.charges_key = charges_key
-        self.output_key = output_key
-        self.model_outputs = [output_key]
-        self.use_neighbors_lr = use_neighbors_lr
-        self.screening_fn = screening_fn
-        self.register_buffer("alpha", torch.Tensor([alpha]))
+        super().__init__(alpha, energy_unit, position_unit, output_key, charges_key, use_neighbors_lr, screening_fn)
         self.k_max = k_max
         self.register_buffer("kvecs", self._generate_kvecs())
-        self._host = _HostScalars()
 
     def _generate_kvecs(self) -> torch.Tensor:
         """electrostatic.py:209-224."""
@@ -257,48 +305,95 @@ class EnergyEwald(nn.Module):
         norm = norm[norm <= self.k_max ** 2 + 2]
         return kvecs[norm != 0, :]
 
-    def _screen(self):
-        sw = self.screening_fn
-        if sw is None:
-            return None
-        if type(sw).__name__ != "SwitchFunction":
-            raise NotImplementedError(f"EnergyEwald: screening_fn {type(sw).__name__} has no CUDA kernel "
-                                      "(SwitchFunction or None)")
-        return sw
-
     @ops.on_tensor_device
     def forward(self, inputs: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
         if self.training and torch.is_grad_enabled():      # no parameters: the charges carry the training graph
             from .. import functional_torch as T
 
             return T.energy_ewald(self, inputs)
-        sw = self._screen()
-        ke, alpha, s_on, s_off = self._host.get(self.ke, self.alpha, sw.switch_on if sw is not None else None,
-                                                sw.switch_off if sw is not None else None)
-        q = inputs[self.charges_key].reshape(-1)
-        if q.dtype != torch.float32:
-            raise TypeError("EnergyEwald: the charges must be float32 on the kernel path")
-        idx_m, n_sys, sys_ptr = _systems(inputs, "EnergyEwald")
-        if self.use_neighbors_lr:
-            r_ij, idx_i, idx_j, graph = _edges(inputs, properties.Rij_lr, properties.idx_i_lr, properties.idx_j_lr,
-                                               q.shape[0])
-            d_max = None
-        else:
-            r_ij, idx_i, idx_j, graph = _edges(inputs, properties.Rij, properties.idx_i, properties.idx_j, q.shape[0])
-            d_max = _short_range_d_max(inputs)
-        if self.list_cutoff is not None:
-            d_max = self.list_cutoff if d_max is None else min(d_max, self.list_cutoff)
-        params, keep = ops.pair_params(ops.PAIR_EWALD_REAL, ke, switch_on=s_on or 0.0, switch_off=s_off or 0.0,
-                                       d_max=d_max, alpha=alpha)
+        r_ij, q, cell, holder = self._kernel_inputs(inputs)
         kvecs = self.kvecs if self.kvecs.dtype == torch.float32 else self.kvecs.float()
-        holder = dict(params=params, keep=keep, idx_i=idx_i, idx_j=idx_j, idx_m=idx_m, graph=graph, sys_ptr=sys_ptr,
-                      n_sys=n_sys, kvecs=kvecs.contiguous(), ke=ke, alpha=alpha,
-                      sink=inputs.get(properties.virial_sink))
-        cell = inputs[properties.cell]
-        if cell.dtype != torch.float32 or cell.numel() != 9 * n_sys:
-            raise TypeError(f"EnergyEwald: the cell must be float32 [{n_sys}, 3, 3] on the kernel path")
+        holder["kvecs"] = kvecs.contiguous()
         inputs[self.output_key] = K.EwaldFunction.apply(r_ij, inputs[properties.R], q, cell, holder)
         return inputs
+
+
+PME_FFT_PRIMES = (2, 3, 5, 7)
+
+
+def _fft_friendly(n: int) -> bool:
+    for p in PME_FFT_PRIMES:
+        while n % p == 0:
+            n //= p
+    return n == 1
+
+
+def pme_mesh(cell: torch.Tensor, spacing: float, order: int = 4) -> tuple:
+    """The smallest mesh (n1, n2, n3) whose sizes have no prime factor above 7 and give every system of the batch a
+    spacing |h_a| / n_a <= ``spacing`` along each lattice vector h_a, and at least ``order`` points per axis."""
+    h = torch.as_tensor(cell, dtype=torch.float64).detach().cpu().reshape(-1, 3, 3)
+    lengths = torch.linalg.norm(h, dim=2).amax(0)
+    out = []
+    for length in lengths.tolist():
+        n = max(int(order), int(math.ceil(length / float(spacing) - 1e-9)))
+        while not _fft_friendly(n):
+            n += 1
+        out.append(n)
+    return tuple(out)
+
+
+class EnergyPME(_EwaldSum):
+    """Coulomb energy of the charges under ``charges_key`` in a periodic box by smooth particle-mesh Ewald (Essmann et
+    al., J. Chem. Phys. 103, 8577 (1995)): E = E_real + E_rec - E_self, where E_real and E_self are ``EnergyEwald``'s (the
+    same kernels, screen and list handling) and E_rec = ke (2 pi / V) sum_k f_k |b(k)|^2 |Q^(k)|^2 over the mesh
+    frequencies k != 0 (a Nyquist frequency of an even axis left out), with Q the B-spline charge mesh of order ``order``
+    in fractional coordinates.  The cost is O(N order^3 + M log M) for M mesh points instead of Ewald's O(N K), so PME
+    wins on large boxes and Ewald on small ones.  ``mesh`` = (n1, n2, n3) is one mesh for every system of a batch
+    (``pme_mesh`` picks one from a spacing); ``order`` in {4, 6, 8}, each axis at least ``order`` points.
+
+    The buffers and keys are ``EnergyEwald``'s without ``kvecs``; ``use_pme`` swaps the modules of a converted model.  No
+    background term for non-neutral systems, NaN for a zero-volume cell (the drivers refuse one at construction).  The
+    kernel path only: ``train()`` under grad mode raises (train with ``EnergyEwald``)."""
+
+    def __init__(self, alpha: float, mesh, order: int, energy_unit: Union[str, float], position_unit: Union[str, float],
+                 output_key: str, charges_key: str = properties.partial_charges, use_neighbors_lr: bool = True,
+                 screening_fn: Optional[nn.Module] = None):
+        super().__init__(alpha, energy_unit, position_unit, output_key, charges_key, use_neighbors_lr, screening_fn)
+        mesh = tuple(int(n) for n in mesh)
+        if int(order) not in ops.PME_ORDERS:
+            raise ValueError(f"EnergyPME: order {order} is not one of {ops.PME_ORDERS}")
+        if len(mesh) != 3 or any(n < int(order) for n in mesh):
+            raise ValueError(f"EnergyPME: mesh {mesh} must have 3 axes of at least order = {order} points (an atom's "
+                             "support along an axis must be distinct mesh points)")
+        self.mesh = mesh
+        self.order = int(order)
+
+    def extra_repr(self) -> str:
+        return f"mesh={self.mesh}, order={self.order}"
+
+    @ops.on_tensor_device
+    def forward(self, inputs: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        if self.training and torch.is_grad_enabled():
+            raise NotImplementedError("EnergyPME has no training path; train with EnergyEwald and switch with use_pme")
+        r_ij, q, cell, holder = self._kernel_inputs(inputs)
+        holder["mesh"], holder["order"] = self.mesh, self.order
+        inputs[self.output_key] = K.PMEFunction.apply(r_ij, inputs[properties.R], q, cell, holder)
+        return inputs
+
+
+def use_pme(model: nn.Module, mesh, order: int) -> nn.Module:
+    """Replace every ``EnergyEwald`` of ``model`` by an ``EnergyPME`` with the same ke, alpha, keys, list choice and
+    screen, in place, and return the model: train and convert with Ewald, then run MD or relaxation with PME."""
+    for parent in list(model.modules()):
+        for name, child in list(parent.named_children()):
+            if type(child).__name__ != "EnergyEwald":
+                continue
+            new = EnergyPME(1.0, mesh, order, 1.0, 1.0, child.output_key, charges_key=child.charges_key,
+                            use_neighbors_lr=child.use_neighbors_lr, screening_fn=child.screening_fn)
+            new.ke = child.ke.detach().clone()
+            new.alpha = child.alpha.detach().clone()
+            setattr(parent, name, new.to(child.ke.device).train(child.training))
+    return model
 
 
 class Aggregation(nn.Module):
@@ -385,11 +480,12 @@ def check_padded_pair_terms(model: nn.Module, list_cutoff: float, who: str) -> N
 
 @contextlib.contextmanager
 def padded_list_cutoff(model: nn.Module, list_cutoff: float):
-    """Evaluate ``model`` on a padded fixed-capacity neighbour list of cutoff ``list_cutoff``: every ``EnergyEwald`` of it
+    """Evaluate ``model`` on a padded fixed-capacity neighbour list of cutoff ``list_cutoff``: every ``EnergyEwald`` or
+    ``EnergyPME`` of it
     masks real-space pairs with d > list_cutoff for the duration (the padding self pairs sit at 2 list_cutoff).  A plain
     module attribute, read when the forward is traced, so nothing enters the batch and a captured graph keeps it.  Models
-    without an ``EnergyEwald`` are untouched."""
-    mods = [m for m in model.modules() if isinstance(m, EnergyEwald)]
+    without either are untouched."""
+    mods = [m for m in model.modules() if isinstance(m, _EwaldSum)]
     old = [m.list_cutoff for m in mods]
     for m in mods:
         m.list_cutoff = float(list_cutoff)
@@ -402,22 +498,24 @@ def padded_list_cutoff(model: nn.Module, list_cutoff: float):
 
 def check_ewald_cells(model: nn.Module, batch: Dict[str, torch.Tensor], who: str) -> None:
     """electrostatic.py:333-336 at the construction of a device driver: raise ``EnergyEwaldError`` when the model has an
-    ``EnergyEwald`` and a system's cell has (close to) zero volume.  One host read, outside the captured step."""
-    if not any(type(m).__name__ == "EnergyEwald" for m in model.modules()):
+    ``EnergyEwald`` or ``EnergyPME`` and a system's cell has (close to) zero volume.  One host read, outside the captured
+    step."""
+    names = {type(m).__name__ for m in model.modules()} & {"EnergyEwald", "EnergyPME"}
+    if not names:
         return
     cell = batch.get(properties.cell)
     if cell is None:
-        raise ValueError(f"{who}: EnergyEwald needs a periodic batch with a '{properties.cell}'")
+        raise ValueError(f"{who}: {sorted(names)[0]} needs a periodic batch with a '{properties.cell}'")
     v_box = torch.abs(torch.linalg.det(cell.detach().reshape(-1, 3, 3).double()))
     if bool(torch.any(torch.isclose(v_box, torch.zeros_like(v_box)))):
         raise EnergyEwaldError("Simulation box has no volume.")
 
 
 def link_charges(output_modules) -> None:
-    """Make the charges of a ``DipoleMoment`` differentiable when an ``EnergyCoulomb`` or ``EnergyEwald`` of the same
-    model reads them (the kernel head returns plain charges otherwise, so models that only output charges are
+    """Make the charges of a ``DipoleMoment`` differentiable when an ``EnergyCoulomb``, ``EnergyEwald`` or ``EnergyPME``
+    of the same model reads them (the kernel head returns plain charges otherwise, so models that only output charges are
     unchanged)."""
-    keys = {m.charges_key for m in output_modules if type(m).__name__ in ("EnergyCoulomb", "EnergyEwald")}
+    keys = {m.charges_key for m in output_modules if type(m).__name__ in ("EnergyCoulomb", "EnergyEwald", "EnergyPME")}
     for m in output_modules:
         if hasattr(m, "differentiable_charges") and m.return_charges and m.charges_key in keys:
             m.differentiable_charges = True

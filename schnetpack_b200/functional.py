@@ -828,3 +828,43 @@ class EwaldFunction(torch.autograd.Function):
             g_R, g_cell = ops.ewald_bwd(Rd, qd, cd, h["kvecs"], h["idx_m"], h["sys_ptr"], h["n_sys"], h["ke"], h["alpha"],
                                         g_E, ws, want_R, g_q, want_cell, virial, acc)
         return g_rij, g_R, g_q, (g_cell.view(ctx.cell_shape) if g_cell is not None else None), None
+
+
+class PMEFunction(torch.autograd.Function):
+    """``EwaldFunction`` with the reciprocal term by smooth particle-mesh Ewald (csrc/pme.cu, fp64 FFTs between its
+    launches): the same inputs, backward outputs and virial-sink protocol; ``holder["mesh"]`` and ``holder["order"]``
+    replace the k-vectors."""
+
+    @staticmethod
+    def forward(ctx, r_ij, R, q, cell, holder):
+        rd, Rd, qd = r_ij.detach().contiguous(), R.detach().contiguous(), q.detach().contiguous()
+        cd = cell.detach().reshape(-1, 3, 3).contiguous()
+        with ops.device_of(rd, Rd, qd, cd):
+            e_real = ops.pair_energy_fwd(holder["params"], rd, holder["idx_i"], holder["idx_j"], None, qd, holder["idx_m"],
+                                         holder["graph"], holder["sys_ptr"], holder["n_sys"])
+            energy, conv, ws = ops.pme_fwd(Rd, qd, cd, holder["idx_m"], holder["sys_ptr"], holder["n_sys"],
+                                           holder["mesh"], holder["order"], holder["ke"], holder["alpha"], addend=e_real)
+        ctx.h = (holder, rd, Rd, qd, conv, ws)
+        ctx.cell_shape = cell.shape
+        ctx.set_materialize_grads(False)
+        return energy
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_E):
+        if g_E is None:
+            return None, None, None, None, None
+        h, rd, Rd, qd, conv, ws = ctx.h
+        _, want_R, want_q, want_cell, _ = ctx.needs_input_grad
+        sink = h.get("sink")
+        virial, acc = None, False
+        if sink is not None:
+            virial, acc = sink["virial"], sink.get("virial_deposited", False)
+            sink["virial_deposited"] = True
+        with ops.device_of(rd):
+            g_E = g_E.contiguous()
+            g_rij, g_q = ops.pair_energy_bwd(h["params"], rd, h["idx_i"], h["idx_j"], None, qd, h["idx_m"], g_E, h["graph"],
+                                             want_q)
+            g_R, g_cell = ops.pme_bwd(Rd, qd, h["idx_m"], h["sys_ptr"], h["n_sys"], h["mesh"], h["order"], h["ke"],
+                                      h["alpha"], g_E, conv, ws, want_R, g_q, want_cell, virial, acc)
+        return g_rij, g_R, g_q, (g_cell.view(ctx.cell_shape) if g_cell is not None else None), None

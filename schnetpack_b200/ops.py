@@ -886,6 +886,53 @@ def ewald_bwd(R: Tensor, q: Tensor, cell: Tensor, kvecs: Tensor, idx_m: Tensor, 
     return g_R, g_cell
 
 
+# ------------------------------------------------------------------------------------------------------------ PME
+PME_ORDERS = (4, 6, 8)
+
+
+def pme_workspace(n_atoms: int, n_sys: int, mesh, order: int, device) -> Tensor:
+    nbytes = int(_lib.lib().spk_pme_workspace_bytes(n_atoms, n_sys, *mesh, order))
+    if nbytes == 0:
+        raise ValueError(f"PME: invalid mesh {tuple(mesh)} or order {order}")
+    return torch.empty(nbytes, dtype=torch.uint8, device=device)
+
+
+def pme_fwd(R: Tensor, q: Tensor, cell: Tensor, idx_m: Tensor, sys_ptr: Tensor, n_sys: int, mesh, order: int, ke: float,
+            alpha: float, addend: Optional[Tensor] = None):
+    """-> (energy [n_sys] = addend + E_rec - E_self, conv [n_sys, n1, n2, n3 // 2 + 1] complex128, workspace): the charge
+    mesh of csrc/pme.cu, its fp64 rfftn, and the influence pass; ``conv`` and the workspace are what the reverse reads."""
+    dev = R.device
+    N = R.shape[0]
+    n1, n2, n3 = mesh
+    ws = pme_workspace(N, n_sys, mesh, order, dev)
+    Q = torch.empty((n_sys, n1, n2, n3), dtype=torch.float64, device=dev)
+    R, q, cell, idx_m = f32(R, "_positions"), f32(q, "charges"), f32(cell, "_cell"), i64(idx_m, "_idx_m")
+    _lib.call("spk_pme_spread", _p(R), _p(q), _p(cell), _p(idx_m), _p(sys_ptr), N, n_sys, n1, n2, n3, int(order), _p(Q),
+              _p(ws), ws.numel(), _stream(), launches=8 if N > 0 else 4)
+    spec = torch.fft.rfftn(Q, dim=(1, 2, 3)).contiguous()
+    energy = torch.empty((n_sys,), dtype=torch.float32, device=dev)
+    conv = torch.empty_like(spec)
+    _lib.call("spk_pme_energy", _p(q), _p(sys_ptr), _p(spec), N, n_sys, n1, n2, n3, int(order), float(ke), float(alpha),
+              _p(f32(addend, "energy")) if addend is not None else None, _p(energy), _p(conv), _p(ws), ws.numel(),
+              _stream())
+    return energy, conv, ws
+
+
+def pme_bwd(R: Tensor, q: Tensor, idx_m: Tensor, sys_ptr: Tensor, n_sys: int, mesh, order: int, ke: float, alpha: float,
+            g_E: Tensor, conv: Tensor, ws: Tensor, want_R: bool, g_q: Optional[Tensor], want_cell: bool,
+            virial: Optional[Tensor] = None, accumulate_virial: bool = False):
+    """The reverse of ``pme_fwd``: potential mesh = irfftn(conv), then the gather; outputs as ``ewald_bwd``."""
+    dev = R.device
+    N = R.shape[0]
+    phi = torch.fft.irfftn(conv, s=tuple(mesh), dim=(1, 2, 3)).contiguous()
+    g_R = torch.empty((N, 3), dtype=torch.float32, device=dev) if want_R else None
+    g_cell = torch.empty((n_sys, 3, 3), dtype=torch.float32, device=dev) if want_cell else None
+    _lib.call("spk_pme_bwd", _p(R), _p(q), _p(idx_m), _p(sys_ptr), _p(phi), N, n_sys, *mesh, int(order), float(ke),
+              float(alpha), _p(f32(g_E, "g_E")), _p(g_R), _p(g_q), 1, _p(g_cell), _p(virial), int(accumulate_virial),
+              _p(ws), ws.numel(), _stream(), launches=int(N > 0) + int(want_cell or virial is not None))
+    return g_R, g_cell
+
+
 # ------------------------------------------------------------------------------------------------------- vibrations
 def vib_displace(params: "_lib.VibParams"):
     """replica positions and realised steps of the chunk the counter names (csrc/vibrations.cu)"""

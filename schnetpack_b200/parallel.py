@@ -418,6 +418,9 @@ class PartitionedPotential:
         rep = model.representation
         if type(rep).__name__ != "PaiNN":
             raise NotImplementedError("PartitionedPotential: PaiNN representation (the named large-system configs)")
+        if any(type(m).__name__ == "EnergyPME" for m in model.output_modules):
+            raise NotImplementedError("PartitionedPotential: EnergyPME (its charge mesh spans the atoms of every rank); "
+                                      "evaluate the model on one device")
         self.rep = rep
         self.head = [m for m in model.output_modules if type(m).__name__ == "Atomwise"][0]
         dev = self.device

@@ -382,7 +382,7 @@ def to_scriptable(model: NeuralNetworkPotential) -> ScriptedPotential:
         elif n == "Forces":
             outs.append(ScriptForces(m))
         elif n in ("DipoleMoment", "Polarizability", "ZBLRepulsionEnergy", "EnergyCoulomb", "EnergyEwald",
-                   "Aggregation"):
+                   "EnergyPME", "Aggregation"):
             raise NotImplementedError(f"to_scriptable: {n} has no TorchScript twin (its kernels run through "
                                       "torch.autograd.Function); evaluate the model in Python")
         else:
