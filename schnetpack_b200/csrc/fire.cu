@@ -8,12 +8,13 @@
 //                    dot products (seg_partials of segscan.cuh);
 //     k_fire_system  one CTA per system: the partials in CTA order, the 3 cell rows of g (filter), the largest row
 //                    |g_row|^2, the convergence test;
-//     k_fire_count   the count of unconverged systems;
+//     k_count_unconverged  the count of unconverged systems (relax_common.cuh);
 //   step (spk_fire_step):
 //     k_fire_coef    one thread per system: dt, a, Nsteps, the cap of |dr| and the cell's 9 components (it owns them);
 //     k_fire_move    one thread per atom: v, s, x = s F^T and the fp32 model positions.
 // |v'|^2 after the mixing follows from v.v, v.g and g.g (v' = c1 v + c2 g with c1, c2 >= 0), so no second reduction pass
 // is needed.  Every sum has a fixed order given the layout and there are no atomics: replays are bitwise reproducible.
+#include "relax_common.cuh"
 #include "segscan.cuh"
 
 namespace {
@@ -26,10 +27,6 @@ constexpr int COEF_T = 128;
 // coefficients the per-system thread leaves for k_fire_move, [n_sys][COEF_N]
 enum { C_MODE = 0, C_ONE_MINUS_A, C_A, C_GNORM, C_VNORM, C_DT, C_NORMDR, COEF_N };
 enum { MODE_FROZEN = 0, MODE_START = 1, MODE_MIX = 2, MODE_RESET = 3 };
-
-__device__ __forceinline__ double dot3(double x0, double x1, double x2, double y0, double y1, double y2) {
-    return __dadd_rn(__dadd_rn(__dmul_rn(x0, y0), __dmul_rn(x1, y1)), __dmul_rn(x2, y2));
-}
 
 // F = h / cell_factor of system m, row-major [3][3]
 __device__ __forceinline__ void load_F(const spk_fire_t& st, int64_t m, double (&F)[9]) {
@@ -44,7 +41,7 @@ __device__ __forceinline__ void atom_force(const spk_fire_t& st, const float* __
     const bool fixed = st.fixed && st.fixed[a];
     double f[3];
 #pragma unroll
-    for (int c = 0; c < 3; ++c) f[c] = fixed ? 0.0 : (double)forces[3 * a + c] * st.force_conversion;
+    for (int c = 0; c < 3; ++c) f[c] = optimizer_force(fixed, forces, st.force_conversion, a, c);
     if (!st.filter) {
 #pragma unroll
         for (int c = 0; c < 3; ++c) g[c] = f[c];
@@ -53,7 +50,7 @@ __device__ __forceinline__ void atom_force(const spk_fire_t& st, const float* __
     double F[9];
     load_F(st, m, F);
 #pragma unroll
-    for (int k = 0; k < 3; ++k) g[k] = dot3(f[0], f[1], f[2], F[k], F[3 + k], F[6 + k]);
+    for (int k = 0; k < 3; ++k) g[k] = dot3_rn(f[0], f[1], f[2], F[k], F[3 + k], F[6 + k]);
 }
 
 __device__ __forceinline__ double* ws_sys_part(const spk_fire_t& st) { return st.workspace; }
@@ -73,9 +70,9 @@ __global__ void __launch_bounds__(FIRE_T) k_fire_atoms(spk_fire_t st, const floa
         const double v0 = st.v[3 * a], v1 = st.v[3 * a + 1], v2 = st.v[3 * a + 2];
 #pragma unroll
         for (int c = 0; c < 3; ++c) st.g[3 * a + c] = g[c];
-        v[0] = dot3(v0, v1, v2, g[0], g[1], g[2]);
-        v[1] = dot3(v0, v1, v2, v0, v1, v2);
-        v[2] = dot3(g[0], g[1], g[2], g[0], g[1], g[2]);
+        v[0] = dot3_rn(v0, v1, v2, g[0], g[1], g[2]);
+        v[1] = dot3_rn(v0, v1, v2, v0, v1, v2);
+        v[2] = dot3_rn(g[0], g[1], g[2], g[0], g[1], g[2]);
     }
     seg_partials<FIRE_T, NSUM>(v, st.n_atoms, m, first, end, ws_sys_part(st), ws_head(st));
 }
@@ -102,7 +99,8 @@ __device__ __forceinline__ void current_cell(const spk_fire_t& st, int64_t m, co
 #pragma unroll
     for (int i = 0; i < 3; ++i)
 #pragma unroll
-        for (int j = 0; j < 3; ++j) cell[3 * i + j] = dot3(c0[3 * i], c0[3 * i + 1], c0[3 * i + 2], F[3 * j], F[3 * j + 1], F[3 * j + 2]);
+        for (int j = 0; j < 3; ++j)
+            cell[3 * i + j] = dot3_rn(c0[3 * i], c0[3 * i + 1], c0[3 * i + 2], F[3 * j], F[3 * j + 1], F[3 * j + 2]);
 }
 
 // The generalized cell forces of UnitCellFilter.get_forces: Vir = -(energy_conversion sym(W) + p V I), Vir F^-T, the
@@ -128,7 +126,7 @@ __device__ void cell_forces(const spk_fire_t& st, int64_t m, const double* __res
     for (int i = 0; i < 3; ++i)
 #pragma unroll
         for (int j = 0; j < 3; ++j)
-            t[3 * i + j] = dot3(vir[3 * i], vir[3 * i + 1], vir[3 * i + 2], Fi[3 * j], Fi[3 * j + 1], Fi[3 * j + 2]);
+            t[3 * i + j] = dot3_rn(vir[3 * i], vir[3 * i + 1], vir[3 * i + 2], Fi[3 * j], Fi[3 * j + 1], Fi[3 * j + 2]);
     if (st.hydrostatic_strain) {
         const double tr3 = (t[0] + t[4] + t[8]) / 3.0;
 #pragma unroll
@@ -160,7 +158,7 @@ __global__ void __launch_bounds__(SEG_FIN_T) k_fire_system(spk_fire_t st, const 
     double mx = 0.0;
     for (int64_t a = a0 + t; a < a1; a += SEG_FIN_T) {
         const double* g = st.g + 3 * a;
-        mx = fmax(mx, dot3(g[0], g[1], g[2], g[0], g[1], g[2]));
+        mx = fmax(mx, dot3_rn(g[0], g[1], g[2], g[0], g[1], g[2]));
     }
     mx_red[t] = mx;
     __syncthreads();
@@ -180,9 +178,9 @@ __global__ void __launch_bounds__(SEG_FIN_T) k_fire_system(spk_fire_t st, const 
         for (int r = 0; r < 3; ++r) {
             const double* gr = hg + 3 * r;
             const double* vr = hv + 3 * r;
-            vg += dot3(vr[0], vr[1], vr[2], gr[0], gr[1], gr[2]);
-            vv += dot3(vr[0], vr[1], vr[2], vr[0], vr[1], vr[2]);
-            const double g2 = dot3(gr[0], gr[1], gr[2], gr[0], gr[1], gr[2]);
+            vg += dot3_rn(vr[0], vr[1], vr[2], gr[0], gr[1], gr[2]);
+            vv += dot3_rn(vr[0], vr[1], vr[2], vr[0], vr[1], vr[2]);
+            const double g2 = dot3_rn(gr[0], gr[1], gr[2], gr[0], gr[1], gr[2]);
             gg += g2;
             mx = fmax(mx, g2);
         }
@@ -192,30 +190,7 @@ __global__ void __launch_bounds__(SEG_FIN_T) k_fire_system(spk_fire_t st, const 
     st.sums[NSUM * m] = vg;
     st.sums[NSUM * m + 1] = vv;
     st.sums[NSUM * m + 2] = gg;
-    const double fm = *st.fmax;
-    const bool conv = mx < fm * fm;
-    st.fmax_sys[m] = sqrt(mx);
-    st.converged[m] = conv ? 1 : 0;
-    const int64_t prev = st.steps[m];
-    st.steps[m] = conv ? (prev >= 0 ? prev : st.counter[1]) : -1;
-}
-
-// count of unconverged systems; the step counter read by the next step catches up with the one the last step wrote
-__global__ void __launch_bounds__(256) k_fire_count(spk_fire_t st) {
-    __shared__ int red[8];
-    SPK_PDL_ENTER();
-    int cnt = 0;
-    for (int64_t m = threadIdx.x; m < st.n_sys; m += 256) cnt += st.converged[m] ? 0 : 1;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = cnt;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int t = 0;
-        for (int k = 0; k < 8; ++k) t += red[k];
-        *st.n_unconverged = t;
-        st.counter[0] = st.counter[1];
-    }
+    record_convergence(st, m, mx);
 }
 
 // ASE's velocity update of one component: the mixing (or the reset) with the old a, then v += dt g with the new dt
@@ -323,7 +298,7 @@ __global__ void __launch_bounds__(MOVE_T) k_fire_move(spk_fire_t st) {
         double F[9];
         load_F(st, m, F);
 #pragma unroll
-        for (int j = 0; j < 3; ++j) x[j] = dot3(s[0], s[1], s[2], F[3 * j], F[3 * j + 1], F[3 * j + 2]);
+        for (int j = 0; j < 3; ++j) x[j] = dot3_rn(s[0], s[1], s[2], F[3 * j], F[3 * j + 1], F[3 * j + 2]);
     }
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -358,7 +333,7 @@ extern "C" int spk_fire_forces(const spk_fire_t* st, const float* forces, const 
     }
     spk_launch(k_fire_system, (unsigned)st->n_sys, SEG_FIN_T, 0, s, *st, virial);
     SPK_LAUNCH_CHECK();
-    spk_launch(k_fire_count, 1, 256, 0, s, *st);
+    spk_launch(k_count_unconverged<spk_fire_t>, 1, 256, 0, s, *st);
     SPK_LAUNCH_CHECK();
     return SPK_OK;
 }

@@ -9,6 +9,7 @@
 //   k_neb_image     one CTA per interior image: the sums in CTA order, the tangent branch, the climbing image, gamma;
 //   k_neb_assemble  one thread per atom: F_NEB = F + gamma (alpha D+ + beta D-), fp32, 0 on fixed atoms.
 // Every sum has a fixed order given the layout and there are no atomics: replays are bitwise reproducible.
+#include "relax_common.cuh"
 #include "segscan.cuh"
 
 namespace {
@@ -44,12 +45,8 @@ __device__ __forceinline__ void atom_terms(const spk_neb_t& st, const float* __r
     for (int c = 0; c < 3; ++c) {
         t.dp[c] = next[c] - x[c];
         t.dm[c] = x[c] - prev[c];
-        t.f[c] = fixed ? 0.0 : (double)forces[3 * a + c] * st.force_conversion;
+        t.f[c] = optimizer_force(fixed, forces, st.force_conversion, a, c);
     }
-}
-
-__device__ __forceinline__ double dot3(const double (&x)[3], const double (&y)[3]) {
-    return __dadd_rn(__dadd_rn(__dmul_rn(x[0], y[0]), __dmul_rn(x[1], y[1])), __dmul_rn(x[2], y[2]));
 }
 
 __global__ void __launch_bounds__(NEB_T) k_neb_partials(spk_neb_t st, const float* __restrict__ forces) {
@@ -63,11 +60,12 @@ __global__ void __launch_bounds__(NEB_T) k_neb_partials(spk_neb_t st, const floa
         end = st.img_ptr[m + 1];
         AtomTerms t;
         atom_terms(st, forces, a, m, t);
-        v[0] = dot3(t.dp, t.dp);
-        v[1] = dot3(t.dm, t.dm);
-        v[2] = dot3(t.dp, t.dm);
-        v[3] = dot3(t.f, t.dp);
-        v[4] = dot3(t.f, t.dm);
+        const double *dp = t.dp, *dm = t.dm, *f = t.f;
+        v[0] = dot3_rn(dp[0], dp[1], dp[2], dp[0], dp[1], dp[2]);
+        v[1] = dot3_rn(dm[0], dm[1], dm[2], dm[0], dm[1], dm[2]);
+        v[2] = dot3_rn(dp[0], dp[1], dp[2], dm[0], dm[1], dm[2]);
+        v[3] = dot3_rn(f[0], f[1], f[2], dp[0], dp[1], dp[2]);
+        v[4] = dot3_rn(f[0], f[1], f[2], dm[0], dm[1], dm[2]);
     }
     seg_partials<NEB_T, NSUM>(v, st.n_atoms, m, first, end, ws_img_part(st), ws_head(st));
 }

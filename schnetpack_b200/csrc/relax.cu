@@ -11,7 +11,7 @@
 // Every sum has a fixed order given the layout, so a replay is bitwise reproducible; there are no atomics.
 #include <cooperative_groups.h>
 
-#include "common.cuh"
+#include "relax_common.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -35,18 +35,6 @@ __device__ __forceinline__ double warp_max_d(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
-}
-
-// force component in optimizer units, zero on fixed atoms (get_forces, :196-197)
-__device__ __forceinline__ double relax_force(const spk_lbfgs_t& st, const float* __restrict__ forces, int64_t atom,
-                                              int c) {
-    if (st.fixed && st.fixed[atom]) return 0.0;
-    return (double)forces[3 * atom + c] * st.force_conversion;
-}
-
-// |v|^2 of a 3-vector summed as numpy does along the last axis: (x^2 + y^2) + z^2, no contraction
-__device__ __forceinline__ double norm2_3(double x, double y, double z) {
-    return __dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z));
 }
 
 // ---- warp per system -----------------------------------------------------------------------------------------------
@@ -78,7 +66,8 @@ __global__ void __launch_bounds__(WARP_CTA_WARPS * 32) k_lbfgs_warp(spk_lbfgs_t 
             q[3 * k + c] = 0.0;
             if (la < n) {
                 const int64_t e = 3 * (a0 + la) + c;
-                const double f = relax_force(st, forces, a0 + la, c);
+                const double f =
+                    optimizer_force(st.fixed && st.fixed[a0 + la], forces, st.force_conversion, a0 + la, c);
                 if (it > 0) {
                     const int64_t sl = (it - 1) % M;
                     const double s = st.r[e] - st.r0[e];
@@ -156,7 +145,10 @@ __global__ void __launch_bounds__(WARP_CTA_WARPS * 32) k_lbfgs_warp(spk_lbfgs_t 
     for (int k = 0; k < WARP_KA; ++k) {
 #pragma unroll
         for (int c = 0; c < 3; ++c) q[3 * k + c] = conv ? 0.0 : -q[3 * k + c];
-        if (lane + 32 * k < n) longest2 = fmax(longest2, norm2_3(q[3 * k], q[3 * k + 1], q[3 * k + 2]));
+        if (lane + 32 * k < n) {
+            const double x = q[3 * k], y = q[3 * k + 1], z = q[3 * k + 2];
+            longest2 = fmax(longest2, dot3_rn(x, y, z, x, y, z));
+        }
     }
     const double longest = sqrt(warp_max_d(longest2));
     const bool cap = longest >= st.maxstep;
@@ -174,7 +166,7 @@ __global__ void __launch_bounds__(WARP_CTA_WARPS * 32) k_lbfgs_warp(spk_lbfgs_t 
                 const double rn = r + p * st.damping;
                 st.p[e] = p;
                 st.r0[e] = r;
-                st.f0[e] = relax_force(st, forces, a0 + la, c);
+                st.f0[e] = optimizer_force(st.fixed && st.fixed[a0 + la], forces, st.force_conversion, a0 + la, c);
                 st.r[e] = rn;
                 st.model_positions[e] = (float)(rn / st.position_conversion);
             }
@@ -230,7 +222,7 @@ __global__ void __cluster_dims__(RELAX_CL_CTAS, 1, 1) __launch_bounds__(RELAX_CL
     for (int64_t la = g; la < n; la += G) {
         for (int c = 0; c < 3; ++c) {
             const int64_t e = 3 * (a0 + la) + c;
-            const double f = relax_force(st, forces, a0 + la, c);
+            const double f = optimizer_force(st.fixed && st.fixed[a0 + la], forces, st.force_conversion, a0 + la, c);
             if (it > 0) {
                 const int64_t sl = (it - 1) % M;
                 const double s = st.r[e] - st.r0[e];
@@ -296,7 +288,7 @@ __global__ void __cluster_dims__(RELAX_CL_CTAS, 1, 1) __launch_bounds__(RELAX_CL
         const int64_t e = 3 * (a0 + la);
         double* v = q + e;
         for (int c = 0; c < 3; ++c) v[c] = conv ? 0.0 : -v[c];
-        longest2 = fmax(longest2, norm2_3(v[0], v[1], v[2]));
+        longest2 = fmax(longest2, dot3_rn(v[0], v[1], v[2], v[0], v[1], v[2]));
     }
     const double longest = sqrt(cluster_reduce<true>(longest2, red, part, phase, cl));
     const bool cap = longest >= st.maxstep;
@@ -309,7 +301,7 @@ __global__ void __cluster_dims__(RELAX_CL_CTAS, 1, 1) __launch_bounds__(RELAX_CL
             const double rn = r + p * st.damping;
             st.p[e] = p;
             st.r0[e] = r;
-            st.f0[e] = relax_force(st, forces, a0 + la, c);
+            st.f0[e] = optimizer_force(st.fixed && st.fixed[a0 + la], forces, st.force_conversion, a0 + la, c);
             st.r[e] = rn;
             st.model_positions[e] = (float)(rn / st.position_conversion);
         }
@@ -324,35 +316,14 @@ __global__ void __launch_bounds__(CONV_WARPS * 32) k_relax_converged(spk_lbfgs_t
     if (m >= st.n_sys) return;
     const int64_t a0 = st.sys_ptr[m], a1 = st.sys_ptr[m + 1];
     double mx = 0.0;
-    for (int64_t a = a0 + lane; a < a1; a += 32)
-        mx = fmax(mx, norm2_3(relax_force(st, forces, a, 0), relax_force(st, forces, a, 1), relax_force(st, forces, a, 2)));
+    for (int64_t a = a0 + lane; a < a1; a += 32) {
+        const double x = optimizer_force(st.fixed && st.fixed[a], forces, st.force_conversion, a, 0);
+        const double y = optimizer_force(st.fixed && st.fixed[a], forces, st.force_conversion, a, 1);
+        const double z = optimizer_force(st.fixed && st.fixed[a], forces, st.force_conversion, a, 2);
+        mx = fmax(mx, dot3_rn(x, y, z, x, y, z));
+    }
     mx = warp_max_d(mx);
-    if (lane == 0) {
-        const double fm = *st.fmax;
-        const bool conv = mx < fm * fm;
-        st.fmax_sys[m] = sqrt(mx);
-        st.converged[m] = conv ? 1 : 0;
-        const int64_t prev = st.steps[m];
-        st.steps[m] = conv ? (prev >= 0 ? prev : st.counter[1]) : -1;
-    }
-}
-
-// count of unconverged systems; the step counter read by the next step catches up with the one the last step wrote
-__global__ void __launch_bounds__(256) k_relax_count(spk_lbfgs_t st) {
-    __shared__ int red[8];
-    SPK_PDL_ENTER();
-    int cnt = 0;
-    for (int64_t m = threadIdx.x; m < st.n_sys; m += 256) cnt += st.converged[m] ? 0 : 1;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = cnt;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int t = 0;
-        for (int k = 0; k < 8; ++k) t += red[k];
-        *st.n_unconverged = t;
-        st.counter[0] = st.counter[1];
-    }
+    if (lane == 0) record_convergence(st, m, mx);
 }
 
 SpkSmemOnce g_warp_smem, g_cluster_smem;
@@ -395,7 +366,7 @@ extern "C" int spk_relax_converged(const spk_lbfgs_t* st, const float* forces, s
     const cudaStream_t s = spk_st(stream);
     spk_launch(k_relax_converged, (unsigned)spk_cdiv(st->n_sys, CONV_WARPS), CONV_WARPS * 32, 0, s, *st, forces);
     SPK_LAUNCH_CHECK();
-    spk_launch(k_relax_count, 1, 256, 0, s, *st);
+    spk_launch(k_count_unconverged<spk_lbfgs_t>, 1, 256, 0, s, *st);
     SPK_LAUNCH_CHECK();
     return SPK_OK;
 }

@@ -1012,7 +1012,8 @@ class _CapturedEvaluation:
     """The force evaluation of a device-resident loop (calculator.calculate) and the capture of one whole step with it:
     neighbour list on the fixed-capacity ``self.nl``, ``self.model`` on ``self.static`` and copies of the outputs into
     ``self.energy`` / ``self.forces``, with the sticky overflow watch ``self.nl_watch``.  ``DeviceMD``,
-    ``relax.DeviceLBFGS`` and ``vibrations.DeviceVibrations`` build their steps around it: each defines ``_step()`` and
+    ``vibrations.DeviceVibrations`` and the batchwise optimizers of ``relax._BatchOptimizer`` (``relax.DeviceLBFGS``,
+    ``relax.DeviceFIRE`` and ``neb.DeviceNEB``) build their steps around it: each defines ``_step()`` and
     ``_step_state()``, the (nested) dict of every tensor the step writes."""
 
     energy_key = P.energy

@@ -19,8 +19,8 @@ import torch
 
 from . import _lib, ops
 from . import properties as P
-from .md import _CapturedEvaluation, _clone_state, _load_state, _TensorState
-from .relax import DEFAULT_MAX_STEPS, FIREState, _check_fire_keywords, _ensemble_uncertainty, _fixed_mask
+from .md import _TensorState
+from .relax import FIREState, _BatchOptimizer, _check_fire_keywords, _fixed_mask
 
 __all__ = ["DeviceNEB", "NEBState", "interpolate"]
 
@@ -227,7 +227,7 @@ class NEBState(_TensorState):
 
 
 # ---- the captured NEB relaxation -----------------------------------------------------------------------------------------
-class DeviceNEB(_CapturedEvaluation):
+class DeviceNEB(_BatchOptimizer):
     """Climbing-image NEB between the systems of ``initial`` and ``final`` (collated batches in model units, one band per
     system; the endpoints of a band have the same atoms in the same order, the same cell and pbc), relaxed by ASE's FIRE
     (its keywords and defaults) with each band as one optimizer.  The ``n_images`` interior images of every band are the
@@ -242,7 +242,9 @@ class DeviceNEB(_CapturedEvaluation):
     is the FIRE step, the neighbour list, the model on the interior images, the NEB forces and FIRE's force side and
     convergence test, captured once as a CUDA graph (``use_graph``).  A band converges when the largest NEB force on its
     moving atoms is below ``fmax``; converged bands take no step.  ``model`` may be a list of at least two members, as in
-    ``DeviceFIRE``."""
+    ``DeviceFIRE``.  Results are per band (``fmax``: the largest NEB force, ``converged``, ``steps_to_converge``) or
+    cover the interior images (``positions``, band-major and image-major; ``get_forces``: the NEB forces;
+    ``get_uncertainty``: their energies and forces)."""
 
     def __init__(self, model: torch.nn.Module, initial: Dict[str, Tensor], final: Dict[str, Tensor], cutoff: float,
                  capacity: int, n_images: int = 5, images: Optional[Dict[str, Tensor]] = None, k: float = 0.1,
@@ -261,16 +263,11 @@ class DeviceNEB(_CapturedEvaluation):
         self.fire_keywords = dict(dt=dt, maxstep=maxstep, dtmax=dtmax, Nmin=Nmin, finc=finc, fdec=fdec, astart=astart,
                                   fa=fa, a=a)
         _check_fire_keywords(self.fire_keywords)
-        outputs = getattr(model, "model_outputs", None)
-        if outputs is not None and (force_key not in outputs or energy_key not in outputs):
-            raise ValueError(f"DeviceNEB: the model must output '{energy_key}' and '{force_key}' (it outputs "
-                             f"{sorted(outputs)})")
+        self._check_outputs(model, energy_key, force_key)
         if initial[P.R].device.type != "cuda":
             raise ValueError("DeviceNEB needs CUDA batches (no CPU fallback)")
-        self.energy_key, self.force_key = energy_key, force_key
         n = self.n_images = int(n_images)
-        self.p_conv, self.e_conv = float(position_conversion), float(energy_conversion)
-        self.f_conv = self.e_conv / self.p_conv
+        self._set_conversions(position_conversion, energy_conversion)
         ends = [_Systems(initial, "DeviceNEB: initial"), _Systems(final, "DeviceNEB: final")]
         self.bands = bands = ends[0]
         _check_same(bands, ends[1], "DeviceNEB: final endpoints")
@@ -311,18 +308,16 @@ class DeviceNEB(_CapturedEvaluation):
                             climb=climb, fixed_atoms_mask=fixed, force_conversion=self.f_conv,
                             energy_conversion=self.e_conv)
         self.climb = bool(climb)
-        self.iterations = 0
-        self.nsteps = 0
-        self._calculate()
-        self.opt.check(self.neb.forces(self.forces, self.energy))
+        self._start()
 
-    def _step(self):
+    def _advance(self):
         self.opt.step()
-        self._calculate()
+
+    def _check(self):
         self.opt.check(self.neb.forces(self.forces, self.energy))
 
     def _step_state(self) -> Dict[str, object]:
-        return dict(opt=self.opt.tensors(), neb=self.neb.tensors(), **self._evaluation_state())
+        return dict(super()._step_state(), neb=self.neb.tensors())
 
     def _reset_fire(self):
         """the state of a new FIRE optimizer for every band (v = 0, dt, a, Nsteps), in place"""
@@ -338,38 +333,15 @@ class DeviceNEB(_CapturedEvaluation):
         """Relax until every band's largest NEB force is below ``fmax`` or ``steps`` steps (default: unlimited) were taken
         in this call; returns whether every band converged.  ``climb`` turns the climbing image on or off first; when that
         changes it, every band's FIRE state is reset, as a new optimizer would start (the captured step stays valid)."""
-        if int(check_every) < 1:
+        if int(check_every) < 1:                 # refused before the climb flag changes
             raise ValueError("DeviceNEB: check_every must be >= 1")
         if climb is not None and bool(climb) != self.climb:
             self.climb = bool(climb)
             self.neb.set_climb(self.climb)
             self._reset_fire()
-        budget = DEFAULT_MAX_STEPS if not steps else int(steps)
-        self.opt.set_fmax(fmax)
-        self.opt.check(self.neb.forces(self.forces, self.energy))
-        done = 0
-        left = int(self.opt.n_unconverged.item())
-        while left and done < budget:
-            kk = min(int(check_every), budget - done)
-            self._run_steps(kk)
-            done += kk
-            self.iterations += kk
-            left = int(self.opt.n_unconverged.item())
-        self.check_neighbor_list()
-        self.nsteps = int(self.opt.steps_to_converge.max().item()) if left == 0 else self.iterations
-        return left == 0
+        return super().run(fmax, steps, check_every)
 
     # ---- results, in optimizer units ------------------------------------------------------------------------------------
-    @property
-    def positions(self) -> Tensor:
-        """[N, 3] fp64 positions of the interior images (band-major, image-major)"""
-        return self.opt.r
-
-    @property
-    def model_positions(self) -> Tensor:
-        """[N, 3] fp32 positions the model reads (positions / position_conversion)"""
-        return self.static[P.R]
-
     def path(self) -> List[Tensor]:
         """per band, [n_images + 2, A_b, 3] fp64: the endpoints and the interior images"""
         out, p, e = [], 0, 0
@@ -415,33 +387,9 @@ class DeviceNEB(_CapturedEvaluation):
         """the NEB forces [N, 3] fp64 of the current positions (0 on fixed atoms)"""
         return self.neb.neb_forces.double()
 
-    def get_uncertainty(self) -> Dict[str, Tensor]:
-        """Ensemble runs: the unbiased std over the members of the energies [n_bands * n_images] and forces [N, 3] of
-        the interior images"""
-        return _ensemble_uncertainty(self)
-
-    @property
-    def fmax(self) -> Tensor:
-        """largest NEB force per band [n_bands] fp64 (the quantity the convergence test compares with ``fmax``)"""
-        return self.opt.fmax
-
-    @property
-    def converged(self) -> Tensor:
-        return self.opt.converged.bool()
-
-    @property
-    def steps_to_converge(self) -> Tensor:
-        """[n_bands] the step count at which each band met the criterion (-1 while it has not)"""
-        return self.opt.steps_to_converge
-
     def state_dict(self) -> Dict[str, object]:
-        """Everything a restart needs to continue bitwise."""
-        return dict(_clone_state(self._step_state()), iterations=self.iterations, nsteps=self.nsteps,
-                    climb_on=self.climb)
+        return dict(super().state_dict(), climb_on=self.climb)
 
     def load_state_dict(self, state: Dict[str, object]):
-        """Copy a ``state_dict`` into the existing buffers (a captured graph stays valid)."""
-        _load_state(self._step_state(), state)
-        self.iterations = int(state["iterations"])
-        self.nsteps = int(state["nsteps"])
+        super().load_state_dict(state)
         self.climb = bool(state["climb_on"])

@@ -52,19 +52,38 @@ def _fixed_mask(fixed_atoms_mask, n_atoms: int, dev) -> Optional[Tensor]:
     return out.to(torch.uint8).to(dev)
 
 
-def _ensemble_uncertainty(driver) -> Dict[str, Tensor]:
-    """the unbiased std over the ensemble members of the energies [n_sys] and forces [N, 3] at the current positions,
-    in optimizer units (BatchwiseEnsembleCalculator.calculate, :329-335)"""
-    if driver.ensemble is None:
-        raise RuntimeError(f"{type(driver).__name__}: get_uncertainty needs an ensemble (model=[m1, m2, ...])")
-    from .ensemble import ensemble_moments
+class _ConvergenceState(_TensorState):
+    """The convergence test's device buffers, which the optimizer kernels keep alike: the step counter pair, the fmax
+    target, the largest force, the converged flag and the step count at which it was met per system, and the count of
+    unconverged systems.  Subclasses set ``n_atoms`` and define ``tensors()``, every buffer a step writes."""
 
-    e = ensemble_moments(driver.stacks[driver.energy_key], ddof=1, spread_scale=driver.e_conv, var=False, std=True)[2]
-    f = ensemble_moments(driver.stacks[driver.force_key], ddof=1, spread_scale=driver.f_conv, var=False, std=True)[2]
-    return {"energy_uncertainty": e, "forces_uncertainty": f}
+    def _init_convergence(self, n_sys: int, fmax: float, dev):
+        self.counter = torch.zeros(2, dtype=torch.int64, device=dev)
+        self.fmax_target = torch.full((1,), float(fmax), dtype=torch.float64, device=dev)
+        self.fmax = torch.zeros(n_sys, dtype=torch.float64, device=dev)
+        self.converged = torch.zeros(n_sys, dtype=torch.int32, device=dev)
+        self.steps_to_converge = torch.full((n_sys,), -1, dtype=torch.int64, device=dev)
+        self.n_unconverged = torch.full((1,), n_sys, dtype=torch.int32, device=dev)
+
+    def _convergence_tensors(self) -> Dict[str, Tensor]:
+        return {"counter": self.counter, "fmax_target": self.fmax_target, "fmax": self.fmax,
+                "converged": self.converged, "steps_to_converge": self.steps_to_converge,
+                "n_unconverged": self.n_unconverged}
+
+    def _forces(self, forces: Tensor) -> Tensor:
+        f = ops.f32(forces, "forces")
+        if f.numel() != 3 * self.n_atoms:
+            raise ValueError(f"{type(self).__name__}: forces of {f.numel()} values for {self.n_atoms} atoms")
+        return f
+
+    def set_fmax(self, fmax: float):
+        self.fmax_target.fill_(float(fmax))
+
+    def _state(self) -> Dict[str, Tensor]:
+        return self.tensors()
 
 
-class LBFGSState(_TensorState):
+class LBFGSState(_ConvergenceState):
     """Optimizer state of a batch and the launches of its kernels (the step and the convergence test), given a forces
     tensor.  ``positions`` [N, 3] are the starting positions in optimizer units (model positions x
     ``position_conversion``); forces are model forces, multiplied by ``force_conversion`` in the kernels.  Systems are
@@ -92,12 +111,7 @@ class LBFGSState(_TensorState):
         self.y = torch.zeros_like(self.s)
         self.rho = torch.ones(self.memory, n_sys, **f64)
         self.p = torch.zeros_like(self.r)
-        self.counter = torch.zeros(2, dtype=torch.int64, device=dev)
-        self.fmax_target = torch.full((1,), float(fmax), **f64)
-        self.fmax = torch.zeros(n_sys, **f64)
-        self.converged = torch.zeros(n_sys, dtype=torch.int32, device=dev)
-        self.steps_to_converge = torch.full((n_sys,), -1, dtype=torch.int64, device=dev)
-        self.n_unconverged = torch.full((1,), n_sys, dtype=torch.int32, device=dev)
+        self._init_convergence(n_sys, fmax, dev)
         self.fixed = _fixed_mask(fixed_atoms_mask, n, dev)
         p_conv = float(position_conversion)
         if model_positions is None:
@@ -118,12 +132,6 @@ class LBFGSState(_TensorState):
             p(self.fixed), p(self.model_positions), p(self.sys_ptr), p(self.order), n, n_sys, self.n_warp,
             self.memory, float(force_conversion), p_conv, float(maxstep), float(damping), 1.0 / float(alpha))
 
-    def _forces(self, forces: Tensor) -> Tensor:
-        f = ops.f32(forces, "forces")
-        if f.numel() != 3 * self.n_atoms:
-            raise ValueError(f"LBFGSState: forces of {f.numel()} values for {self.n_atoms} atoms")
-        return f
-
     def check(self, forces: Tensor):
         """the convergence test of the forces at the current positions (fmax, converged, steps_to_converge and the
         unconverged count, on the device)"""
@@ -134,80 +142,65 @@ class LBFGSState(_TensorState):
         _lib.call("spk_relax_step", ctypes.byref(self._params), ops._p(self._forces(forces)), ops._stream(),
                   launches=int(self.n_warp > 0) + int(self.n_warp < self.n_sys))
 
-    def set_fmax(self, fmax: float):
-        self.fmax_target.fill_(float(fmax))
-
     def tensors(self) -> Dict[str, Tensor]:
         """every buffer the step writes"""
         return {"r": self.r, "r0": self.r0, "f0": self.f0, "s": self.s, "y": self.y, "rho": self.rho, "p": self.p,
-                "counter": self.counter, "fmax_target": self.fmax_target, "fmax": self.fmax,
-                "converged": self.converged, "steps_to_converge": self.steps_to_converge,
-                "n_unconverged": self.n_unconverged, "model_positions": self.model_positions}
-
-    def _state(self) -> Dict[str, Tensor]:
-        return self.tensors()
+                **self._convergence_tensors(), "model_positions": self.model_positions}
 
 
-class DeviceLBFGS(_CapturedEvaluation):
-    """Relax every system of ``batch`` with the reference's batchwise L-BFGS (keywords and defaults of
-    ASEBatchwiseLBFGS; ``alpha`` gives H0 = 1 / alpha).  ``batch[_positions]`` is in model units;
-    ``position_conversion`` and ``energy_conversion`` turn model lengths and energies into the optimizer's units (Angstrom
-    and eV in the reference), so ``maxstep`` and ``fmax`` are in those.  ``fixed_atoms_mask`` (boolean mask or atom
-    indices) zeroes the forces of atoms that must not move.  ``cutoff`` and ``capacity`` size the device neighbour list,
-    which is rebuilt at every step.
+class _BatchOptimizer(_CapturedEvaluation):
+    """The driver of a batchwise optimizer in the captured step: ``self.opt`` (a ``_ConvergenceState``) holds the
+    optimizer state and the convergence buffers.  A driver defines ``_advance()``, its optimizer step, and ``_check()``,
+    the force side and convergence test on the current evaluation; one step is ``_advance()``, the evaluation and
+    ``_check()``.  Results are in optimizer units."""
 
-    One step is the optimizer kernels, the neighbour list, the model and the convergence test, captured once as a CUDA
-    graph (``use_graph``).  ``run`` replays it in chunks of ``check_every`` steps and reads the count of unconverged
-    systems once per chunk; steps replayed after every system has converged leave the positions bitwise unchanged.
-
-    ``model`` may be a list (or ``nn.ModuleList``) of at least two members, as the reference's
-    BatchwiseEnsembleCalculator (interfaces/batchwise_optimization.py:229-347): the mean forces drive the optimizer
-    and its ``fmax`` test, and ``get_uncertainty`` gives the unbiased std over the members."""
-
-    def __init__(self, model: torch.nn.Module, batch: Dict[str, Tensor], cutoff: float, capacity: int,
-                 maxstep: float = 0.2, memory: int = 100, damping: float = 1.0, alpha: float = 70.0,
-                 fixed_atoms_mask=None, position_conversion: float = 1.0, energy_conversion: float = 1.0,
-                 energy_key: str = P.energy, force_key: str = P.forces, use_graph: bool = True):
-        if float(maxstep) > 1.0:                                                 # batchwise_optimization.py:711-715
-            raise ValueError("You are using a much too large value for the maximum step size: %.1f Angstrom"
-                             % float(maxstep))
+    def _check_outputs(self, model, energy_key: str, force_key: str):
+        """refuse a model that does not output both keys, and take them as the evaluation's keys"""
         outputs = getattr(model, "model_outputs", None)
         if outputs is not None and (force_key not in outputs or energy_key not in outputs):
-            raise ValueError(f"DeviceLBFGS: the model must output '{energy_key}' and '{force_key}' (it outputs "
+            raise ValueError(f"{type(self).__name__}: the model must output '{energy_key}' and '{force_key}' (it outputs "
                              f"{sorted(outputs)})")
         self.energy_key, self.force_key = energy_key, force_key
-        idx_m, n_sys = self._setup(model, batch, cutoff, capacity, use_graph)
+
+    def _set_conversions(self, position_conversion: float, energy_conversion: float):
         self.p_conv = float(position_conversion)
         self.e_conv = float(energy_conversion)
         self.f_conv = self.e_conv / self.p_conv
+
+    def _fp32_positions(self) -> Tensor:
+        """the model positions ``static[_positions]``, checked to be a contiguous fp32 tensor"""
         mp = self.static[P.R]
         if mp.dtype != torch.float32 or not mp.is_contiguous():
-            raise ValueError("DeviceLBFGS: '_positions' must be a contiguous float32 tensor")
-        self.opt = LBFGSState(mp.double() * self.p_conv, idx_m, n_sys, memory=memory, maxstep=maxstep,
-                              damping=damping, alpha=alpha, fixed_atoms_mask=fixed_atoms_mask,
-                              position_conversion=self.p_conv, force_conversion=self.f_conv, model_positions=mp)
+            raise ValueError(f"{type(self).__name__}: '_positions' must be a contiguous float32 tensor")
+        return mp
+
+    def _start(self):
+        """the step counts and the convergence test of the starting positions"""
         self.iterations = 0                      # steps taken (host mirror of the device counter)
         self.nsteps = 0
         self._calculate()                        # forces of the starting positions (irun, :417)
-        self.opt.check(self.forces)
+        self._check()
 
     def _step(self):
-        self.opt.step(self.forces)
+        self._advance()
         self._calculate()
-        self.opt.check(self.forces)
+        self._check()
 
     def _step_state(self) -> Dict[str, object]:
-        return dict(opt=self.opt.tensors(), **self._evaluation_state())
+        state = dict(opt=self.opt.tensors(), **self._evaluation_state())
+        if self.virial is not None:
+            state["virial"] = self.virial
+        return state
 
     def run(self, fmax: float = 0.05, steps: Optional[int] = None, check_every: int = 10) -> bool:
         """Relax until every system's largest force is below ``fmax`` or ``steps`` steps (default: unlimited) were taken
         in this call; returns whether every system converged.  ``nsteps`` is then the step count at which the reference's
         loop would have stopped."""
         if int(check_every) < 1:
-            raise ValueError("DeviceLBFGS: check_every must be >= 1")
+            raise ValueError(f"{type(self).__name__}: check_every must be >= 1")
         budget = DEFAULT_MAX_STEPS if not steps else int(steps)
         self.opt.set_fmax(fmax)
-        self.opt.check(self.forces)              # the convergence test under this fmax
+        self._check()                            # the convergence test under this fmax
         done = 0
         left = int(self.opt.n_unconverged.item())
         while left and done < budget:
@@ -231,10 +224,6 @@ class DeviceLBFGS(_CapturedEvaluation):
         """[N, 3] fp32 positions the model reads (positions / position_conversion)"""
         return self.static[P.R]
 
-    def get_energy(self) -> Tensor:
-        """energies of the current positions [n_sys] in optimizer units"""
-        return self.energy * self.e_conv
-
     def get_forces(self) -> Tensor:
         """forces of the current positions [N, 3] fp64 in optimizer units, zero on fixed atoms (get_forces, :182-198)"""
         f = self.forces.double() * self.f_conv
@@ -245,7 +234,13 @@ class DeviceLBFGS(_CapturedEvaluation):
     def get_uncertainty(self) -> Dict[str, Tensor]:
         """Ensemble runs: the unbiased std over the members of the energies [n_sys] and forces [N, 3] at the current
         positions, in optimizer units (BatchwiseEnsembleCalculator.calculate, :329-335)"""
-        return _ensemble_uncertainty(self)
+        if self.ensemble is None:
+            raise RuntimeError(f"{type(self).__name__}: get_uncertainty needs an ensemble (model=[m1, m2, ...])")
+        from .ensemble import ensemble_moments
+
+        e = ensemble_moments(self.stacks[self.energy_key], ddof=1, spread_scale=self.e_conv, var=False, std=True)[2]
+        f = ensemble_moments(self.stacks[self.force_key], ddof=1, spread_scale=self.f_conv, var=False, std=True)[2]
+        return {"energy_uncertainty": e, "forces_uncertainty": f}
 
     @property
     def fmax(self) -> Tensor:
@@ -270,6 +265,49 @@ class DeviceLBFGS(_CapturedEvaluation):
         _load_state(self._step_state(), state)
         self.iterations = int(state["iterations"])
         self.nsteps = int(state["nsteps"])
+
+
+class DeviceLBFGS(_BatchOptimizer):
+    """Relax every system of ``batch`` with the reference's batchwise L-BFGS (keywords and defaults of
+    ASEBatchwiseLBFGS; ``alpha`` gives H0 = 1 / alpha).  ``batch[_positions]`` is in model units;
+    ``position_conversion`` and ``energy_conversion`` turn model lengths and energies into the optimizer's units (Angstrom
+    and eV in the reference), so ``maxstep`` and ``fmax`` are in those.  ``fixed_atoms_mask`` (boolean mask or atom
+    indices) zeroes the forces of atoms that must not move.  ``cutoff`` and ``capacity`` size the device neighbour list,
+    which is rebuilt at every step.
+
+    One step is the optimizer kernels, the neighbour list, the model and the convergence test, captured once as a CUDA
+    graph (``use_graph``).  ``run`` replays it in chunks of ``check_every`` steps and reads the count of unconverged
+    systems once per chunk; steps replayed after every system has converged leave the positions bitwise unchanged.
+
+    ``model`` may be a list (or ``nn.ModuleList``) of at least two members, as the reference's
+    BatchwiseEnsembleCalculator (interfaces/batchwise_optimization.py:229-347): the mean forces drive the optimizer
+    and its ``fmax`` test, and ``get_uncertainty`` gives the unbiased std over the members."""
+
+    def __init__(self, model: torch.nn.Module, batch: Dict[str, Tensor], cutoff: float, capacity: int,
+                 maxstep: float = 0.2, memory: int = 100, damping: float = 1.0, alpha: float = 70.0,
+                 fixed_atoms_mask=None, position_conversion: float = 1.0, energy_conversion: float = 1.0,
+                 energy_key: str = P.energy, force_key: str = P.forces, use_graph: bool = True):
+        if float(maxstep) > 1.0:                                                 # batchwise_optimization.py:711-715
+            raise ValueError("You are using a much too large value for the maximum step size: %.1f Angstrom"
+                             % float(maxstep))
+        self._check_outputs(model, energy_key, force_key)
+        idx_m, n_sys = self._setup(model, batch, cutoff, capacity, use_graph)
+        self._set_conversions(position_conversion, energy_conversion)
+        mp = self._fp32_positions()
+        self.opt = LBFGSState(mp.double() * self.p_conv, idx_m, n_sys, memory=memory, maxstep=maxstep,
+                              damping=damping, alpha=alpha, fixed_atoms_mask=fixed_atoms_mask,
+                              position_conversion=self.p_conv, force_conversion=self.f_conv, model_positions=mp)
+        self._start()
+
+    def _advance(self):
+        self.opt.step(self.forces)
+
+    def _check(self):
+        self.opt.check(self.forces)
+
+    def get_energy(self) -> Tensor:
+        """energies of the current positions [n_sys] in optimizer units"""
+        return self.energy * self.e_conv
 
 
 # ---- FIRE and the unit-cell filter -------------------------------------------------------------------------------------
@@ -320,7 +358,7 @@ def _check_fire_keywords(kw: Dict[str, float]):
         raise ValueError(f"FIRE: Nmin must be a non-negative integer, got {kw['Nmin']}")
 
 
-class FIREState(_TensorState):
+class FIREState(_ConvergenceState):
     """FIRE state of a batch and the launches of its kernels, given a forces tensor (and, with ``cell_filter``, the fp64
     model virial [n_sys, 3, 3]).  ``positions`` [N, 3] are the starting positions in optimizer units (model positions x
     ``position_conversion``), ``cell`` [n_sys, 3, 3] the starting cells in the same units (needed with the filter);
@@ -362,12 +400,7 @@ class FIREState(_TensorState):
         self.coef = torch.zeros(n_sys, _lib.FIRE_COEF, **f64)
         nbytes = int(_lib.lib().spk_fire_workspace_bytes(n, n_sys))
         self.workspace = torch.zeros(max(nbytes // 8, 1), **f64)
-        self.counter = torch.zeros(2, dtype=torch.int64, device=dev)
-        self.fmax_target = torch.full((1,), float(fmax), **f64)
-        self.fmax = torch.zeros(n_sys, **f64)
-        self.converged = torch.zeros(n_sys, dtype=torch.int32, device=dev)
-        self.steps_to_converge = torch.full((n_sys,), -1, dtype=torch.int64, device=dev)
-        self.n_unconverged = torch.full((1,), n_sys, dtype=torch.int32, device=dev)
+        self._init_convergence(n_sys, fmax, dev)
         self.fixed = _fixed_mask(fixed_atoms_mask, n, dev)
         if model_positions is None:
             model_positions = (self.s / p_conv).float()
@@ -408,9 +441,7 @@ class FIREState(_TensorState):
     def check(self, forces: Tensor, virial: Optional[Tensor] = None):
         """the generalized forces at the current positions and the convergence test (fmax, converged,
         steps_to_converge and the unconverged count, on the device)"""
-        f = ops.f32(forces, "forces")
-        if f.numel() != 3 * self.n_atoms:
-            raise ValueError(f"FIREState: forces of {f.numel()} values for {self.n_atoms} atoms")
+        f = self._forces(forces)
         w = None
         if self.filter is not None:
             if (virial is None or virial.dtype != torch.float64 or not virial.is_contiguous()
@@ -423,9 +454,6 @@ class FIREState(_TensorState):
     def step(self):
         """one FIRE step with the generalized forces of the last ``check``"""
         _lib.call("spk_fire_step", ctypes.byref(self._params), ops._stream(), launches=1 + int(self.n_atoms > 0))
-
-    def set_fmax(self, fmax: float):
-        self.fmax_target.fill_(float(fmax))
 
     def deformation_gradient(self) -> Optional[Tensor]:
         """F [n_sys, 3, 3] fp64 (cell = cell0 F^T), None without a filter"""
@@ -442,18 +470,14 @@ class FIREState(_TensorState):
     def tensors(self) -> Dict[str, Tensor]:
         """every buffer the step and the force side write and a later step reads"""
         out = {"s": self.s, "v": self.v, "g": self.g, "dt": self.dt, "a": self.a, "nsteps": self.nsteps,
-               "started": self.started, "sums": self.sums, "counter": self.counter, "fmax_target": self.fmax_target,
-               "fmax": self.fmax, "converged": self.converged, "steps_to_converge": self.steps_to_converge,
-               "n_unconverged": self.n_unconverged, "model_positions": self.model_positions}
+               "started": self.started, "sums": self.sums, **self._convergence_tensors(),
+               "model_positions": self.model_positions}
         if self.filter is not None:
             out.update(r=self.r, h=self.h, hv=self.hv, hg=self.hg, model_cell=self.model_cell)
         return out
 
-    def _state(self) -> Dict[str, Tensor]:
-        return self.tensors()
 
-
-class DeviceFIRE(_CapturedEvaluation):
+class DeviceFIRE(_BatchOptimizer):
     """Relax every system of ``batch`` with ASE's FIRE (its keywords and defaults; no ``downhill_check``), one optimizer
     per system, with the batch semantics of ``DeviceLBFGS``: a system whose largest (generalized) force is below
     ``fmax`` takes no step and keeps its optimizer state, and systems may differ in size.  ``batch[_positions]`` (and
@@ -468,7 +492,9 @@ class DeviceFIRE(_CapturedEvaluation):
 
     One step is the optimizer kernels, the neighbour list, the model and the convergence test, captured once as a CUDA
     graph (``use_graph``).  ``model`` may be a list of at least two members: their mean forces drive a fixed-cell
-    relaxation and ``get_uncertainty`` gives the unbiased std over the members, as in ``DeviceLBFGS``."""
+    relaxation and ``get_uncertainty`` gives the unbiased std over the members, as in ``DeviceLBFGS``.  ``fmax`` is the
+    largest generalized force per system (atom rows and, under the filter, cell rows); ``positions`` and ``get_forces``
+    are Cartesian."""
 
     def __init__(self, model: torch.nn.Module, batch: Dict[str, Tensor], cutoff: float, capacity: int,
                  dt: float = 0.1, maxstep: float = 0.2, dtmax: float = 1.0, Nmin: int = 5, finc: float = 1.1,
@@ -480,21 +506,13 @@ class DeviceFIRE(_CapturedEvaluation):
                                   astart=astart, fa=fa, a=a))
         if cell_filter is not None and not isinstance(cell_filter, UnitCellFilter):
             raise TypeError("DeviceFIRE: cell_filter must be a UnitCellFilter")
-        outputs = getattr(model, "model_outputs", None)
-        if outputs is not None and (force_key not in outputs or energy_key not in outputs):
-            raise ValueError(f"DeviceFIRE: the model must output '{energy_key}' and '{force_key}' (it outputs "
-                             f"{sorted(outputs)})")
-        self.energy_key, self.force_key = energy_key, force_key
+        self._check_outputs(model, energy_key, force_key)
         idx_m, n_sys = self._setup(model, batch, cutoff, capacity, use_graph)
         if cell_filter is not None and self.ensemble is not None:
             raise NotImplementedError("DeviceFIRE: a cell filter needs the stress, which an ensemble does not have (the "
                                       "reference's EnsembleCalculator._activate_stress raises)")
-        self.p_conv = float(position_conversion)
-        self.e_conv = float(energy_conversion)
-        self.f_conv = self.e_conv / self.p_conv
-        mp = self.static[P.R]
-        if mp.dtype != torch.float32 or not mp.is_contiguous():
-            raise ValueError("DeviceFIRE: '_positions' must be a contiguous float32 tensor")
+        self._set_conversions(position_conversion, energy_conversion)
+        mp = self._fp32_positions()
         cell = model_cell = None
         if cell_filter is not None:
             model_cell = self._setup_virial(n_sys, "a cell filter")
@@ -505,53 +523,15 @@ class DeviceFIRE(_CapturedEvaluation):
                              cell=cell, cell_filter=cell_filter, position_conversion=self.p_conv,
                              force_conversion=self.f_conv, energy_conversion=self.e_conv, model_positions=mp,
                              model_cell=model_cell)
-        self.iterations = 0
-        self.nsteps = 0
-        self._calculate()
-        self.opt.check(self.forces, self.virial)
+        self._start()
 
-    def _step(self):
+    def _advance(self):
         self.opt.step()
-        self._calculate()
-        self.opt.check(self.forces, self.virial)
 
-    def _step_state(self) -> Dict[str, object]:
-        state = dict(opt=self.opt.tensors(), **self._evaluation_state())
-        if self.virial is not None:
-            state["virial"] = self.virial
-        return state
-
-    def run(self, fmax: float = 0.05, steps: Optional[int] = None, check_every: int = 10) -> bool:
-        """Relax until every system's largest generalized force is below ``fmax`` or ``steps`` steps (default:
-        unlimited) were taken in this call; returns whether every system converged."""
-        if int(check_every) < 1:
-            raise ValueError("DeviceFIRE: check_every must be >= 1")
-        budget = DEFAULT_MAX_STEPS if not steps else int(steps)
-        self.opt.set_fmax(fmax)
+    def _check(self):
         self.opt.check(self.forces, self.virial)
-        done = 0
-        left = int(self.opt.n_unconverged.item())
-        while left and done < budget:
-            k = min(int(check_every), budget - done)
-            self._run_steps(k)
-            done += k
-            self.iterations += k
-            left = int(self.opt.n_unconverged.item())
-        self.check_neighbor_list()
-        self.nsteps = int(self.opt.steps_to_converge.max().item()) if left == 0 else self.iterations
-        return left == 0
 
     # ---- results, in optimizer units ----------------------------------------------------------------------------------
-    @property
-    def positions(self) -> Tensor:
-        """[N, 3] fp64 positions"""
-        return self.opt.r
-
-    @property
-    def model_positions(self) -> Tensor:
-        """[N, 3] fp32 positions the model reads (positions / position_conversion)"""
-        return self.static[P.R]
-
     @property
     def cell(self) -> Optional[Tensor]:
         """[n_sys, 3, 3] fp64 cells (rows = lattice vectors) under a cell filter, else None"""
@@ -560,13 +540,6 @@ class DeviceFIRE(_CapturedEvaluation):
     def get_energy(self) -> Tensor:
         """energies of the current positions [n_sys]"""
         return self.energy * self.e_conv
-
-    def get_forces(self) -> Tensor:
-        """Cartesian forces of the current positions [N, 3] fp64, zero on fixed atoms"""
-        f = self.forces.double() * self.f_conv
-        if self.opt.fixed is not None:
-            f = f * (1 - self.opt.fixed.double())[:, None]
-        return f
 
     def get_stress(self) -> Tensor:
         """stress of the current cells [n_sys, 3, 3] fp64: the symmetric part of W / V (cell filter only)"""
@@ -581,31 +554,3 @@ class DeviceFIRE(_CapturedEvaluation):
         if self.opt.filter is None:
             return e
         return e + self.opt.filter.scalar_pressure * torch.linalg.det(self.cell).abs()
-
-    def get_uncertainty(self) -> Dict[str, Tensor]:
-        """Ensemble runs: the unbiased std over the members of the energies [n_sys] and forces [N, 3]"""
-        return _ensemble_uncertainty(self)
-
-    @property
-    def fmax(self) -> Tensor:
-        """largest generalized force per system [n_sys] fp64 (the quantity the convergence test compares with fmax)"""
-        return self.opt.fmax
-
-    @property
-    def converged(self) -> Tensor:
-        return self.opt.converged.bool()
-
-    @property
-    def steps_to_converge(self) -> Tensor:
-        """[n_sys] the step count at which each system met the criterion (-1 while it has not)"""
-        return self.opt.steps_to_converge
-
-    def state_dict(self) -> Dict[str, object]:
-        """Everything a restart needs to continue bitwise."""
-        return dict(_clone_state(self._step_state()), iterations=self.iterations, nsteps=self.nsteps)
-
-    def load_state_dict(self, state: Dict[str, object]):
-        """Copy a ``state_dict`` into the existing buffers (a captured graph stays valid)."""
-        _load_state(self._step_state(), state)
-        self.iterations = int(state["iterations"])
-        self.nsteps = int(state["nsteps"])
