@@ -895,19 +895,22 @@ int spk_ensemble_uncertainty(const float* energy, double energy_scale, const dou
  * coordinates d = 3 a + k) from C = n_cols * nfree replica-major copies: copy c = d_local * nfree + s holds atoms
  * [c N, (c+1) N) and systems [c B, (c+1) B) and displaces coordinate d = chunk * n_cols + d_local of every system by
  * (float)(o_s * delta), o = (-1, +1) for nfree 2 and (-2, -1, +1, +2) for nfree 4; systems with d >= 3 n_m stay
- * undisplaced in that copy (idle).  counter (int64[2]) = (chunk the next displacement reads, chunk the last displacement
- * wrote + 1); zero it before the first chunk.
+ * undisplaced in that copy (idle).  n_displaced (int64[B], optional) restricts the displaced coordinates of system m to
+ * those of its first n_displaced[m] atoms, d < 3 n_displaced[m] (NULL: all n_m atoms).  counter (int64[2]) = (chunk the
+ * next displacement reads, chunk the last displacement wrote + 1); zero it before the first chunk.
  *
  * spk_vib_displace: positions [C N, 3] = base with the displacement rounded to fp32 (__fadd_rn); steps [C, B] fp64 =
  *   (double)displaced - (double)base of the displaced coordinate (0 for idle copies); counter[1] = counter[0] + 1.
  * spk_vib_assemble, after the model wrote forces [C N, 3] (and dipole [C B, 3] / polar [C B, 3, 3]): for chunk =
  *   counter[1] - 1 and every non-idle (system, d): with w_s the weights of the derivative at 0 of the polynomial through
  *   (steps[c_s, m], y_s), h_raw[hess_ptr[m] + d 3 n_m + r] = -sum_s w_s forces_r (column d, stored transposed),
+ *   for d < 3 n_displaced[m] (the block of system m then holds 9 n_displaced[m] n_m values),
  *   dipole_deriv [N, 3, 3] element [i, comp, dir] and polar_deriv [N, 3, 3, 3] element [i, a, b, dir] (each optional)
  *   = sum_s w_s y_s with atom i = sys_ptr[m] + d / 3, dir = d % 3; counter[0] = counter[1].
  * spk_vib_finish, once after the last chunk: H = (h_raw + h_raw^T) / 2 per system; hessian [sum n_m^2, 3, 3] fp64 in
  *   the Response layout (row i n_m + j, block [a, b] = H[3 i + a, 3 j + b]) at hess_ptr[m] (= 9 sum_{m' < m} n_m'^2) and
  *   hessian_mw [3 n_m, 3 n_m] at the same offset = H * mw_scale / sqrt(masses[i] masses[j]).  max_atoms = max_m n_m.
+ *   Needs n_displaced == NULL.
  * No atomics; every value is written once: bitwise reproducible. */
 typedef struct {
     const float* base;         /* [N, 3] undisplaced model positions */
@@ -919,9 +922,10 @@ typedef struct {
     const float* polar;        /* [C B, 3, 3] or NULL */
     const int64_t* idx_m;      /* [N] */
     const int32_t* sys_ptr;    /* [B + 1] */
+    const int64_t* n_displaced;   /* [B] displaced atoms per system (the first ones), or NULL: all */
     const int64_t* hess_ptr;   /* [B + 1] */
     const double* masses;      /* [N] */
-    double* h_raw;             /* [sum 9 n_m^2] */
+    double* h_raw;             /* [sum 9 n_m^2], or [sum 9 n_displaced[m] n_m] */
     double* hessian;           /* [sum n_m^2, 3, 3] */
     double* hessian_mw;        /* [sum 9 n_m^2] */
     double* dipole_deriv;      /* [N, 3, 3] or NULL */
@@ -933,6 +937,70 @@ typedef struct {
 int spk_vib_displace(const spk_vib_t* params, spk_stream_t stream);
 int spk_vib_assemble(const spk_vib_t* params, spk_stream_t stream);
 int spk_vib_finish(const spk_vib_t* params, spk_stream_t stream);
+
+/* ---- phonons of crystals (csrc/phonons.cu; the method of ASE's Phonons) ------------------------------------------------
+ * System m (of B) has n_m primitive atoms [prim_ptr[m], prim_ptr[m+1]) and a supercell of L = n_cells primitive cells
+ * (supercell matrix M, rows of the supercell = M . cell); supercell atom j = l n_m + b is primitive atom b translated by
+ * lattice[l] (int32 [L, 3], lattice[0] = 0), and neg[l] is the index of -lattice[l] modulo the supercell.  Row
+ * fc_ptr[m] + a n_m L + j (fc_ptr[m] = sum_{m' < m} n_m'^2 L, n_rows = fc_ptr[B]) holds the block Phi(a, 0; j) [3, 3].
+ *
+ * spk_ph_force_constants: h_raw = the finite differences of spk_vib_assemble with n_displaced[m] = n_m (per system rows
+ *   d = 3 a + alpha of 3 n_m L columns, at 9 fc_ptr[m]) -> force_constants [n_rows, 3, 3] after `rounds` rounds of:
+ *   Phi(a, 0; b, l) <- (Phi(a, 0; b, l) + Phi(b, 0; a, neg[l])^T) / 2, then, if acoustic, Phi(a, 0; a, 0) -= sum_j
+ *   Phi(a, 0; j) (the sum in ascending j).  Without acoustic at most one round runs (a second one is the identity).
+ *   work: [n_rows, 3, 3] scratch.  1 + rounds launches.
+ * spk_ph_images: for every row, the supercell-lattice images of atom j closest to atom a (positions [N_prim, 3], cell
+ *   [B, 3, 3] primitive rows, super_cell / super_inv [B, 3, 3] = M . cell and its inverse, heights [B, 3] = the
+ *   supercell's plane spacings, all fp64): the images within tie_tol of the shortest distance; img_count[row] = their
+ *   number (may exceed SPK_PH_MAX_IMAGES: then only the first SPK_PH_MAX_IMAGES are stored and the table is unusable),
+ *   img_lattice [n_rows, SPK_PH_MAX_IMAGES, 3] = their primitive lattice translations.
+ * spk_ph_dynmat: dyn [n_q, dyn_ptr[B]] complex128 (re, im), system m at dyn_ptr[m] (= 9 sum_{m' < m} n_m'^2) as
+ *   [3 n_m, 3 n_m]: D_{a alpha, b beta}(q) = sum_l sum_images Phi(a, 0; l n_m + b)[alpha, beta] e^{2 pi i q . n_image}
+ *   / img_count * mw_scale / sqrt(masses[a] masses[b]) for q [n_q, 3] in reduced reciprocal coordinates.  max_atoms =
+ *   max_m n_m.
+ * spk_ph_dos: out [B, n_grid] = sum_{q, k} exp(-(grid - freq[q, 3 prim_ptr[m] + k])^2 / (2 width^2)) / (width sqrt(2 pi)
+ *   n_q) over the 3 n_m modes of system m; freq [n_q, n_modes], n_modes = 3 prim_ptr[B].  Fixed loop order (q, k).
+ * spk_ph_thermo: per segment s = t B + m (items [seg_ptr[s], seg_ptr[s+1]) = the n_q 3 n_m modes of system m, n_items =
+ *   seg_ptr[n_temps B]): out [n_temps B, 6] = per primitive cell, with e = freq ev_per_invcm, x = e / (k_b T):
+ *   (sum e / 2, sum e / 2 + k_b T ln(1 - e^-x), k_b sum (x / (e^x - 1) - ln(1 - e^-x)), k_b sum (x / (2 sinh(x/2)))^2) / n_q
+ *   over the modes with freq >= min_freq (T = 0: zero-point terms only), then the number of modes left out and of those
+ *   with freq < 0.  Segmented fp64 sums of segscan.cuh (2 launches) in spk_ph_thermo_workspace_bytes(n_items, n_temps B)
+ *   bytes of workspace.
+ * No atomics; every value is written once: bitwise reproducible. */
+#define SPK_PH_MAX_IMAGES 8
+typedef struct {
+    const double* h_raw;       /* [9 n_rows] finite differences (spk_vib_assemble) */
+    double* force_constants;   /* [n_rows, 3, 3] */
+    double* work;              /* [n_rows, 3, 3] */
+    const int32_t* prim_ptr;   /* [B + 1] */
+    const int64_t* fc_ptr;     /* [B + 1] */
+    const int32_t* lattice;    /* [L, 3] */
+    const int32_t* neg;        /* [L] */
+    const double* positions;   /* [N_prim, 3] primitive positions */
+    const double* cell;        /* [B, 3, 3] */
+    const double* super_cell;  /* [B, 3, 3] */
+    const double* super_inv;   /* [B, 3, 3] */
+    const double* heights;     /* [B, 3] */
+    const double* masses;      /* [N_prim] */
+    int32_t* img_count;        /* [n_rows] */
+    int32_t* img_lattice;      /* [n_rows, SPK_PH_MAX_IMAGES, 3] */
+    int32_t supercell[9];      /* M, row-major */
+    int64_t n_sys, n_prim, n_rows, n_cells, max_atoms, rounds;
+    int32_t acoustic, reserved;
+    double tie_tol;            /* model length units */
+    double mw_scale;           /* energy_conversion / position_conversion^2 */
+} spk_ph_t;
+int spk_ph_force_constants(const spk_ph_t* params, spk_stream_t stream);
+int spk_ph_images(const spk_ph_t* params, spk_stream_t stream);
+int spk_ph_dynmat(const spk_ph_t* params, const double* q, int64_t n_q, const int64_t* dyn_ptr, void* dyn,
+                  spk_stream_t stream);
+int spk_ph_dos(const double* freq, int64_t n_q, int64_t n_modes, const int32_t* prim_ptr, int64_t n_sys,
+               const double* grid, int64_t n_grid, double width, double* out, spk_stream_t stream);
+size_t spk_ph_thermo_workspace_bytes(int64_t n_items, int64_t n_seg);
+int spk_ph_thermo(const double* freq, int64_t n_q, int64_t n_modes, const int32_t* prim_ptr, int64_t n_sys,
+                  const double* temperatures, int64_t n_temps, const int32_t* seg_ptr, int64_t n_items, double min_freq,
+                  double ev_per_invcm, double k_b, double* out, void* workspace, size_t workspace_bytes,
+                  spk_stream_t stream);
 
 /* ---- vibrational spectra from recorded MD series (csrc/spectra.cu; md/data/spectra.py) ------------------------------
  * spk_spectrum_series: records [T, P, stride] fp32 (P replicas).  Output field f (of F) is

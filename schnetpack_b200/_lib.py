@@ -67,10 +67,26 @@ class VibParams(Structure):
     """spk_vib_t of include/spk_b200.h (device pointers of the replica batch and the vibrational-analysis buffers)."""
     _fields_ = [("base", c_void_p), ("positions", c_void_p), ("steps", c_void_p), ("counter", c_void_p),
                 ("forces", c_void_p), ("dipole", c_void_p), ("polar", c_void_p), ("idx_m", c_void_p),
-                ("sys_ptr", c_void_p), ("hess_ptr", c_void_p), ("masses", c_void_p), ("h_raw", c_void_p),
+                ("sys_ptr", c_void_p), ("n_displaced", c_void_p), ("hess_ptr", c_void_p), ("masses", c_void_p),
+                ("h_raw", c_void_p),
                 ("hessian", c_void_p), ("hessian_mw", c_void_p), ("dipole_deriv", c_void_p), ("polar_deriv", c_void_p),
                 ("n_atoms", c_int64), ("n_sys", c_int64), ("n_cols", c_int64), ("nfree", c_int64),
                 ("max_atoms", c_int64), ("delta", c_double), ("mw_scale", c_double)]
+
+
+class PhononParams(Structure):
+    """spk_ph_t of include/spk_b200.h (the supercell layout, force-constant and minimum-image buffers of a phonon run)."""
+    _fields_ = [("h_raw", c_void_p), ("force_constants", c_void_p), ("work", c_void_p), ("prim_ptr", c_void_p),
+                ("fc_ptr", c_void_p), ("lattice", c_void_p), ("neg", c_void_p), ("positions", c_void_p),
+                ("cell", c_void_p), ("super_cell", c_void_p), ("super_inv", c_void_p), ("heights", c_void_p),
+                ("masses", c_void_p), ("img_count", c_void_p), ("img_lattice", c_void_p), ("supercell", c_int32 * 9),
+                ("n_sys", c_int64), ("n_prim", c_int64), ("n_rows", c_int64), ("n_cells", c_int64),
+                ("max_atoms", c_int64), ("rounds", c_int64), ("acoustic", c_int32), ("reserved", c_int32),
+                ("tie_tol", c_double), ("mw_scale", c_double)]
+
+
+PH_MAX_IMAGES = 8           # SPK_PH_MAX_IMAGES
+PH_THERMO_FIELDS = 6        # spk_ph_thermo: zero-point energy, F, S, C_v, modes left out, imaginary modes
 
 
 class FIREState(Structure):
@@ -219,6 +235,13 @@ SIGNATURES = {
     "spk_vib_displace": [POINTER(VibParams), P],
     "spk_vib_assemble": [POINTER(VibParams), P],
     "spk_vib_finish": [POINTER(VibParams), P],
+    "spk_ph_force_constants": [POINTER(PhononParams), P],
+    "spk_ph_images": [POINTER(PhononParams), P],
+    "spk_ph_dynmat": [POINTER(PhononParams), P, c_int64, P, P, P],
+    "spk_ph_dos": [P, c_int64, c_int64, P, c_int64, P, c_int64, c_double, P, P],
+    "spk_ph_thermo_workspace_bytes": [c_int64, c_int64],
+    "spk_ph_thermo": [P, c_int64, c_int64, P, c_int64, P, c_int64, P, c_int64, c_double, c_double, c_double, P, P,
+                      c_size_t, P],
     "spk_md_record_velocities": [P, P, c_int64, P, c_int64, c_int64, P, P],
     "spk_spectrum_workspace_bytes": [c_int64, c_int64, c_int64],
     "spk_spectrum_series": [P, c_int64, c_int64, c_int64, P, P, c_int64, c_int, c_double, P, P, P, P],
@@ -257,7 +280,7 @@ _RESTYPE = {"spk_graph_workspace_bytes": c_size_t, "spk_tc_packed_floats": c_siz
             "spk_spectrum_workspace_bytes": c_size_t, "spk_fire_workspace_bytes": c_size_t,
             "spk_md_motion_workspace_bytes": c_size_t, "spk_spectrum_stream_state_bytes": c_size_t,
             "spk_spectrum_stream_finalise_workspace_bytes": c_size_t, "spk_neb_workspace_bytes": c_size_t,
-            "spk_pme_workspace_bytes": c_size_t}
+            "spk_pme_workspace_bytes": c_size_t, "spk_ph_thermo_workspace_bytes": c_size_t}
 
 _lib = None
 
@@ -305,8 +328,9 @@ LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out
             "spk_pairwise_virial_add": 2, "spk_spectrum_autocorrelation": 2, "spk_spectrum_transform": 2,
             "spk_fire_forces": 3, "spk_fire_step": 2, "spk_md_remove_motion": 3, "spk_spectrum_stream_push": 2,
             "spk_spectrum_stream_finalise": 2, "spk_neb_forces": 3, "spk_pme_spread": 8,
-            "spk_pme_energy": 2, "spk_pme_bwd": 2}
+            "spk_pme_energy": 2, "spk_pme_bwd": 2, "spk_ph_thermo": 2}
 # spk_pme_spread: 4 without atoms (cell, setup, scan, spread); spk_pme_bwd: 1 per part present (atoms, cell or virial);
+# spk_ph_force_constants: 1 + the rounds run;
 # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global; spk_md_initial_momenta: 4 if uniform
 MOTION_CENTER_OF_MASS, MOTION_TRANSLATION, MOTION_ROTATION = 1, 2, 4       # SPK_MOTION_*
 launch_count = 0

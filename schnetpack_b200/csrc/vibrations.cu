@@ -4,7 +4,9 @@
 //
 // The B-system batch is replicated replica-major into C = n_cols * nfree copies (copy c = d_local * nfree + s holds the
 // atoms [c N, (c+1) N) and the systems [c B, (c+1) B)).  Copy (d_local, s) displaces coordinate d = chunk * n_cols +
-// d_local of every system by stencil offset s; a system with d >= 3 n_m is left undisplaced in that copy (idle).  One
+// d_local of every system by stencil offset s; a system with d >= 3 n_m is left undisplaced in that copy (idle).  With
+// n_displaced given, only the first n_displaced[m] atoms of system m are displaced (phonons.py displaces the primitive
+// atoms of a supercell) and the Hessian columns run over their coordinates only.  One
 // chunk is: k_vib_displace, the model on the replica batch, k_vib_assemble.  The chunk index lives in a device counter
 // pair, so one captured step serves every chunk:
 //   counter[0] = the chunk the next displacement reads, counter[1] = the chunk the last displacement wrote plus one;
@@ -30,6 +32,11 @@ __device__ __forceinline__ float stencil_offset(int s, int nfree, double h) {
     return (float)((double)mult * h);
 }
 
+// atoms of system m whose coordinates are displaced: the first n_displaced[m], or all
+__device__ __forceinline__ int64_t displaced_atoms(const spk_vib_t& p, int64_t m, int64_t first) {
+    return p.n_displaced ? p.n_displaced[m] : p.sys_ptr[m + 1] - first;
+}
+
 __global__ void __launch_bounds__(VD_T) k_vib_displace(spk_vib_t p) {
     SPK_PDL_ENTER();
     const int64_t t = (int64_t)blockIdx.x * VD_T + threadIdx.x;
@@ -39,7 +46,7 @@ __global__ void __launch_bounds__(VD_T) k_vib_displace(spk_vib_t p) {
     if (t < C * N) {
         const int64_t c = t / N, a = t - c * N;
         const int64_t m = p.idx_m[a];
-        const int64_t first = p.sys_ptr[m], n_m = p.sys_ptr[m + 1] - first;
+        const int64_t first = p.sys_ptr[m], n_m = displaced_atoms(p, m, first);
         const int64_t d = chunk * p.n_cols + c / p.nfree;
         const int k = (d < 3 * n_m && a == first + d / 3) ? (int)(d % 3) : -1;     // the displaced component, if any
         const float off = stencil_offset((int)(c % p.nfree), p.nfree, p.delta);
@@ -51,7 +58,7 @@ __global__ void __launch_bounds__(VD_T) k_vib_displace(spk_vib_t p) {
     }
     if (t < C * B) {
         const int64_t c = t / B, m = t - c * B;
-        const int64_t first = p.sys_ptr[m], n_m = p.sys_ptr[m + 1] - first;
+        const int64_t first = p.sys_ptr[m], n_m = displaced_atoms(p, m, first);
         const int64_t d = chunk * p.n_cols + c / p.nfree;
         double step = 0.0;
         if (d < 3 * n_m) {
@@ -90,7 +97,7 @@ __device__ __forceinline__ void assemble_column(const spk_vib_t& p, int64_t chun
     const int64_t m = p.idx_m[a];
     const int64_t first = p.sys_ptr[m], n3 = 3 * (p.sys_ptr[m + 1] - first);
     const int64_t d = chunk * p.n_cols + d_local;
-    if (d >= n3) return;                                                    // idle copy of this system
+    if (d >= 3 * displaced_atoms(p, m, first)) return;                     // idle copy of this system
     double t[NF], w[NF];
     int64_t c[NF];
 #pragma unroll
@@ -192,7 +199,7 @@ extern "C" int spk_vib_assemble(const spk_vib_t* p, spk_stream_t stream) {
 
 extern "C" int spk_vib_finish(const spk_vib_t* p, spk_stream_t stream) {
     if (check_params(p) != SPK_OK || !p->h_raw || !p->hessian || !p->hessian_mw || (p->n_atoms > 0 && !p->masses) ||
-        p->max_atoms < 0)
+        p->max_atoms < 0 || p->n_displaced)         // the finish symmetrises square blocks: every atom displaced
         return SPK_ERR_ARG;
     const int64_t n3 = 3 * p->max_atoms;
     if (n3 == 0) return SPK_OK;

@@ -947,3 +947,45 @@ def vib_assemble(params: "_lib.VibParams"):
 def vib_finish(params: "_lib.VibParams"):
     """symmetrised Hessian in the Response layout and its mass-weighted blocks, once after the last chunk"""
     _lib.call("spk_vib_finish", ctypes.byref(params), _stream())
+
+
+# ------------------------------------------------------------------------------------------------------- phonons
+def ph_force_constants(params: "_lib.PhononParams", rounds: int):
+    """force constants in the block layout after ``rounds`` symmetrisation / sum-rule rounds (csrc/phonons.cu)"""
+    _lib.call("spk_ph_force_constants", ctypes.byref(params), _stream(), launches=1 + rounds)
+
+
+def ph_images(params: "_lib.PhononParams"):
+    """the minimum-image table of every force-constant row"""
+    _lib.call("spk_ph_images", ctypes.byref(params), _stream())
+
+
+def ph_dynmat(params: "_lib.PhononParams", q: Tensor, dyn_ptr: Tensor, n_el: int) -> Tensor:
+    """[Q, n_el] complex128 mass-weighted dynamical matrices at q [Q, 3] (reduced reciprocal coordinates); n_el =
+    dyn_ptr[-1], system m at dyn_ptr[m] as [3 n_m, 3 n_m]"""
+    q = q.to(torch.float64).contiguous()
+    out = torch.empty(q.shape[0], n_el, dtype=torch.complex128, device=q.device)
+    _lib.call("spk_ph_dynmat", ctypes.byref(params), _p(q), q.shape[0], _p(dyn_ptr), _p(out), _stream())
+    return out
+
+
+def ph_dos(freq: Tensor, prim_ptr: Tensor, grid: Tensor, width: float) -> Tensor:
+    """[B, G] Gaussian density of states of the frequencies [Q, 3 N_prim] on ``grid`` [G] (same unit as freq)"""
+    n_sys = prim_ptr.shape[0] - 1
+    out = torch.empty(n_sys, grid.shape[0], dtype=torch.float64, device=freq.device)
+    _lib.call("spk_ph_dos", _p(freq), freq.shape[0], freq.shape[1], _p(prim_ptr), n_sys, _p(grid), grid.shape[0],
+              float(width), _p(out), _stream())
+    return out
+
+
+def ph_thermo(freq: Tensor, prim_ptr: Tensor, temperatures: Tensor, seg_ptr: Tensor, n_items: int, min_freq: float,
+              ev_per_invcm: float, k_b: float) -> Tensor:
+    """[T B, 6] per-cell harmonic thermodynamics of the frequencies [Q, 3 N_prim] in cm^-1 (csrc/phonons.cu)"""
+    n_sys, n_t = prim_ptr.shape[0] - 1, temperatures.shape[0]
+    nbytes = _lib.lib().spk_ph_thermo_workspace_bytes(n_items, n_sys * n_t)
+    ws = torch.empty(-(-nbytes // 8), dtype=torch.float64, device=freq.device)
+    out = torch.empty(n_t * n_sys, _lib.PH_THERMO_FIELDS, dtype=torch.float64, device=freq.device)
+    _lib.call("spk_ph_thermo", _p(freq), freq.shape[0], freq.shape[1], _p(prim_ptr), n_sys, _p(temperatures), n_t,
+              _p(seg_ptr), n_items, float(min_freq), float(ev_per_invcm), float(k_b), _p(out), _p(ws), nbytes,
+              _stream())
+    return out

@@ -129,7 +129,7 @@ class DeviceVibrations(_CapturedEvaluation):
         self._params = _lib.VibParams(
             p(self.base_positions), p(self.static[P.R]), p(self.steps), p(self.counter), p(self.forces),
             p(self.outputs.get(P.dipole_moment)), p(self.outputs.get(P.polarizability)), p(self.idx_m),
-            p(self.sys_ptr), p(self.hess_ptr), p(self.masses), p(self.h_raw), p(self.hessian), p(self.hessian_mw),
+            p(self.sys_ptr), None, p(self.hess_ptr), p(self.masses), p(self.h_raw), p(self.hessian), p(self.hessian_mw),
             p(self.dipole_derivatives), p(self.polarizability_derivatives), n, n_sys, self.n_cols, self.nfree,
             self.max_atoms, self.delta / self.p_conv, self.e_conv / self.p_conv ** 2)
 
