@@ -8,16 +8,19 @@ reference's HDF5Loader takes for ``replica_idx=None``, so the reference runs in 
 Each file holds the records (rec:velocities [T, P, N, 3], rec:dipole_moment [T, P, B, 3], rec:polarizability
 [T, P, B, 3, 3]), sys_ptr, n_replicas, dt_fs and a JSON list of runs; run r of system m stores
 ``r{r}:m{m}:freq``, ``r{r}:m{m}:I{j}`` (the reference's intensities) and ``r{r}:m{m}:acf`` (``_compute_autocorrelations``
-of the reference's data, flattened to [F, n - 1]).
+of the reference's data, flattened to [F, n - 1]; spectra_long keeps its first min(resolution, n - 1) lags).
 
 Cases:
   * spectra_power: three ragged systems (3, 1 and 4 atoms), P = 4 replicas, at resolutions above and below n - 1;
   * spectra_ir: two systems, P = 1, resolution above and below n - 1;
   * spectra_raman: two systems, P = 2, averaged and not;
   * spectra_short: the shortest series (T = 3 for power, T = 5 for IR and Raman);
-  * spectra_zero: a zero-variance field (an atom at rest along x, a constant dipole component): NaN channels.
+  * spectra_zero: a zero-variance field (an atom at rest along x, a constant dipole component): NaN channels;
+  * spectra_long: T = 5200 records (three time chunks of the device autocorrelation), one atom and one dipole, P = 2;
+    power at resolution 5120 and IR at 1024 (both placements of the transform's cosine table), acf stored for the used
+    lags only.  It has its own generator, so it is made alone without rewriting the others.
 
-Run from the repository root:  python tests/golden/make_golden_spectra.py
+Run from the repository root:  python tests/golden/make_golden_spectra.py [case ...]  (default: every case)
 """
 import importlib
 import json
@@ -90,7 +93,8 @@ def signal(rng, T, shape, dt_fs, n_modes=4):
     return out.astype(np.float32)
 
 
-def run_case(mod, name, records, sys_ptr, n_replicas, runs):
+def run_case(mod, name, records, sys_ptr, n_replicas, runs, acf_lags=False):
+    """``acf_lags``: store only the lags the spectrum uses, acf[:, :min(resolution, n - 1)], not all n - 1"""
     loader = StubLoader(records, sys_ptr, DT_FS)
     out = {f"rec:{k}": v for k, v in records.items()}
     out.update(sys_ptr=np.asarray(sys_ptr, np.int64), n_replicas=np.int64(n_replicas), dt_fs=np.float64(DT_FS))
@@ -107,7 +111,8 @@ def run_case(mod, name, records, sys_ptr, n_replicas, runs):
                 data = spec._get_data(m)
                 acf = spec._compute_autocorrelations(data.copy())
                 spec.compute_spectrum(m)
-            out[f"r{r}:m{m}:acf"] = acf.reshape(-1, acf.shape[-1])
+            acf = acf.reshape(-1, acf.shape[-1])
+            out[f"r{r}:m{m}:acf"] = acf[:, :res] if acf_lags else acf
             out[f"r{r}:m{m}:freq"] = np.asarray(spec.frequencies[0])
             for j, v in enumerate(spec.intensities):
                 out[f"r{r}:m{m}:I{j}"] = np.asarray(v)
@@ -116,8 +121,28 @@ def run_case(mod, name, records, sys_ptr, n_replicas, runs):
     print("wrote", name, {k: v.shape for k, v in out.items() if k.startswith("rec:")})
 
 
-def main():
+def long_case(mod):
+    """one atom and one dipole, P = 2, T = 5200 records (three time chunks of the device autocorrelation): power at
+    resolution 5120 (the transform's cosine table in global memory) and IR at 1024 (in shared memory).  The records
+    sit on a 2^-10 grid (far finer than their 0.05 noise) and only the used lags are stored, so the file stays small."""
+    rng = np.random.default_rng(11)
+    T = 5200
+
+    def grid(x):
+        return (np.round(x.astype(np.float64) * 1024.0) / 1024.0).astype(np.float32)
+
+    records = {"velocities": grid(signal(rng, T, (2, 1, 3), DT_FS)),
+               "dipole_moment": grid(signal(rng, T, (2, 1, 3), DT_FS))}
+    run_case(mod, "spectra_long", records, [0, 1], 2,
+             [dict(kind="power", resolution=5120), dict(kind="ir", resolution=1024)], acf_lags=True)
+
+
+def main(names=None):
     mod = load_spectra()
+    if names:
+        assert set(names) <= {"spectra_long"}, "only spectra_long is made alone; the others share one generator"
+        long_case(mod)
+        return
     rng = np.random.default_rng(7)
     # power: ragged systems, one of them a single atom, 4 replicas
     sys_ptr = [0, 3, 4, 8]
@@ -151,7 +176,8 @@ def main():
     run_case(mod, "spectra_zero", {"velocities": vel, "dipole_moment": dip, "polarizability": pol}, [0, 2, 3], 1,
              [dict(kind="power", resolution=4096), dict(kind="ir", resolution=4096),
               dict(kind="raman", resolution=4096, averaged=False), dict(kind="raman", resolution=4096, averaged=True)])
+    long_case(mod)
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1:])

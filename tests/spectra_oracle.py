@@ -1,11 +1,14 @@
 """fp64 numpy restatement of md/data/spectra.py in the form of csrc/spectra.cu: centroid, central difference and field
 combinations, per-field normalisation, the autocorrelation as direct lag sums with channel weights, and the spectrum as
-the DCT-II of the windowed lags (no FFT anywhere).  ``fft_autocorrelation`` restates the reference's FFT route for the
-identity test."""
+the DCT-II of the windowed lags.  ``fft_autocorrelation`` restates the reference's FFT route for the identity test.
+
+The direct forms cost n^2 and (4L) L; above DIRECT_MAX (series of a few thousand points) ``spectrum`` takes the
+zero-padded FFT routes instead (``fft_acf``, ``fft_spectrum``), which the CPU tests check against the direct forms."""
 import numpy as np
 
 C_LIGHT = 299792458.0                     # ase.units._c
 RAMAN_FACTOR = 4.160440e-18
+DIRECT_MAX = 10 ** 7                      # largest n (n - 1) and 4 L^2 evaluated directly
 
 
 def cosine_sq_window(n):
@@ -30,8 +33,8 @@ def fields(kind, sys_ptr, m, averaged=False):
     return idx, coef, [(0, [1.0]), (1, [0.5, 0.5, 0.5, 3.0, 3.0, 3.0])]
 
 
-def series(records, index, coef, derivative, dt_fs):
-    """records [T, P, S] -> normalised fields z [F, n] (fp64)"""
+def combine(records, index, coef, derivative, dt_fs):
+    """records [T, P, S] -> the fields x [F, n] before normalisation (fp64)"""
     T, P = records.shape[:2]
     c = records.reshape(T, P, -1).astype(np.float64).mean(axis=1)
     d = (c[2:] - c[:-2]) / (2 * dt_fs) if derivative else c
@@ -40,6 +43,12 @@ def series(records, index, coef, derivative, dt_fs):
         for i, w in zip(ii, cc):
             if i >= 0:
                 x[f] += w * d[:, i]
+    return x
+
+
+def series(records, index, coef, derivative, dt_fs):
+    """records [T, P, S] -> normalised fields z [F, n] (fp64)"""
+    x = combine(records, index, coef, derivative, dt_fs)
     with np.errstate(invalid="ignore", divide="ignore"):
         return (x - x.mean(axis=1, keepdims=True)) / x.std(axis=1, keepdims=True)
 
@@ -48,6 +57,24 @@ def direct_acf(z, n_lags):
     """C[f, k] = (1/n) sum_{t < n-k} z_f[t] z_f[t+k], k < n_lags"""
     n = z.shape[1]
     return np.stack([np.einsum("ft,ft->f", z[:, : n - k], z[:, k:]) / n for k in range(n_lags)], axis=1)
+
+
+def fft_acf(z, n_lags):
+    """direct_acf through the FFT of z zero-padded to 2n (no circular wrap), k < n_lags <= n"""
+    n = z.shape[1]
+    f = np.fft.rfft(z, n=2 * n, axis=1)
+    return np.fft.irfft(f.real ** 2 + f.imag ** 2, n=2 * n, axis=1)[:, :n_lags] / n
+
+
+def fft_spectrum(a, window, dt_fs):
+    """dct_spectrum by the reference's route: |dt FFT| of a [..., L] zero-padded to 4L and mirrored to 8L"""
+    L = a.shape[-1]
+    if window is not None:
+        a = a * window
+    padded = np.zeros(a.shape[:-1] + (4 * L,))
+    padded[..., :L] = a
+    mirrored = np.concatenate((padded[..., ::-1], padded), axis=-1)
+    return 2 * dt_fs * np.abs(0.5 * np.fft.fft(mirrored, n=8 * L, axis=-1)[..., : 4 * L])
 
 
 def fft_autocorrelation(x, n_lags):
@@ -82,14 +109,15 @@ def spectrum(kind, records, sys_ptr, n_replicas, dt_fs, m, resolution=4096, aver
     T = records.shape[0]
     z = series(records.reshape(T, n_replicas, -1), idx, coef, derivative, dt_fs)
     n = z.shape[1]
-    acf_fields = direct_acf(z, n - 1)
+    acf_fields = direct_acf(z, n - 1) if n * (n - 1) <= DIRECT_MAX else fft_acf(z, n - 1)
     L = min(resolution, n - 1)
     chans = []
     for first, w in channels:
         chans.append(sum(wf * acf_fields[first + j] for j, wf in enumerate(w))[:L])
     chans = np.stack(chans)
     win = window(L) if window is not None else None
-    out = [dct_spectrum(a, win, dt_fs) for a in chans]
+    transform = dct_spectrum if 4 * L * L <= DIRECT_MAX else fft_spectrum
+    out = [transform(a, win, dt_fs) for a in chans]
     freq = frequencies(L, dt_fs)
     if kind == "raman":
         with np.errstate(invalid="ignore", divide="ignore"):
@@ -104,7 +132,7 @@ def spectrum(kind, records, sys_ptr, n_replicas, dt_fs, m, resolution=4096, aver
 
 
 PROP = {"power": "velocities", "ir": "dipole_moment", "raman": "polarizability"}
-GOLDEN = ("spectra_power", "spectra_ir", "spectra_raman", "spectra_short", "spectra_zero")
+GOLDEN = ("spectra_power", "spectra_ir", "spectra_raman", "spectra_short", "spectra_zero", "spectra_long")
 
 
 def golden(name):
