@@ -671,7 +671,7 @@ def so3_take_l0(x, lmax: int, F: int):
 
 
 # ------------------------------------------------------------------------------------------------------------ output heads
-HEAD_DIPOLE, HEAD_POLAR = 0, 1
+HEAD_DIPOLE, HEAD_POLAR = _lib.CONSTANTS["SPK_HEAD_DIPOLE"], _lib.CONSTANTS["SPK_HEAD_POLAR"]
 
 
 def geq_ctx(s: Tensor, VW: Tensor, Fi: int, Fo: int) -> Tensor:

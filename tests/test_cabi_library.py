@@ -1,5 +1,6 @@
-"""CPU: the C-ABI shared library builds for sm_90a, loads, and exports every symbol include/spk_b200.h declares
-(no compute calls -- there is no GPU here)."""
+"""CPU: the C-ABI shared library builds for sm_90a, loads, and exports every symbol include/spk_b200.h declares, and the
+binding _lib reads from the header lays the structs out as the C compiler does (no compute calls -- there is no GPU
+here)."""
 import ctypes
 import os
 import re
@@ -29,6 +30,46 @@ def test_header_symbols_exported():
     assert sorted(_lib.SIGNATURES) == declared
     assert h.spk_version() >= 1
     assert h.spk_graph_workspace_bytes  # callable without a device
+
+
+def test_struct_layouts_match_the_c_compiler(tmp_path):
+    """Every parameter struct _lib reads from the header has the C compiler's size and field offsets: field order, types
+    and padding."""
+    import shutil
+    import subprocess
+
+    from schnetpack_b200 import _lib
+
+    cc = shutil.which("cc")
+    if cc is None:
+        pytest.skip("no C compiler")
+    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "spk_b200.h")).read(), flags=re.S)
+    assert sorted(_lib.STRUCTS) == sorted(re.findall(r"\}\s*(\w+)\s*;", text))
+    expected, prints = {}, []
+    for name, struct in _lib.STRUCTS.items():
+        expected[name] = ctypes.sizeof(struct)
+        prints.append(f'printf("{name} %zu\\n", sizeof({name}));')
+        for field, _ in struct._fields_:
+            expected[f"{name}.{field}"] = getattr(struct, field).offset
+            prints.append(f'printf("{name}.{field} %zu\\n", offsetof({name}, {field}));')
+    src = tmp_path / "layout.c"
+    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "spk_b200.h"\nint main(void) {\n'
+                   + "\n".join(prints) + "\nreturn 0;\n}\n")
+    subprocess.run([cc, "-I", os.path.join(ROOT, "include"), str(src), "-o", str(tmp_path / "layout")], check=True)
+    out = subprocess.run([str(tmp_path / "layout")], capture_output=True, text=True, check=True).stdout
+    assert {k: int(v) for k, v in (line.split() for line in out.splitlines())} == expected
+
+
+@pytest.mark.parametrize("header, message", [
+    ("int spk_f(long n, spk_stream_t stream);", "unknown type 'long'"),
+    ("void spk_f(int n);", "spk_f returns 'void'"),
+    ("typedef struct { int16_t n; } spk_s_t;", "unknown type 'int16_t'"),
+])
+def test_header_reader_refuses_unknown_constructs(header, message):
+    from schnetpack_b200 import _lib
+
+    with pytest.raises(ValueError, match=message):
+        _lib.read_header(header)
 
 
 def test_sm100a_sass_present():
