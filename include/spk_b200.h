@@ -1098,6 +1098,48 @@ int spk_md_initial_momenta(float* momenta, const float* masses, const int64_t* i
                            void* workspace, size_t workspace_bytes, spk_stream_t stream);
 int spk_md_step_advance(int64_t* step, spk_stream_t stream);
 
+/* ---- structural observables of the device MD (csrc/structure.cu; DESIGN.md section 24) ------------------------------
+ * Both entry points are hooks inside the captured step: with step (nullable, a device int64 step counter, not advanced)
+ * every kernel returns at once unless step[0] % every == 0.  No float atomics; every fp64 sum has a fixed order.
+ * spk_rdf_accumulate: the pairs the neighbour list lists at cutoff r_max (spk_neighbor_list: ordered (i, j, S) with
+ *   |R_j - R_i + S cell| < r_max, (i, i, 0) excluded, self images included; R [n_atoms, 3], cell [n_sys, 9] fp32, pbc
+ *   [n_sys, 3], all systems periodic) are binned by distance, bin floor(d n_bins / r_max), without being written out.
+ *   Atom i of type ti = type[i] and j of type tj count in slot slot_of[ti n_types + tj] (-1: none) and in total_slot
+ *   (-1: none), as integers.  Then acc [n_out, n_slots, n_bins] fp64 += sum_r V_s counts[s] over the systems
+ *   s = r n_out + o (r ascending; n_out divides n_sys: the beads of a ring polymer fold onto their system),
+ *   volume_sum [n_out] += sum_r V_s and frames[0] += 1, with V_s = |det(volume_cell + s volume_cell_stride)| x
+ *   volume_scale (fp64, stride 0 or 9).  Workspace: spk_rdf_workspace_bytes(n_atoms, n_sys, n_slots, n_bins) bytes,
+ *   zero-initialised once: its count region is left zero by every call.  Seven launches (sampling flag, grid setup,
+ *   bin, sort, cell bounds, traversal, fold); only the sort does work on steps that do not sample.
+ * spk_msd_accumulate: per atom a of n_atoms (ring polymers: the centroid of the n_beads copies positions[r n_atoms + a],
+ *   replica-major) in systems idx_m / sys_ptr [n_sys + 1], species[a] in [0, n_species), n_species <= 8.  State, zero at
+ *   the start: track [n_atoms, 6] fp64 (unwrapped position u, last sampled position), origins [n_slots, n_atoms, 3],
+ *   origin_com [n_slots, n_sys, 3], acc [n_sys, n_species, n_lags] fp64, count [n_lags] int64, meta [2] int64 (samples
+ *   taken, jump flag).  Sample n: u += x - last with the fractional components of the periodic axes wrapped to
+ *   [-1/2, 1/2) in the cell of the atom's system (cell fp64 [*, 9] with stride 0 or 9, pbc [*, 3] with stride 0 or 3;
+ *   both NULL for open systems); meta[1] = 1 if that displacement is longer than half the shortest periodic height.
+ *   Every origin_every samples u (and, with remove_com, the mass-weighted centre of u per system) goes to origin slot
+ *   (n / origin_every) % n_slots, n_slots = ceil(n_lags / origin_every); then for every held origin o with lag
+ *   n - n_o < n_lags, acc[s, c, lag] += sum over the atoms of species c in s of |u - u_o - (com - com_o)|^2 and
+ *   count[lag] += 1.  Workspace: spk_msd_workspace_bytes(n_atoms, n_sys, n_species, n_slots) = 8 (1 + 7 n_sys + 4 n_cta +
+ *   n_slots + n_slots (n_sys + n_cta) W) bytes, n_cta = ceil(n_atoms / 256), W = n_species rounded up to 1, 2, 4 or 8.
+ *   Seven launches with remove_com, five without. */
+size_t spk_rdf_workspace_bytes(int64_t n_atoms, int64_t n_sys, int64_t n_slots, int64_t n_bins);
+int spk_rdf_accumulate(const float* R, const float* cell, const uint8_t* pbc, const int32_t* sys_ptr, int64_t n_atoms,
+                       int64_t n_sys, const int32_t* type, int64_t n_types, const int32_t* slot_of, int32_t total_slot,
+                       int64_t n_slots, float r_max, int64_t n_bins, const double* volume_cell,
+                       int64_t volume_cell_stride, double volume_scale, int64_t n_out, const int64_t* step,
+                       int64_t every, double* acc, double* volume_sum, int64_t* frames, void* workspace,
+                       size_t workspace_bytes, spk_stream_t stream);
+size_t spk_msd_workspace_bytes(int64_t n_atoms, int64_t n_sys, int64_t n_species, int64_t n_slots);
+int spk_msd_accumulate(const float* positions, int64_t n_atoms, int32_t n_beads, const float* masses,
+                       const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_sys, const int32_t* species,
+                       int64_t n_species, const double* cell, int64_t cell_stride, const uint8_t* pbc,
+                       int64_t pbc_stride, int remove_com, int64_t n_lags, int64_t origin_every, int64_t n_slots,
+                       const int64_t* step, int64_t every, double* track, double* origins, double* origin_com,
+                       double* acc, int64_t* count, int64_t* meta, void* workspace, size_t workspace_bytes,
+                       spk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1236,9 +1236,10 @@ class DeviceMD(_CapturedEvaluation):
         ``initializer`` (a ``MaxwellBoltzmannInit`` or ``UniformInit``) sets the starting state as the reference's
         system.initializer does (md/cli.py:154-157): after ring-polymer replication and the binding of the thermostat and
         barostat, before the forces at t = 0; it replaces ``momenta``, which it refuses next to it.  ``hooks`` (a list of
-        ``RemoveCOMMotion`` / ``WrapPositions``) run in the listed order after the step's thermostat or barostat and
-        before the recorder, as the reference's simulation hooks at on_step_finalize; they are gated by a device step
-        counter, which ``state_dict`` carries, so a restarted run keeps their phase.
+        ``RemoveCOMMotion`` / ``WrapPositions`` / ``structure.RadialDistribution`` / ``structure.MeanSquaredDisplacement``)
+        run in the listed order after the step's thermostat or barostat and before the recorder, as the reference's
+        simulation hooks at on_step_finalize; they are gated by a device step counter, which ``state_dict`` carries with
+        the structure hooks' accumulators, so a restarted run keeps their phase and continues bitwise.
 
         ``stream`` (a ``spectra.SpectrumStream``) accumulates the autocorrelations the spectra need inside the step, on
         the steps the recorder would record, before the step counter advances; it works without a recorder, reads the
@@ -1315,6 +1316,9 @@ class DeviceMD(_CapturedEvaluation):
         if initializer is not None:
             initializer.initialize(self)        # md/cli.py:154-157
         self._calculate()                       # forces at t = 0 (simulator.py:118)
+        for h in self.hooks:                    # the accumulators of the structure hooks
+            if hasattr(h, "_bind"):
+                h._bind(self)
         if stream is not None:
             base = self._rp_base if self.ring_polymer is not None else self.systems
             stream._bind(self, base.sys_ptr.tolist(), self._n_replicas())
@@ -1342,10 +1346,15 @@ class DeviceMD(_CapturedEvaluation):
                                 f"{type(initializer).__name__}")
             if momenta is not None:
                 raise ValueError("DeviceMD: pass either momenta or an initializer, which draws them")
+        from .structure import MeanSquaredDisplacement, RadialDistribution
+
         hooks = list(hooks or [])
         for h in hooks:
-            if not isinstance(h, (RemoveCOMMotion, WrapPositions)):
-                raise TypeError(f"DeviceMD: hooks take RemoveCOMMotion and WrapPositions, got {type(h).__name__}")
+            if not isinstance(h, (RemoveCOMMotion, WrapPositions, RadialDistribution, MeanSquaredDisplacement)):
+                raise TypeError(f"DeviceMD: hooks take RemoveCOMMotion, WrapPositions, structure.RadialDistribution and "
+                                f"structure.MeanSquaredDisplacement, got {type(h).__name__}")
+            if getattr(h, "_md", None) is not None:
+                raise ValueError(f"DeviceMD: this {type(h).__name__} already belongs to another DeviceMD")
         return hooks
 
     # ---- motion removal and wrapping (system.py:258-315,652-684) -------------------------------------------------------
@@ -1696,6 +1705,9 @@ class DeviceMD(_CapturedEvaluation):
             state["step_counter"] = self._rec_counter
         if self.stream is not None:
             state["stream"] = self.stream._state()
+        accumulators = {str(k): h._state() for k, h in enumerate(self.hooks) if hasattr(h, "_state")}
+        if accumulators:
+            state["hooks"] = accumulators
         return state
 
     def run(self, n_steps: int):
@@ -1713,6 +1725,9 @@ class DeviceMD(_CapturedEvaluation):
             self._n_records += self._records_in(int(n_steps))
         self.steps_done += int(n_steps)
         self.check_neighbor_list()
+        for h in self.hooks:
+            if hasattr(h, "_check"):
+                h._check()
         return self.energy, self.forces
 
     def kinetic_energy(self) -> Tensor:
