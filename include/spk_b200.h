@@ -300,7 +300,12 @@ int spk_md_velocity_verlet(float* momenta, float* positions, float* model_positi
  *                          counter [2] uint64 on the DEVICE: [0] = application index, advanced by one in stream order by
  *                          every call (so a replayed graph draws fresh noise each time), [1] = 0 (internal ticket).
  *   spk_philox4x32_10      out[4 i + k] = word k of the Philox4x32-10 draw for element i, application counter[0], key
- *                          seed (counter not advanced): the raw bits behind spk_md_langevin. */
+ *                          seed (counter not advanced): the raw bits behind spk_md_langevin.
+ * Per-system bath temperatures (DESIGN.md section 25): kb_temperature_sys [n_sys] fp64 on the device holds kB T_s of every
+ * system.  spk_md_langevin_per_system is spk_md_langevin with kB T_s of the atom's system idx_m[a]; spk_md_nhc_per_system
+ * is spk_md_nhc with every chain forced at kB T_s of its system (of its atom's system when massive; idx_m is read then),
+ * params->kb_temperature unused.  The chain masses chain_m must be built from the same kB T_s.  With every kB T_s equal to
+ * kb_temperature they give bitwise the results of the scalar entry points. */
 typedef struct {
     int32_t chain_length;  /* >= 1 */
     int32_t multi_step;    /* >= 1 */
@@ -323,6 +328,13 @@ int spk_md_nhc(float* momenta, const float* masses, const int64_t* idx_m, const 
 int spk_md_langevin(float* momenta, const float* masses, int64_t n_atoms, double c1, double c2, double kb_temperature,
                     uint64_t seed, uint64_t* counter, spk_stream_t stream);
 int spk_philox4x32_10(uint64_t seed, const uint64_t* counter, int64_t n, uint32_t* out, spk_stream_t stream);
+int spk_md_langevin_per_system(float* momenta, const float* masses, const int64_t* idx_m, int64_t n_atoms, double c1,
+                               double c2, const double* kb_temperature_sys, uint64_t seed, uint64_t* counter,
+                               spk_stream_t stream);
+int spk_md_nhc_per_system(float* momenta, const float* masses, const int64_t* idx_m, const int32_t* sys_ptr,
+                          int64_t n_atoms, int64_t n_sys, const spk_nhc_params_t* params,
+                          const double* kb_temperature_sys, double* chain_v, double* chain_f, const double* chain_m,
+                          void* workspace, size_t workspace_bytes, spk_stream_t stream);
 
 /* ---- per-system virial (csrc/geometry.cu): W[m][b][a] = sum_{e in m} g_rij[e][b] * r_ij[e][a] in fp64, the strain
  * derivative dE/d(strain) of atomistic/response.py:78-90 (Strain maps r_e -> r_e (1 + strain^T)); the stress is W / V.
@@ -1139,6 +1151,33 @@ int spk_msd_accumulate(const float* positions, int64_t n_atoms, int32_t n_beads,
                        const int64_t* step, int64_t every, double* track, double* origins, double* origin_com,
                        double* acc, int64_t* count, int64_t* meta, void* workspace, size_t workspace_bytes,
                        spk_stream_t stream);
+
+/* ---- temperature replica exchange in the device MD (csrc/exchange.cu; DESIGN.md section 25) ------------------------
+ * spk_remd_exchange: one exchange attempt over n_groups * n_rungs systems, rung-major (system k n_groups + g is rung k of
+ *   group g; the systems of a group have equal atom counts, so atom a of system s sits at sys_ptr[s] + a).  With step
+ *   (nullable, a device int64 step counter, not advanced) both kernels return at once unless step[0] % every == 0.
+ *   Attempt n = attempt[0] (device int64, advanced by one) tries the pairs (k, k + 1) with k = n (mod 2) of every group:
+ *   Delta = (1 / (kB T_k) - 1 / (kB T_k+1)) (U_k - U_k+1) in fp64 with U = energy[s] * energy_conversion and T =
+ *   temperature[s] (fp64, K); the pair is accepted iff Delta >= 0 or u < exp(Delta), u = (x + 1/2) 2^-32 with x word 0
+ *   of the Philox4x32-10 draw of key seed and counter (g (n_rungs - 1) + k, 2^63 + n).  decision [n_groups, n_rungs - 1]
+ *   uint8 is set to 1 for the pairs that swap on this attempt and 0 for the others; attempted / accepted
+ *   [n_groups, n_rungs - 1] int64 count the tried and accepted pairs; walker [n_rungs n_groups] int32 exchanges its two
+ *   entries on every swap.  A swap exchanges the momenta [n_atoms, 3] of the two systems, rescaled by
+ *   sqrt(T_new / T_old) in fp64 and rounded once to fp32, and the rows of every buffer of *buffers (nullable: none): per
+ *   atom or per system, width floats each, copied unchanged.  No atomics.  Two launches (decide, swap). */
+#define SPK_REMD_MAX_BUFFERS 16
+typedef struct {
+    int32_t n_buffers;     /* buffers used, <= SPK_REMD_MAX_BUFFERS */
+    int32_t per_atom[16];  /* 1: one row per atom, 0: one row per system */
+    int64_t width[16];     /* floats per row, >= 1 */
+    float* data[16];       /* device fp32 buffers, swapped in place */
+} spk_remd_buffers_t;
+
+int spk_remd_exchange(const float* energy, double energy_conversion, const double* temperature, double kB,
+                      const int64_t* idx_m, const int32_t* sys_ptr, int64_t n_atoms, int64_t n_groups, int32_t n_rungs,
+                      uint64_t seed, const int64_t* step, int64_t every, int64_t* attempt, int32_t* walker,
+                      int64_t* attempted, int64_t* accepted, uint8_t* decision, float* momenta,
+                      const spk_remd_buffers_t* buffers, spk_stream_t stream);
 
 #ifdef __cplusplus
 }

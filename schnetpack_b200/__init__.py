@@ -7,7 +7,8 @@ callers either side of the path: ``neighbors.CellListNeighborList`` (device-resi
 (CUDA-graph velocity-Verlet step), ``relax.DeviceLBFGS`` (batchwise L-BFGS relaxation in a CUDA graph), ``neb.DeviceNEB``
 (climbing-image nudged elastic band, every image of every band in one captured step), ``parallel``
 (batch sharding, graph partition + halo exchange), ``structure`` (radial distribution functions and mean-squared
-displacements accumulated inside the captured MD step).
+displacements accumulated inside the captured MD step), ``exchange`` (temperature replica exchange in the captured MD
+step).
 All arithmetic runs in the hand-written CUDA library ``csrc/libspk_b200.so`` (C ABI: ``include/spk_b200.h``).
 """
 from . import properties  # noqa: F401
@@ -18,6 +19,7 @@ from . import model  # noqa: F401
 from . import neighbors  # noqa: F401
 from . import md  # noqa: F401
 from . import structure  # noqa: F401
+from . import exchange  # noqa: F401
 from . import relax  # noqa: F401
 from . import neb  # noqa: F401
 from . import parallel  # noqa: F401

@@ -165,11 +165,12 @@ LAUNCHES = {"spk_graph_build": 8, "spk_graph_build_active": 8, "spk_atomwise_out
             "spk_fire_forces": 3, "spk_fire_step": 2, "spk_md_remove_motion": 3, "spk_spectrum_stream_push": 2,
             "spk_spectrum_stream_finalise": 2, "spk_neb_forces": 3, "spk_pme_spread": 8,
             "spk_pme_energy": 2, "spk_pme_bwd": 2, "spk_ph_thermo": 2, "spk_rdf_accumulate": 7,
-            "spk_msd_accumulate": 7}
+            "spk_msd_accumulate": 7, "spk_md_nhc_per_system": 3, "spk_remd_exchange": 2}
 # spk_pme_spread: 4 without atoms (cell, setup, scan, spread); spk_pme_bwd: 1 per part present (atoms, cell or virial);
 # spk_ph_force_constants: 1 + the rounds run;
 # spk_rdf_accumulate: 2 without atoms (gate, fold); spk_msd_accumulate: 5 without remove_com;
 # spk_relax_step: 1 per size path present; spk_rpmd_pile / spk_rpmd_nhc: 3 if global; spk_md_initial_momenta: 4 if uniform
+# spk_md_nhc_per_system: 1 if massive (no kinetic-energy passes)
 launch_count = 0
 
 

@@ -90,7 +90,7 @@ __global__ void k_baro_thermostat(const __grid_constant__ spk_nhc_barostat_t b, 
         double ke2, k2[9];
         system_ke(sys_ptr, w, s, ke2, k2);
         const double dof = 3.0 * (double)(sys_ptr[s + 1] - sys_ptr[s]);
-        w.scale[s] = nhc_propagate(ke2, dof, q, b.t_v + s * L, b.t_f + s * L, b.t_m + s * L);
+        w.scale[s] = nhc_propagate(ke2, dof, q, q.kb_temperature, b.t_v + s * L, b.t_f + s * L, b.t_m + s * L);
     }
     const int nb = b.anisotropic ? 9 : 1;
     double* bv = b.b_v + s * nb;
@@ -102,7 +102,8 @@ __global__ void k_baro_thermostat(const __grid_constant__ spk_nhc_barostat_t b, 
     } else {
         ke_cell = b.b_m[s] * (bv[0] * bv[0]);
     }
-    const double sc = nhc_propagate(ke_cell, b.anisotropic ? 6.0 : 1.0, q, b.c_v + s * L, b.c_f + s * L, b.c_m + s * L);
+    const double sc = nhc_propagate(ke_cell, b.anisotropic ? 6.0 : 1.0, q, q.kb_temperature, b.c_v + s * L, b.c_f + s * L,
+                                    b.c_m + s * L);
     for (int k = 0; k < nb; ++k) bv[k] = bv[k] * sc;          // :473-481, :798-808
 }
 
@@ -295,7 +296,7 @@ extern "C" int spk_md_barostat_thermostat(const spk_nhc_barostat_t* b, float* mo
             spk_nhc_params_t q = {b->chain_length, b->multi_step, b->order, 1, b->kb_temperature, {}};
             for (int k = 0; k < 7; ++k) q.time_step[k] = b->ys_time_step[k];
             spk_launch(k_nhc_massive, (unsigned)spk_cdiv(n_atoms * 3, 128), 128, 0, st, momenta, masses, n_atoms * 3, q,
-                       b->t_v, b->t_f, b->t_m);
+                       nullptr, nullptr, b->t_v, b->t_f, b->t_m);
         } else {
             spk_launch(k_scale_momenta, (unsigned)spk_cdiv(n_atoms * 3, ELT_T), ELT_T, 0, st, momenta, idx_m, w.scale,
                        n_atoms * 3);

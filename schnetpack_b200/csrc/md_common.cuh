@@ -8,11 +8,11 @@
 namespace {
 
 // thermostats.py:398-468 for one chain (barostats.py:408-481 runs the same propagation on the particle and on the cell
-// chains); v, f, M point at its chain_length entries.  Operation order as in the reference.
-__device__ double nhc_propagate(double ke, double dof, const spk_nhc_params_t& q, double* __restrict__ v,
+// chains); v, f, M point at its chain_length entries and kbt is the chain's kB T (q.kb_temperature, or the bath
+// temperature of the chain's system).  Operation order as in the reference.
+__device__ double nhc_propagate(double ke, double dof, const spk_nhc_params_t& q, double kbt, double* __restrict__ v,
                                 double* __restrict__ f, const double* __restrict__ M) {
     const int L = q.chain_length;
-    const double kbt = q.kb_temperature;
     f[0] = (ke - dof * kbt) / M[0];
     double scaling = 1.0;
     for (int ms = 0; ms < q.multi_step; ++ms) {
@@ -44,18 +44,20 @@ __global__ void k_scale_momenta(float* __restrict__ p, const int64_t* __restrict
     p[i] = (float)(scale[idx_m[i / 3]] * (double)p[i]);
 }
 
-// massive NHC: one chain per degree of freedom (thermostats.py:348-354,483-487), one thread per chain
+// massive NHC: one chain per degree of freedom (thermostats.py:348-354,483-487), one thread per chain.  kbt_sys (nullable)
+// holds kB T per system, read through idx_m; without it every chain uses q.kb_temperature.
 __global__ void k_nhc_massive(float* __restrict__ p, const float* __restrict__ m, int64_t n_dof,
-                              const __grid_constant__ spk_nhc_params_t q,
-                              double* __restrict__ chain_v, double* __restrict__ chain_f,
-                              const double* __restrict__ chain_m) {
+                              const __grid_constant__ spk_nhc_params_t q, const int64_t* __restrict__ idx_m,
+                              const double* __restrict__ kbt_sys, double* __restrict__ chain_v,
+                              double* __restrict__ chain_f, const double* __restrict__ chain_m) {
     SPK_PDL_ENTER();
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= n_dof) return;
     const double pi = (double)p[i];
     const double ke = pi * pi / (double)m[i / 3];
     const int L = q.chain_length;
-    const double sc = nhc_propagate(ke, 1.0, q, chain_v + i * L, chain_f + i * L, chain_m + i * L);
+    const double kbt = kbt_sys ? kbt_sys[idx_m[i / 3]] : q.kb_temperature;
+    const double sc = nhc_propagate(ke, 1.0, q, kbt, chain_v + i * L, chain_f + i * L, chain_m + i * L);
     p[i] = (float)(pi * sc);
 }
 

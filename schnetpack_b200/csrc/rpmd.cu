@@ -212,7 +212,8 @@ __global__ void __launch_bounds__(RP_THREADS) k_rpmd_modes(const __grid_constant
             }
             const int L = A.q.chain_length;
             const int64_t row = (int64_t)k * n_dof + i;
-            pn *= nhc_propagate(ke, dof, A.q, A.chain_v + row * L, A.chain_f + row * L, A.chain_m + row * L);
+            pn *= nhc_propagate(ke, dof, A.q, A.q.kb_temperature, A.chain_v + row * L, A.chain_f + row * L,
+                                A.chain_m + row * L);
         }
         if (HAS_X) mx[j] = xn;
         mp[j] = pn;

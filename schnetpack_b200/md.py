@@ -121,10 +121,10 @@ class _Systems:
             ws = self._workspaces[size_fn] = torch.empty(nbytes, dtype=torch.uint8, device=self.masses.device)
         return ws
 
-    def call(self, name: str, momenta: Tensor, *args):
+    def call(self, name: str, momenta: Tensor, *args, launches: Optional[int] = None):
         ws = self.workspace("spk_md_thermostat_workspace_bytes")
         _lib.call(name, ops._p(momenta), ops._p(self.masses), ops._p(self.idx_m), ops._p(self.sys_ptr), self.n_atoms,
-                  self.n_sys, *args, ops._p(ws), ws.numel(), ops._stream())
+                  self.n_sys, *args, ops._p(ws), ws.numel(), ops._stream(), launches=launches)
 
     def kinetic_energy_and_temperature(self, momenta: Tensor, kB: float):
         dev = momenta.device
@@ -204,6 +204,29 @@ class _TensorState:
         _load_state(self._state(), state)
 
 
+def _bath_temperature(value, who: str, per_system: bool = False):
+    """``temperature_bath`` as one float in K, or as a list of floats when it is a sequence or tensor of them, which only
+    thermostats with ``per_system`` take"""
+    if isinstance(value, (int, float)):
+        return float(value)
+    temps = torch.as_tensor(value, dtype=torch.float64)
+    if temps.dim() == 0:
+        return float(temps)
+    if not per_system:
+        raise ValueError(f"{who}: temperature_bath must be one number; only LangevinThermostat and NHCThermostat take one "
+                         "temperature per system")
+    if temps.numel() == 0:
+        raise ValueError(f"{who}: temperature_bath is an empty sequence")
+    return [float(t) for t in temps.reshape(-1).tolist()]
+
+
+def _one_per_system(temps: List[float], n_sys: int, who: str) -> Tensor:
+    """[n_sys] fp64 (host) from one temperature or one per system"""
+    if len(temps) not in (1, n_sys):
+        raise ValueError(f"{who}: {len(temps)} temperatures for {n_sys} systems; give one temperature or one per system")
+    return torch.tensor(temps * (n_sys if len(temps) == 1 else 1), dtype=torch.float64)
+
+
 def _noise(seed: int, device) -> tuple:
     """(seed, counter) of a Philox noise hook: the seed taken to 64 bits and a fresh device counter laid out as
     advance_counter (md_common.cuh) reads it, [0] = application index, [1] = the kernel's internal ticket (zero between
@@ -233,10 +256,15 @@ def _ys_steps(time_step: float, multi_step: int, integration_order: int):
     return (ctypes.c_double * 7)(*([time_step * wk / multi_step for wk in w] + [0.0] * (7 - len(w))))
 
 
-def _chain_masses(n_chains: int, dof, chain_length: int, kbt: float, frequency: float, device) -> Tensor:
+def _chain_masses(n_chains: int, dof, chain_length: int, kbt, frequency: float, device) -> Tensor:
     """[n_chains, chain_length] fp64 chain masses kB T / omega^2, the first link times the degrees of freedom ``dof`` of
-    its chain (a number or an [n_chains] tensor) (thermostats.py:387-396)"""
-    masses = torch.full((n_chains, chain_length), kbt / frequency ** 2, dtype=torch.float64, device=device)
+    its chain (a number or an [n_chains] tensor) (thermostats.py:387-396).  ``kbt`` is a number or an [n_chains] tensor;
+    a tensor goes through the same fp64 operations, elementwise, so equal values give the same bits."""
+    if isinstance(kbt, Tensor):       # true division (torch divides a device tensor by a number via its reciprocal)
+        link = torch.from_numpy(kbt.cpu().numpy() / frequency ** 2).to(device)
+        masses = link[:, None].repeat(1, chain_length)
+    else:
+        masses = torch.full((n_chains, chain_length), kbt / frequency ** 2, dtype=torch.float64, device=device)
     masses[:, 0] = dof * kbt / frequency ** 2
     return masses
 
@@ -245,18 +273,36 @@ class _Thermostat(_TensorState):
     """Common part of the device thermostats (ThermostatHook, thermostats.py:41-146): bath temperature in K, time constant
     in fs.  ``kB`` (MD energy per kelvin) and ``fs`` (one femtosecond in MD time) define the caller's MD units; the
     defaults are the reference's (kJ/mol, nm, Da).  ``bind`` sizes the state for a batch, ``apply`` updates the momenta in
-    place (enqueue-only, capturable)."""
+    place (enqueue-only, capturable).
 
-    def __init__(self, temperature_bath: float, time_constant: float, kB: float = KB_MD, fs: float = FS_MD):
-        self.temperature_bath = float(temperature_bath)
+    Thermostats with ``takes_per_system`` (Langevin, NHC) also take a sequence or tensor of bath temperatures: one, or one
+    per system of the batch, checked by ``bind``, which keeps them as ``temperatures`` (fp64 [n_sys] on the device) and
+    ``kb_temperatures`` (kB T_s).  ``temperatures`` is None with one number."""
+
+    takes_per_system = False
+
+    def __init__(self, temperature_bath, time_constant: float, kB: float = KB_MD, fs: float = FS_MD):
+        self.temperature_bath = _bath_temperature(temperature_bath, type(self).__name__, self.takes_per_system)
         self.time_constant = float(time_constant) * float(fs)          # thermostats.py:57-59
         self.kB = float(kB)
         self.systems: Optional[_Systems] = None
         self.time_step: Optional[float] = None
+        self.temperatures: Optional[Tensor] = None
+        self.kb_temperatures: Optional[Tensor] = None
+
+    @property
+    def per_system(self) -> bool:
+        return isinstance(self.temperature_bath, list)
 
     def bind(self, systems: _Systems, time_step: float):
         self.systems = systems
         self.time_step = float(time_step)
+        if self.per_system:
+            t = _one_per_system(self.temperature_bath, systems.n_sys, type(self).__name__)
+            if not bool((t >= 0.0).all()):
+                raise ValueError(f"{type(self).__name__}: bath temperatures must be >= 0 K, got {t.min().item()}")
+            self.temperatures = t.to(systems.masses.device)
+            self.kb_temperatures = self.temperatures * self.kB          # the scalar path's kB * T, elementwise
         self._init_state()
 
     def _init_state(self):
@@ -278,9 +324,12 @@ class BerendsenThermostat(_Thermostat):
 class LangevinThermostat(_Thermostat):
     """Langevin thermostat (thermostats.py:192-261): p = c1 p + c2 sqrt(m kB T_bath) xi with c1 = exp(-dt / (2 tau)),
     c2 = sqrt(1 - c1^2).  xi comes from Philox4x32-10 keyed by ``seed`` with the counter (atom, application); the
-    application index lives on the device and advances with every application, also inside a replayed graph."""
+    application index lives on the device and advances with every application, also inside a replayed graph.
+    ``temperature_bath`` may give one temperature per system: T_bath is then that of the atom's system."""
 
-    def __init__(self, temperature_bath: float, time_constant: float, seed: int = 0, kB: float = KB_MD,
+    takes_per_system = True
+
+    def __init__(self, temperature_bath, time_constant: float, seed: int = 0, kB: float = KB_MD,
                  fs: float = FS_MD):
         super().__init__(temperature_bath, time_constant, kB=kB, fs=fs)
         self.seed = seed
@@ -293,6 +342,10 @@ class LangevinThermostat(_Thermostat):
 
     def apply(self, momenta: Tensor):
         s = self.systems
+        if self.per_system:
+            _lib.call("spk_md_langevin_per_system", ops._p(momenta), ops._p(s.masses), ops._p(s.idx_m), s.n_atoms,
+                      self.c1, self.c2, ops._p(self.kb_temperatures), self.seed, ops._p(self.counter), ops._stream())
+            return
         _lib.call("spk_md_langevin", ops._p(momenta), ops._p(s.masses), s.n_atoms, self.c1, self.c2,
                   self.kB * self.temperature_bath, self.seed, ops._p(self.counter), ops._stream())
 
@@ -303,9 +356,12 @@ class LangevinThermostat(_Thermostat):
 class NHCThermostat(_Thermostat):
     """Nose-Hoover chain thermostat (thermostats.py:264-513) with the reference's keywords and defaults: one chain per
     system, or per degree of freedom with ``massive``; ``multi_step`` sub-steps of a Yoshida-Suzuki scheme of order
-    ``integration_order`` (3, 5 or 7).  The chain state is fp64 on the device."""
+    ``integration_order`` (3, 5 or 7).  The chain state is fp64 on the device.  With one ``temperature_bath`` per system,
+    the masses and forces of every chain use kB T_s of its system (of its atom's system with ``massive``)."""
 
-    def __init__(self, temperature_bath: float, time_constant: float, chain_length: int = 3, massive: bool = False,
+    takes_per_system = True
+
+    def __init__(self, temperature_bath, time_constant: float, chain_length: int = 3, massive: bool = False,
                  multi_step: int = 2, integration_order: int = 3, kB: float = KB_MD, fs: float = FS_MD):
         super().__init__(temperature_bath, time_constant, kB=kB, fs=fs)
         _check_nhc(chain_length, multi_step, integration_order)
@@ -318,18 +374,29 @@ class NHCThermostat(_Thermostat):
     def _init_state(self):
         s = self.systems
         dev = s.masses.device
-        kbt = self.temperature_bath * self.kB                             # :308
+        if self.per_system and not bool((self.temperatures > 0.0).all()):
+            raise ValueError("NHCThermostat: bath temperatures must be > 0 K (they set the chain masses)")
+        kbt = self.kb_temperatures if self.per_system else self.temperature_bath * self.kB     # :308
         if self.massive:                                                  # :348-359
             dof = torch.ones(3 * s.n_atoms, dtype=torch.float64, device=dev)
+            chain_kbt = kbt[s.idx_m].repeat_interleave(3) if self.per_system else kbt
         else:
             dof = 3.0 * s.n_atoms_sys
-        self.masses = _chain_masses(dof.shape[0], dof, self.chain_length, kbt, 1.0 / self.time_constant, dev)  # :304
+            chain_kbt = kbt
+        self.masses = _chain_masses(dof.shape[0], dof, self.chain_length, chain_kbt, 1.0 / self.time_constant,  # :304
+                                    dev)
         self.velocities = torch.zeros_like(self.masses)
         self.forces = torch.zeros_like(self.masses)
-        self.params = _lib.NHCParams(self.chain_length, self.multi_step, self.integration_order, int(self.massive), kbt,
+        self.params = _lib.NHCParams(self.chain_length, self.multi_step, self.integration_order, int(self.massive),
+                                     0.0 if self.per_system else kbt,
                                      _ys_steps(self.time_step, self.multi_step, self.integration_order))
 
     def apply(self, momenta: Tensor):
+        if self.per_system:
+            self.systems.call("spk_md_nhc_per_system", momenta, ctypes.byref(self.params), ops._p(self.kb_temperatures),
+                              ops._p(self.velocities), ops._p(self.forces), ops._p(self.masses),
+                              launches=1 if self.massive else None)
+            return
         self.systems.call("spk_md_nhc", momenta, ctypes.byref(self.params), ops._p(self.velocities),
                           ops._p(self.forces), ops._p(self.masses))
 
@@ -354,7 +421,7 @@ class _NHCBarostat(_TensorState):
                  kB: float = KB_MD, fs: float = FS_MD, bar: float = BAR_MD):
         _check_nhc(chain_length, multi_step, integration_order)
         self.target_pressure = float(target_pressure) * float(bar)               # :51-53
-        self.temperature_bath = float(temperature_bath)
+        self.temperature_bath = _bath_temperature(temperature_bath, type(self).__name__)
         self.time_constant = float(time_constant) * float(fs)
         self.frequency = 1.0 / self.time_constant                               # :209
         self.cell_frequency = self.frequency if time_constant_cell is None else 1.0 / (float(time_constant_cell) * fs)
@@ -842,7 +909,7 @@ class PILEBarostat(_TensorState):
     def __init__(self, target_pressure: float, temperature_bath: float, time_constant: float, seed: int = 0,
                  kB: float = KB_MD, fs: float = FS_MD, bar: float = BAR_MD):
         self.target_pressure = float(target_pressure) * float(bar)               # barostats.py:51-53
-        self.temperature_bath = float(temperature_bath)
+        self.temperature_bath = _bath_temperature(temperature_bath, type(self).__name__)
         self.time_constant = float(time_constant) * float(fs)
         self.frequency = 1.0 / self.time_constant                               # barostats_rpmd.py:53
         self.kB = float(kB)
@@ -931,12 +998,7 @@ class _Initializer:
 
     def system_temperatures(self, n_sys: int, n_copies: int, device) -> Tensor:
         """[n_copies n_sys] fp64 target temperature of every (bead) system (initial_conditions.py:57-61)"""
-        t = self.temperature
-        if len(t) not in (1, n_sys):
-            raise ValueError(f"{type(self).__name__}: {len(t)} temperatures for {n_sys} systems; give one temperature or "
-                             "one per system")
-        t = torch.tensor(t * (n_sys if len(t) == 1 else 1), dtype=torch.float64)
-        return t.repeat(n_copies).to(device)
+        return _one_per_system(self.temperature, n_sys, type(self).__name__).repeat(n_copies).to(device)
 
     def initialize(self, md: "DeviceMD"):
         """initialize_system (initial_conditions.py:50-75) on the state of ``md``, in place"""
@@ -1236,10 +1298,11 @@ class DeviceMD(_CapturedEvaluation):
         ``initializer`` (a ``MaxwellBoltzmannInit`` or ``UniformInit``) sets the starting state as the reference's
         system.initializer does (md/cli.py:154-157): after ring-polymer replication and the binding of the thermostat and
         barostat, before the forces at t = 0; it replaces ``momenta``, which it refuses next to it.  ``hooks`` (a list of
-        ``RemoveCOMMotion`` / ``WrapPositions`` / ``structure.RadialDistribution`` / ``structure.MeanSquaredDisplacement``)
-        run in the listed order after the step's thermostat or barostat and before the recorder, as the reference's
-        simulation hooks at on_step_finalize; they are gated by a device step counter, which ``state_dict`` carries with
-        the structure hooks' accumulators, so a restarted run keeps their phase and continues bitwise.
+        ``RemoveCOMMotion`` / ``WrapPositions`` / ``structure.RadialDistribution`` / ``structure.MeanSquaredDisplacement`` /
+        ``exchange.ReplicaExchange``) run in the listed order after the step's thermostat or barostat and before the
+        recorder, as the reference's simulation hooks at on_step_finalize; they are gated by a device step counter, which
+        ``state_dict`` carries with the structure hooks' accumulators and the exchange statistics, so a restarted run keeps
+        their phase and continues bitwise.
 
         ``stream`` (a ``spectra.SpectrumStream``) accumulates the autocorrelations the spectra need inside the step, on
         the steps the recorder would record, before the step counter advances; it works without a recorder, reads the
@@ -1346,13 +1409,16 @@ class DeviceMD(_CapturedEvaluation):
                                 f"{type(initializer).__name__}")
             if momenta is not None:
                 raise ValueError("DeviceMD: pass either momenta or an initializer, which draws them")
+        from .exchange import ReplicaExchange
         from .structure import MeanSquaredDisplacement, RadialDistribution
 
         hooks = list(hooks or [])
         for h in hooks:
-            if not isinstance(h, (RemoveCOMMotion, WrapPositions, RadialDistribution, MeanSquaredDisplacement)):
-                raise TypeError(f"DeviceMD: hooks take RemoveCOMMotion, WrapPositions, structure.RadialDistribution and "
-                                f"structure.MeanSquaredDisplacement, got {type(h).__name__}")
+            if not isinstance(h, (RemoveCOMMotion, WrapPositions, RadialDistribution, MeanSquaredDisplacement,
+                                  ReplicaExchange)):
+                raise TypeError(f"DeviceMD: hooks take RemoveCOMMotion, WrapPositions, structure.RadialDistribution, "
+                                f"structure.MeanSquaredDisplacement and exchange.ReplicaExchange, got "
+                                f"{type(h).__name__}")
             if getattr(h, "_md", None) is not None:
                 raise ValueError(f"DeviceMD: this {type(h).__name__} already belongs to another DeviceMD")
         return hooks
@@ -1492,6 +1558,7 @@ class DeviceMD(_CapturedEvaluation):
             n_rep = self._n_replicas()
             self._records["velocities"] = torch.zeros(self.record_capacity, n_rep, self.positions.shape[0] // n_rep, 3,
                                                       dtype=torch.float32, device=self.positions.device)
+        self._hook_series: Dict[str, Tensor] = {}    # series a hook records from its own buffer (name -> source)
         self._n_records = 0                      # host mirror of the device count: the record count is deterministic
         self._rec_counter = torch.zeros(2, dtype=torch.int64, device=self.positions.device)
 
@@ -1573,7 +1640,7 @@ class DeviceMD(_CapturedEvaluation):
                           ops._p(self._rec_counter), self.record_every, self.record_capacity, ops._p(rec),
                           ops._stream())
                 continue
-            buf = self.properties[p]
+            buf = self._hook_series[p] if p in self._hook_series else self.properties[p]
             _lib.call("spk_md_record", ops._p(buf), buf.numel(), ops._p(self._rec_counter), self.record_every,
                       self.record_capacity, ops._p(rec), ops._stream())
         _lib.call("spk_md_record_advance", ops._p(self._rec_counter), self.record_every, self.record_capacity,
@@ -1603,7 +1670,8 @@ class DeviceMD(_CapturedEvaluation):
         vel = self._records.get("velocities")
         return RecordedSeries(self.record_every * self.dt / FS_MD, base.sys_ptr, self._n_replicas(),
                               velocities=None if vel is None else vel[:n],
-                              properties={p: v[:n] for p, v in self._records.items() if p != "velocities"})
+                              properties={p: v[:n] for p, v in self._records.items()
+                                          if p != "velocities" and p not in self._hook_series})
 
     def drain(self) -> Dict[str, Tensor]:
         """Return every recorded series (as ``recorded``) and empty the recorder."""
